@@ -137,6 +137,52 @@ int b200sa_doc_ids_dev(b200sa_ctx *ctx, const uint32_t *d_pos, uint64_t count,
 int b200sa_lcp_intervals_dev(b200sa_ctx *ctx, const uint32_t *d_lcp, uint64_t n,
                              uint32_t *d_psv, uint32_t *d_nsv, void *stream);
 
+/* ---- suffix tree (SURVEY.md 8f-5; reference suffix_tree/src/lib.rs:392-505) ----
+ * SuffixTree::from_suffix_table (:74-76) builds its tree with a serial insertion loop over
+ * table() and lcp_lens() (to_suffix_tree, :392-505).  These entry points build the same tree
+ * (structure, child order, string depths, label bytes, terminals) data-parallel from SA + LCP
+ * and return it as arrays indexed by preorder id.  The reference's preorder is lexicographic
+ * (children are keyed by the first byte of their label).  With lcp[n] := 0,
+ * psv[i] = largest j < i with lcp[j] < lcp[i], nsv[i] = smallest j > i with lcp[j] < lcp[i] (or n),
+ * pse[i] = largest j < i with lcp[j] <= lcp[i]:
+ *   1. root: range [0, n), depth 0, parent 0xFFFFFFFF; its terminal is n (suffix_tree :84).
+ *   2. internal nodes: one per boundary i in [1, n) with lcp[i] > 0 and pse[i] == psv[i];
+ *      range [psv[i], nsv[i]), depth lcp[i].
+ *   3. rank r is merged iff r+1 < n and lcp[r+1] == n - sa[r]: suffix sa[r] ends at the internal
+ *      node of boundary r+1 (which keeps it as terminal and has children, :128-131, :432).  Every
+ *      other rank r is a leaf: range [r, r+1), depth n - sa[r].
+ *   4. preorder = ascending (sa_lo, depth); N = 1 + #internal + n - #merged <= 2n.
+ *   5. parent of [lo, hi) (not the root): pd = max(lcp[lo], lcp[hi]); pd == 0: the root, else
+ *      the node (plo, pd) with plo = lo if lcp[hi] > lcp[lo], else psv[lo].
+ *   6. label = text[sa[lo] + pd, sa[lo] + depth); the node carries terminal sa[lo] iff
+ *      depth == n - sa[lo].  (The reference's own label offsets of internal nodes depend on its
+ *      insertion history, :474-480; the bytes are the same.)
+ *   7. subtree_end = first[hi] (smallest id with sa_lo == hi) if hi < n, else N.
+ *   8. children of v: v+1, then subtree_end of each child, while below subtree_end[v].
+ * Every array of `out` holds at least `cap` entries; cap must be >= max(1, 2n).  On success
+ * *num_nodes = N and entries [0, N) are written.  n = 0 gives the root alone (subtree_end 1).
+ * Inputs are checked on the device (sa[r] < n, lcp[0] == 0, lcp[r] <= n - sa[r-1] and
+ * <= n - sa[r], and every parent lookup finds its node): B200SA_ERR_BAD_ARG with a
+ * b200sa_last_error detail otherwise.  Node ids are u32 with 0xFFFFFFFF reserved, so
+ * n > B200SA_TREE_MAX_N returns B200SA_ERR_TOO_LARGE.  Device workspace is about 66 bytes per
+ * text byte (the host entry point adds 56 for staging); B200SA_ERR_OOM if it cannot be had.
+ * Measured on one H100 80GB HBM3 (400 W limit), device entry with the inputs and the six
+ * arrays on the same card: n = 671,088,640 fits, n = 805,306,368 returns B200SA_ERR_OOM. */
+#define B200SA_TREE_MAX_N 0x7FFFFFFFull
+typedef struct {
+    uint32_t *parent;       /* preorder id of the parent; 0xFFFFFFFF for the root (id 0)     */
+    uint32_t *depth;        /* string depth (the reference's path_len)                       */
+    uint32_t *sa_lo, *sa_hi;/* the subtree holds exactly the suffixes sa[sa_lo..sa_hi)       */
+    uint32_t *label_start;  /* label = text[label_start, label_start + depth - depth[parent]) */
+    uint32_t *subtree_end;  /* preorder id one past the node's last descendant               */
+} b200sa_tree;
+/* device buffers (sa, lcp in; the six arrays out); synchronises the stream before returning */
+int b200sa_suffix_tree_dev(b200sa_ctx *ctx, uint64_t n, const uint32_t *d_sa, const uint32_t *d_lcp,
+                           const b200sa_tree *out, uint64_t cap, uint64_t *num_nodes, void *stream);
+/* host buffers: SuffixTree::from_suffix_table(table) with sa = table(), lcp = lcp_lens() */
+int b200sa_suffix_tree(b200sa_ctx *ctx, uint64_t n, const uint32_t *sa, const uint32_t *lcp,
+                       const b200sa_tree *out, uint64_t cap, uint64_t *num_nodes);
+
 /* ---- multi-GPU: communicator + sharded LMS-suffix sort (SURVEY.md 8e, config 5) ----
  * One process (or thread) and one context per GPU.  NCCL is resolved at run time
  * (the copy already loaded in the process, else libnccl.so.2); the single-GPU entry

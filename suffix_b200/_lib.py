@@ -30,6 +30,13 @@ class ShardStats(ctypes.Structure):
                 ("kc", ctypes.c_uint32), ("nranks", ctypes.c_uint32), ("rank", ctypes.c_uint32), ("reserved", ctypes.c_uint32)]
 
 
+class Tree(ctypes.Structure):
+    """b200sa_tree: six u32 arrays indexed by preorder id."""
+    _fields_ = [(f, ctypes.c_void_p) for f in ("parent", "depth", "sa_lo", "sa_hi", "label_start", "subtree_end")]
+
+
+TREE_FIELDS = tuple(f for f, _ in Tree._fields_)
+
 _lib = None
 
 
@@ -63,6 +70,8 @@ def lib():
         "b200sa_doc_ids_dev": ([vp, vp, u64, vp, u32, vp, vp, vp], ci),
         "b200sa_lcp_intervals_dev": ([vp, vp, u64, vp, vp, vp], ci),
         "b200sa_lcp_sharded": ([vp, vp, u64, vp, vp, ci, vp], ci),
+        "b200sa_suffix_tree_dev": ([vp, u64, vp, vp, ctypes.POINTER(Tree), u64, ctypes.POINTER(u64), vp], ci),
+        "b200sa_suffix_tree": ([vp, u64, vp, vp, ctypes.POINTER(Tree), u64, ctypes.POINTER(u64)], ci),
         "b200sa_last_stats": ([vp, ctypes.POINTER(Stats)], ci),
         "b200sa_set_timing": ([vp, ci], ci),
         "b200sa_last_phase_times": ([vp, ctypes.POINTER(ctypes.c_char_p), ctypes.POINTER(ctypes.c_float), ci], ci),
@@ -189,6 +198,28 @@ class Context:
 
     def lcp_intervals_dev(self, d_lcp: int, n: int, d_psv: int, d_nsv: int, stream: int = 0):
         self._check(lib().b200sa_lcp_intervals_dev(self._h, d_lcp, n, d_psv, d_nsv, stream))
+
+    def suffix_tree(self, sa: np.ndarray, lcp: np.ndarray) -> dict:
+        """b200sa_suffix_tree: the reference's suffix tree as six u32 arrays of N entries."""
+        sa = np.ascontiguousarray(sa, dtype=np.uint32)
+        lcp = np.ascontiguousarray(lcp, dtype=np.uint32)
+        if len(sa) != len(lcp):
+            raise ValueError("sa and lcp lengths differ")
+        n = len(sa)
+        cap = max(1, 2 * n)
+        arrs = {f: np.empty(cap, dtype=np.uint32) for f in TREE_FIELDS}
+        t = Tree(*[arrs[f].ctypes.data for f in TREE_FIELDS])
+        N = ctypes.c_uint64(0)
+        self._check(lib().b200sa_suffix_tree(self._h, n, sa.ctypes.data, lcp.ctypes.data, ctypes.byref(t), cap,
+                                             ctypes.byref(N)))
+        return {f: a[:N.value] for f, a in arrs.items()}
+
+    def suffix_tree_dev(self, n: int, d_sa: int, d_lcp: int, out_ptrs, cap: int, stream: int = 0) -> int:
+        """b200sa_suffix_tree_dev; out_ptrs: six device pointers in TREE_FIELDS order.  Returns N."""
+        t = Tree(*out_ptrs)
+        N = ctypes.c_uint64(0)
+        self._check(lib().b200sa_suffix_tree_dev(self._h, n, d_sa, d_lcp, ctypes.byref(t), cap, ctypes.byref(N), stream))
+        return int(N.value)
 
     def lcp_sharded(self, d_text: int, n: int, d_sa: int, d_lcp: int, replicated: bool = False, stream: int = 0):
         self._check(lib().b200sa_lcp_sharded(self._h, d_text, n, d_sa, d_lcp, 1 if replicated else 0, stream))

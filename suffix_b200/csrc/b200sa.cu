@@ -28,6 +28,7 @@
 #include "pipeline_kernels.cuh"
 #include "lms_sort.cuh"
 #include "shard.cuh"
+#include "tree.cuh"
 #include "nccl_dyn.h"
 
 using namespace b200sa;
@@ -72,6 +73,7 @@ struct b200sa_ctx {
     DevBuf os_hist, os_status, phik, phiv, runscr, plcp_samp;
     DevBuf k32b, k64a, k64b, v0, v1, p0, p1, g0, g1, rank, isa, qbuf;
     DevBuf packed, scan_state, cls_state, lmsdesc, steplog, hist_copies;
+    DevBuf tree_out;                           // output staging of b200sa_suffix_tree
     uint32_t cls_calls = 0;
     // multi-GPU (SURVEY 8e): communicator owned or attached, NCCL resolved at run time
     ncclComm_t comm = nullptr;
@@ -1227,7 +1229,7 @@ void b200sa_ctx_destroy(b200sa_ctx *c) {
     DevBuf *bufs[] = {&c->text, &c->sa, &c->lcp, &c->pred, &c->stype, &c->lmsb, &c->lmsrank, &c->lmspos, &c->lmslist,
                       &c->lmspred, &c->sorted, &c->flag, &c->reduced, &c->sa_r, &c->blkstate, &c->carry, &c->tables,
                       &c->small, &c->scan_partial, &c->radix_cnt, &c->blkcnt, &c->k32b, &c->k64a, &c->k64b, &c->v0,
-                      &c->v1, &c->p0, &c->p1, &c->g0, &c->g1, &c->rank, &c->isa, &c->qbuf, &c->os_hist, &c->os_status, &c->packed, &c->phik, &c->phiv, &c->runscr, &c->plcp_samp, &c->scan_state, &c->cls_state, &c->lmsdesc, &c->steplog, &c->hist_copies, &c->sh_a, &c->sh_b, &c->sh_c, &c->sh_d, &c->sh_e, &c->sh_f, &c->sh_small};
+                      &c->v1, &c->p0, &c->p1, &c->g0, &c->g1, &c->rank, &c->isa, &c->qbuf, &c->os_hist, &c->os_status, &c->packed, &c->phik, &c->phiv, &c->runscr, &c->plcp_samp, &c->scan_state, &c->cls_state, &c->lmsdesc, &c->steplog, &c->hist_copies, &c->tree_out, &c->sh_a, &c->sh_b, &c->sh_c, &c->sh_d, &c->sh_e, &c->sh_f, &c->sh_small};
     for (DevBuf *b : bufs) if (b->p) cudaFree(b->p);
     for (cudaEvent_t e : c->event_pool) cudaEventDestroy(e);
     if (c->h_pin) cudaFreeHost(c->h_pin);
@@ -1458,6 +1460,25 @@ int b200sa_doc_ids_dev(b200sa_ctx *c, const uint32_t *d_pos, uint64_t count, con
     return end_call(c);
 }
 
+// Block minima of the LCP array over 32^k entries (in c->qbuf) for the ANSV searches.
+static int ansv_levels(b200sa_ctx *c, const uint32_t *d_lcp, uint64_t n, AnsvLevels *L) {
+    memset(L, 0, sizeof *L);
+    L->lv[0] = d_lcp; L->cnt[0] = n; L->nlev = 1;
+    uint64_t total = 0;
+    for (uint64_t k = (n + 31) / 32; ; k = (k + 31) / 32) { total += k; if (k <= 32) break; }
+    TRY(ensure(c, c->qbuf, (total + 64) * 4));
+    uint32_t *lvbuf = ptr<uint32_t>(c->qbuf);
+    uint64_t cnt = n;
+    while (cnt > 32 && L->nlev < 8) {
+        uint64_t nxt = (cnt + 31) / 32;
+        LAUNCH(c, k_min32, cdiv(nxt, BLK), L->lv[L->nlev - 1], cnt, lvbuf);
+        L->lv[L->nlev] = lvbuf; L->cnt[L->nlev] = nxt; L->nlev++;
+        lvbuf += nxt;
+        cnt = nxt;
+    }
+    return B200SA_OK;
+}
+
 int b200sa_lcp_intervals_dev(b200sa_ctx *c, const uint32_t *d_lcp, uint64_t n, uint32_t *d_psv, uint32_t *d_nsv,
                              void *stream) {
     if (!c || (n > 0 && (!d_lcp || !d_psv || !d_nsv))) return B200SA_ERR_BAD_ARG;
@@ -1466,23 +1487,165 @@ int b200sa_lcp_intervals_dev(b200sa_ctx *c, const uint32_t *d_lcp, uint64_t n, u
     begin_call(c, stream);
     if (n == 0) return end_call(c);
     AnsvLevels L;
-    memset(&L, 0, sizeof L);
-    L.lv[0] = d_lcp; L.cnt[0] = n; L.nlev = 1;
-    uint64_t total = 0;
-    for (uint64_t k = (n + 31) / 32; ; k = (k + 31) / 32) { total += k; if (k <= 32) break; }
-    TRY(ensure(c, c->qbuf, (total + 64) * 4));
-    uint32_t *lvbuf = ptr<uint32_t>(c->qbuf);
-    uint64_t cnt = n;
-    while (cnt > 32 && L.nlev < 8) {
-        uint64_t nxt = (cnt + 31) / 32;
-        LAUNCH(c, k_min32, cdiv(nxt, BLK), L.lv[L.nlev - 1], cnt, lvbuf);
-        L.lv[L.nlev] = lvbuf; L.cnt[L.nlev] = nxt; L.nlev++;
-        lvbuf += nxt;
-        cnt = nxt;
-    }
+    TRY(ansv_levels(c, d_lcp, n, &L));
     LAUNCH(c, k_ansv, cdiv(n, BLK), L, n, d_psv, d_nsv);
     CU_TRY(c, cudaGetLastError());
     return end_call(c);
+}
+
+// ------------------------------------------------------------ suffix tree from SA + LCP (SURVEY 8f-5)
+static int tree_bad(b200sa_ctx *c, uint32_t bits) {
+    std::string m = "suffix tree input rejected:";
+    if (bits & TREE_BAD_SA) m += " sa[r] >= n;";
+    if (bits & TREE_BAD_LCP0) m += " lcp[0] != 0;";
+    if (bits & TREE_BAD_LCP) m += " lcp[r] longer than suffix sa[r-1] or sa[r];";
+    if (bits & TREE_BAD_PARENT) m += " a parent node is missing (lcp is not the LCP array of sa);";
+    if (bits & TREE_BAD_FIRST) m += " a rank starts no node (lcp is not the LCP array of sa);";
+    c->last_error = m;
+    return B200SA_ERR_BAD_ARG;
+}
+
+// n >= 1, device inputs and outputs (capacity >= 2n each).  Phases: tree_ansv, tree_emit, tree_sort,
+// tree_first, tree_nodes.
+static int suffix_tree_core(b200sa_ctx *c, uint32_t n, const uint32_t *d_sa, const uint32_t *d_lcp, const TreeOut &o,
+                            uint64_t *num_nodes) {
+    const uint64_t cap = 2 * (uint64_t)n;
+    const int B = bit_length(n);                       // depth <= n and sa_lo < n both fit in B bits
+    TRY(ensure(c, c->p0, (size_t)n * 4));
+    TRY(ensure(c, c->p1, (size_t)n * 4));
+    TRY(ensure(c, c->flag, n));
+    TRY(ensure(c, c->g0, ((size_t)n + 1) * 4));
+    TRY(ensure(c, c->k64a, cap * 8));
+    TRY(ensure(c, c->k64b, cap * 8));
+    TRY(ensure(c, c->v0, cap * 4));
+    TRY(ensure(c, c->v1, cap * 4));
+    TRY(ensure(c, c->small, 4096));
+    uint32_t *psv = ptr<uint32_t>(c->p0), *nsv = ptr<uint32_t>(c->p1), *first = ptr<uint32_t>(c->g0);
+    uint8_t *rep = ptr<uint8_t>(c->flag);
+    uint32_t *words = ptr<uint32_t>(c->small);          // [0] nodes below the root, [1] check bits
+    TRY(mark(c, "tree_ansv"));
+    AnsvLevels L;
+    TRY(ansv_levels(c, d_lcp, n, &L));
+    LAUNCH(c, k_tree_ansv, cdiv(n, BLK), L, (uint64_t)n, psv, nsv, rep);
+    TRY(mark(c, "tree_emit"));
+    CU_TRY(c, cudaMemsetAsync(words, 0, 8, c->stream));
+    TreeCount tin{d_sa, d_lcp, rep, n, words + 1};
+    TreeEmit tout{d_sa, d_lcp, psv, nsv, rep, n, B, ptr<uint64_t>(c->k64a), ptr<uint32_t>(c->v0)};
+    TRY((dev_scan<OpSum>(c, tin, tout, n, words)));
+    TRY(read_words(c, words, 2));
+    if (c->h_pin[1]) return tree_bad(c, c->h_pin[1]);
+    const uint32_t N = c->h_pin[0] + 1;
+    TRY(mark(c, "tree_sort"));
+    uint64_t *K;
+    uint32_t *V;
+    TRY(sort_pairs<uint64_t>(c, ptr<uint64_t>(c->k64a), ptr<uint32_t>(c->v0), ptr<uint64_t>(c->k64b),
+                             ptr<uint32_t>(c->v1), N, 2 * B, &K, &V));
+    TRY(mark(c, "tree_first"));
+    CU_TRY(c, cudaMemsetAsync(first, 0xff, ((size_t)n + 1) * 4, c->stream));
+    LAUNCH(c, k_tree_first, cdiv(N, BLK), K, N, B, n, first);
+    TRY(mark(c, "tree_nodes"));
+    uint32_t grid_n = N > n + 1 ? N : n + 1;
+    LAUNCH(c, k_tree_nodes, cdiv(grid_n, BLK), K, V, N, B, d_sa, d_lcp, psv, first, n, o, words + 1);
+    TRY(mark(c, "end"));
+    CU_TRY(c, cudaGetLastError());
+    TRY(read_words(c, words + 1, 1));
+    if (c->h_pin[0]) return tree_bad(c, c->h_pin[0]);
+    *num_nodes = N;
+    return B200SA_OK;
+}
+
+static int tree_args(b200sa_ctx *c, uint64_t n, const void *sa, const void *lcp, const b200sa_tree *out,
+                     uint64_t cap, uint64_t *num_nodes) {
+    if (!c || !out || !num_nodes) return B200SA_ERR_BAD_ARG;
+    if (!out->parent || !out->depth || !out->sa_lo || !out->sa_hi || !out->label_start || !out->subtree_end ||
+        (n > 0 && (!sa || !lcp))) {
+        c->last_error = "null pointer";
+        return B200SA_ERR_BAD_ARG;
+    }
+    if (n > B200SA_TREE_MAX_N) {
+        c->last_error = "suffix tree: n >= 2^31 (node ids are u32 with 0xFFFFFFFF reserved)";
+        return B200SA_ERR_TOO_LARGE;
+    }
+    if (cap < (n ? 2 * n : 1)) {
+        c->last_error = "suffix tree: cap < max(1, 2n)";
+        return B200SA_ERR_BAD_ARG;
+    }
+    return B200SA_OK;
+}
+
+// Every failing exit of the tree entry points passes through here (like host_build).
+static int tree_exit(b200sa_ctx *c, int rc) {
+    if (rc != B200SA_OK) {
+        if (c->stream) cudaStreamSynchronize(c->stream);
+        cudaGetLastError();
+        return rc;
+    }
+    return end_call(c);
+}
+
+int b200sa_suffix_tree_dev(b200sa_ctx *c, uint64_t n, const uint32_t *d_sa, const uint32_t *d_lcp,
+                           const b200sa_tree *out, uint64_t cap, uint64_t *num_nodes, void *stream) {
+    TRY(tree_args(c, n, d_sa, d_lcp, out, cap, num_nodes));
+    CU_TRY(c, cudaSetDevice(c->device));
+    begin_call(c, stream);
+    *num_nodes = 0;
+    int rc = B200SA_OK;
+    if (n == 0) {
+        // the root alone: parent none, depth 0, range [0, 0), empty label, subtree [0, 1)
+        const uint32_t root[6] = {TREE_NONE, 0, 0, 0, 0, 1};
+        uint32_t *dst[6] = {out->parent, out->depth, out->sa_lo, out->sa_hi, out->label_start, out->subtree_end};
+        for (int k = 0; k < 6 && rc == B200SA_OK; k++) {
+            cudaError_t e = cudaMemcpyAsync(dst[k], &root[k], 4, cudaMemcpyHostToDevice, c->stream);
+            if (e != cudaSuccess) { c->last_error = cudaGetErrorString(e); rc = B200SA_ERR_CUDA; }
+        }
+        if (rc == B200SA_OK && cudaStreamSynchronize(c->stream) != cudaSuccess) rc = B200SA_ERR_CUDA;
+        if (rc == B200SA_OK) *num_nodes = 1;
+        return tree_exit(c, rc);
+    }
+    TreeOut o{out->parent, out->depth, out->sa_lo, out->sa_hi, out->label_start, out->subtree_end};
+    rc = suffix_tree_core(c, (uint32_t)n, d_sa, d_lcp, o, num_nodes);
+    return tree_exit(c, rc);
+}
+
+static int suffix_tree_host(b200sa_ctx *c, uint64_t n, const uint32_t *sa, const uint32_t *lcp, const b200sa_tree *out,
+                            uint64_t *num_nodes) {
+    const uint64_t cap = 2 * n;
+    TRY(ensure(c, c->sa, n * 4));
+    TRY(ensure(c, c->lcp, n * 4));
+    TRY(ensure(c, c->tree_out, cap * 4 * 6));
+    TRY(mark(c, "h2d"));
+    CU_TRY(c, cudaMemcpyAsync(c->sa.p, sa, n * 4, cudaMemcpyHostToDevice, c->stream));
+    CU_TRY(c, cudaMemcpyAsync(c->lcp.p, lcp, n * 4, cudaMemcpyHostToDevice, c->stream));
+    uint32_t *dev[6];
+    for (int k = 0; k < 6; k++) dev[k] = ptr<uint32_t>(c->tree_out) + k * cap;
+    TreeOut o{dev[0], dev[1], dev[2], dev[3], dev[4], dev[5]};
+    uint64_t N = 0;
+    TRY(suffix_tree_core(c, (uint32_t)n, ptr<uint32_t>(c->sa), ptr<uint32_t>(c->lcp), o, &N));
+    if (!c->marks.empty()) c->marks.pop_back();        // the copy-out replaces the core's "end"
+    TRY(mark(c, "d2h"));
+    uint32_t *host[6] = {out->parent, out->depth, out->sa_lo, out->sa_hi, out->label_start, out->subtree_end};
+    for (int k = 0; k < 6; k++)
+        CU_TRY(c, cudaMemcpyAsync(host[k], dev[k], N * 4, cudaMemcpyDeviceToHost, c->stream));
+    TRY(mark(c, "end"));
+    CU_TRY(c, cudaStreamSynchronize(c->stream));
+    *num_nodes = N;
+    return B200SA_OK;
+}
+
+int b200sa_suffix_tree(b200sa_ctx *c, uint64_t n, const uint32_t *sa, const uint32_t *lcp, const b200sa_tree *out,
+                       uint64_t cap, uint64_t *num_nodes) {
+    TRY(tree_args(c, n, sa, lcp, out, cap, num_nodes));
+    CU_TRY(c, cudaSetDevice(c->device));
+    begin_call(c, nullptr);
+    *num_nodes = 0;
+    if (n == 0) {
+        out->parent[0] = TREE_NONE;
+        out->depth[0] = out->sa_lo[0] = out->sa_hi[0] = out->label_start[0] = 0;
+        out->subtree_end[0] = 1;
+        *num_nodes = 1;
+        return end_call(c);
+    }
+    return tree_exit(c, suffix_tree_host(c, n, sa, lcp, out, num_nodes));
 }
 
 // ------------------------------------------------------------ multi-GPU: communicator + sharded LMS sort

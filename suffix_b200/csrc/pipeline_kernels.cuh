@@ -614,6 +614,11 @@ struct AnsvLevels {
     uint64_t cnt[8];
     int nlev;
 };
+// STRICT: largest j < i with lv[0][j] < v (psv); otherwise with lv[0][j] <= v (pse, the suffix tree's
+// representative test, tree.cuh).  Block minima serve both: a block holds such a j iff its minimum does.
+template <bool STRICT = true>
+__device__ __forceinline__ bool ansv_hit(uint32_t x, uint32_t v) { return STRICT ? x < v : x <= v; }
+template <bool STRICT = true>
 __device__ __forceinline__ uint32_t ansv_left(const AnsvLevels &L, uint64_t i, uint32_t v) {
     // climb: at level k, scan the siblings to the left inside the parent block; a block with min < v holds the answer
     uint64_t idx = i;
@@ -624,14 +629,14 @@ __device__ __forceinline__ uint32_t ansv_left(const AnsvLevels &L, uint64_t i, u
         bool found = false;
         while (j > first) {
             j--;
-            if (L.lv[k][j] < v) { found = true; break; }
+            if (ansv_hit<STRICT>(L.lv[k][j], v)) { found = true; break; }
         }
         if (found) {                       // descend: rightmost entry < v inside block j of level k
             while (k > 0) {
                 uint64_t base = j * 32, end = base + 32;
                 if (end > L.cnt[k - 1]) end = L.cnt[k - 1];
                 uint64_t q = end;
-                while (q > base) { q--; if (L.lv[k - 1][q] < v) break; }
+                while (q > base) { q--; if (ansv_hit<STRICT>(L.lv[k - 1][q], v)) break; }
                 j = q;
                 k--;
             }
@@ -675,7 +680,7 @@ __global__ void __launch_bounds__(BLK) k_ansv(AnsvLevels L, uint64_t n, uint32_t
     uint64_t i = (uint64_t)blockIdx.x * BLK + threadIdx.x;
     if (i >= n) return;
     uint32_t v = L.lv[0][i];
-    psv[i] = ansv_left(L, i, v);
+    psv[i] = ansv_left<true>(L, i, v);
     nsv[i] = (uint32_t)ansv_right(L, i, v, n);
 }
 

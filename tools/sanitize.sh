@@ -1,6 +1,6 @@
 #!/bin/bash
 # compute-sanitizer on small builds: every path of round 2 (direct / robust LMS sort, induce variants,
-# fused classifier, sharded world-1 entry points, LCP paths, rows f)
+# fused classifier, sharded world-1 entry points, LCP paths, rows f, the suffix tree)
 mkdir -p gpurun_out
 cat > /tmp/san.py <<'PY'
 import sys, os
@@ -37,6 +37,15 @@ for variant in ("", "1", "2", "3", "4", "5", "6:no_cascade", "6:cascade_4096", "
     c2.close()
 for k in ("B200SA_INDUCE", "B200SA_NO_CASCADE", "B200SA_CASCADE_MAX", "B200SA_CLASSIFY_TMA"):
     os.environ.pop(k, None)
+from suffix_b200 import SuffixTree
+sys.path.insert(0, os.path.join(os.getcwd(), "tests"))
+import tree_oracle
+for name, t in cases + [("banana", np.frombuffer(b"banana", np.uint8)), ("a3000", np.full(3000, 97, np.uint8))]:
+    tb = t.tobytes()
+    st_t = SuffixTree(tb)
+    want = oracle.sais(tb)
+    ref = tree_oracle.suffix_tree(want, oracle.lcp_kasai(tb, want))
+    assert all(np.array_equal(st_t.arrays()[f], ref[f]) for f in tree_oracle.FIELDS), name
 for name, t in cases[:4]:
     want = oracle.sais(t)
     os.environ["B200SA_LCP_LINEAR"] = "1"
