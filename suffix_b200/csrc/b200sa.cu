@@ -289,10 +289,11 @@ static int sort_pairs(b200sa_ctx *c, K *ka, uint32_t *va, K *kb, uint32_t *vb, u
 }
 
 // Same sort, but the first pass reads its (key, value) items from functors (no materialised
-// input arrays); at least one pass runs, so the result always lands in a buffer pair.
+// input arrays); at least one pass runs, so the result always lands in a buffer pair.  The passes
+// sort by key bits [shift0, shift0 + bits).
 template <class K, class KeyF, class ValF, int OSI = ITEMS>
 static int sort_pairs_from(b200sa_ctx *c, KeyF keyf, ValF valf, K *ka, uint32_t *va, K *kb, uint32_t *vb, uint64_t n,
-                           int bits, K **kout, uint32_t **vout) {
+                           int bits, K **kout, uint32_t **vout, uint32_t shift0 = 0) {
     *kout = ka;
     *vout = va;
     if (n == 0) return B200SA_OK;
@@ -311,17 +312,17 @@ static int sort_pairs_from(b200sa_ctx *c, KeyF keyf, ValF valf, K *ka, uint32_t 
         size_t shm = (size_t)NWARP * npass * 256 * 4;
         auto kfn = k_os_hist<K, KeyF>;
         CU_TRY(c, cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(NWARP * OS_MAX_PASSES * 256 * 4)));
-        kfn<<<hb, BLK, shm, c->stream>>>(keyf, n, npass, 0u, ghist, kb);      // kb <- the keys (free until pass 2 writes it)
+        kfn<<<hb, BLK, shm, c->stream>>>(keyf, n, npass, shift0, ghist, kb);   // kb <- the keys (free until pass 2 writes it)
         c->launches++;
     }
     LAUNCH(c, k_os_scan, (uint32_t)npass, ghist);
     volatile unsigned long long *status = reinterpret_cast<volatile unsigned long long *>(c->os_status.p);
     CU_TRY(c, cudaMemsetAsync(c->os_status.p, 0, status_bytes, c->stream));
-    LAUNCH(c, (k_os_pass<K, LoadArr<K>, ValF, OSI>), tiles, LoadArr<K>{kb}, valf, ka, va, n, 0u, ghist, status, ticket);
+    LAUNCH(c, (k_os_pass<K, LoadArr<K>, ValF, OSI>), tiles, LoadArr<K>{kb}, valf, ka, va, n, shift0, ghist, status, ticket);
     for (int p = 1; p < npass; p++) {
         CU_TRY(c, cudaMemsetAsync(c->os_status.p, 0, status_bytes, c->stream));
         LAUNCH(c, (k_os_pass<K, LoadArr<K>, LoadArr<uint32_t>, OSI>), tiles, LoadArr<K>{ka}, LoadArr<uint32_t>{va}, kb, vb, n,
-               (uint32_t)(8 * p), ghist + p * 256, status, ticket + p);
+               shift0 + (uint32_t)(8 * p), ghist + p * 256, status, ticket + p);
         K *tk = ka; ka = kb; kb = tk;
         uint32_t *tv = va; va = vb; vb = tv;
     }
@@ -539,23 +540,6 @@ static int lms_direct_sort_t(b200sa_ctx *c, uint32_t n, uint32_t m, uint32_t **l
     TRY(ensure(c, c->small, 4096));
     uint32_t *sm = ptr<uint32_t>(c->small);
     uint32_t *Ks, *Ps;
-    TRY(mark(c, "lms_sort"));
-    {
-        const char *e = getenv("B200SA_SORT_ITEMS");            // keys per thread of the one-sweep passes: 8 | 16
-        const bool wide = e ? atoi(e) == 16 : (m >= (1u << 20) && !getenv("B200SA_SORT_NARROW"));
-        LmsKeyDesc<BITS> kf{W, ptr<uint32_t>(c->lmsdesc)};
-        LmsValDesc vf{ptr<uint32_t>(c->lmsdesc)};
-        if (wide)
-            TRY((sort_pairs_from<uint32_t, LmsKeyDesc<BITS>, LmsValDesc, 16>(c, kf, vf, ptr<uint32_t>(c->k32b), ptr<uint32_t>(c->v0),
-                                                                             ptr<uint32_t>(c->reduced), ptr<uint32_t>(c->v1), m,
-                                                                             bit_length(range - 1), &Ks, &Ps)));
-        else
-            TRY((sort_pairs_from<uint32_t, LmsKeyDesc<BITS>, LmsValDesc, ITEMS>(c, kf, vf, ptr<uint32_t>(c->k32b), ptr<uint32_t>(c->v0),
-                                                                                ptr<uint32_t>(c->reduced), ptr<uint32_t>(c->v1), m,
-                                                                                bit_length(range - 1), &Ks, &Ps)));
-    }
-    // groups of equal windows; members of non-singleton groups -> active list
-    TRY(mark(c, "lms_groups"));
     TRY(ensure(c, c->p0, (size_t)m * 4));
     TRY(ensure(c, c->p1, (size_t)m * 4));
     TRY(ensure(c, c->g0, (size_t)m * 4));
@@ -566,7 +550,59 @@ static int lms_direct_sort_t(b200sa_ctx *c, uint32_t n, uint32_t m, uint32_t **l
     uint32_t *grpA = ptr<uint32_t>(c->g0), *grpB = ptr<uint32_t>(c->g1);
     uint32_t *posA = ptr<uint32_t>(c->sa_r), *posB = ptr<uint32_t>(c->rank);
     unsigned long long *d_tot = reinterpret_cast<unsigned long long *>(sm + 16);
-    {
+    const char *items_env = getenv("B200SA_SORT_ITEMS");            // keys per thread of the one-sweep passes: 8 | 16
+    const bool wide = items_env ? atoi(items_env) == 16 : (m >= (1u << 20) && !getenv("B200SA_SORT_NARROW"));
+    LmsKeyDesc<BITS> kf{W, ptr<uint32_t>(c->lmsdesc)};
+    LmsValDesc vf{ptr<uint32_t>(c->lmsdesc)};
+    // 2-bit text: two passes on the top 16 key bits (the first 8 characters), then k_lms_bucket_sort sorts every
+    // bucket by the low 16 bits in shared memory and finds the round-1 ties with the group ids.  A bucket longer
+    // than BS_CAP sends the sort back to the four full passes below.  B200SA_LMS_SORT4=1 forces those (cross-check).
+    bool bucketed = false;
+    if (BITS == 2 && !getenv("B200SA_LMS_SORT4")) {
+        TRY(mark(c, "lms_sort"));
+        if (wide)
+            TRY((sort_pairs_from<uint32_t, LmsKeyDesc<BITS>, LmsValDesc, 16>(c, kf, vf, ptr<uint32_t>(c->k32b), ptr<uint32_t>(c->v0),
+                                                                             ptr<uint32_t>(c->reduced), ptr<uint32_t>(c->v1), m,
+                                                                             16, &Ks, &Ps, 16u)));
+        else
+            TRY((sort_pairs_from<uint32_t, LmsKeyDesc<BITS>, LmsValDesc, ITEMS>(c, kf, vf, ptr<uint32_t>(c->k32b), ptr<uint32_t>(c->v0),
+                                                                                ptr<uint32_t>(c->reduced), ptr<uint32_t>(c->v1), m,
+                                                                                16, &Ks, &Ps, 16u)));
+        TRY(mark(c, "lms_groups"));
+        uint32_t *Pout = ptr<uint32_t>(c->k32b);                    // keys of the first pass: dead after the second
+        CU_TRY(c, cudaMemsetAsync(sm + 16, 0, 12, c->stream));      // [16] tied count, [18] bucket overflow
+        uint32_t nt = cdiv(m, BS_T);
+        ScanState S;
+        TRY(scan_state_for(c, nt, &S));
+        CU_TRY(c, cudaFuncSetAttribute(k_lms_bucket_sort, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)BS_SMEM));
+        // all of the unified L1 as shared memory: three CTAs per SM (the default carveout may leave room for one)
+        CU_TRY(c, cudaFuncSetAttribute(k_lms_bucket_sort, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
+        if (getenv("B200SA_TRACE")) {
+            int occ = 0;
+            cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_lms_bucket_sort, BLK, BS_SMEM);
+            fprintf(stderr, "[b200sa] k_lms_bucket_sort: %u CTAs, %d per SM\n", nt, occ);
+        }
+        k_lms_bucket_sort<<<nt, BLK, BS_SMEM, c->stream>>>(Ks, Ps, m, n, kc, nt, S, Pout, slotA, posA, grpA, sm + 16, sm + 18);
+        c->launches++;
+        CU_TRY(c, cudaGetLastError());
+        TRY(read_words(c, sm + 16, 3));
+        bucketed = c->h_pin[2] == 0;
+        Ps = Pout;
+        if (!bucketed && getenv("B200SA_TRACE"))
+            fprintf(stderr, "[b200sa] direct LMS sort: a top-16 bucket holds more than %u suffixes: four-pass sort\n", BS_CAP);
+    }
+    if (!bucketed) {
+        TRY(mark(c, "lms_sort"));
+        if (wide)
+            TRY((sort_pairs_from<uint32_t, LmsKeyDesc<BITS>, LmsValDesc, 16>(c, kf, vf, ptr<uint32_t>(c->k32b), ptr<uint32_t>(c->v0),
+                                                                             ptr<uint32_t>(c->reduced), ptr<uint32_t>(c->v1), m,
+                                                                             bit_length(range - 1), &Ks, &Ps)));
+        else
+            TRY((sort_pairs_from<uint32_t, LmsKeyDesc<BITS>, LmsValDesc, ITEMS>(c, kf, vf, ptr<uint32_t>(c->k32b), ptr<uint32_t>(c->v0),
+                                                                                ptr<uint32_t>(c->reduced), ptr<uint32_t>(c->v1), m,
+                                                                                bit_length(range - 1), &Ks, &Ps)));
+        // groups of equal windows; members of non-singleton groups -> active list
+        TRY(mark(c, "lms_groups"));
         size_t fw = ((size_t)m + 31) / 32 + 1;
         TRY(ensure(c, c->flag, fw * 4));
         uint32_t *forced = ptr<uint32_t>(c->flag);
@@ -583,19 +619,20 @@ static int lms_direct_sort_t(b200sa_ctx *c, uint32_t n, uint32_t m, uint32_t **l
             LAUNCH(c, k_lms_groups1, nt, Ks, Ps, forced, m, nt, S, slotA, posA, grpA, sm + 16);
             CU_TRY(c, cudaGetLastError());
         }
+        TRY(read_words(c, sm + 16, 1));
     }
-    TRY(read_words(c, sm + 16, 1));
     uint32_t na = c->h_pin[0];
     c->stats.names = m - na;                       // LMS suffixes settled by the first window
     uint32_t rounds = 1;
     uint32_t max_rounds = BITS == 8 ? 16u : 8u;    // byte windows hold 4-8 chars: natural text needs ~10 of them
     if (const char *e = getenv("B200SA_DIRECT_ROUNDS")) { int v = atoi(e); if (v >= 1) max_rounds = (uint32_t)v; }
-    if (getenv("B200SA_TRACE")) fprintf(stderr, "[b200sa] direct LMS sort: kc=%u, round 1 leaves %u of %u tied\n", kc, na, m);
+    if (getenv("B200SA_TRACE")) fprintf(stderr, "[b200sa] direct LMS sort: kc=%u, round 1 leaves %u of %u tied%s\n", kc, na, m,
+                                        bucketed ? " (bucket sort)" : "");
     const bool force = getenv("B200SA_DIRECT_FORCE") != nullptr;            // experiments: never bail out early
     // the window tells (almost) nothing apart: every suffix has a twin for kc characters -- repeats, not
     // a skewed alphabet (English leaves 99.5 % tied after 5 bytes and still converges in ~10 rounds)
     if (!force && (uint64_t)na * 1000 > (uint64_t)m * 999 && m > 64) return B200SA_OK;
-    if (na > 0)     // group id of every tied element = slot of its group's head
+    if (na > 0 && !bucketed)     // group id of every tied element = slot of its group's head (the bucket sort writes it)
         TRY((dev_scan<OpMax>(c, InArray{grpA}, OutMaxInPlace{grpA}, na, nullptr)));
     uint64_t h = kc;
     const bool allow_local = getenv("B200SA_NO_LOCAL_SORT") == nullptr;

@@ -1,5 +1,6 @@
 #!/bin/bash
-# compute-sanitizer on small builds: every path of round 2 (direct / robust LMS sort, induce variants,
+# compute-sanitizer on small builds: every path of round 2 (direct / robust LMS sort, the 2-bit bucket sort and its
+# overflow, induce variants,
 # fused classifier, sharded world-1 entry points, LCP paths, rows f, the suffix tree)
 mkdir -p gpurun_out
 cat > /tmp/san.py <<'PY'
@@ -21,6 +22,9 @@ for k in range(300):
     runs.append(np.full(int(rng.integers(1, 12)), b"ACGT"[k % 4], dtype=np.uint8))
     runs.append(gen.dna(int(rng.integers(1, 40)), seed=k))
 cases.append(("short_runs", np.concatenate(runs * 8)))
+# 2-bit text with one top-16 bucket of > 4096 LMS suffixes: k_lms_bucket_sort overflows, the four-pass sort reruns
+fill = np.frombuffer(b"ACGT", np.uint8)[rng.integers(0, 4, (4200, 6))]
+cases.append(("bucket_overflow", np.concatenate([gen.dna(20000)] + [np.concatenate([np.frombuffer(b"TACGTACGTC", np.uint8), f]) for f in fill] + [gen.dna(20000)])))
 for variant in ("", "1", "2", "3", "4", "5", "6:no_cascade", "6:cascade_4096", "6:classify_tma"):
     os.environ.pop("B200SA_NO_CASCADE", None); os.environ.pop("B200SA_CASCADE_MAX", None); os.environ.pop("B200SA_CLASSIFY_TMA", None)
     if variant:
@@ -37,6 +41,10 @@ for variant in ("", "1", "2", "3", "4", "5", "6:no_cascade", "6:cascade_4096", "
     c2.close()
 for k in ("B200SA_INDUCE", "B200SA_NO_CASCADE", "B200SA_CASCADE_MAX", "B200SA_CLASSIFY_TMA"):
     os.environ.pop(k, None)
+os.environ["B200SA_LMS_SORT4"] = "1"            # the four-pass LMS sort on 2-bit text
+for name, t in cases[:1] + cases[-1:]:
+    assert np.array_equal(ctx.build(t), oracle.sais(t)), name
+del os.environ["B200SA_LMS_SORT4"]
 from suffix_b200 import SuffixTree
 sys.path.insert(0, os.path.join(os.getcwd(), "tests"))
 import tree_oracle
