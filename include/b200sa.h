@@ -183,6 +183,42 @@ int b200sa_suffix_tree_dev(b200sa_ctx *ctx, uint64_t n, const uint32_t *d_sa, co
 int b200sa_suffix_tree(b200sa_ctx *ctx, uint64_t n, const uint32_t *sa, const uint32_t *lcp,
                        const b200sa_tree *out, uint64_t cap, uint64_t *num_nodes);
 
+/* ---- generalized suffix array without separators (SURVEY.md 8f-6; reference README.md:60-74, TODO:13-18) ----
+ * Documents D_0 .. D_{k-1} (arbitrary bytes, possibly empty) are given as their concatenation C of
+ * n = sum |D_d| bytes, with no separators, and doc_starts[d] = offset of D_d in C (ascending,
+ * doc_starts[0] = 0, every entry <= n).  For a position p of document d, r_p = end_d - p and its
+ * suffix is T_p = C[p, p + r_p).
+ *   gsa   (the generalized suffix array G): all n positions sorted by (T_p, d).  Bytes compare
+ *         lexicographically, a proper prefix sorts first, equal strings are ordered by document.
+ *         This is the suffix array of D_0 $_0 D_1 $_1 ... with $_0 < $_1 < ... < every byte, without
+ *         the terminator positions.  For k = 1 it is the SuffixTable of the single document.
+ *   glcp  glcp[0] = 0, glcp[i] = common prefix length of T_{G[i-1]} and T_{G[i]} (never crosses a
+ *         document end).  glcp_out / d_glcp may be NULL.
+ * Built from SA and LCP of C (b200sa_build_lcp_dev): lo_i = the first rank sharing >= r_p bytes with
+ * p = SA_C[i] (ranks with LCP_C[i] < r_p: i itself), G = the ranks sorted by (lo, r, d), and
+ * glcp = min(r_a, r_b, min LCP_C over (lo_a, lo_b]) for neighbours a, b.  Only the ranks whose suffix
+ * in C reaches past their document end are sorted.
+ * B200SA_ERR_BAD_ARG with a b200sa_last_error detail when doc_starts does not start at 0, is not
+ * ascending or has an entry above n, or when ndocs = 0 with n > 0 (the host entry checks on the host,
+ * the device entry on the device); B200SA_ERR_TOO_LARGE above B200SA_MAX_N.  n = 0 and n = 1 return
+ * without launching.  Device workspace, the SA + LCP build's included, measured on 100 MB on one
+ * H100 80GB HBM3: about 46 bytes per text byte when few suffixes cross their document end (the build
+ * alone holds 25), 78 when all do (n/4 copies of "ACGT"; the build alone 38); the host entry adds 9
+ * for staging.  The phases report to b200sa_last_phase_times.  B200SA_DOCS_SORT2=1 forces the
+ * two-stage sort (by document, then by (lo, r)) that keys of more than 64 bits take. */
+int b200sa_docs_build(b200sa_ctx *ctx, const uint8_t *text, uint64_t n, const uint32_t *doc_starts, uint32_t ndocs,
+                      uint32_t *gsa_out, uint32_t *glcp_out);
+/* device buffers; synchronises the stream only to read the check word and the sort size back */
+int b200sa_docs_build_dev(b200sa_ctx *ctx, const uint8_t *d_text, uint64_t n, const uint32_t *d_doc_starts,
+                          uint32_t ndocs, uint32_t *d_gsa, uint32_t *d_glcp, void *stream);
+/* Batched positions over G (b200sa_positions_dev with every suffix cut at its document end): query q is
+ * bytes [q_off[q], q_off[q+1]) of d_queries (any bytes); writes the range [start[q], end[q]) of G whose
+ * document suffixes start with it.  A match never crosses a document end.  d_gsa and d_doc_starts are
+ * what b200sa_docs_build_dev was given and returned. */
+int b200sa_docs_positions_dev(b200sa_ctx *ctx, const uint8_t *d_text, uint64_t n, const uint32_t *d_gsa,
+                              const uint32_t *d_doc_starts, uint32_t ndocs, const uint8_t *d_queries,
+                              const uint64_t *d_q_off, uint32_t nq, uint32_t *d_start, uint32_t *d_end, void *stream);
+
 /* ---- multi-GPU: communicator + sharded LMS-suffix sort (SURVEY.md 8e, config 5) ----
  * One process (or thread) and one context per GPU.  NCCL is resolved at run time
  * (the copy already loaded in the process, else libnccl.so.2); the single-GPU entry

@@ -72,6 +72,9 @@ def lib():
         "b200sa_lcp_sharded": ([vp, vp, u64, vp, vp, ci, vp], ci),
         "b200sa_suffix_tree_dev": ([vp, u64, vp, vp, ctypes.POINTER(Tree), u64, ctypes.POINTER(u64), vp], ci),
         "b200sa_suffix_tree": ([vp, u64, vp, vp, ctypes.POINTER(Tree), u64, ctypes.POINTER(u64)], ci),
+        "b200sa_docs_build": ([vp, vp, u64, vp, u32, vp, vp], ci),
+        "b200sa_docs_build_dev": ([vp, vp, u64, vp, u32, vp, vp, vp], ci),
+        "b200sa_docs_positions_dev": ([vp, vp, u64, vp, vp, u32, vp, vp, u32, vp, vp, vp], ci),
         "b200sa_last_stats": ([vp, ctypes.POINTER(Stats)], ci),
         "b200sa_set_timing": ([vp, ci], ci),
         "b200sa_last_phase_times": ([vp, ctypes.POINTER(ctypes.c_char_p), ctypes.POINTER(ctypes.c_float), ci], ci),
@@ -220,6 +223,28 @@ class Context:
         N = ctypes.c_uint64(0)
         self._check(lib().b200sa_suffix_tree_dev(self._h, n, d_sa, d_lcp, ctypes.byref(t), cap, ctypes.byref(N), stream))
         return int(N.value)
+
+    def docs_build(self, text: np.ndarray, doc_starts: np.ndarray, with_lcp: bool = True):
+        """b200sa_docs_build: (gsa, glcp) of the documents concatenated in `text`; glcp is None
+        without with_lcp."""
+        text = np.ascontiguousarray(text, dtype=np.uint8)
+        starts = np.ascontiguousarray(doc_starts, dtype=np.uint32)
+        n = len(text)
+        gsa = np.empty(n, dtype=np.uint32)
+        glcp = np.empty(n, dtype=np.uint32) if with_lcp else None
+        self._check(lib().b200sa_docs_build(self._h, text.ctypes.data, n, starts.ctypes.data, len(starts),
+                                            gsa.ctypes.data, glcp.ctypes.data if with_lcp else None))
+        return gsa, glcp
+
+    def docs_build_dev(self, d_text: int, n: int, d_doc_starts: int, ndocs: int, d_gsa: int, d_glcp: int = 0,
+                       stream: int = 0):
+        self._check(lib().b200sa_docs_build_dev(self._h, d_text, n, d_doc_starts, ndocs, d_gsa, d_glcp or None,
+                                                stream))
+
+    def docs_positions_dev(self, d_text, n, d_gsa, d_doc_starts, ndocs, d_q, d_qoff, nq, d_start, d_end,
+                           stream: int = 0):
+        self._check(lib().b200sa_docs_positions_dev(self._h, d_text, n, d_gsa, d_doc_starts, ndocs, d_q, d_qoff, nq,
+                                                    d_start, d_end, stream))
 
     def lcp_sharded(self, d_text: int, n: int, d_sa: int, d_lcp: int, replicated: bool = False, stream: int = 0):
         self._check(lib().b200sa_lcp_sharded(self._h, d_text, n, d_sa, d_lcp, 1 if replicated else 0, stream))

@@ -11,6 +11,7 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <new>
 #include <string>
 #include <vector>
 
@@ -29,6 +30,7 @@
 #include "lms_sort.cuh"
 #include "shard.cuh"
 #include "tree.cuh"
+#include "docs.cuh"
 #include "nccl_dyn.h"
 
 using namespace b200sa;
@@ -74,6 +76,7 @@ struct b200sa_ctx {
     DevBuf k32b, k64a, k64b, v0, v1, p0, p1, g0, g1, rank, isa, qbuf;
     DevBuf packed, scan_state, cls_state, lmsdesc, steplog, hist_copies;
     DevBuf tree_out;                           // output staging of b200sa_suffix_tree
+    DevBuf docs_starts, docs_out;              // doc_starts and output staging of b200sa_docs_build
     uint32_t cls_calls = 0;
     // multi-GPU (SURVEY 8e): communicator owned or attached, NCCL resolved at run time
     ncclComm_t comm = nullptr;
@@ -1175,6 +1178,31 @@ static int test_sort(b200sa_ctx *c, K *keys, uint32_t *vals, uint64_t n, int bit
     return end_call(c);
 }
 
+// SA + LCP of one text, device-resident (b200sa_build_lcp_dev, and step 1 of b200sa_docs_build).
+static int build_lcp_dev(b200sa_ctx *c, const uint8_t *d_text, uint64_t n, uint32_t *d_sa, uint32_t *d_lcp) {
+    int rc = build_dev(c, d_text, n, d_sa);
+    if (rc == B200SA_OK) {
+        // build_dev may have classified an aligned copy of the text; the packed text (or that
+        // copy) is still valid, so the LCP kernels reuse it (n >= 2 means classification ran)
+        const uint8_t *t = (((uintptr_t)d_text & 15) != 0 && n >= 2) ? ptr<uint8_t>(c->text) : d_text;
+        b200sa_stats st = c->stats;
+        rc = lcp_dev(c, t, n, d_sa, d_lcp, n >= 2);
+        c->stats = st;
+    }
+    return rc;
+}
+
+// Sorts the cnt ranks of `vals` (the A ranks of b200sa_docs_build) by the key of kf (wider tiles for large inputs, as sort_pairs).
+template <class K, class KeyF>
+static int docs_sort(b200sa_ctx *c, KeyF kf, const uint32_t *vals, K *ka, uint32_t *va, K *kb, uint32_t *vb,
+                     uint32_t cnt, int bits, K **kout, uint32_t **vout) {
+    LoadArr<uint32_t> vf{vals};
+    if (cnt >= (1u << 20))
+        return sort_pairs_from<K, KeyF, LoadArr<uint32_t>, (sizeof(K) == 4 ? 16 : 12)>(c, kf, vf, ka, va, kb, vb, cnt, bits,
+                                                                                       kout, vout);
+    return sort_pairs_from<K, KeyF, LoadArr<uint32_t>, ITEMS>(c, kf, vf, ka, va, kb, vb, cnt, bits, kout, vout);
+}
+
 // ================================================================= C ABI
 extern "C" {
 
@@ -1266,7 +1294,7 @@ void b200sa_ctx_destroy(b200sa_ctx *c) {
     DevBuf *bufs[] = {&c->text, &c->sa, &c->lcp, &c->pred, &c->stype, &c->lmsb, &c->lmsrank, &c->lmspos, &c->lmslist,
                       &c->lmspred, &c->sorted, &c->flag, &c->reduced, &c->sa_r, &c->blkstate, &c->carry, &c->tables,
                       &c->small, &c->scan_partial, &c->radix_cnt, &c->blkcnt, &c->k32b, &c->k64a, &c->k64b, &c->v0,
-                      &c->v1, &c->p0, &c->p1, &c->g0, &c->g1, &c->rank, &c->isa, &c->qbuf, &c->os_hist, &c->os_status, &c->packed, &c->phik, &c->phiv, &c->runscr, &c->plcp_samp, &c->scan_state, &c->cls_state, &c->lmsdesc, &c->steplog, &c->hist_copies, &c->tree_out, &c->sh_a, &c->sh_b, &c->sh_c, &c->sh_d, &c->sh_e, &c->sh_f, &c->sh_small};
+                      &c->v1, &c->p0, &c->p1, &c->g0, &c->g1, &c->rank, &c->isa, &c->qbuf, &c->os_hist, &c->os_status, &c->packed, &c->phik, &c->phiv, &c->runscr, &c->plcp_samp, &c->scan_state, &c->cls_state, &c->lmsdesc, &c->steplog, &c->hist_copies, &c->tree_out, &c->docs_starts, &c->docs_out, &c->sh_a, &c->sh_b, &c->sh_c, &c->sh_d, &c->sh_e, &c->sh_f, &c->sh_small};
     for (DevBuf *b : bufs) if (b->p) cudaFree(b->p);
     for (cudaEvent_t e : c->event_pool) cudaEventDestroy(e);
     if (c->h_pin) cudaFreeHost(c->h_pin);
@@ -1324,15 +1352,7 @@ int b200sa_build_lcp_dev(b200sa_ctx *c, const uint8_t *d_text, uint64_t n, uint3
     if (!c || (n > 0 && (!d_text || !d_sa || !d_lcp))) return B200SA_ERR_BAD_ARG;
     CU_TRY(c, cudaSetDevice(c->device));
     begin_call(c, stream);
-    int rc = build_dev(c, d_text, n, d_sa);
-    if (rc == B200SA_OK) {
-        // build_dev may have classified an aligned copy of the text; the packed text (or that
-        // copy) is still valid, so the LCP kernels reuse it (n >= 2 means classification ran)
-        const uint8_t *t = (((uintptr_t)d_text & 15) != 0 && n >= 2) ? ptr<uint8_t>(c->text) : d_text;
-        b200sa_stats st = c->stats;
-        rc = lcp_dev(c, t, n, d_sa, d_lcp, n >= 2);
-        c->stats = st;
-    }
+    int rc = build_lcp_dev(c, d_text, n, d_sa, d_lcp);
     if (rc == B200SA_OK) rc = end_call(c);
     return rc;
 }
@@ -1427,7 +1447,8 @@ int b200sa_positions_dev(b200sa_ctx *c, const uint8_t *d_text, uint64_t n, const
     CU_TRY(c, cudaSetDevice(c->device));
     begin_call(c, stream);
     if (nq > 0) {
-        LAUNCH(c, k_positions, cdiv(nq, BLK), d_text, (uint32_t)n, d_sa, d_queries, d_q_off, nq, d_start, d_end);
+        LAUNCH(c, k_positions<TextEnd>, cdiv(nq, BLK), d_text, (uint32_t)n, d_sa, d_queries, d_q_off, nq, d_start, d_end,
+               TextEnd{(uint32_t)n});
         CU_TRY(c, cudaGetLastError());
     }
     return end_call(c);
@@ -1610,7 +1631,7 @@ static int tree_args(b200sa_ctx *c, uint64_t n, const void *sa, const void *lcp,
     return B200SA_OK;
 }
 
-// Every failing exit of the tree entry points passes through here (like host_build).
+// Every failing exit of the tree and docs entry points passes through here (like host_build).
 static int tree_exit(b200sa_ctx *c, int rc) {
     if (rc != B200SA_OK) {
         if (c->stream) cudaStreamSynchronize(c->stream);
@@ -1683,6 +1704,231 @@ int b200sa_suffix_tree(b200sa_ctx *c, uint64_t n, const uint32_t *sa, const uint
         return end_call(c);
     }
     return tree_exit(c, suffix_tree_host(c, n, sa, lcp, out, num_nodes));
+}
+
+// ------------------------------------------------------------ generalized suffix array without separators (SURVEY 8f-6)
+static int docs_bad(b200sa_ctx *c, uint32_t bits) {
+    std::string m = "doc_starts rejected:";
+    if (bits & DOCS_BAD_FIRST) m += " doc_starts[0] != 0;";
+    if (bits & DOCS_BAD_ORDER) m += " not ascending;";
+    if (bits & DOCS_BAD_RANGE) m += " an entry above n;";
+    c->last_error = m;
+    return B200SA_ERR_BAD_ARG;
+}
+
+// The checks of k_docs_check on host entries doc_starts[first, first + count); *prev holds
+// doc_starts[first - 1] on entry and the span's last entry on return.
+static uint32_t docs_check_span(uint64_t n, const uint32_t *starts, uint64_t first, uint64_t count, uint64_t *prev) {
+    uint32_t bad = 0;
+    for (uint64_t k = 0; k < count; k++) {
+        uint64_t v = starts[k], d = first + k;
+        if (d == 0 && v != 0) bad |= DOCS_BAD_FIRST;
+        if (v > n) bad |= DOCS_BAD_RANGE;
+        if (d > 0 && *prev <= n && v < *prev) bad |= DOCS_BAD_ORDER;   // a start above n is flagged itself
+        *prev = v;
+    }
+    return bad;
+}
+
+static int docs_check_host(b200sa_ctx *c, uint64_t n, const uint32_t *starts, uint32_t ndocs) {
+    uint64_t prev = 0;
+    uint32_t bad = docs_check_span(n, starts, 0, ndocs, &prev);
+    return bad ? docs_bad(c, bad) : B200SA_OK;
+}
+
+// The same checks on device entries, copied back through a bounded host buffer (ndocs is not
+// bounded by n: any number of documents may be empty).
+static int docs_check_dev_copy(b200sa_ctx *c, uint64_t n, const uint32_t *d_starts, uint32_t ndocs) {
+    const uint64_t chunk = 1u << 16;
+    std::vector<uint32_t> buf;
+    try {
+        buf.resize(ndocs < chunk ? ndocs : chunk);
+    } catch (const std::bad_alloc &) {
+        c->last_error = "host buffer for the doc_starts check";
+        return B200SA_ERR_OOM;
+    }
+    uint64_t prev = 0;
+    uint32_t bad = 0;
+    for (uint64_t first = 0; first < ndocs; first += chunk) {
+        uint64_t cnt = ndocs - first < chunk ? ndocs - first : chunk;
+        CU_TRY(c, cudaMemcpyAsync(buf.data(), d_starts + first, cnt * 4, cudaMemcpyDeviceToHost, c->stream));
+        CU_TRY(c, cudaStreamSynchronize(c->stream));
+        bad |= docs_check_span(n, buf.data(), first, cnt, &prev);
+    }
+    return bad ? docs_bad(c, bad) : B200SA_OK;
+}
+
+static int docs_args(b200sa_ctx *c, uint64_t n, const void *text, const void *starts, uint32_t ndocs, const void *gsa) {
+    if (!c) return B200SA_ERR_BAD_ARG;
+    if ((n > 0 && (!text || !gsa)) || (ndocs > 0 && !starts)) {
+        c->last_error = "null pointer";
+        return B200SA_ERR_BAD_ARG;
+    }
+    if (n > B200SA_MAX_N) {
+        c->last_error = "text longer than 2^32-4096 bytes";
+        return B200SA_ERR_TOO_LARGE;
+    }
+    if (ndocs == 0 && n > 0) {
+        c->last_error = "doc_starts rejected: ndocs == 0 with n > 0;";
+        return B200SA_ERR_BAD_ARG;
+    }
+    return B200SA_OK;
+}
+
+// n >= 2, ndocs >= 1, device inputs and outputs (d_glcp may be null).  Phases: docs_check, the SA + LCP
+// build's own, docs_split, docs_sort, docs_place, docs_fill, docs_out.
+static int docs_core(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const uint32_t *d_starts, uint32_t ndocs,
+                     uint32_t *d_gsa, uint32_t *d_glcp) {
+    TRY(ensure(c, c->small, 4096));
+    uint32_t *words = ptr<uint32_t>(c->small);           // [0] check bits / |A|, [1] longest document
+    TRY(mark(c, "docs_check"));
+    CU_TRY(c, cudaMemsetAsync(words, 0, 8, c->stream));
+    LAUNCH(c, k_docs_check, cdiv(ndocs, BLK), d_starts, ndocs, n, words);
+    CU_TRY(c, cudaGetLastError());
+    TRY(read_words(c, words, 2));
+    if (c->h_pin[0]) return docs_bad(c, c->h_pin[0]);
+    const uint32_t maxlen = c->h_pin[1];
+
+    // 1. SA and LCP of the concatenation
+    TRY(ensure(c, c->sa, (size_t)n * 4));
+    TRY(ensure(c, c->lcp, (size_t)n * 4));
+    uint32_t *sa = ptr<uint32_t>(c->sa), *lcp = ptr<uint32_t>(c->lcp);
+    TRY(build_lcp_dev(c, d_text, n, sa, lcp));
+    if (!c->marks.empty()) c->marks.pop_back();          // docs_split follows instead of the build's "end"
+
+    // 2-3. r per rank, U / A split, block minima of LCP_C
+    TRY(mark(c, "docs_split"));
+    TRY(ensure(c, c->isa, (size_t)n * 4));
+    TRY(ensure(c, c->rank, (size_t)n * 4));
+    TRY(ensure(c, c->p0, (size_t)n * 4));
+    uint32_t *rem = ptr<uint32_t>(c->isa), *pre = ptr<uint32_t>(c->rank), *list = ptr<uint32_t>(c->p0);
+    TRY((dev_scan<OpSum>(c, DocsSplitIn{sa, lcp, d_starts, ndocs, n, rem}, DocsSplitOut{pre, list, n}, n, words)));
+    AnsvLevels L;
+    TRY(ansv_levels(c, lcp, n, &L));
+    TRY(read_words(c, words, 1));
+    const uint32_t na = c->h_pin[0];
+
+    uint32_t *gr = nullptr, *glo = nullptr;
+    if (na > 0) {
+        // 4. sort A by (lo, r, d), place it, U fills the rest
+        TRY(mark(c, "docs_sort"));
+        TRY(ensure(c, c->k64a, (size_t)na * 8));
+        TRY(ensure(c, c->k64b, (size_t)na * 8));
+        TRY(ensure(c, c->v0, (size_t)na * 4));
+        TRY(ensure(c, c->v1, (size_t)na * 4));
+        const uint32_t *alist = list + (n - na);
+        uint32_t *v0 = ptr<uint32_t>(c->v0), *v1 = ptr<uint32_t>(c->v1);
+        const int lb = bit_length(n - 1), rb = bit_length(maxlen), db = bit_length(ndocs - 1);
+        const char *e2 = getenv("B200SA_DOCS_SORT2");
+        uint64_t *K;
+        uint32_t *V;
+        int shift;
+        if (lb + rb + db <= 64 && !(e2 && atoi(e2) == 1)) {
+            DocsKey kf{L, sa, rem, d_starts, alist, ndocs, rb, db, true};
+            TRY(docs_sort<uint64_t>(c, kf, alist, ptr<uint64_t>(c->k64a), v0, ptr<uint64_t>(c->k64b), v1, na,
+                                    lb + rb + db, &K, &V));
+            shift = rb + db;
+        } else {
+            // (lo, r, d) does not fit 64 bits: a stable sort by d, then one by (lo, r)
+            uint32_t *K1, *V1;
+            DocsDocKey kd{sa, d_starts, alist, ndocs};
+            TRY(docs_sort<uint32_t>(c, kd, alist, ptr<uint32_t>(c->k64a), v0, ptr<uint32_t>(c->k64b), v1, na, db,
+                                    &K1, &V1));
+            uint32_t *other = V1 == v0 ? v1 : v0;          // V1 is read only by the first pass of the second sort
+            DocsKey kf{L, sa, rem, d_starts, V1, ndocs, rb, 0, false};
+            TRY(docs_sort<uint64_t>(c, kf, V1, ptr<uint64_t>(c->k64a), other, ptr<uint64_t>(c->k64b), V1, na,
+                                    lb + rb, &K, &V));
+            shift = rb;
+        }
+        TRY(mark(c, "docs_place"));
+        TRY(ensure(c, c->p1, (size_t)n * 4));
+        TRY(ensure(c, c->g0, (size_t)n * 4));
+        gr = ptr<uint32_t>(c->p1);
+        glo = ptr<uint32_t>(c->g0);
+        CU_TRY(c, cudaMemsetAsync(glo, 0xff, (size_t)n * 4, c->stream));
+        LAUNCH(c, k_docs_place, cdiv(na, BLK), K, V, na, shift, sa, lcp, rem, pre, gr, glo);
+        TRY(mark(c, "docs_fill"));
+        TRY((dev_scan<OpSum>(c, DocsFreeIn{glo}, DocsFreeOut{list, gr, glo}, n, nullptr)));
+    }
+    // 5. G and glcp
+    TRY(mark(c, "docs_out"));
+    LAUNCH(c, k_docs_out, cdiv(n, BLK), gr, glo, n, sa, rem, L, d_gsa, d_glcp);
+    TRY(mark(c, "end"));
+    CU_TRY(c, cudaGetLastError());
+    return B200SA_OK;
+}
+
+int b200sa_docs_build_dev(b200sa_ctx *c, const uint8_t *d_text, uint64_t n, const uint32_t *d_doc_starts,
+                          uint32_t ndocs, uint32_t *d_gsa, uint32_t *d_glcp, void *stream) {
+    TRY(docs_args(c, n, d_text, d_doc_starts, ndocs, d_gsa));
+    CU_TRY(c, cudaSetDevice(c->device));
+    begin_call(c, stream);
+    int rc = B200SA_OK;
+    if (n <= 1) {
+        // nothing to launch: doc_starts is checked from host copies, G = [0] and glcp = [0] for n = 1
+        rc = docs_check_dev_copy(c, n, d_doc_starts, ndocs);
+        if (rc == B200SA_OK && n == 1) {
+            if (cudaMemsetAsync(d_gsa, 0, 4, c->stream) != cudaSuccess ||
+                (d_glcp && cudaMemsetAsync(d_glcp, 0, 4, c->stream) != cudaSuccess)) {
+                c->last_error = "output write failed";
+                rc = B200SA_ERR_CUDA;
+            }
+        }
+        return tree_exit(c, rc);
+    }
+    return tree_exit(c, docs_core(c, d_text, (uint32_t)n, d_doc_starts, ndocs, d_gsa, d_glcp));
+}
+
+static int docs_host(b200sa_ctx *c, const uint8_t *text, uint32_t n, const uint32_t *starts, uint32_t ndocs,
+                     uint32_t *gsa_out, uint32_t *glcp_out) {
+    TRY(ensure(c, c->text, n));
+    TRY(ensure(c, c->docs_starts, (size_t)ndocs * 4));
+    TRY(ensure(c, c->docs_out, (size_t)n * 4 * (glcp_out ? 2 : 1)));
+    uint32_t *d_gsa = ptr<uint32_t>(c->docs_out), *d_glcp = glcp_out ? d_gsa + n : nullptr;
+    TRY(mark(c, "h2d"));
+    CU_TRY(c, cudaMemcpyAsync(c->text.p, text, n, cudaMemcpyHostToDevice, c->stream));
+    CU_TRY(c, cudaMemcpyAsync(c->docs_starts.p, starts, (size_t)ndocs * 4, cudaMemcpyHostToDevice, c->stream));
+    TRY(docs_core(c, ptr<uint8_t>(c->text), n, ptr<uint32_t>(c->docs_starts), ndocs, d_gsa, d_glcp));
+    if (!c->marks.empty()) c->marks.pop_back();          // the copy-out replaces the core's "end"
+    TRY(mark(c, "d2h"));
+    CU_TRY(c, cudaMemcpyAsync(gsa_out, d_gsa, (size_t)n * 4, cudaMemcpyDeviceToHost, c->stream));
+    if (glcp_out) CU_TRY(c, cudaMemcpyAsync(glcp_out, d_glcp, (size_t)n * 4, cudaMemcpyDeviceToHost, c->stream));
+    TRY(mark(c, "end"));
+    CU_TRY(c, cudaStreamSynchronize(c->stream));
+    return B200SA_OK;
+}
+
+int b200sa_docs_build(b200sa_ctx *c, const uint8_t *text, uint64_t n, const uint32_t *doc_starts, uint32_t ndocs,
+                      uint32_t *gsa_out, uint32_t *glcp_out) {
+    TRY(docs_args(c, n, text, doc_starts, ndocs, gsa_out));
+    TRY(docs_check_host(c, n, doc_starts, ndocs));
+    CU_TRY(c, cudaSetDevice(c->device));
+    begin_call(c, nullptr);
+    if (n <= 1) {
+        if (n == 1) {
+            gsa_out[0] = 0;
+            if (glcp_out) glcp_out[0] = 0;
+        }
+        return end_call(c);
+    }
+    return tree_exit(c, docs_host(c, text, (uint32_t)n, doc_starts, ndocs, gsa_out, glcp_out));
+}
+
+int b200sa_docs_positions_dev(b200sa_ctx *c, const uint8_t *d_text, uint64_t n, const uint32_t *d_gsa,
+                              const uint32_t *d_doc_starts, uint32_t ndocs, const uint8_t *d_queries,
+                              const uint64_t *d_q_off, uint32_t nq, uint32_t *d_start, uint32_t *d_end, void *stream) {
+    if (!c || (nq > 0 && (!d_q_off || !d_start || !d_end)) ||
+        (n > 0 && (!d_text || !d_gsa || !d_doc_starts || ndocs == 0)))
+        return B200SA_ERR_BAD_ARG;
+    if (n > B200SA_MAX_N) return B200SA_ERR_TOO_LARGE;
+    CU_TRY(c, cudaSetDevice(c->device));
+    begin_call(c, stream);
+    if (nq > 0) {
+        LAUNCH(c, k_positions<DocsEnd>, cdiv(nq, BLK), d_text, (uint32_t)n, d_gsa, d_queries, d_q_off, nq, d_start,
+               d_end, DocsEnd{d_doc_starts, ndocs, (uint32_t)n});
+        CU_TRY(c, cudaGetLastError());
+    }
+    return end_call(c);
 }
 
 // ------------------------------------------------------------ multi-GPU: communicator + sharded LMS sort

@@ -538,28 +538,36 @@ __device__ __forceinline__ int cmp_query_suffix(const uint8_t *__restrict__ text
     *is_prefix = (m <= ls);
     return (m <= ls) ? (m == ls ? 0 : -1) : 1;
 }
+// End of the suffix that starts at p: the text's end (SuffixTable), or its document's end
+// (the generalized suffix array of docs.cuh supplies that functor).
+struct TextEnd {
+    uint32_t n;
+    __device__ __forceinline__ uint32_t operator()(uint32_t) const { return n; }
+};
 // One thread per query: reference early-outs (src/table.rs:228-235), then the
-// two binary searches (:244-250).
+// two binary searches (:244-250), every suffix cut at end(p).
+template <class EndF>
 __global__ void __launch_bounds__(BLK) k_positions(const uint8_t *__restrict__ text, uint32_t n,
                                                    const uint32_t *__restrict__ sa, const uint8_t *__restrict__ qs,
                                                    const uint64_t *__restrict__ qoff, uint32_t nq,
-                                                   uint32_t *out_start, uint32_t *out_end) {
+                                                   uint32_t *out_start, uint32_t *out_end, EndF end) {
     uint32_t qi = blockIdx.x * BLK + threadIdx.x;
     if (qi >= nq) return;
     const uint8_t *q = qs + qoff[qi];
     uint32_t m = (uint32_t)(qoff[qi + 1] - qoff[qi]);
-    uint32_t start = 0, end = 0;
+    uint32_t start = 0, finish = 0;
+    auto cmp = [&](uint32_t p, bool *pre) { return cmp_query_suffix(text, end(p), p, q, m, pre); };
     if (n > 0 && m > 0) {
         bool pre;
-        int c0 = cmp_query_suffix(text, n, sa[0], q, m, &pre);
+        int c0 = cmp(sa[0], &pre);
         bool out = (c0 < 0 && !pre);
-        if (!out) { bool p2; out = cmp_query_suffix(text, n, sa[n - 1], q, m, &p2) > 0; }
+        if (!out) { bool p2; out = cmp(sa[n - 1], &p2) > 0; }
         if (!out) {
             uint32_t lo = 0, hi = n;
             while (lo < hi) {                               // first suffix >= query
                 uint32_t mid = lo + (hi - lo) / 2;
                 bool p;
-                int c = cmp_query_suffix(text, n, sa[mid], q, m, &p);
+                int c = cmp(sa[mid], &p);
                 if (c <= 0) hi = mid; else lo = mid + 1;
             }
             start = lo;
@@ -567,14 +575,14 @@ __global__ void __launch_bounds__(BLK) k_positions(const uint8_t *__restrict__ t
             while (lo2 < hi2) {                             // first suffix not starting with query
                 uint32_t mid = lo2 + (hi2 - lo2) / 2;
                 bool p;
-                cmp_query_suffix(text, n, sa[start + mid], q, m, &p);
+                cmp(sa[start + mid], &p);
                 if (!p) hi2 = mid; else lo2 = mid + 1;
             }
-            end = start + lo2;
+            finish = start + lo2;
         }
     }
     out_start[qi] = start;
-    out_end[qi] = end;
+    out_end[qi] = finish;
 }
 
 // ------------------------------------------------------------ generalized suffix array (SURVEY 8f-3)

@@ -1,7 +1,7 @@
 #!/bin/bash
 # compute-sanitizer on small builds: every path of round 2 (direct / robust LMS sort, the 2-bit bucket sort and its
 # overflow, induce variants,
-# fused classifier, sharded world-1 entry points, LCP paths, rows f, the suffix tree)
+# fused classifier, sharded world-1 entry points, LCP paths, rows f, the suffix tree, the document suffix array)
 mkdir -p gpurun_out
 cat > /tmp/san.py <<'PY'
 import sys, os
@@ -76,6 +76,21 @@ st_ = SuffixTable(cases[0][1].tobytes())
 st_.lcp_intervals()
 g = GeneralizedSuffixTable([b"ACGT" * 50, b"GATTACA" * 30, b"TTTT"])
 assert len(g.positions(b"TACAG")) > 0
+from suffix_b200 import DocumentSuffixTable
+from tests import model_docs
+dna = gen.dna(60_000).tobytes()
+doc_sets = [[dna[:20000], b"", dna[20000:20007], dna[:20000], dna[20000:]], [b"ACGT"] * 3000,
+            [bytes(range(256)), b"\x00\x00", b"", bytes(range(256))[:7]], [b"banana"]]
+for k, docs in enumerate(doc_sets):
+    for two in ("", "1"):                        # the (lo, r, d) sort and the two-stage sort
+        os.environ["B200SA_DOCS_SORT2"] = two
+        dt = DocumentSuffixTable(docs)
+        if len(dt) < 3000:
+            g, l = model_docs.brute(docs)
+            assert np.array_equal(dt.table(), g) and np.array_equal(dt.lcp_lens(), l), k
+    s_, e_ = dt.positions_batch([b"ACG", b"TA", b"\x00", b"", b"GTAC"])
+    assert all(int(a) <= int(b) for a, b in zip(s_, e_)), k
+del os.environ["B200SA_DOCS_SORT2"]
 print("sanitize workload ok")
 PY
 for tool in memcheck racecheck; do
