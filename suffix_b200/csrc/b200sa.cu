@@ -21,10 +21,6 @@
 #include "classify.cuh"
 #include "classify2.cuh"
 #include "induce.cuh"
-#include "induce2.cuh"
-#include "induce3.cuh"
-#include "induce4.cuh"
-#include "induce5.cuh"
 #include "induce6.cuh"
 #include "pipeline_kernels.cuh"
 #include "lms_sort.cuh"
@@ -49,9 +45,9 @@ struct b200sa_ctx {
     cudaEvent_t ev_sa = nullptr;
     int sm_count = 0;
     int induce_blocks = 0;          // largest co-resident grid (workspace is sized for it)
-    int induce_bps_max = 1;         // occupancy bound over all variants, blocks per SM
-    int induce_occ[3] = {1, 1, 1};  // occupancy bound per text packing (2, 4, 8 bits) of the default variant
-    int induce_occ_v[7][3] = {{1, 1, 1}, {1, 1, 1}, {1, 1, 1}, {1, 1, 1}, {1, 1, 1}, {1, 1, 1}, {1, 1, 1}};   // per kernel variant
+    int induce_bps_max = 1;         // occupancy bound over both kernels, blocks per SM
+    int induce_occ[3] = {1, 1, 1};  // occupancy bound per text packing (2, 4, 8 bits) of the default kernel
+    int induce_occ_v[2][3] = {{1, 1, 1}, {1, 1, 1}};   // per kernel: [0] k_induce, [1] k_induce6 (k_induce for 4 / 8 bits)
     int induce_bps_env = 0;         // B200SA_INDUCE_BPS override (0 = adaptive)
     int cur_induce_blocks = 0;      // grid of the current build
     std::string last_error;
@@ -85,8 +81,6 @@ struct b200sa_ctx {
     DevBuf sh_a, sh_b, sh_c, sh_d, sh_e, sh_f, sh_small;
     bool lms_asc_ready = false;       // c->lmspos / c->lmsrank (text order) valid for the current text
     uint32_t scan_epoch = 0, scan_tiles_cap = 0;
-    bool l2_persist = false;          // access policy window for the packed text (B200SA_L2PERSIST)
-    size_t l2_max_window = 0, l2_set_aside = 0;
     uint32_t sigma = 256;            // distinct bytes of the current text
     int bits = 8;                    // bits per char of the packed text of the current call (2, 4 or 8 = raw)
     const void *ptext = nullptr;     // packed words, or the byte text when bits == 8
@@ -152,9 +146,7 @@ static void begin_call(b200sa_ctx *c, void *stream) {
     c->launches = 0;
     c->last_error.clear();
 }
-static void l2_window(b200sa_ctx *c, const void *p, size_t bytes);
 static int end_call(b200sa_ctx *c) {
-    if (c->l2_persist) l2_window(c, nullptr, 0);              // the caller's stream leaves without our policy
     c->stats.kernel_launches = c->launches;
     c->stats.workspace_bytes = c->ws_bytes;
     c->phase_names.clear();
@@ -475,22 +467,6 @@ static int reduced_sa(b200sa_ctx *c, uint32_t *R, uint32_t m, uint32_t names, ui
     return B200SA_OK;
 }
 
-// ------------------------------------------------------- L2 residency of the packed text
-// The induce, the window keys of the LMS sort and the direct LCP all gather from the packed
-// text at random while hundreds of MB of suffix-array data stream through L2.  An access
-// policy window marks the packed text persisting (evict-last) for the kernels of this call.
-static void l2_window(b200sa_ctx *c, const void *p, size_t bytes) {
-    if (!c->l2_persist || c->l2_max_window == 0) return;
-    cudaStreamAttrValue v;
-    memset(&v, 0, sizeof v);
-    v.accessPolicyWindow.base_ptr = const_cast<void *>(p);
-    v.accessPolicyWindow.num_bytes = bytes < c->l2_max_window ? bytes : c->l2_max_window;
-    v.accessPolicyWindow.hitRatio = bytes ? 1.0f : 0.0f;
-    v.accessPolicyWindow.hitProp = cudaAccessPropertyPersisting;
-    v.accessPolicyWindow.missProp = cudaAccessPropertyStreaming;
-    if (cudaStreamSetAttribute(c->stream, cudaStreamAttributeAccessPolicyWindow, &v) != cudaSuccess) cudaGetLastError();
-}
-
 // ------------------------------------------------------- packed text
 // Chooses 2 / 4 bits per char when the alphabet allows it and packs the text;
 // code_of/alpha live in the tables buffer.
@@ -508,7 +484,6 @@ static int pack_text(b200sa_ctx *c, const uint8_t *text, uint64_t n, uint32_t si
     else LAUNCH(c, (k_pack<4>), cdiv(words, BLK), text, n, tab + T_CODE, ptr<uint32_t>(c->packed));
     CU_TRY(c, cudaGetLastError());
     c->ptext = c->packed.p;
-    if (words * 4 <= c->l2_set_aside) l2_window(c, c->packed.p, words * 4 + 8);
     return B200SA_OK;
 }
 
@@ -703,32 +678,18 @@ static int lms_direct_sort(b200sa_ctx *c, uint32_t n, uint32_t m, uint32_t **lis
 }
 
 // ------------------------------------------------------- induce launcher
-// Kernel variants of the induce passes (B200SA_INDUCE=1..6 forces one):
-//   1  one-round steps with MATCH ranking (any packing; the default for 4-bit and byte text)
-//   2  multi-round bucket steps (packed text)
-//   3  packed-counter ranking on physically aligned tiles (2-bit text)
-//   4  3 + three carried predecessor chars per byte + staged coalesced stores (2-bit text)
-//   5  warp-private tile streams + 16-bit carried chars with producer-side refresh (2-bit text)
-//   6  3's block-wide tiles + 5's carried chars + cascade steps for short chain lists (2-bit text; default there;
-//      B200SA_NO_CASCADE / B200SA_CASCADE_MAX=<entries> switch the cascade steps off / limit them)
-static int induce_variant_env() {
-    const char *e = getenv("B200SA_INDUCE");       // read per call: tests switch variants inside one process
-    return e ? atoi(e) : 0;
-}
+// Kernel variants of the induce passes:
+//   1  k_induce: one-round steps with MATCH ranking (any packing; the default for 4-bit and byte text)
+//   6  k_induce6: packed-counter ranking on physically aligned tiles + 16-bit carried chars + cascade steps for
+//      short chain lists (2-bit text; default there; B200SA_NO_CASCADE / B200SA_CASCADE_MAX=<entries> switch the
+//      cascade steps off / limit them)
+// B200SA_INDUCE=1 forces variant 1 on 2-bit text, which also runs there when sa or lms is not 16-byte aligned.
 static int induce_variant(int bits) {
-    int v = induce_variant_env();
-    if (v == 2 && bits < 8) return 2;
-    if (v == 1) return 1;
-    if (bits == 2) return (v >= 3 && v <= 5) ? v : 6;
-    return 1;
+    const char *e = getenv("B200SA_INDUCE");       // read per call: tests switch variants inside one process
+    return (bits == 2 && !(e && atoi(e) == 1)) ? 6 : 1;
 }
 static const void *induce_fn_v(bool spass, int bits, int variant) {
     if (variant == 6 && bits == 2) return spass ? (const void *)k_induce6<true> : (const void *)k_induce6<false>;
-    if (variant == 5 && bits == 2) return spass ? (const void *)k_induce5<true> : (const void *)k_induce5<false>;
-    if (variant == 4 && bits == 2) return spass ? (const void *)k_induce4<true> : (const void *)k_induce4<false>;
-    if (variant == 3 && bits == 2) return spass ? (const void *)k_induce3<true> : (const void *)k_induce3<false>;
-    if (variant == 2 && bits == 2) return spass ? (const void *)k_induce2<true, 2> : (const void *)k_induce2<false, 2>;
-    if (variant == 2 && bits == 4) return spass ? (const void *)k_induce2<true, 4> : (const void *)k_induce2<false, 4>;
     if (bits == 2) return spass ? (const void *)k_induce<true, 2> : (const void *)k_induce<false, 2>;
     if (bits == 4) return spass ? (const void *)k_induce<true, 4> : (const void *)k_induce<false, 4>;
     return spass ? (const void *)k_induce<true, 8> : (const void *)k_induce<false, 8>;
@@ -764,10 +725,10 @@ static int launch_induce(b200sa_ctx *c, bool spass, const uint8_t *text, uint32_
     }
     void *args[] = {&A};
     int variant = induce_variant(c->bits);
-    if (variant >= 3 && (((uintptr_t)sa | (uintptr_t)lms) & 15) != 0) variant = 1;      // 16-byte loads need aligned arrays
-    A.carry = (variant >= 5) ? 2 : (variant == 4 ? 1 : 0);
+    if (variant == 6 && (((uintptr_t)sa | (uintptr_t)lms) & 15) != 0) variant = 1;      // 16-byte loads need aligned arrays
+    A.carry = variant == 6 ? 2 : 0;
     int bi = c->bits == 2 ? 0 : (c->bits == 4 ? 1 : 2);
-    int blocks = c->cur_induce_blocks, cap = c->sm_count * c->induce_occ_v[variant][bi];
+    int blocks = c->cur_induce_blocks, cap = c->sm_count * c->induce_occ_v[variant == 6][bi];
     if (blocks > cap) blocks = cap;
     A.cascade = 0;
     if (variant == 6 && !getenv("B200SA_NO_CASCADE")) {          // multi-round steps for the short lists of every bucket's cascade
@@ -935,7 +896,7 @@ static int build_dev(b200sa_ctx *c, const uint8_t *d_text, uint64_t n, uint32_t 
     }
     c->stats.m = m; c->last_m = m;
     c->stats.induce_blocks = c->cur_induce_blocks;
-    TRY(ensure(c, c->pred, 2 * n + 64));          // bytes (variants 1-4) or 16-bit carried words (variant 5)
+    TRY(ensure(c, c->pred, 2 * n + 64));          // bytes (variant 1) or 16-bit carried words (variant 6)
     TRY(ensure(c, c->lmslist, (size_t)m * 4));
     TRY(ensure(c, c->lmspred, 2 * (size_t)m + 64));
     TRY(ensure(c, c->blkcnt, (size_t)2 * c->induce_blocks * 256 * 4));
@@ -1236,23 +1197,7 @@ int b200sa_ctx_create(int device, b200sa_ctx **out) {
     if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) { delete c; return B200SA_ERR_CUDA; }
     if (prop.major != 9 || prop.minor != 0) { delete c; return B200SA_ERR_NO_DEVICE; }   // sm_90a code: H100 class only
     c->sm_count = prop.multiProcessorCount;
-    if (const char *e = getenv("B200SA_L2FETCH")) {   // experiment: L2 fetch granularity for random gathers
-        int v = atoi(e);
-        if (v == 32 || v == 64 || v == 128) cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, (size_t)v);
-    }
     if (!prop.cooperativeLaunch) { delete c; return B200SA_ERR_NO_DEVICE; }
-    if (const char *e = getenv("B200SA_L2PERSIST")) {
-        int mb = atoi(e);                                       // MB of L2 set aside for persisting lines
-        if (mb > 0 && prop.persistingL2CacheMaxSize > 0) {
-            size_t want = (size_t)mb << 20;
-            if (want > (size_t)prop.persistingL2CacheMaxSize) want = (size_t)prop.persistingL2CacheMaxSize;
-            if (cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, want) == cudaSuccess) {
-                c->l2_persist = true;
-                c->l2_set_aside = want;
-                c->l2_max_window = (size_t)prop.accessPolicyMaxWindowSize;
-            } else cudaGetLastError();
-        }
-    }
     if (cudaStreamCreateWithFlags(&c->own_stream, cudaStreamNonBlocking) != cudaSuccess) { delete c; return B200SA_ERR_CUDA; }
     c->stream = c->own_stream;
     if (cudaStreamCreateWithFlags(&c->copy_stream, cudaStreamNonBlocking) != cudaSuccess ||
@@ -1262,19 +1207,19 @@ int b200sa_ctx_create(int device, b200sa_ctx **out) {
     int occ = 0;
     {
         const int bb[3] = {2, 4, 8};
-        for (int v = 1; v <= 6; v++)
+        for (int v = 0; v < 2; v++)
             for (int k = 0; k < 3; k++) {
                 int ok = 1 << 30;
                 for (int sp = 0; sp < 2; sp++) {
                     int o = 0;
-                    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&o, induce_fn_v(sp != 0, bb[k], v), BLK, 0);
+                    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&o, induce_fn_v(sp != 0, bb[k], v ? 6 : 1), BLK, 0);
                     if (o < ok) ok = o;
                 }
                 c->induce_occ_v[v][k] = ok > 4 ? 4 : ok;
             }
         for (int k = 0; k < 3; k++) {
-            c->induce_occ[k] = c->induce_occ_v[induce_variant(bb[k])][k];
-            for (int v = 1; v <= 6; v++) if (c->induce_occ_v[v][k] > occ) occ = c->induce_occ_v[v][k];
+            c->induce_occ[k] = c->induce_occ_v[induce_variant(bb[k]) == 6][k];
+            for (int v = 0; v < 2; v++) if (c->induce_occ_v[v][k] > occ) occ = c->induce_occ_v[v][k];
         }
     }
     if (occ < 1) { cudaFreeHost(c->h_pin); delete c; return B200SA_ERR_CUDA; }

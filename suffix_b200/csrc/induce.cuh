@@ -45,8 +45,8 @@ struct InduceArgs {
     uint32_t *run_scratch;   // [TILE] run-skipping: terminal entries in scan order
     uint32_t *run_alive;     // [TILE] run-skipping: alive entries of the epoch being emitted grid-wide
     uint32_t *cmd;           // [8]    block 0 -> grid: {cmd, a, t_prev, rounds, base pos, bucket}
-    int carry;               // 1: pred[] carries predecessor chars per SA slot as bytes (k_induce4), 2: as 16-bit words
-                             // (k_induce5); products of the shared small-step code mark theirs "unknown" (0)
+    int carry;               // 2: pred[] carries predecessor chars per SA slot as 16-bit words (k_induce6); products of
+                             // the shared small-step code mark theirs "unknown" (0).  0: k_induce
     uint32_t cascade;        // k_induce6: chain lists of at most this many entries take cascade steps (0: off)
     uint32_t run_streak;     // small chain rounds in one bucket before the chain is finished at once (0: RUN_STREAK)
     uint32_t blocklog_step;  // diagnostics: every block logs its phase times of big step number blocklog_step-1 at steplog[4096 + 6*bid ..]

@@ -1,18 +1,94 @@
-// induce6.cuh -- K4/K5 for 2-bit packed text (sigma <= 4): the block-wide packed-counter steps of
-// induce3.cuh (reference src/table.rs:421-448, :543-573, :723-736) with the 16-bit CARRIED CHARS of
-// induce5.cuh.  The reasoning behind it (step timelines of the persistent kernels): the count phases
-// of induce3 are bound by one divergent T[s-1] gather per entry; with six chars carried next to
-// every SA slot (written by the producer, refreshed by the producer when they would run out) a
-// count phase only reads 2 bytes per entry -- except for LMS lists, whose entries gather once.  The
-// block-wide 2048-entry tiles of induce3 scatter about twice as fast as the warp-private tiles of
-// induce5, so this variant keeps them.
+// induce6.cuh -- K4/K5 for 2-bit packed text (sigma <= 4): the one-round bucket steps of
+// induce.cuh (reference src/table.rs:421-448, :543-573, head_insert/tail_insert :723-736) with
+//   * PACKED-COUNTER RANKING on physically aligned tiles: tiles are cut in physical index space at
+//     multiples of TILE, so thread t owns 8 consecutive, 32-byte aligned entries (two 16-byte
+//     loads); the logical (scan) order is thread-major, ascending or descending.  With at most 4
+//     destination buckets the per-thread counts of all buckets fit ONE 64-bit word (4 fields of 16
+//     bits; a tile has 2048 entries), so one block-wide add-scan of that word ranks the whole tile
+//     stably for every bucket at once, and the count matrix of a step is G x 4 words, not G x 256;
+//   * 16-bit CARRIED CHARS: a word next to every SA slot holds the next six text chars to the left
+//     of the entry, b = c1 | c2 << 2 | ... | c6 << 10 | cnt << 12, written by the step that
+//     PRODUCES the entry; a child inherits (b >> 2, cnt - 1) without touching memory, and the
+//     producer refreshes a child that would run dry.  Without them the count phases are bound by one
+//     divergent T[s-1] gather per entry; with them a count phase reads 2 bytes per entry -- except
+//     for LMS lists, whose entries gather once, and the rare entries made by the shared small-step
+//     code (marked 0);
+//   * CASCADE STEPS for the short chain lists at the end of every bucket (below).
+// Control flow (peek, big / small steps, run skipping, fill accounting, invariants) is the one
+// of induce.cuh.
 #pragma once
-#include "induce5.cuh"
+#include "induce.cuh"
 #ifndef IND6_MINB
 #define IND6_MINB 3
 #endif
 
 namespace b200sa {
+
+struct Ind6Shared {
+    unsigned long long wtot[2][NWARP];   // per-warp packed totals, double buffered over tiles
+    uint32_t cbase[4];                   // running destination position per code (inside the bucket part)
+    uint32_t ctot[4];                    // step totals per code
+    uint32_t code_of[256];
+    uint32_t nsig;
+};
+
+// Physical chunk of thread t in tile T of a segment: 8 consecutive entries in PHYSICAL order
+// (no data movement after the load: the registers are consumed an iteration later, so the
+// loads stay in flight under the work on the previous tile).  Logical (scan) order is
+// ascending physical index in the L pass and descending in the S pass.
+__device__ __forceinline__ void ind6_load8(const uint32_t *__restrict__ src, uint32_t chunk, uint32_t limit,
+                                           uint32_t (&raw)[ITEMS]) {
+    if (chunk + ITEMS <= limit) {
+        const uint4 *q = reinterpret_cast<const uint4 *>(src + chunk);
+        uint4 a = __ldcg(q), b = __ldcg(q + 1);
+        raw[0] = a.x; raw[1] = a.y; raw[2] = a.z; raw[3] = a.w;
+        raw[4] = b.x; raw[5] = b.y; raw[6] = b.z; raw[7] = b.w;
+    } else {
+#pragma unroll
+        for (int i = 0; i < ITEMS; i++) raw[i] = (chunk + i < limit) ? __ldcg(src + chunk + i) : 0u;
+    }
+}
+
+// pair-reversal of 16 two-bit groups (same as lms_sort.cuh::rev_pairs, which is included later)
+__device__ __forceinline__ uint32_t rev_pairs16(uint32_t x) {
+    uint32_t y = __brev(x);
+    return ((y & 0x55555555u) << 1) | ((y >> 1) & 0x55555555u);
+}
+// carried word of the entry at text position e from the ONE aligned text word that holds T[e-1]
+// (up to six chars; fewer when the word starts within six chars)
+__device__ __forceinline__ uint32_t carry_from_word(uint32_t e, uint32_t wd) {
+    uint32_t q = e - 1u;                          // position of c1 (e > 0)
+    uint32_t av = (q & 15u) + 1u;                 // chars of this word at or below q
+    uint32_t x = wd << (2u * (15u - (q & 15u)));  // c1 in the top pair
+    uint32_t cnt = av < 6u ? av : 6u;
+    return (rev_pairs16(x) & 0xfffu) | (cnt << 12);
+}
+__device__ __forceinline__ uint32_t fresh_carry(const void *__restrict__ ptext, uint32_t e) {
+    if (e == 0) return 0u;
+    return carry_from_word(e, __ldg(reinterpret_cast<const uint32_t *>(ptext) + ((e - 1u) >> 4)));
+}
+// 8 carried words of a lane's chunk (16 bytes)
+__device__ __forceinline__ void load_carry8(const uint16_t *__restrict__ pc, uint32_t chunk, uint32_t limit, uint32_t (&v)[4]) {
+    if (chunk + ITEMS <= limit) {
+        uint4 a = __ldcg(reinterpret_cast<const uint4 *>(pc + chunk));
+        v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w;
+    } else {
+#pragma unroll
+        for (int i = 0; i < 4; i++) {
+            uint32_t lo = (chunk + 2 * i < limit) ? pc[chunk + 2 * i] : 0u, hi = (chunk + 2 * i + 1 < limit) ? pc[chunk + 2 * i + 1] : 0u;
+            v[i] = lo | (hi << 16);
+        }
+    }
+}
+__device__ __forceinline__ uint32_t carry_at(const uint32_t (&v)[4], int i) { return (v[i >> 1] >> ((i & 1) * 16)) & 0xffffu; }
+
+// diagnostics (B200SA_STEPLOG): block 0 logs the phase boundaries of a big step
+#define IND_MARK(code)                                                                                   \
+    if (A.steplog && bid == 0 && tid == 0) {                                                             \
+        unsigned long long now_, k_ = A.steplog[0];                                                      \
+        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(now_));                                         \
+        if (k_ < 2000) { A.steplog[1 + 2 * k_] = now_; A.steplog[2 + 2 * k_] = 0xF0000000ull | (code); A.steplog[0] = k_ + 1; } \
+    }
 
 // ---------------------------------------------------------------- cascade steps
 // The entries a chain list induces into its OWN bucket are the next list of that bucket, a
@@ -47,7 +123,7 @@ __device__ __forceinline__ unsigned long long sel4(uint32_t k, unsigned long lon
 // products of the last round.  The code is kept SMALL on purpose (rolled loops over a shared-memory copy
 // of the tile): it runs a few times per pass, from a cold instruction cache.
 template <bool SPASS>
-__device__ __noinline__ void cascade_step(const InduceArgs &A, IndShared &sh, Ind4Shared &s4, cg::grid_group &grid,
+__device__ __noinline__ void cascade_step(const InduceArgs &A, IndShared &sh, Ind6Shared &s4, cg::grid_group &grid,
                                           uint32_t cbyte, uint32_t tiles, uint32_t *cntbuf, bool local) {
     const uint32_t G = gridDim.x, bid = blockIdx.x, tid = threadIdx.x;
     const uint32_t w = warp_id(), l = lane_id();
@@ -211,7 +287,7 @@ __device__ __noinline__ void cascade_step(const InduceArgs &A, IndShared &sh, In
 
 // Small episode of k_induce6: induce_small_episode (induce.cuh) with cascade steps for chain lists.
 template <bool SPASS>
-__device__ __noinline__ void induce6_small_episode(const InduceArgs &A, IndShared &sh, Ind4Shared &s4, cg::grid_group &grid,
+__device__ __noinline__ void induce6_small_episode(const InduceArgs &A, IndShared &sh, Ind6Shared &s4, cg::grid_group &grid,
                                                    uint32_t &smallcount) {
     const uint32_t bid = blockIdx.x, tid = threadIdx.x;
     if (bid == 0) {
@@ -274,7 +350,7 @@ __device__ __noinline__ void induce6_small_episode(const InduceArgs &A, IndShare
 // One ordinary (one-round) big step of k_induce6 over sh.seg, all blocks.  A function of its own so that the
 // registers of its two tile loops are allocated without regard to the rest of the kernel.
 template <bool SPASS>
-__device__ __noinline__ void induce6_big_step(const InduceArgs &A, IndShared &sh, Ind4Shared &s4, cg::grid_group &grid,
+__device__ __noinline__ void induce6_big_step(const InduceArgs &A, IndShared &sh, Ind6Shared &s4, cg::grid_group &grid,
                                               uint32_t bigcount, uint32_t &bigtiles) {
     const uint32_t G = gridDim.x, bid = blockIdx.x, tid = threadIdx.x;
     const uint32_t w = warp_id(), l = lane_id();
@@ -316,9 +392,9 @@ __device__ __noinline__ void induce6_big_step(const InduceArgs &A, IndShared &sh
     uint32_t c0 = 0, c1 = 0, c2 = 0, c3 = 0;
     if (gather_all) {
         uint32_t s0[ITEMS], s1[ITEMS], wv[ITEMS];
-        if (tb0 < tb1) ind4_load8(src, chunk_of(tb0), limit, s0);
+        if (tb0 < tb1) ind6_load8(src, chunk_of(tb0), limit, s0);
         for (uint32_t k = tb0; k < tb1; k++) {
-            if (k + 1 < tb1) ind4_load8(src, chunk_of(k + 1), limit, s1);
+            if (k + 1 < tb1) ind6_load8(src, chunk_of(k + 1), limit, s1);
             const uint32_t chunk = chunk_of(k);
 #pragma unroll
             for (int i = 0; i < ITEMS; i++)           // one aligned text word per entry, all eight in flight
@@ -356,7 +432,7 @@ __device__ __noinline__ void induce6_big_step(const InduceArgs &A, IndShared &sh
             }
             if (need) {                               // products of small steps / the seed: chars not carried
                 uint32_t sv[ITEMS];
-                ind4_load8(src, chunk, limit, sv);
+                ind6_load8(src, chunk, limit, sv);
 #pragma unroll
                 for (int i = 0; i < ITEMS; i++) {
                     if ((need >> i) & 1u) {
@@ -429,12 +505,12 @@ __device__ __noinline__ void induce6_big_step(const InduceArgs &A, IndShared &sh
         const uint32_t bs2 = SPASS ? sh.bstart[sh.alpha[2] + 1] - 1u : sh.bstart[sh.alpha[2]];
         const uint32_t bs3 = SPASS ? sh.bstart[sh.alpha[3] + 1] - 1u : sh.bstart[sh.alpha[3]];
         uint32_t s_cur[ITEMS], s_nxt[ITEMS], p_cur[4], p_nxt[4] = {0, 0, 0, 0};
-        ind4_load8(src, chunk_of(tb0), limit, s_cur);
+        ind6_load8(src, chunk_of(tb0), limit, s_cur);
         load_carry8(pc, chunk_of(tb0), limit, p_cur);
         uint32_t par = 0;
         for (uint32_t k = tb0; k < tb1; k++) {
             if (k + 1 < tb1) {
-                ind4_load8(src, chunk_of(k + 1), limit, s_nxt);
+                ind6_load8(src, chunk_of(k + 1), limit, s_nxt);
                 load_carry8(pc, chunk_of(k + 1), limit, p_nxt);
             }
             const uint32_t chunk = chunk_of(k);
@@ -526,7 +602,7 @@ __device__ __noinline__ void induce6_big_step(const InduceArgs &A, IndShared &sh
 template <bool SPASS>
 __global__ void __launch_bounds__(BLK, IND6_MINB) k_induce6(InduceArgs A) {
     __shared__ IndShared sh;
-    __shared__ Ind4Shared s4;
+    __shared__ Ind6Shared s4;
     cg::grid_group grid = cg::this_grid();
     const uint32_t G = gridDim.x, bid = blockIdx.x, tid = threadIdx.x;
     const uint32_t w = warp_id(), l = lane_id();
