@@ -219,6 +219,58 @@ int b200sa_docs_positions_dev(b200sa_ctx *ctx, const uint8_t *d_text, uint64_t n
                               const uint32_t *d_doc_starts, uint32_t ndocs, const uint8_t *d_queries,
                               const uint64_t *d_q_off, uint32_t nq, uint32_t *d_start, uint32_t *d_end, void *stream);
 
+/* ---- generalized suffix tree with document counts (SURVEY.md 8f-7) ----
+ * Documents D_0 .. D_{k-1} are given as for b200sa_docs_build: their concatenation C (n bytes) and
+ * doc_starts.  For a position p of document d, len(p) = end_d - p and T_p = C[p, p + len(p)); G and
+ * glcp are what b200sa_docs_build returns.
+ * The tree is the compressed trie of the strings T_p.  Its nodes are the root, every distinct T_p,
+ * and every string followed, among the T_p, by at least two distinct next bytes.  Children are
+ * ordered by the first byte of their label and preorder is lexicographic, as for b200sa_suffix_tree.
+ * The terminals of a node are all positions p whose T_p equals its string: a suffix that is a proper
+ * prefix of another stays a terminal of a node with children (the reference's no-terminator
+ * convention), and equal suffixes of different documents share one node.  The root has none.
+ * As rules over (G, glcp), with len[r] = len(G[r]) and glcp[n] := 0: rules 1-8 of b200sa_suffix_tree,
+ * with sa = G and lcp = glcp, except that
+ *   3'. rank r is merged iff (r+1 < n and glcp[r+1] == len[r]) or (r > 0 and glcp[r] == len[r]); every
+ *       other rank is a leaf with range [r, r+1) and depth len[r].  (For k = 1 the second condition never
+ *       holds: the six arrays equal b200sa_suffix_tree's.)
+ *   6.  label_start = G[lo] + pd as before; since depth <= len[lo], a label never crosses a document end.
+ * and two more arrays per node v:
+ *   term_end[v]   the terminals of v are G[sa_lo[v], term_end[v]) (== sa_lo[v] when there are none): a
+ *                 prefix of the range, since proper prefixes sort first and equal strings are adjacent,
+ *                 ordered by document;
+ *   doc_count[v]  the number of distinct documents among G[sa_lo[v], sa_hi[v]); the root's is the number
+ *                 of non-empty documents.
+ * Inputs as for b200sa_suffix_tree (cap >= max(1, 2n), n <= B200SA_TREE_MAX_N, every array of `out` holds
+ * cap entries) and b200sa_docs_build (doc_starts; the host entry checks it on the host, the device entry
+ * on the device).  G and glcp are checked on the device with the tree's checks, glcp[r] bounded by the
+ * len of both neighbours; every failure returns B200SA_ERR_BAD_ARG with a b200sa_last_error detail.
+ * n = 0 gives the root alone (doc_count 0).  The phases report to b200sa_last_phase_times.  Device
+ * workspace, measured on 100 MB on one H100 80GB HBM3: about 81 bytes per text byte (74 for n/4 copies
+ * of "ACGT"); the caller's eight arrays add 64, G and glcp 8, and the host entry stages all of them.
+ * (The output struct is b200sa_docs_tree_out: C gives a type and a function one namespace.) */
+typedef struct {
+    b200sa_tree tree;       /* rules 1-8 with 3' and document suffix lengths   */
+    uint32_t *term_end;     /* terminals of v: G[sa_lo[v], term_end[v])        */
+    uint32_t *doc_count;    /* distinct documents among G[sa_lo[v], sa_hi[v])  */
+} b200sa_docs_tree_out;
+/* device buffers (G, glcp, doc_starts in; the eight arrays out); synchronises the stream before returning */
+int b200sa_docs_tree_dev(b200sa_ctx *ctx, uint64_t n, const uint32_t *d_gsa, const uint32_t *d_glcp,
+                         const uint32_t *d_doc_starts, uint32_t ndocs, const b200sa_docs_tree_out *out,
+                         uint64_t cap, uint64_t *num_nodes, void *stream);
+/* host buffers */
+int b200sa_docs_tree(b200sa_ctx *ctx, uint64_t n, const uint32_t *gsa, const uint32_t *glcp,
+                     const uint32_t *doc_starts, uint32_t ndocs, const b200sa_docs_tree_out *out,
+                     uint64_t cap, uint64_t *num_nodes);
+/* Document frequency of a batch of ranges of G: d_start / d_end as b200sa_docs_positions_dev writes them.
+ * d_count[q] = 0 for an empty range, else doc_count of a node whose range is [start[q], end[q]) (every node
+ * with that range has the same count): the number of documents that contain query q.  A non-empty range
+ * that is no node's returns B200SA_ERR_BAD_ARG.  The arrays are the first num_nodes entries of
+ * b200sa_docs_tree_dev's sa_lo, sa_hi and doc_count.  Synchronises the stream. */
+int b200sa_docs_tree_counts_dev(b200sa_ctx *ctx, const uint32_t *d_sa_lo, const uint32_t *d_sa_hi,
+                                const uint32_t *d_doc_count, uint64_t num_nodes, const uint32_t *d_start,
+                                const uint32_t *d_end, uint32_t nq, uint32_t *d_count, void *stream);
+
 /* ---- multi-GPU: communicator + sharded LMS-suffix sort (SURVEY.md 8e, config 5) ----
  * One process (or thread) and one context per GPU.  NCCL is resolved at run time
  * (the copy already loaded in the process, else libnccl.so.2); the single-GPU entry

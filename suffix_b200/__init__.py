@@ -7,3 +7,4 @@ from .table import SuffixTable  # noqa: F401
 from .generalized import GeneralizedSuffixTable  # noqa: F401,E402
 from .tree import Node, SuffixTree  # noqa: F401,E402
 from .docs import DocumentSuffixTable  # noqa: F401,E402
+from .docs_tree import DocumentNode, DocumentSuffixTree  # noqa: F401,E402

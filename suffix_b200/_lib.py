@@ -37,6 +37,14 @@ class Tree(ctypes.Structure):
 
 TREE_FIELDS = tuple(f for f, _ in Tree._fields_)
 
+
+class DocsTree(ctypes.Structure):
+    """b200sa_docs_tree_out: the six tree arrays, term_end and doc_count, indexed by preorder id."""
+    _fields_ = [("tree", Tree), ("term_end", ctypes.c_void_p), ("doc_count", ctypes.c_void_p)]
+
+
+DOCS_TREE_FIELDS = TREE_FIELDS + ("term_end", "doc_count")
+
 _lib = None
 
 
@@ -75,6 +83,9 @@ def lib():
         "b200sa_docs_build": ([vp, vp, u64, vp, u32, vp, vp], ci),
         "b200sa_docs_build_dev": ([vp, vp, u64, vp, u32, vp, vp, vp], ci),
         "b200sa_docs_positions_dev": ([vp, vp, u64, vp, vp, u32, vp, vp, u32, vp, vp, vp], ci),
+        "b200sa_docs_tree_dev": ([vp, u64, vp, vp, vp, u32, ctypes.POINTER(DocsTree), u64, ctypes.POINTER(u64), vp], ci),
+        "b200sa_docs_tree": ([vp, u64, vp, vp, vp, u32, ctypes.POINTER(DocsTree), u64, ctypes.POINTER(u64)], ci),
+        "b200sa_docs_tree_counts_dev": ([vp, vp, vp, vp, u64, vp, vp, u32, vp, vp], ci),
         "b200sa_last_stats": ([vp, ctypes.POINTER(Stats)], ci),
         "b200sa_set_timing": ([vp, ci], ci),
         "b200sa_last_phase_times": ([vp, ctypes.POINTER(ctypes.c_char_p), ctypes.POINTER(ctypes.c_float), ci], ci),
@@ -245,6 +256,38 @@ class Context:
                            stream: int = 0):
         self._check(lib().b200sa_docs_positions_dev(self._h, d_text, n, d_gsa, d_doc_starts, ndocs, d_q, d_qoff, nq,
                                                     d_start, d_end, stream))
+
+    def docs_tree(self, gsa: np.ndarray, glcp: np.ndarray, doc_starts: np.ndarray) -> dict:
+        """b200sa_docs_tree: the generalized suffix tree of (G, glcp) as eight u32 arrays of N entries."""
+        gsa = np.ascontiguousarray(gsa, dtype=np.uint32)
+        glcp = np.ascontiguousarray(glcp, dtype=np.uint32)
+        starts = np.ascontiguousarray(doc_starts, dtype=np.uint32)
+        if len(gsa) != len(glcp):
+            raise ValueError("gsa and glcp lengths differ")
+        n = len(gsa)
+        cap = max(1, 2 * n)
+        arrs = {f: np.empty(cap, dtype=np.uint32) for f in DOCS_TREE_FIELDS}
+        t = DocsTree(Tree(*[arrs[f].ctypes.data for f in TREE_FIELDS]), arrs["term_end"].ctypes.data,
+                     arrs["doc_count"].ctypes.data)
+        N = ctypes.c_uint64(0)
+        self._check(lib().b200sa_docs_tree(self._h, n, gsa.ctypes.data, glcp.ctypes.data,
+                                           starts.ctypes.data if len(starts) else None, len(starts), ctypes.byref(t),
+                                           cap, ctypes.byref(N)))
+        return {f: a[:N.value] for f, a in arrs.items()}
+
+    def docs_tree_dev(self, n: int, d_gsa: int, d_glcp: int, d_doc_starts: int, ndocs: int, out_ptrs, cap: int,
+                      stream: int = 0) -> int:
+        """b200sa_docs_tree_dev; out_ptrs: eight device pointers in DOCS_TREE_FIELDS order.  Returns N."""
+        t = DocsTree(Tree(*out_ptrs[:6]), out_ptrs[6], out_ptrs[7])
+        N = ctypes.c_uint64(0)
+        self._check(lib().b200sa_docs_tree_dev(self._h, n, d_gsa, d_glcp, d_doc_starts or None, ndocs, ctypes.byref(t),
+                                               cap, ctypes.byref(N), stream))
+        return int(N.value)
+
+    def docs_tree_counts_dev(self, d_sa_lo, d_sa_hi, d_doc_count, num_nodes, d_start, d_end, nq, d_count,
+                             stream: int = 0):
+        self._check(lib().b200sa_docs_tree_counts_dev(self._h, d_sa_lo, d_sa_hi, d_doc_count, num_nodes, d_start,
+                                                      d_end, nq, d_count, stream))
 
     def lcp_sharded(self, d_text: int, n: int, d_sa: int, d_lcp: int, replicated: bool = False, stream: int = 0):
         self._check(lib().b200sa_lcp_sharded(self._h, d_text, n, d_sa, d_lcp, 1 if replicated else 0, stream))

@@ -27,6 +27,7 @@
 #include "shard.cuh"
 #include "tree.cuh"
 #include "docs.cuh"
+#include "docs_tree.cuh"
 #include "nccl_dyn.h"
 
 using namespace b200sa;
@@ -1504,14 +1505,18 @@ static int tree_bad(b200sa_ctx *c, uint32_t bits) {
     if (bits & TREE_BAD_LCP) m += " lcp[r] longer than suffix sa[r-1] or sa[r];";
     if (bits & TREE_BAD_PARENT) m += " a parent node is missing (lcp is not the LCP array of sa);";
     if (bits & TREE_BAD_FIRST) m += " a rank starts no node (lcp is not the LCP array of sa);";
+    if (bits & TREE_BAD_NODE) m += " the node of a document string is missing (glcp is not the LCP array of G);";
     c->last_error = m;
     return B200SA_ERR_BAD_ARG;
 }
 
 // n >= 1, device inputs and outputs (capacity >= 2n each).  Phases: tree_ansv, tree_emit, tree_sort,
-// tree_first, tree_nodes.
+// tree_first, tree_nodes.  len gives the suffix length of a rank (TextLen: one text; DocsLen: the
+// generalized tree, whose sorted keys and first[] b200sa_docs_tree reads afterwards in k64a/k64b and g0).
+extern "C++" {   // templates inside the C-ABI block
+template <class LenF>
 static int suffix_tree_core(b200sa_ctx *c, uint32_t n, const uint32_t *d_sa, const uint32_t *d_lcp, const TreeOut &o,
-                            uint64_t *num_nodes) {
+                            uint64_t *num_nodes, LenF len, uint64_t **keys_out = nullptr) {
     const uint64_t cap = 2 * (uint64_t)n;
     const int B = bit_length(n);                       // depth <= n and sa_lo < n both fit in B bits
     TRY(ensure(c, c->p0, (size_t)n * 4));
@@ -1532,8 +1537,8 @@ static int suffix_tree_core(b200sa_ctx *c, uint32_t n, const uint32_t *d_sa, con
     LAUNCH(c, k_tree_ansv, cdiv(n, BLK), L, (uint64_t)n, psv, nsv, rep);
     TRY(mark(c, "tree_emit"));
     CU_TRY(c, cudaMemsetAsync(words, 0, 8, c->stream));
-    TreeCount tin{d_sa, d_lcp, rep, n, words + 1};
-    TreeEmit tout{d_sa, d_lcp, psv, nsv, rep, n, B, ptr<uint64_t>(c->k64a), ptr<uint32_t>(c->v0)};
+    TreeCount<LenF> tin{len, d_sa, d_lcp, rep, n, words + 1};
+    TreeEmit<LenF> tout{len, d_sa, d_lcp, psv, nsv, rep, n, B, ptr<uint64_t>(c->k64a), ptr<uint32_t>(c->v0)};
     TRY((dev_scan<OpSum>(c, tin, tout, n, words)));
     TRY(read_words(c, words, 2));
     if (c->h_pin[1]) return tree_bad(c, c->h_pin[1]);
@@ -1544,8 +1549,14 @@ static int suffix_tree_core(b200sa_ctx *c, uint32_t n, const uint32_t *d_sa, con
     TRY(sort_pairs<uint64_t>(c, ptr<uint64_t>(c->k64a), ptr<uint32_t>(c->v0), ptr<uint64_t>(c->k64b),
                              ptr<uint32_t>(c->v1), N, 2 * B, &K, &V));
     TRY(mark(c, "tree_first"));
-    CU_TRY(c, cudaMemsetAsync(first, 0xff, ((size_t)n + 1) * 4, c->stream));
-    LAUNCH(c, k_tree_first, cdiv(N, BLK), K, N, B, n, first);
+    if (LenF::DOCS) {
+        CU_TRY(c, cudaMemsetAsync(first, 0, ((size_t)n + 1) * 4, c->stream));
+        LAUNCH(c, k_tree_last, cdiv(N, BLK), K, N, B, first);
+        TRY((dev_scan<OpMax>(c, InArray{first}, OutStoreExcl{first}, (uint64_t)n + 1, nullptr)));
+    } else {
+        CU_TRY(c, cudaMemsetAsync(first, 0xff, ((size_t)n + 1) * 4, c->stream));
+        LAUNCH(c, k_tree_first, cdiv(N, BLK), K, N, B, n, first);
+    }
     TRY(mark(c, "tree_nodes"));
     uint32_t grid_n = N > n + 1 ? N : n + 1;
     LAUNCH(c, k_tree_nodes, cdiv(grid_n, BLK), K, V, N, B, d_sa, d_lcp, psv, first, n, o, words + 1);
@@ -1554,8 +1565,10 @@ static int suffix_tree_core(b200sa_ctx *c, uint32_t n, const uint32_t *d_sa, con
     TRY(read_words(c, words + 1, 1));
     if (c->h_pin[0]) return tree_bad(c, c->h_pin[0]);
     *num_nodes = N;
+    if (keys_out) *keys_out = K;
     return B200SA_OK;
 }
+}  // extern "C++"
 
 static int tree_args(b200sa_ctx *c, uint64_t n, const void *sa, const void *lcp, const b200sa_tree *out,
                      uint64_t cap, uint64_t *num_nodes) {
@@ -1606,7 +1619,7 @@ int b200sa_suffix_tree_dev(b200sa_ctx *c, uint64_t n, const uint32_t *d_sa, cons
         return tree_exit(c, rc);
     }
     TreeOut o{out->parent, out->depth, out->sa_lo, out->sa_hi, out->label_start, out->subtree_end};
-    rc = suffix_tree_core(c, (uint32_t)n, d_sa, d_lcp, o, num_nodes);
+    rc = suffix_tree_core(c, (uint32_t)n, d_sa, d_lcp, o, num_nodes, TextLen{});
     return tree_exit(c, rc);
 }
 
@@ -1623,7 +1636,7 @@ static int suffix_tree_host(b200sa_ctx *c, uint64_t n, const uint32_t *sa, const
     for (int k = 0; k < 6; k++) dev[k] = ptr<uint32_t>(c->tree_out) + k * cap;
     TreeOut o{dev[0], dev[1], dev[2], dev[3], dev[4], dev[5]};
     uint64_t N = 0;
-    TRY(suffix_tree_core(c, (uint32_t)n, ptr<uint32_t>(c->sa), ptr<uint32_t>(c->lcp), o, &N));
+    TRY(suffix_tree_core(c, (uint32_t)n, ptr<uint32_t>(c->sa), ptr<uint32_t>(c->lcp), o, &N, TextLen{}));
     if (!c->marks.empty()) c->marks.pop_back();        // the copy-out replaces the core's "end"
     TRY(mark(c, "d2h"));
     uint32_t *host[6] = {out->parent, out->depth, out->sa_lo, out->sa_hi, out->label_start, out->subtree_end};
@@ -1874,6 +1887,199 @@ int b200sa_docs_positions_dev(b200sa_ctx *c, const uint8_t *d_text, uint64_t n, 
         CU_TRY(c, cudaGetLastError());
     }
     return end_call(c);
+}
+
+// ------------------------------------------------------------ generalized suffix tree with document counts (SURVEY 8f-7)
+static int docs_tree_args(b200sa_ctx *c, uint64_t n, const void *gsa, const void *glcp, const void *starts,
+                          uint32_t ndocs, const b200sa_docs_tree_out *out, uint64_t cap, uint64_t *num_nodes) {
+    if (!c || !out || !num_nodes) return B200SA_ERR_BAD_ARG;
+    TRY(tree_args(c, n, gsa, glcp, &out->tree, cap, num_nodes));
+    if (!out->term_end || !out->doc_count || (ndocs > 0 && !starts)) {
+        c->last_error = "null pointer";
+        return B200SA_ERR_BAD_ARG;
+    }
+    if (ndocs == 0 && n > 0) {
+        c->last_error = "doc_starts rejected: ndocs == 0 with n > 0;";
+        return B200SA_ERR_BAD_ARG;
+    }
+    return B200SA_OK;
+}
+
+extern "C++" {
+// The tree's document-sort key: the document of a rank.
+template <int OSI>
+static int dtree_sort(b200sa_ctx *c, const uint32_t *doc, uint32_t n, int bits, uint32_t **kout, uint32_t **vout) {
+    return sort_pairs_from<uint32_t, LoadArr<uint32_t>, LoadIndex, OSI>(
+        c, LoadArr<uint32_t>{doc}, LoadIndex{}, ptr<uint32_t>(c->p0), ptr<uint32_t>(c->p1), ptr<uint32_t>(c->v0),
+        ptr<uint32_t>(c->v1), n, bits, kout, vout);
+}
+}  // extern "C++"
+
+// n >= 1, ndocs >= 1, device inputs and outputs (capacity >= 2n each).  Phases: docs_check (when
+// check_starts), dtree_len, the tree's five, dtree_term, dtree_sort, dtree_pairs, dtree_count.
+static int docs_tree_core(b200sa_ctx *c, uint32_t n, const uint32_t *d_g, const uint32_t *d_glcp,
+                          const uint32_t *d_starts, uint32_t ndocs, bool check_starts, const b200sa_docs_tree_out *out,
+                          uint64_t *num_nodes) {
+    TRY(ensure(c, c->small, 4096));
+    uint32_t *words = ptr<uint32_t>(c->small);           // [0, 2) the tree's, [2] the check bits of the stages after it
+    if (check_starts) {
+        TRY(mark(c, "docs_check"));
+        CU_TRY(c, cudaMemsetAsync(words, 0, 8, c->stream));
+        LAUNCH(c, k_docs_check, cdiv(ndocs, BLK), d_starts, ndocs, n, words);
+        CU_TRY(c, cudaGetLastError());
+        TRY(read_words(c, words, 1));
+        if (c->h_pin[0]) return docs_bad(c, c->h_pin[0]);
+    }
+    // document and suffix length of every rank, then the tree with rule 3'
+    TRY(mark(c, "dtree_len"));
+    TRY(ensure(c, c->isa, (size_t)n * 4));
+    TRY(ensure(c, c->rank, (size_t)n * 4));
+    uint32_t *len = ptr<uint32_t>(c->isa), *doc = ptr<uint32_t>(c->rank);
+    LAUNCH(c, k_dtree_len, cdiv(n, BLK), d_g, n, d_starts, ndocs, len, doc);
+    const b200sa_tree &t = out->tree;
+    TreeOut o{t.parent, t.depth, t.sa_lo, t.sa_hi, t.label_start, t.subtree_end};
+    uint64_t N64 = 0, *K = nullptr;
+    TRY(suffix_tree_core(c, n, d_g, d_glcp, o, &N64, DocsLen{len}, &K));
+    if (!c->marks.empty()) c->marks.pop_back();          // dtree_term follows instead of the tree's "end"
+    const uint32_t N = (uint32_t)N64, *first = ptr<uint32_t>(c->g0);
+    const int B = bit_length(n);                         // as in suffix_tree_core
+
+    // terminals
+    TRY(mark(c, "dtree_term"));
+    AnsvLevels L;
+    TRY(ansv_levels(c, d_glcp, n, &L));
+    CU_TRY(c, cudaMemsetAsync(words + 2, 0, 4, c->stream));
+    CU_TRY(c, cudaMemcpyAsync(out->term_end, t.sa_lo, (size_t)N * 4, cudaMemcpyDeviceToDevice, c->stream));
+    LAUNCH(c, k_dtree_term, cdiv(n, BLK), L, len, n, K, first, N, B, out->term_end, words + 2);
+
+    // Hui's counts: ranks stably by document, one add per pair at its lowest common ancestor, one scan
+    TRY(mark(c, "dtree_sort"));
+    TRY(ensure(c, c->p0, (size_t)n * 4));
+    TRY(ensure(c, c->p1, (size_t)n * 4));
+    uint32_t *dk, *rk;
+    const int db = bit_length(ndocs - 1);
+    if (n >= (1u << 20)) TRY(dtree_sort<16>(c, doc, n, db, &dk, &rk));
+    else TRY(dtree_sort<ITEMS>(c, doc, n, db, &dk, &rk));
+    TRY(mark(c, "dtree_pairs"));
+    TRY(ensure(c, c->g1, ((size_t)N + 1) * 4));
+    uint32_t *pairs = ptr<uint32_t>(c->g1);
+    CU_TRY(c, cudaMemsetAsync(pairs, 0, ((size_t)N + 1) * 4, c->stream));
+    LAUNCH(c, k_dtree_pairs, cdiv(n, BLK), L, dk, rk, len, n, K, first, N, B, pairs, words + 2);
+    TRY(mark(c, "dtree_count"));
+    TRY((dev_scan<OpSum>(c, InArray{pairs}, OutStoreExcl{pairs}, (uint64_t)N + 1, nullptr)));
+    LAUNCH(c, k_dtree_count, cdiv(N, BLK), t.sa_lo, t.sa_hi, t.subtree_end, pairs, N, out->doc_count);
+    TRY(mark(c, "end"));
+    CU_TRY(c, cudaGetLastError());
+    TRY(read_words(c, words + 2, 1));
+    if (c->h_pin[0]) return tree_bad(c, c->h_pin[0]);
+    *num_nodes = N;
+    return B200SA_OK;
+}
+
+int b200sa_docs_tree_dev(b200sa_ctx *c, uint64_t n, const uint32_t *d_gsa, const uint32_t *d_glcp,
+                         const uint32_t *d_doc_starts, uint32_t ndocs, const b200sa_docs_tree_out *out, uint64_t cap,
+                         uint64_t *num_nodes, void *stream) {
+    TRY(docs_tree_args(c, n, d_gsa, d_glcp, d_doc_starts, ndocs, out, cap, num_nodes));
+    CU_TRY(c, cudaSetDevice(c->device));
+    begin_call(c, stream);
+    *num_nodes = 0;
+    if (n == 0) {
+        // doc_starts checked from host copies; the root alone, without terminals or documents
+        int rc = docs_check_dev_copy(c, 0, d_doc_starts, ndocs);
+        const uint32_t root[8] = {TREE_NONE, 0, 0, 0, 0, 1, 0, 0};
+        const b200sa_tree &t = out->tree;
+        uint32_t *dst[8] = {t.parent, t.depth, t.sa_lo, t.sa_hi, t.label_start, t.subtree_end, out->term_end,
+                            out->doc_count};
+        for (int k = 0; k < 8 && rc == B200SA_OK; k++) {
+            cudaError_t e = cudaMemcpyAsync(dst[k], &root[k], 4, cudaMemcpyHostToDevice, c->stream);
+            if (e != cudaSuccess) { c->last_error = cudaGetErrorString(e); rc = B200SA_ERR_CUDA; }
+        }
+        if (rc == B200SA_OK && cudaStreamSynchronize(c->stream) != cudaSuccess) rc = B200SA_ERR_CUDA;
+        if (rc == B200SA_OK) *num_nodes = 1;
+        return tree_exit(c, rc);
+    }
+    return tree_exit(c, docs_tree_core(c, (uint32_t)n, d_gsa, d_glcp, d_doc_starts, ndocs, true, out, num_nodes));
+}
+
+static int docs_tree_host(b200sa_ctx *c, uint32_t n, const uint32_t *gsa, const uint32_t *glcp, const uint32_t *starts,
+                          uint32_t ndocs, const b200sa_docs_tree_out *out, uint64_t *num_nodes) {
+    const uint64_t cap = 2 * (uint64_t)n;
+    TRY(ensure(c, c->sa, (size_t)n * 4));
+    TRY(ensure(c, c->lcp, (size_t)n * 4));
+    TRY(ensure(c, c->docs_starts, (size_t)ndocs * 4));
+    TRY(ensure(c, c->tree_out, cap * 4 * 8));
+    TRY(mark(c, "h2d"));
+    CU_TRY(c, cudaMemcpyAsync(c->sa.p, gsa, (size_t)n * 4, cudaMemcpyHostToDevice, c->stream));
+    CU_TRY(c, cudaMemcpyAsync(c->lcp.p, glcp, (size_t)n * 4, cudaMemcpyHostToDevice, c->stream));
+    CU_TRY(c, cudaMemcpyAsync(c->docs_starts.p, starts, (size_t)ndocs * 4, cudaMemcpyHostToDevice, c->stream));
+    uint32_t *dev[8];
+    for (int k = 0; k < 8; k++) dev[k] = ptr<uint32_t>(c->tree_out) + k * cap;
+    b200sa_docs_tree_out o{{dev[0], dev[1], dev[2], dev[3], dev[4], dev[5]}, dev[6], dev[7]};
+    uint64_t N = 0;
+    TRY(docs_tree_core(c, n, ptr<uint32_t>(c->sa), ptr<uint32_t>(c->lcp), ptr<uint32_t>(c->docs_starts), ndocs, false,
+                       &o, &N));
+    if (!c->marks.empty()) c->marks.pop_back();          // the copy-out replaces the core's "end"
+    TRY(mark(c, "d2h"));
+    const b200sa_tree &t = out->tree;
+    uint32_t *host[8] = {t.parent, t.depth, t.sa_lo, t.sa_hi, t.label_start, t.subtree_end, out->term_end,
+                         out->doc_count};
+    for (int k = 0; k < 8; k++)
+        CU_TRY(c, cudaMemcpyAsync(host[k], dev[k], N * 4, cudaMemcpyDeviceToHost, c->stream));
+    TRY(mark(c, "end"));
+    CU_TRY(c, cudaStreamSynchronize(c->stream));
+    *num_nodes = N;
+    return B200SA_OK;
+}
+
+int b200sa_docs_tree(b200sa_ctx *c, uint64_t n, const uint32_t *gsa, const uint32_t *glcp, const uint32_t *doc_starts,
+                     uint32_t ndocs, const b200sa_docs_tree_out *out, uint64_t cap, uint64_t *num_nodes) {
+    TRY(docs_tree_args(c, n, gsa, glcp, doc_starts, ndocs, out, cap, num_nodes));
+    TRY(docs_check_host(c, n, doc_starts, ndocs));
+    CU_TRY(c, cudaSetDevice(c->device));
+    begin_call(c, nullptr);
+    *num_nodes = 0;
+    if (n == 0) {
+        const b200sa_tree &t = out->tree;
+        t.parent[0] = TREE_NONE;
+        t.depth[0] = t.sa_lo[0] = t.sa_hi[0] = t.label_start[0] = 0;
+        t.subtree_end[0] = 1;
+        out->term_end[0] = out->doc_count[0] = 0;
+        *num_nodes = 1;
+        return end_call(c);
+    }
+    return tree_exit(c, docs_tree_host(c, (uint32_t)n, gsa, glcp, doc_starts, ndocs, out, num_nodes));
+}
+
+int b200sa_docs_tree_counts_dev(b200sa_ctx *c, const uint32_t *d_sa_lo, const uint32_t *d_sa_hi,
+                                const uint32_t *d_doc_count, uint64_t num_nodes, const uint32_t *d_start,
+                                const uint32_t *d_end, uint32_t nq, uint32_t *d_count, void *stream) {
+    if (!c) return B200SA_ERR_BAD_ARG;
+    if (nq > 0 && (!d_sa_lo || !d_sa_hi || !d_doc_count || !d_start || !d_end || !d_count)) {
+        c->last_error = "null pointer";
+        return B200SA_ERR_BAD_ARG;
+    }
+    if (nq > 0 && (num_nodes == 0 || num_nodes > 2 * B200SA_TREE_MAX_N)) {
+        c->last_error = "docs tree counts: num_nodes must be in [1, 2 * B200SA_TREE_MAX_N]";
+        return B200SA_ERR_BAD_ARG;
+    }
+    CU_TRY(c, cudaSetDevice(c->device));
+    begin_call(c, stream);
+    if (nq == 0) return end_call(c);
+    int rc = ensure(c, c->small, 4096);
+    uint32_t *flag = ptr<uint32_t>(c->small);
+    if (rc == B200SA_OK && cudaMemsetAsync(flag, 0, 4, c->stream) != cudaSuccess) rc = B200SA_ERR_CUDA;
+    if (rc == B200SA_OK) {
+        LAUNCH(c, k_dtree_counts, cdiv(nq, BLK), d_sa_lo, d_sa_hi, d_doc_count, (uint32_t)num_nodes, d_start, d_end, nq,
+               d_count, flag);
+        if (cudaGetLastError() != cudaSuccess) rc = B200SA_ERR_CUDA;
+    }
+    if (rc == B200SA_OK) rc = read_words(c, flag, 1);
+    if (rc == B200SA_OK && c->h_pin[0]) {
+        c->last_error = "docs tree counts: a range [start, end) is the range of no node";
+        rc = B200SA_ERR_BAD_ARG;
+    }
+    if (rc == B200SA_ERR_CUDA && c->last_error.empty()) c->last_error = "kernel launch failed";
+    return tree_exit(c, rc);
 }
 
 // ------------------------------------------------------------ multi-GPU: communicator + sharded LMS sort

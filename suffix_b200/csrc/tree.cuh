@@ -10,6 +10,8 @@
 //                  range [r, r+1), string depth n - sa[r]
 //   root           range [0, n), depth 0
 // Preorder (the reference's, lexicographic) is the ascending order of the keys (sa_lo, depth).
+// The kernels that use a suffix's length take it from a functor: n - sa[r] for one text (TextLen),
+// the length to the document's end for the generalized tree of docs_tree.cuh (DocsLen, rule 3').
 #pragma once
 #include "pipeline_kernels.cuh"
 
@@ -17,7 +19,8 @@ namespace b200sa {
 
 constexpr uint32_t TREE_NONE = 0xffffffffu;
 // bits of the check word (b200sa_suffix_tree_dev reports them through last_error)
-constexpr uint32_t TREE_BAD_SA = 1, TREE_BAD_LCP0 = 2, TREE_BAD_LCP = 4, TREE_BAD_PARENT = 8, TREE_BAD_FIRST = 16;
+constexpr uint32_t TREE_BAD_SA = 1, TREE_BAD_LCP0 = 2, TREE_BAD_LCP = 4, TREE_BAD_PARENT = 8, TREE_BAD_FIRST = 16,
+                   TREE_BAD_NODE = 32;   // b200sa_docs_tree: the node of a document string or of a pair is missing
 
 // psv of every rank (exactly k_ansv's), and for the representative boundaries (rule 2) their nsv.
 // rep[i] = 1 iff i is representative; the non-strict left search (pse) is only run where lcp[i] > 0.
@@ -33,33 +36,53 @@ __global__ void __launch_bounds__(BLK) k_tree_ansv(AnsvLevels L, uint64_t n, uin
     if (r) nsv[i] = (uint32_t)ansv_right(L, i, v, n);
 }
 
-__device__ __forceinline__ bool tree_merged(const uint32_t *sa, const uint32_t *lcp, uint32_t n, uint32_t r) {
-    return r + 1 < n && lcp[r + 1] == n - sa[r];
+// Length of the suffix of rank r (s = sa[r]): to the text's end for one text (SuffixTree), or to its
+// document's end, read from a per-rank array, for the generalized tree (docs_tree.cuh).
+// The scan functors derive from it, so the empty TextLen leaves their parameter layout as it was.
+struct TextLen {
+    static constexpr bool DOCS = false;
+    __device__ __forceinline__ uint32_t operator()(uint32_t, uint32_t s, uint32_t n) const { return n - s; }
+};
+struct DocsLen {
+    static constexpr bool DOCS = true;
+    const uint32_t *len;
+    __device__ __forceinline__ uint32_t operator()(uint32_t r, uint32_t, uint32_t) const { return len[r]; }
+};
+
+// Rule 3 (one text): suffix sa[r] is a proper prefix of sa[r+1].  Rule 3' (documents) also merges a
+// rank whose string equals the previous one's.
+template <class LenF>
+__device__ __forceinline__ bool tree_merged(const uint32_t *sa, const uint32_t *lcp, uint32_t n, uint32_t r,
+                                            const LenF &len) {
+    return (r + 1 < n && lcp[r + 1] == len(r, sa[r], n)) || (LenF::DOCS && r > 0 && lcp[r] == len(r, sa[r], n));
 }
 
 // Scan input: nodes emitted by rank r (its representative internal node, its leaf), plus the input
 // checks.  Every check runs before a value of sa or lcp is used to address memory (none is, before
 // the host has read the check word back).
-struct TreeCount {
+template <class LenF>
+struct TreeCount : LenF {
     const uint32_t *sa, *lcp;
     const uint8_t *rep;
     uint32_t n;
     uint32_t *flag;
+    __device__ __forceinline__ uint32_t len(uint32_t r, uint32_t s) const { return LenF::operator()(r, s, n); }
     __device__ uint32_t operator()(uint64_t i) const {
         uint32_t r = (uint32_t)i, s = sa[r], l = lcp[r], bad = 0;
         if (s >= n) bad |= TREE_BAD_SA;
-        else if (l > n - s) bad |= TREE_BAD_LCP;
+        else if (l > len(r, s)) bad |= TREE_BAD_LCP;
         if (r == 0 && l != 0) bad |= TREE_BAD_LCP0;
         if (r > 0) {
             uint32_t s1 = sa[r - 1];
-            if (s1 < n && l > n - s1) bad |= TREE_BAD_LCP;
+            if (s1 < n && l > len(r - 1, s1)) bad |= TREE_BAD_LCP;
         }
         if (bad) atomicOr(flag, bad);
-        return (uint32_t)rep[r] + (tree_merged(sa, lcp, n, r) ? 0u : 1u);
+        return (uint32_t)rep[r] + (tree_merged(sa, lcp, n, r, static_cast<const LenF &>(*this)) ? 0u : 1u);
     }
 };
 // Scan output: key (sa_lo << B | depth) and payload sa_hi of each node; the root goes last.
-struct TreeEmit {
+template <class LenF>
+struct TreeEmit : LenF {
     const uint32_t *sa, *lcp, *psv, *nsv;
     const uint8_t *rep;
     uint32_t n;
@@ -75,7 +98,7 @@ struct TreeEmit {
             o++;
         }
         if (v > isrep) {
-            key[o] = ((uint64_t)r << B) | (n - sa[r]);
+            key[o] = ((uint64_t)r << B) | LenF::operator()(r, sa[r], n);
             hi[o] = r + 1;
             o++;
         }
@@ -94,6 +117,34 @@ __global__ void __launch_bounds__(BLK) k_tree_first(const uint64_t *key, uint32_
     uint32_t l = (uint32_t)(key[j] >> B);
     if (j == 0 || (uint32_t)(key[j - 1] >> B) != l) first[l] = j;
     if (j == N - 1) first[n] = N;
+}
+
+// Finds the node (lo, d): *id = the lower bound of its key among the nodes that start at lo,
+// key[first[lo], first[lo + 1]); false (and *id untouched) if there is none.
+__device__ __forceinline__ bool tree_find(const uint64_t *key, const uint32_t *first, uint32_t N, int B, uint32_t n,
+                                          uint32_t lo, uint32_t d, uint32_t *id) {
+    uint32_t a = lo < n ? first[lo] : TREE_NONE, b = lo < n ? first[lo + 1] : TREE_NONE;
+    uint64_t want = ((uint64_t)lo << B) | d;
+    bool found = false;
+    if (a != TREE_NONE && b != TREE_NONE && a < b && b <= N) {
+        while (a < b) {                               // lower bound of want in key[a, b)
+            uint32_t m = a + (b - a) / 2;
+            if (key[m] < want) a = m + 1; else b = m;
+        }
+        found = a < N && key[a] == want;
+    }
+    if (found) *id = a;
+    return found;
+}
+
+// With documents a rank inside a run of equal strings starts no node, so first[l] is the smallest id
+// whose sa_lo >= l instead: the exclusive max-scan over l of last[l] = 1 + the largest id that starts
+// at l (0 if none), which this kernel writes into a zeroed array.
+__global__ void __launch_bounds__(BLK) k_tree_last(const uint64_t *key, uint32_t N, int B, uint32_t *last) {
+    uint32_t j = blockIdx.x * BLK + threadIdx.x;
+    if (j >= N) return;
+    uint32_t l = (uint32_t)(key[j] >> B);
+    if (j == N - 1 || (uint32_t)(key[j + 1] >> B) != l) last[l] = j + 1;
 }
 
 struct TreeOut {
@@ -120,18 +171,7 @@ __global__ void __launch_bounds__(BLK) k_tree_nodes(const uint64_t *key, const u
         par = 0;
         if (pd > 0) {
             uint32_t plo = lhi > llo ? lo : psv[lo];
-            uint32_t a = plo < n ? first[plo] : TREE_NONE, b = plo < n ? first[plo + 1] : TREE_NONE;
-            uint64_t want = ((uint64_t)plo << B) | pd;
-            bool found = false;
-            if (a != TREE_NONE && b != TREE_NONE && a < b && b <= N) {
-                while (a < b) {                       // lower bound of want in key[a, b)
-                    uint32_t m = a + (b - a) / 2;
-                    if (key[m] < want) a = m + 1; else b = m;
-                }
-                found = a < N && key[a] == want;
-            }
-            if (found) par = a;
-            else atomicOr(flag, TREE_BAD_PARENT);
+            if (!tree_find(key, first, N, B, n, plo, pd, &par)) atomicOr(flag, TREE_BAD_PARENT);
         }
         ls = sa[lo] + pd;
         if (hi < n) {

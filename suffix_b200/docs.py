@@ -165,15 +165,20 @@ class DocumentSuffixTable:
         """Per query the range [start, end) of table() whose document suffixes start with it
         (b200sa_docs_positions_dev): two u32 arrays.  The first call copies the concatenation,
         G and doc_starts to the device; they stay there for later calls."""
+        d_start, d_end = self._positions_dev(queries)
+        return d_start.cpu().numpy().view(np.uint32), d_end.cpu().numpy().view(np.uint32)
+
+    def _positions_dev(self, queries):
+        """positions_batch with the ranges left on the device: two int32 tensors of u32 values."""
         import torch
         qs = [_as_bytes(q) for q in queries]
         nq = len(qs)
+        dev = torch.device("cuda", self._device)
         if nq == 0:
-            return np.zeros(0, dtype=np.uint32), np.zeros(0, dtype=np.uint32)
+            return torch.zeros(0, dtype=torch.int32, device=dev), torch.zeros(0, dtype=torch.int32, device=dev)
         off = np.zeros(nq + 1, dtype=np.uint64)
         off[1:] = np.cumsum([len(q) for q in qs])
         blob = np.frombuffer(b"".join(qs) or b"\0", dtype=np.uint8)
-        dev = torch.device("cuda", self._device)
         n = len(self._text)
         d_t, d_g, d_s = self._device_arrays()
         d_q = torch.from_numpy(blob.copy()).to(dev)
@@ -185,7 +190,7 @@ class DocumentSuffixTable:
                 d_t.data_ptr(), n, d_g.data_ptr(), d_s.data_ptr(), len(self._starts), d_q.data_ptr(),
                 d_off.data_ptr(), nq, d_start.data_ptr(), d_end.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
         torch.cuda.synchronize(dev)
-        return d_start.cpu().numpy().view(np.uint32), d_end.cpu().numpy().view(np.uint32)
+        return d_start, d_end
 
     def __repr__(self):
         return "DocumentSuffixTable(docs=%d, n=%d)" % (len(self._starts), len(self._table))

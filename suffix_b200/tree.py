@@ -51,7 +51,7 @@ class SuffixTree:
         return self._text
 
     def root(self) -> "Node":
-        return Node(self, 0)
+        return self._node(self, 0)
 
     def label(self, node: "Node") -> bytes:
         """The path label into `node` (:97-100)."""
@@ -102,7 +102,7 @@ class Node:
 
     def parent(self):
         p = int(self.tree._parent[self.id])
-        return None if p == NONE else Node(self.tree, p)
+        return None if p == NONE else type(self)(self.tree, p)
 
     def children(self):
         """Children in byte order of their labels' first bytes (:108-111)."""
@@ -110,21 +110,21 @@ class Node:
         end = int(t._subtree_end[self.id])
         c = self.id + 1
         while c < end:
-            yield Node(t, c)
+            yield type(self)(t, c)
             c = int(t._subtree_end[c])
 
     def ancestors(self):
         """This node, its parent, ..., the root (:113-118)."""
         t, v = self.tree, self.id
         while v != NONE:
-            yield Node(t, v)
+            yield type(self)(t, v)
             v = int(t._parent[v])
 
     def preorder(self):
         """This node and its descendants in preorder, which is lexicographic (:120-125)."""
         t = self.tree
         for v in range(self.id, int(t._subtree_end[self.id])):
-            yield Node(t, v)
+            yield type(self)(t, v)
 
     def leaves(self):
         """Nodes of the preorder with len() > 0 and terminals; they may have children (:127-134, :357)."""
@@ -156,3 +156,6 @@ class Node:
             return [n]
         s = int(t._table[int(t._sa_lo[self.id])])
         return [s] if int(t._depth[self.id]) == n - s else []
+
+
+SuffixTree._node = Node          # the handle class of a tree's nodes (DocumentSuffixTree uses its own)

@@ -91,6 +91,11 @@ for k, docs in enumerate(doc_sets):
     s_, e_ = dt.positions_batch([b"ACG", b"TA", b"\x00", b"", b"GTAC"])
     assert all(int(a) <= int(b) for a, b in zip(s_, e_)), k
 del os.environ["B200SA_DOCS_SORT2"]
+from suffix_b200 import DocumentSuffixTree      # the generalized suffix tree and its document counts
+for k, docs in enumerate(doc_sets + [[b"ACGT"] * 2000 + [b""]]):
+    dtr = DocumentSuffixTree(docs)
+    assert dtr.root().doc_count() == sum(1 for d in docs if d), k
+    assert len(dtr.document_counts([b"ACG", b"TA", b"\x00", b"", b"GTAC"])) == 5, k
 print("sanitize workload ok")
 PY
 for tool in memcheck racecheck; do
