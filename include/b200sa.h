@@ -271,6 +271,42 @@ int b200sa_docs_tree_counts_dev(b200sa_ctx *ctx, const uint32_t *d_sa_lo, const 
                                 const uint32_t *d_doc_count, uint64_t num_nodes, const uint32_t *d_start,
                                 const uint32_t *d_end, uint32_t nq, uint32_t *d_count, void *stream);
 
+/* ---- document listing (SURVEY.md 8f-8) ----
+ * Documents D_0 .. D_{k-1}, their concatenation C (n bytes), doc_starts, G and doc(p) as for
+ * b200sa_docs_build.  Which documents contain a query, and how often, without the tree:
+ *   byd   (n x u32) the ranks 0..n-1 sorted stably by (doc(G[r]), r).  Every position of document d has
+ *         exactly one rank, so d's ranks are byd[doc_starts[d], doc_starts[d+1]) in increasing order.
+ *   prev  (n x u32) for rank r of document d: prev[r] = r' + 1, where r' is the previous rank of d in
+ *         byd, or 0 if r is d's first rank (the +1 keeps "none" below every threshold).
+ * For a range [s, e) of G (b200sa_docs_positions_dev):
+ *   listing  the ranks i in [s, e) with prev[i] <= s: the first rank of each document inside the range,
+ *            so exactly one entry per distinct document of G[s, e), in ascending i (the table order of
+ *            each document's first occurrence);
+ *   docs     entry i reports d = doc(G[i]);
+ *   tf       entry i optionally reports #{ranks of d in [s, e)}: the occurrences of the query in D_d
+ *            (overlapping ones count, none crosses a document end).
+ * b200sa_docs_list_index_dev writes byd and prev into caller buffers of n entries.  doc_starts is checked
+ * on the device (B200SA_ERR_BAD_ARG with a b200sa_last_error detail, as b200sa_docs_tree_dev);
+ * B200SA_ERR_TOO_LARGE above B200SA_MAX_N; n = 0 returns without launching.  Synchronises the stream
+ * only to read the check word back.  Phases: docs_check, dlist_len, dlist_sort, dlist_prev. */
+int b200sa_docs_list_index_dev(b200sa_ctx *ctx, uint64_t n, const uint32_t *d_gsa, const uint32_t *d_doc_starts,
+                               uint32_t ndocs, uint32_t *d_byd, uint32_t *d_prev, void *stream);
+/* Document listing of a batch of ranges d_start / d_end of G.  Always writes d_offsets (nq + 1 x u64,
+ * exclusive: query q's entries are [offsets[q], offsets[q+1])) and *total = offsets[nq].  Writes
+ * d_docs[offsets[q], offsets[q+1]) and, if d_tf is non-NULL, d_tf at the same places, only when
+ * total <= cap; otherwise it returns B200SA_OK with nothing written past the offsets, so that the caller
+ * can size the buffers and call again.  cap = 0 (d_docs may then be NULL) is the document-frequency
+ * query: offsets[q+1] - offsets[q] is the number of documents that contain query q.  byd and prev must
+ * be what b200sa_docs_list_index_dev wrote for the same G and doc_starts; they are not verified.  A range
+ * with start > end or end > n returns B200SA_ERR_BAD_ARG (checked on the device).  Block minima over
+ * prev are rebuilt on every call (one read of 4n bytes); device workspace besides them is 12 bytes per
+ * chunk of 1024 ranks of every range plus 8 per query.  Synchronises the stream (it reads the chunk
+ * count and the total back).  Phases: dlist_levels, dlist_count, dlist_scan, dlist_emit. */
+int b200sa_docs_list_dev(b200sa_ctx *ctx, uint64_t n, const uint32_t *d_gsa, const uint32_t *d_doc_starts,
+                         uint32_t ndocs, const uint32_t *d_byd, const uint32_t *d_prev, const uint32_t *d_start,
+                         const uint32_t *d_end, uint32_t nq, uint64_t *d_offsets, uint32_t *d_docs, uint32_t *d_tf,
+                         uint64_t cap, uint64_t *total, void *stream);
+
 /* ---- multi-GPU: communicator + sharded LMS-suffix sort (SURVEY.md 8e, config 5) ----
  * One process (or thread) and one context per GPU.  NCCL is resolved at run time
  * (the copy already loaded in the process, else libnccl.so.2); the single-GPU entry

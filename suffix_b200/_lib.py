@@ -86,6 +86,9 @@ def lib():
         "b200sa_docs_tree_dev": ([vp, u64, vp, vp, vp, u32, ctypes.POINTER(DocsTree), u64, ctypes.POINTER(u64), vp], ci),
         "b200sa_docs_tree": ([vp, u64, vp, vp, vp, u32, ctypes.POINTER(DocsTree), u64, ctypes.POINTER(u64)], ci),
         "b200sa_docs_tree_counts_dev": ([vp, vp, vp, vp, u64, vp, vp, u32, vp, vp], ci),
+        "b200sa_docs_list_index_dev": ([vp, u64, vp, vp, u32, vp, vp, vp], ci),
+        "b200sa_docs_list_dev": ([vp, u64, vp, vp, u32, vp, vp, vp, vp, u32, vp, vp, vp, u64, ctypes.POINTER(u64), vp],
+                                 ci),
         "b200sa_last_stats": ([vp, ctypes.POINTER(Stats)], ci),
         "b200sa_set_timing": ([vp, ci], ci),
         "b200sa_last_phase_times": ([vp, ctypes.POINTER(ctypes.c_char_p), ctypes.POINTER(ctypes.c_float), ci], ci),
@@ -288,6 +291,20 @@ class Context:
                              stream: int = 0):
         self._check(lib().b200sa_docs_tree_counts_dev(self._h, d_sa_lo, d_sa_hi, d_doc_count, num_nodes, d_start,
                                                       d_end, nq, d_count, stream))
+
+    def docs_list_index_dev(self, n, d_gsa, d_doc_starts, ndocs, d_byd, d_prev, stream: int = 0):
+        """b200sa_docs_list_index_dev: byd and prev (n u32 each) of G for document listing."""
+        self._check(lib().b200sa_docs_list_index_dev(self._h, n, d_gsa, d_doc_starts or None, ndocs, d_byd, d_prev,
+                                                     stream))
+
+    def docs_list_dev(self, n, d_gsa, d_doc_starts, ndocs, d_byd, d_prev, d_start, d_end, nq, d_offsets, d_docs,
+                      d_tf, cap, stream: int = 0) -> int:
+        """b200sa_docs_list_dev: writes the offsets, and docs / tf when the listing fits in cap.  Returns the total."""
+        total = ctypes.c_uint64(0)
+        self._check(lib().b200sa_docs_list_dev(self._h, n, d_gsa, d_doc_starts or None, ndocs, d_byd, d_prev, d_start,
+                                               d_end, nq, d_offsets, d_docs or None, d_tf or None, cap,
+                                               ctypes.byref(total), stream))
+        return int(total.value)
 
     def lcp_sharded(self, d_text: int, n: int, d_sa: int, d_lcp: int, replicated: bool = False, stream: int = 0):
         self._check(lib().b200sa_lcp_sharded(self._h, d_text, n, d_sa, d_lcp, 1 if replicated else 0, stream))

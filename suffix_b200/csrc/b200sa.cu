@@ -28,6 +28,7 @@
 #include "tree.cuh"
 #include "docs.cuh"
 #include "docs_tree.cuh"
+#include "docs_list.cuh"
 #include "nccl_dyn.h"
 
 using namespace b200sa;
@@ -2080,6 +2081,135 @@ int b200sa_docs_tree_counts_dev(b200sa_ctx *c, const uint32_t *d_sa_lo, const ui
     }
     if (rc == B200SA_ERR_CUDA && c->last_error.empty()) c->last_error = "kernel launch failed";
     return tree_exit(c, rc);
+}
+
+// ------------------------------------------------------------ document listing (SURVEY 8f-8)
+// n >= 1, ndocs >= 1.  Phases: docs_check, dlist_len, dlist_sort, dlist_prev.
+static int docs_list_index_core(b200sa_ctx *c, uint32_t n, const uint32_t *d_g, const uint32_t *d_starts,
+                                uint32_t ndocs, uint32_t *d_byd, uint32_t *d_prev) {
+    TRY(ensure(c, c->small, 4096));
+    uint32_t *words = ptr<uint32_t>(c->small);
+    TRY(mark(c, "docs_check"));
+    CU_TRY(c, cudaMemsetAsync(words, 0, 8, c->stream));
+    LAUNCH(c, k_docs_check, cdiv(ndocs, BLK), d_starts, ndocs, n, words);
+    CU_TRY(c, cudaGetLastError());
+    TRY(read_words(c, words, 1));
+    if (c->h_pin[0]) return docs_bad(c, c->h_pin[0]);
+    TRY(mark(c, "dlist_len"));                          // the document of every rank (its length is not used)
+    TRY(ensure(c, c->isa, (size_t)n * 4));
+    TRY(ensure(c, c->rank, (size_t)n * 4));
+    uint32_t *len = ptr<uint32_t>(c->isa), *doc = ptr<uint32_t>(c->rank);
+    LAUNCH(c, k_dtree_len, cdiv(n, BLK), d_g, n, d_starts, ndocs, len, doc);
+    TRY(mark(c, "dlist_sort"));
+    TRY(ensure(c, c->p0, (size_t)n * 4));
+    TRY(ensure(c, c->p1, (size_t)n * 4));
+    TRY(ensure(c, c->v0, (size_t)n * 4));
+    TRY(ensure(c, c->v1, (size_t)n * 4));
+    uint32_t *dk, *rk;
+    const int db = bit_length(ndocs - 1);
+    if (n >= (1u << 20)) TRY(dtree_sort<16>(c, doc, n, db, &dk, &rk));
+    else TRY(dtree_sort<ITEMS>(c, doc, n, db, &dk, &rk));
+    TRY(mark(c, "dlist_prev"));
+    LAUNCH(c, k_dlist_prev, cdiv(n, BLK), dk, rk, n, d_byd, d_prev);
+    TRY(mark(c, "end"));
+    CU_TRY(c, cudaGetLastError());
+    return B200SA_OK;
+}
+
+int b200sa_docs_list_index_dev(b200sa_ctx *c, uint64_t n, const uint32_t *d_gsa, const uint32_t *d_doc_starts,
+                               uint32_t ndocs, uint32_t *d_byd, uint32_t *d_prev, void *stream) {
+    if (!c) return B200SA_ERR_BAD_ARG;
+    if ((n > 0 && (!d_gsa || !d_byd || !d_prev)) || (ndocs > 0 && !d_doc_starts)) {
+        c->last_error = "null pointer";
+        return B200SA_ERR_BAD_ARG;
+    }
+    if (ndocs == 0 && n > 0) {
+        c->last_error = "doc_starts rejected: ndocs == 0 with n > 0;";
+        return B200SA_ERR_BAD_ARG;
+    }
+    if (n > B200SA_MAX_N) return B200SA_ERR_TOO_LARGE;
+    CU_TRY(c, cudaSetDevice(c->device));
+    begin_call(c, stream);
+    if (n == 0) return tree_exit(c, docs_check_dev_copy(c, 0, d_doc_starts, ndocs));
+    return tree_exit(c, docs_list_index_core(c, (uint32_t)n, d_gsa, d_doc_starts, ndocs, d_byd, d_prev));
+}
+
+// nq >= 1.  Phases: dlist_levels, dlist_count, dlist_scan, dlist_emit (when the listing fits in cap).
+static int docs_list_core(b200sa_ctx *c, uint32_t n, const uint32_t *d_g, const uint32_t *d_starts, uint32_t ndocs,
+                          const uint32_t *d_byd, const uint32_t *d_prev, const uint32_t *d_start,
+                          const uint32_t *d_end, uint32_t nq, uint64_t *d_offsets, uint32_t *d_docs, uint32_t *d_tf,
+                          uint64_t cap, uint64_t *total) {
+    typedef unsigned long long u64;
+    TRY(ensure(c, c->small, 4096));
+    uint32_t *words = ptr<uint32_t>(c->small);           // [0] check bits, [2, 4) items, [4, 6) total
+    u64 *d_items = reinterpret_cast<u64 *>(words + 2), *d_total = reinterpret_cast<u64 *>(words + 4);
+    TRY(mark(c, "dlist_levels"));
+    DListArgs A;
+    TRY(ansv_levels(c, d_prev, n, &A.L));
+    TRY(mark(c, "dlist_count"));
+    CU_TRY(c, cudaMemsetAsync(words, 0, 24, c->stream));
+    TRY(ensure(c, c->k64a, ((size_t)nq + 1) * 8));
+    u64 *item_start = ptr<u64>(c->k64a);
+    TRY((dev_scan<OpSum64>(c, DListChunks{d_start, d_end, nq, n, words}, OutStoreExcl64{item_start}, (uint64_t)nq + 1,
+                           d_items)));
+    TRY(read_words(c, words, 4));
+    if (c->h_pin[0] & DLIST_BAD_RANGE) {
+        c->last_error = "docs list: a range [start, end) has start > end or end > n";
+        return B200SA_ERR_BAD_ARG;
+    }
+    const uint64_t items = c->h_pin[2] | ((uint64_t)c->h_pin[3] << 32);
+    if (items > (uint64_t)0x7fffffff * NWARP) {
+        c->last_error = "docs list: more than 2^31 * 8 chunks of 1024 ranks in one batch";
+        return B200SA_ERR_TOO_LARGE;
+    }
+    A.qs = d_start; A.qe = d_end; A.item_start = item_start; A.nq = nq; A.items = items;
+    TRY(ensure(c, c->p0, (size_t)items * 4));
+    TRY(ensure(c, c->k64b, ((size_t)items + 1) * 8));
+    uint32_t *cnt = ptr<uint32_t>(c->p0);
+    u64 *item_off = ptr<u64>(c->k64b);
+    const uint32_t grid = cdiv(items, NWARP);
+    if (items) LAUNCH(c, k_dlist<false>, grid, A, cnt, (const u64 *)nullptr, d_g, d_starts, ndocs, n, d_byd,
+                      (uint32_t *)nullptr, (uint32_t *)nullptr);
+    TRY(mark(c, "dlist_scan"));
+    TRY((dev_scan<OpSum64>(c, InCount64{cnt, items}, OutStoreExcl64{item_off}, items + 1, d_total)));
+    LAUNCH(c, k_dlist_qoff, cdiv((uint64_t)nq + 1, BLK), item_start, item_off, nq, reinterpret_cast<u64 *>(d_offsets));
+    TRY(read_words(c, words + 4, 2));
+    *total = c->h_pin[0] | ((uint64_t)c->h_pin[1] << 32);
+    if (*total > 0 && *total <= cap) {
+        TRY(mark(c, "dlist_emit"));
+        LAUNCH(c, k_dlist<true>, grid, A, cnt, item_off, d_g, d_starts, ndocs, n, d_byd, d_docs, d_tf);
+    }
+    TRY(mark(c, "end"));
+    CU_TRY(c, cudaGetLastError());
+    CU_TRY(c, cudaStreamSynchronize(c->stream));
+    return B200SA_OK;
+}
+
+int b200sa_docs_list_dev(b200sa_ctx *c, uint64_t n, const uint32_t *d_gsa, const uint32_t *d_doc_starts,
+                         uint32_t ndocs, const uint32_t *d_byd, const uint32_t *d_prev, const uint32_t *d_start,
+                         const uint32_t *d_end, uint32_t nq, uint64_t *d_offsets, uint32_t *d_docs, uint32_t *d_tf,
+                         uint64_t cap, uint64_t *total, void *stream) {
+    if (!c) return B200SA_ERR_BAD_ARG;
+    if (!total || !d_offsets || (nq > 0 && (!d_start || !d_end)) || (cap > 0 && !d_docs) ||
+        (n > 0 && (!d_gsa || !d_doc_starts || !d_byd || !d_prev))) {
+        c->last_error = "null pointer";
+        return B200SA_ERR_BAD_ARG;
+    }
+    if (ndocs == 0 && n > 0) {
+        c->last_error = "doc_starts rejected: ndocs == 0 with n > 0;";
+        return B200SA_ERR_BAD_ARG;
+    }
+    if (n > B200SA_MAX_N) return B200SA_ERR_TOO_LARGE;
+    CU_TRY(c, cudaSetDevice(c->device));
+    begin_call(c, stream);
+    *total = 0;
+    if (nq == 0) {
+        CU_TRY(c, cudaMemsetAsync(d_offsets, 0, 8, c->stream));
+        CU_TRY(c, cudaStreamSynchronize(c->stream));
+        return end_call(c);
+    }
+    return tree_exit(c, docs_list_core(c, (uint32_t)n, d_gsa, d_doc_starts, ndocs, d_byd, d_prev, d_start, d_end, nq,
+                                       d_offsets, d_docs, d_tf, cap, total));
 }
 
 // ------------------------------------------------------------ multi-GPU: communicator + sharded LMS sort

@@ -50,6 +50,11 @@ struct OpSum {
     __device__ __forceinline__ static uint32_t id() { return 0u; }
     __device__ __forceinline__ static uint32_t op(uint32_t a, uint32_t b) { return a + b; }
 };
+struct OpSum64 {                    // sums that may pass 2^32 (document listing totals)
+    using T = unsigned long long;
+    __device__ __forceinline__ static T id() { return 0ull; }
+    __device__ __forceinline__ static T op(T a, T b) { return a + b; }
+};
 struct OpMax {
     using T = uint32_t;
     __device__ __forceinline__ static uint32_t id() { return 0u; }

@@ -34,6 +34,7 @@ class DocumentSuffixTable:
         self._starts = np.asarray(starts, dtype=np.uint32)
         self._ends = np.append(self._starts[1:], np.uint32(len(self._text))).astype(np.uint32) if docs else self._starts
         self._dev = None
+        self._dlist = None
         t = np.frombuffer(self._text, dtype=np.uint8)
         with _lock:                           # default context is not thread-safe
             self._table, self._lcp = _lib.default_context(device).docs_build(t, self._starts, with_lcp=True)
@@ -191,6 +192,92 @@ class DocumentSuffixTable:
                 d_off.data_ptr(), nq, d_start.data_ptr(), d_end.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
         torch.cuda.synchronize(dev)
         return d_start, d_end
+
+    # ---- document listing
+    def _list_arrays(self):
+        """byd and prev of b200sa_docs_list_index_dev (two int32 tensors of u32 values), built on the device
+        on first use and kept while the table lives: 8 bytes per text byte of device memory."""
+        if self._dlist is None:
+            import torch
+            d_t, d_g, d_s = self._device_arrays()
+            dev = d_g.device
+            n = len(self._table)
+            byd = torch.empty(max(n, 1), dtype=torch.int32, device=dev)
+            prev = torch.empty(max(n, 1), dtype=torch.int32, device=dev)
+            with _lock:
+                if self._dlist is None:
+                    _lib.default_context(self._device).docs_list_index_dev(
+                        n, d_g.data_ptr(), d_s.data_ptr(), len(self._starts), byd.data_ptr(), prev.data_ptr(),
+                        torch.cuda.current_stream(dev).cuda_stream)
+                    torch.cuda.synchronize(dev)
+                    self._dlist = (byd, prev)
+        return self._dlist
+
+    def _list_dev(self, queries, cap_guess, with_tf=True):
+        """b200sa_docs_list_dev over the ranges of positions_batch: (offsets, docs, tf) as device tensors
+        (u64 offsets as int64, u32 entries as int32, tf None without with_tf).  cap_guess = 0 asks for the
+        offsets alone; otherwise the buffers hold cap_guess entries and a larger listing is fetched by a
+        second call sized to it."""
+        import torch
+        d_start, d_end = self._positions_dev(queries)
+        nq = len(d_start)
+        dev = d_start.device
+        d_off = torch.zeros(nq + 1, dtype=torch.int64, device=dev)
+        if nq == 0:
+            e = torch.zeros(0, dtype=torch.int32, device=dev)
+            return d_off, e, e if with_tf else None
+        byd, prev = self._list_arrays()
+        _, d_g, d_s = self._device_arrays()
+        n = len(self._table)
+
+        def call(cap):
+            docs = torch.empty(max(cap, 1), dtype=torch.int32, device=dev)
+            tf = torch.empty(max(cap, 1), dtype=torch.int32, device=dev) if with_tf else None
+            with _lock:
+                total = _lib.default_context(self._device).docs_list_dev(
+                    n, d_g.data_ptr(), d_s.data_ptr(), len(self._starts), byd.data_ptr(), prev.data_ptr(),
+                    d_start.data_ptr(), d_end.data_ptr(), nq, d_off.data_ptr(), docs.data_ptr() if cap else 0,
+                    tf.data_ptr() if cap and with_tf else 0, cap, torch.cuda.current_stream(dev).cuda_stream)
+            return total, docs, tf
+
+        total, docs, tf = call(cap_guess)
+        if cap_guess and total > cap_guess:
+            total, docs, tf = call(total)
+        return d_off, docs[:total] if cap_guess else docs[:0], (tf[:total] if cap_guess else tf[:0]) if with_tf else None
+
+    def documents_batch(self, queries, *, _cap_guess=None):
+        """Per query the documents that contain it and its number of occurrences in each (overlapping
+        occurrences count; a match never crosses a document end): (offsets u64[nq + 1], docs u32[],
+        counts u32[]), query q's rows at [offsets[q], offsets[q+1]), sorted by document.  The listing runs
+        on the device (b200sa_docs_list_dev, Muthukrishnan's array over the ranges of positions_batch); its
+        index, built on the first call and kept, holds 8 bytes per text byte of device memory.  b"" lists
+        nothing."""
+        import torch
+        qs = list(queries)
+        if _cap_guess is None:
+            _cap_guess = max(1, min(1 << 24, 64 * len(qs)))
+        d_off, docs, tf = self._list_dev(qs, _cap_guess)
+        nq = len(qs)
+        if len(docs):
+            # rank order -> document order per query: one sort of (query, document) keys
+            q = torch.repeat_interleave(torch.arange(nq, device=docs.device, dtype=torch.int64), d_off.diff())
+            key = (q << 32) | (docs.to(torch.int64) & 0xFFFFFFFF)
+            order = torch.argsort(key)
+            docs, tf = docs[order], tf[order]
+        torch.cuda.synchronize(docs.device)
+        return (d_off.cpu().numpy().view(np.uint64), docs.cpu().numpy().view(np.uint32),
+                tf.cpu().numpy().view(np.uint32))
+
+    def documents(self, query) -> np.ndarray:
+        """(document, count) rows of the documents that contain `query`, by ascending document: a batch of one."""
+        _, docs, tf = self.documents_batch([query])
+        return np.stack([docs, tf], axis=1)
+
+    def document_frequencies(self, queries) -> np.ndarray:
+        """For each query, the number of documents that contain it (0 for b""): the listing's counts alone
+        (b200sa_docs_list_dev with cap = 0), without building the tree of DocumentSuffixTree."""
+        d_off, _, _ = self._list_dev(list(queries), 0, with_tf=False)
+        return d_off.diff().cpu().numpy().astype(np.uint32)
 
     def __repr__(self):
         return "DocumentSuffixTable(docs=%d, n=%d)" % (len(self._starts), len(self._table))

@@ -96,6 +96,14 @@ for k, docs in enumerate(doc_sets + [[b"ACGT"] * 2000 + [b""]]):
     dtr = DocumentSuffixTree(docs)
     assert dtr.root().doc_count() == sum(1 for d in docs if d), k
     assert len(dtr.document_counts([b"ACG", b"TA", b"\x00", b"", b"GTAC"])) == 5, k
+for k, docs in enumerate(doc_sets + [[b"ACGT"] * 2000 + [b""]]):   # document listing: index, listing, tf on / off
+    dl = DocumentSuffixTable(docs)
+    qs = [b"ACG", b"TA", b"\x00", b"", b"GTAC", b"A"]
+    off, dd, tf = dl.documents_batch(qs, _cap_guess=1)             # cap too small, then sufficient
+    assert np.array_equal(dl.documents_batch(qs)[1], dd), k
+    assert np.array_equal(dl.document_frequencies(qs), np.diff(off.astype(np.int64))), k
+    d_off, d_docs, _ = dl._list_dev(qs, max(1, int(off[-1])), with_tf=False)
+    assert int(d_off[-1]) == int(off[-1]), k
 print("sanitize workload ok")
 PY
 for tool in memcheck racecheck; do
