@@ -307,6 +307,31 @@ int b200sa_docs_list_dev(b200sa_ctx *ctx, uint64_t n, const uint32_t *d_gsa, con
                          const uint32_t *d_end, uint32_t nq, uint64_t *d_offsets, uint32_t *d_docs, uint32_t *d_tf,
                          uint64_t cap, uint64_t *total, void *stream);
 
+/* ---- top-k document retrieval (SURVEY.md 8f-9) ----
+ * For a range [s, e) of G the listing above gives one entry (d, tf) per distinct document.  Then
+ *   key(d, tf)   orders entries by tf descending, then d ascending (((u64)tf << 32) | (0xFFFFFFFF - d),
+ *                largest first); documents are distinct within a query, so the order is total;
+ *   top_k(s, e)  the min(k, df) entries with the largest keys, in key order;
+ * an empty range (s = e: b"" or an absent query) has no entries.
+ * b200sa_docs_topk_dev writes d_count[q] = min(k, df(q)) and, for j < d_count[q], d_docs[q*k + j] and
+ * d_tf[q*k + j]: query q's top-k in key order.  Slots j >= d_count[q] are not written.  Arguments as for
+ * b200sa_docs_list_dev (byd and prev are not verified; a range with start > end or end > n returns
+ * B200SA_ERR_BAD_ARG, checked on the device); k = 0 or k > B200SA_TOPK_MAX returns B200SA_ERR_BAD_ARG
+ * (one block sorts the survivors of a query in shared memory; for larger k list with
+ * b200sa_docs_list_dev); nq = 0 returns without launching; n = 0 gives all counts 0.
+ * The listing is materialised in rounds: runs of consecutive queries whose entries fit
+ * B200SA_TOPK_ROUND_ENTRIES (a larger query, at most ndocs entries, is a round of its own); more than
+ * one round reads the per-query offsets back.  Device workspace: the listing's (block minima, 12 bytes per
+ * chunk of 1024 ranks of every range) plus 20 bytes per query and 16 bytes per entry of the largest round;
+ * with more than one round, 8 more per query and per chunk of that round.  Synchronises the stream.
+ * Phases: dlist_levels, dlist_count, dlist_scan, then per round topk_emit, topk_select. */
+#define B200SA_TOPK_MAX 1024
+#define B200SA_TOPK_ROUND_ENTRIES (1ull << 26)
+int b200sa_docs_topk_dev(b200sa_ctx *ctx, uint64_t n, const uint32_t *d_gsa, const uint32_t *d_doc_starts,
+                         uint32_t ndocs, const uint32_t *d_byd, const uint32_t *d_prev, const uint32_t *d_start,
+                         const uint32_t *d_end, uint32_t nq, uint32_t k, uint32_t *d_count, uint32_t *d_docs,
+                         uint32_t *d_tf, void *stream);
+
 /* ---- multi-GPU: communicator + sharded LMS-suffix sort (SURVEY.md 8e, config 5) ----
  * One process (or thread) and one context per GPU.  NCCL is resolved at run time
  * (the copy already loaded in the process, else libnccl.so.2); the single-GPU entry

@@ -89,6 +89,7 @@ def lib():
         "b200sa_docs_list_index_dev": ([vp, u64, vp, vp, u32, vp, vp, vp], ci),
         "b200sa_docs_list_dev": ([vp, u64, vp, vp, u32, vp, vp, vp, vp, u32, vp, vp, vp, u64, ctypes.POINTER(u64), vp],
                                  ci),
+        "b200sa_docs_topk_dev": ([vp, u64, vp, vp, u32, vp, vp, vp, vp, u32, u32, vp, vp, vp, vp], ci),
         "b200sa_last_stats": ([vp, ctypes.POINTER(Stats)], ci),
         "b200sa_set_timing": ([vp, ci], ci),
         "b200sa_last_phase_times": ([vp, ctypes.POINTER(ctypes.c_char_p), ctypes.POINTER(ctypes.c_float), ci], ci),
@@ -305,6 +306,12 @@ class Context:
                                                d_end, nq, d_offsets, d_docs or None, d_tf or None, cap,
                                                ctypes.byref(total), stream))
         return int(total.value)
+
+    def docs_topk_dev(self, n, d_gsa, d_doc_starts, ndocs, d_byd, d_prev, d_start, d_end, nq, k, d_count, d_docs, d_tf,
+                      stream: int = 0):
+        """b200sa_docs_topk_dev: count[q] = min(k, df(q)); docs / tf[q*k + j] for j < count[q], best first."""
+        self._check(lib().b200sa_docs_topk_dev(self._h, n, d_gsa, d_doc_starts or None, ndocs, d_byd, d_prev, d_start,
+                                               d_end, nq, k, d_count, d_docs, d_tf, stream))
 
     def lcp_sharded(self, d_text: int, n: int, d_sa: int, d_lcp: int, replicated: bool = False, stream: int = 0):
         self._check(lib().b200sa_lcp_sharded(self._h, d_text, n, d_sa, d_lcp, 1 if replicated else 0, stream))

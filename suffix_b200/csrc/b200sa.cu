@@ -11,6 +11,7 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <algorithm>
 #include <new>
 #include <string>
 #include <vector>
@@ -29,6 +30,7 @@
 #include "docs.cuh"
 #include "docs_tree.cuh"
 #include "docs_list.cuh"
+#include "docs_topk.cuh"
 #include "nccl_dyn.h"
 
 using namespace b200sa;
@@ -2134,11 +2136,13 @@ int b200sa_docs_list_index_dev(b200sa_ctx *c, uint64_t n, const uint32_t *d_gsa,
     return tree_exit(c, docs_list_index_core(c, (uint32_t)n, d_gsa, d_doc_starts, ndocs, d_byd, d_prev));
 }
 
-// nq >= 1.  Phases: dlist_levels, dlist_count, dlist_scan, dlist_emit (when the listing fits in cap).
-static int docs_list_core(b200sa_ctx *c, uint32_t n, const uint32_t *d_g, const uint32_t *d_starts, uint32_t ndocs,
-                          const uint32_t *d_byd, const uint32_t *d_prev, const uint32_t *d_start,
-                          const uint32_t *d_end, uint32_t nq, uint64_t *d_offsets, uint32_t *d_docs, uint32_t *d_tf,
-                          uint64_t cap, uint64_t *total) {
+// The listing's front half, shared by the listing and top-k: nq >= 1.  Writes the offsets (nq + 1) and
+// *total, and leaves in *A and *item_off (c->k64a, c->k64b) what k_dlist<true> needs to emit.  Phases:
+// dlist_levels, dlist_count, dlist_scan.
+static int docs_list_front(b200sa_ctx *c, uint32_t n, const uint32_t *d_g, const uint32_t *d_starts, uint32_t ndocs,
+                           const uint32_t *d_byd, const uint32_t *d_prev, const uint32_t *d_start,
+                           const uint32_t *d_end, uint32_t nq, uint64_t *d_offsets, DListArgs *Aout,
+                           unsigned long long **item_off_out, uint64_t *total) {
     typedef unsigned long long u64;
     TRY(ensure(c, c->small, 4096));
     uint32_t *words = ptr<uint32_t>(c->small);           // [0] check bits, [2, 4) items, [4, 6) total
@@ -2175,9 +2179,24 @@ static int docs_list_core(b200sa_ctx *c, uint32_t n, const uint32_t *d_g, const 
     LAUNCH(c, k_dlist_qoff, cdiv((uint64_t)nq + 1, BLK), item_start, item_off, nq, reinterpret_cast<u64 *>(d_offsets));
     TRY(read_words(c, words + 4, 2));
     *total = c->h_pin[0] | ((uint64_t)c->h_pin[1] << 32);
+    *Aout = A;
+    *item_off_out = item_off;
+    return B200SA_OK;
+}
+
+// nq >= 1.  Phases: dlist_levels, dlist_count, dlist_scan, dlist_emit (when the listing fits in cap).
+static int docs_list_core(b200sa_ctx *c, uint32_t n, const uint32_t *d_g, const uint32_t *d_starts, uint32_t ndocs,
+                          const uint32_t *d_byd, const uint32_t *d_prev, const uint32_t *d_start,
+                          const uint32_t *d_end, uint32_t nq, uint64_t *d_offsets, uint32_t *d_docs, uint32_t *d_tf,
+                          uint64_t cap, uint64_t *total) {
+    typedef unsigned long long u64;
+    DListArgs A;
+    u64 *item_off;
+    TRY(docs_list_front(c, n, d_g, d_starts, ndocs, d_byd, d_prev, d_start, d_end, nq, d_offsets, &A, &item_off, total));
     if (*total > 0 && *total <= cap) {
         TRY(mark(c, "dlist_emit"));
-        LAUNCH(c, k_dlist<true>, grid, A, cnt, item_off, d_g, d_starts, ndocs, n, d_byd, d_docs, d_tf);
+        LAUNCH(c, k_dlist<true>, cdiv(A.items, NWARP), A, ptr<uint32_t>(c->p0), item_off, d_g, d_starts, ndocs, n,
+               d_byd, d_docs, d_tf);
     }
     TRY(mark(c, "end"));
     CU_TRY(c, cudaGetLastError());
@@ -2210,6 +2229,132 @@ int b200sa_docs_list_dev(b200sa_ctx *c, uint64_t n, const uint32_t *d_gsa, const
     }
     return tree_exit(c, docs_list_core(c, (uint32_t)n, d_gsa, d_doc_starts, ndocs, d_byd, d_prev, d_start, d_end, nq,
                                        d_offsets, d_docs, d_tf, cap, total));
+}
+
+// ------------------------------------------------------------ top-k document retrieval (SURVEY 8f-9)
+// Launches of k_topk_tile that a round needs when its largest query lists lmax entries (topk_tiles on the host).
+static uint32_t topk_levels(uint64_t lmax, uint32_t k) {
+    if (lmax <= TOPK_WARP) return 0;
+    uint32_t lv = 1;
+    for (uint64_t L = lmax; L > TOPK_TILE; lv++) {
+        const uint64_t t1 = (L - 1) / TOPK_TILE, last = L - t1 * TOPK_TILE;
+        L = t1 * k + (last < k ? last : k);
+    }
+    return lv;
+}
+
+// nq >= 1, 1 <= k <= B200SA_TOPK_MAX.  Phases: dlist_levels, dlist_count, dlist_scan, then per round
+// topk_emit and topk_select.
+static int docs_topk_core(b200sa_ctx *c, uint32_t n, const uint32_t *d_g, const uint32_t *d_starts, uint32_t ndocs,
+                          const uint32_t *d_byd, const uint32_t *d_prev, const uint32_t *d_start,
+                          const uint32_t *d_end, uint32_t nq, uint32_t k, uint32_t *d_count, uint32_t *d_docs,
+                          uint32_t *d_tf) {
+    typedef unsigned long long u64;
+    static_assert(TOPK_KMAX == B200SA_TOPK_MAX, "one block sorts the survivors of a tile");
+    TRY(ensure(c, c->g0, ((size_t)nq + 1) * 8));
+    u64 *off = ptr<u64>(c->g0);
+    DListArgs A;
+    u64 *item_off;
+    uint64_t total;
+    TRY(docs_list_front(c, n, d_g, d_starts, ndocs, d_byd, d_prev, d_start, d_end, nq,
+                        reinterpret_cast<uint64_t *>(off), &A, &item_off, &total));
+    LAUNCH(c, k_topk_count, cdiv(nq, BLK), off, nq, k, d_count);
+
+    // Rounds: runs of consecutive queries whose listing fits the budget; a larger query is a round of its own.
+    uint64_t budget = B200SA_TOPK_ROUND_ENTRIES;
+    if (const char *e = getenv("B200SA_TOPK_ROUND")) { long long v = atoll(e); if (v >= 1) budget = (uint64_t)v; }
+    struct Round { uint32_t q0, q1; uint64_t lmax; };
+    std::vector<Round> rounds{{0, nq, total < ndocs ? total : (uint64_t)ndocs}};
+    std::vector<u64> h_off, h_is;
+    uint64_t rcap = total, max_items = 0;
+    const bool multi = total > budget;
+    if (multi) {                                         // cut the batch on the host
+        h_off.resize((size_t)nq + 1);
+        h_is.resize((size_t)nq + 1);
+        CU_TRY(c, cudaMemcpyAsync(h_off.data(), off, ((size_t)nq + 1) * 8, cudaMemcpyDeviceToHost, c->stream));
+        CU_TRY(c, cudaMemcpyAsync(h_is.data(), A.item_start, ((size_t)nq + 1) * 8, cudaMemcpyDeviceToHost, c->stream));
+        CU_TRY(c, cudaStreamSynchronize(c->stream));
+        rounds.clear();
+        rcap = 0;
+        for (uint32_t q0 = 0, q1; q0 < nq; q0 = q1) {
+            uint64_t lmax = h_off[q0 + 1] - h_off[q0];
+            for (q1 = q0 + 1; q1 < nq && h_off[q1 + 1] - h_off[q0] <= budget; q1++)
+                lmax = std::max<uint64_t>(lmax, h_off[q1 + 1] - h_off[q1]);
+            rounds.push_back({q0, q1, lmax});
+            rcap = std::max<uint64_t>(rcap, h_off[q1] - h_off[q0]);
+            max_items = std::max<uint64_t>(max_items, h_is[q1] - h_is[q0]);
+        }
+        TRY(ensure(c, c->p1, ((size_t)nq + 1) * 8));
+        TRY(ensure(c, c->rank, (size_t)max_items * 8));
+    }
+    TRY(ensure(c, c->v0, (size_t)rcap * 8));             // X: the round's documents | tf, later keys
+    TRY(ensure(c, c->v1, (size_t)rcap * 8));             // Y: keys
+    TRY(ensure(c, c->g1, ((size_t)nq + 1) * 4));
+    uint32_t *X = ptr<uint32_t>(c->v0), *tile_start = ptr<uint32_t>(c->g1);
+    u64 *KX = ptr<u64>(c->v0), *KY = ptr<u64>(c->v1);
+    uint32_t *d_ntiles = ptr<uint32_t>(c->small) + 8;
+    const uint32_t tile_grid = (uint32_t)c->sm_count * 4;
+    for (const Round &r : rounds) {
+        const uint32_t nqr = r.q1 - r.q0;
+        const uint64_t e0 = multi ? h_off[r.q0] : 0, entries = multi ? h_off[r.q1] - e0 : total;
+        if (entries == 0) continue;                      // every count is 0
+        TRY(mark(c, "topk_emit"));
+        DListArgs Ar = A;
+        const u64 *io = item_off;
+        if (multi) {
+            const uint64_t i0 = h_is[r.q0], items = h_is[r.q1] - i0;
+            LAUNCH(c, k_topk_rebase, cdiv(std::max<uint64_t>((uint64_t)nqr + 1, items), BLK), A.item_start, item_off,
+                   r.q0, nqr, i0, items, e0, ptr<u64>(c->p1), ptr<u64>(c->rank));
+            Ar.qs = d_start + r.q0; Ar.qe = d_end + r.q0; Ar.item_start = ptr<u64>(c->p1); Ar.nq = nqr;
+            Ar.items = items;
+            io = ptr<u64>(c->rank);
+        }
+        LAUNCH(c, k_dlist<true>, cdiv(Ar.items, NWARP), Ar, ptr<uint32_t>(c->p0), io, d_g, d_starts, ndocs, n, d_byd,
+               X, X + rcap);
+        TRY(mark(c, "topk_select"));
+        const TopkArgs P{off, e0, rcap, r.q0, nqr, k, ndocs, (uint32_t)bit_length(ndocs - 1), d_docs, d_tf};
+        LAUNCH(c, k_topk_warp, cdiv(nqr, NWARP), P, (const uint32_t *)X);
+        const uint32_t levels = topk_levels(r.lmax, k);
+        for (uint32_t lv = 0; lv < levels; lv++) {
+            TRY((dev_scan<OpSum>(c, TopkTileCount{off, r.q0, nqr, k, lv}, OutStoreExcl{tile_start}, nqr, d_ntiles)));
+            if (lv == 0)
+                LAUNCH(c, k_topk_tile<true>, tile_grid, P, lv, (const uint32_t *)tile_start, (const uint32_t *)d_ntiles,
+                       (const uint32_t *)X, (const u64 *)nullptr, KY);
+            else
+                LAUNCH(c, k_topk_tile<false>, tile_grid, P, lv, (const uint32_t *)tile_start, (const uint32_t *)d_ntiles,
+                       (const uint32_t *)nullptr, (const u64 *)(lv & 1 ? KY : KX), lv & 1 ? KX : KY);
+        }
+    }
+    TRY(mark(c, "end"));
+    CU_TRY(c, cudaGetLastError());
+    CU_TRY(c, cudaStreamSynchronize(c->stream));
+    return B200SA_OK;
+}
+
+int b200sa_docs_topk_dev(b200sa_ctx *c, uint64_t n, const uint32_t *d_gsa, const uint32_t *d_doc_starts,
+                         uint32_t ndocs, const uint32_t *d_byd, const uint32_t *d_prev, const uint32_t *d_start,
+                         const uint32_t *d_end, uint32_t nq, uint32_t k, uint32_t *d_count, uint32_t *d_docs,
+                         uint32_t *d_tf, void *stream) {
+    if (!c) return B200SA_ERR_BAD_ARG;
+    if (!d_count || !d_docs || !d_tf || (nq > 0 && (!d_start || !d_end)) ||
+        (n > 0 && (!d_gsa || !d_doc_starts || !d_byd || !d_prev))) {
+        c->last_error = "null pointer";
+        return B200SA_ERR_BAD_ARG;
+    }
+    if (ndocs == 0 && n > 0) {
+        c->last_error = "doc_starts rejected: ndocs == 0 with n > 0;";
+        return B200SA_ERR_BAD_ARG;
+    }
+    if (k == 0 || k > B200SA_TOPK_MAX) {
+        c->last_error = "docs topk: k must be in 1 .. B200SA_TOPK_MAX";
+        return B200SA_ERR_BAD_ARG;
+    }
+    if (n > B200SA_MAX_N) return B200SA_ERR_TOO_LARGE;
+    CU_TRY(c, cudaSetDevice(c->device));
+    begin_call(c, stream);
+    if (nq == 0) return end_call(c);
+    return tree_exit(c, docs_topk_core(c, (uint32_t)n, d_gsa, d_doc_starts, ndocs, d_byd, d_prev, d_start, d_end, nq,
+                                       k, d_count, d_docs, d_tf));
 }
 
 // ------------------------------------------------------------ multi-GPU: communicator + sharded LMS sort

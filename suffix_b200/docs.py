@@ -16,6 +16,7 @@ from . import _lib
 from .table import _as_bytes, _lock      # the lock of the per-device default context, shared with SuffixTable
 
 MAX_N = 0xFFFFF000        # B200SA_MAX_N
+TOPK_MAX = 1024           # B200SA_TOPK_MAX
 
 
 class DocumentSuffixTable:
@@ -278,6 +279,46 @@ class DocumentSuffixTable:
         (b200sa_docs_list_dev with cap = 0), without building the tree of DocumentSuffixTree."""
         d_off, _, _ = self._list_dev(list(queries), 0, with_tf=False)
         return d_off.diff().cpu().numpy().astype(np.uint32)
+
+    # ---- top-k document retrieval
+    def top_documents_batch(self, queries, k):
+        """Per query the min(k, df) documents that contain it most often, by occurrence count descending and
+        then by ascending document: (offsets u64[nq + 1], docs u32[], counts u32[]), query q's rows at
+        [offsets[q], offsets[q+1]) in that order.  1 <= k <= TOPK_MAX (for a longer answer use
+        documents_batch).  Runs on the device (b200sa_docs_topk_dev over the ranges of positions_batch) with
+        the index of documents_batch; the device output is nq * k rows, whatever the listing's size.  b"" and
+        absent queries have no rows."""
+        import torch
+        k = int(k)
+        if not 1 <= k <= TOPK_MAX:
+            raise ValueError("k must be in 1 .. %d, got %d" % (TOPK_MAX, k))
+        d_start, d_end = self._positions_dev(queries)
+        nq = len(d_start)
+        if nq == 0:
+            return np.zeros(1, dtype=np.uint64), np.zeros(0, dtype=np.uint32), np.zeros(0, dtype=np.uint32)
+        dev = d_start.device
+        byd, prev = self._list_arrays()
+        _, d_g, d_s = self._device_arrays()
+        count = torch.empty(nq, dtype=torch.int32, device=dev)
+        docs = torch.empty(nq * k, dtype=torch.int32, device=dev)
+        tf = torch.empty(nq * k, dtype=torch.int32, device=dev)
+        with _lock:
+            _lib.default_context(self._device).docs_topk_dev(
+                len(self._table), d_g.data_ptr(), d_s.data_ptr(), len(self._starts), byd.data_ptr(), prev.data_ptr(),
+                d_start.data_ptr(), d_end.data_ptr(), nq, k, count.data_ptr(), docs.data_ptr(), tf.data_ptr(),
+                torch.cuda.current_stream(dev).cuda_stream)
+        keep = torch.arange(k, device=dev, dtype=torch.int32)[None, :] < count[:, None]
+        off = torch.zeros(nq + 1, dtype=torch.int64, device=dev)
+        off[1:] = torch.cumsum(count, 0)
+        docs, tf = docs.view(nq, k)[keep], tf.view(nq, k)[keep]
+        torch.cuda.synchronize(dev)
+        return off.cpu().numpy().view(np.uint64), docs.cpu().numpy().view(np.uint32), tf.cpu().numpy().view(np.uint32)
+
+    def top_documents(self, query, k) -> np.ndarray:
+        """(document, count) rows of the min(k, df) documents that contain `query` most often, by count
+        descending, then by ascending document: a batch of one."""
+        _, docs, tf = self.top_documents_batch([query], k)
+        return np.stack([docs, tf], axis=1)
 
     def __repr__(self):
         return "DocumentSuffixTable(docs=%d, n=%d)" % (len(self._starts), len(self._table))

@@ -104,6 +104,16 @@ for k, docs in enumerate(doc_sets + [[b"ACGT"] * 2000 + [b""]]):   # document li
     assert np.array_equal(dl.document_frequencies(qs), np.diff(off.astype(np.int64))), k
     d_off, d_docs, _ = dl._list_dev(qs, max(1, int(off[-1])), with_tf=False)
     assert int(d_off[-1]) == int(off[-1]), k
+# top-k: every size class (b"A" of 9000 copies: two levels of tiles), k = 1 / B200SA_TOPK_MAX, one and many rounds
+for k, docs in enumerate(doc_sets + [[b"ACGT"] * 9000 + [b""]]):
+    dl = DocumentSuffixTable(docs)
+    qs = [b"ACG", b"TA", b"\x00", b"", b"GTAC", b"A", b"C"]
+    for kk in (1, 1024):
+        want = dl.top_documents_batch(qs, kk)
+        os.environ["B200SA_TOPK_ROUND"] = "50"
+        got = dl.top_documents_batch(qs, kk)
+        del os.environ["B200SA_TOPK_ROUND"]
+        assert all(np.array_equal(x, y) for x, y in zip(want, got)), (k, kk)
 print("sanitize workload ok")
 PY
 for tool in memcheck racecheck; do
