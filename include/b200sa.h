@@ -332,6 +332,58 @@ int b200sa_docs_topk_dev(b200sa_ctx *ctx, uint64_t n, const uint32_t *d_gsa, con
                          const uint32_t *d_end, uint32_t nq, uint32_t k, uint32_t *d_count, uint32_t *d_docs,
                          uint32_t *d_tf, void *stream);
 
+/* ---- matching statistics and super-maximal exact matches (DESIGN.md 6b f-10) ----
+ * Index: a text T of n bytes with sa and lcp as b200sa_build_lcp_dev returns them, or the documents'
+ * concatenation C with G, glcp and doc_starts as b200sa_docs_build_dev takes and returns them.  S_p is the
+ * suffix at p: T[p, n), or C[p, end of p's document).  A string occurs if it is a prefix of some S_p; with
+ * documents an occurrence never crosses a document end.
+ * Queries as for b200sa_positions_dev: query q is bytes [q_off[q], q_off[q+1]) of d_queries, and
+ * q_bytes = q_off[nq] is passed by the caller, so that no read-back is needed to size the launch.  A pattern
+ * position is a byte index x in [0, q_bytes); it lies in query q(x), whose end is E(x) = q_off[q(x)+1].
+ * For every pattern position x:
+ *   len[x]              the largest l <= E(x) - x such that queries[x, x+l) occurs: a match never runs past
+ *                       the end of its own query;
+ *   [start[x], end[x])  the range of the table (sa or G) whose suffixes start with queries[x, x+len[x]):
+ *                       what b200sa_positions_dev / b200sa_docs_positions_dev return for that string when
+ *                       len[x] > 0, and (0, 0) when len[x] = 0 (b"" matches nothing).
+ * d_len, d_start and d_end hold q_bytes u32 each.  d_start and d_end are both given or both NULL; without
+ * them only len is written, d_lcp / d_glcp may be NULL and no block minima are built.  One binary search
+ * per position carries the common-prefix lengths of its two bounds, so it ends with the longest match and
+ * a rank that attains it; the range is the LCP interval of depth len[x] around that rank.  Block minima
+ * over lcp are rebuilt on every call (one read of 4n bytes).
+ * sa and lcp (G and glcp) must be what the build returned; they are not verified.  q_off is checked on the
+ * device (q_off[0] = 0, ascending, q_off[nq] = q_bytes), and so is doc_starts by the documents entry:
+ * B200SA_ERR_BAD_ARG with a b200sa_last_error detail, as for a required NULL pointer.  n or q_bytes above
+ * B200SA_MAX_N returns B200SA_ERR_TOO_LARGE.  nq = 0 or q_bytes = 0 return without launching; n = 0 gives
+ * len = start = end = 0 everywhere.  No byte outside [d_text, d_text + n) and [d_queries, d_queries + q_bytes)
+ * is read: the buffers need no padding and no alignment.  Synchronises the stream only to read the check
+ * words back.  Phases: match_check, match_levels (with ranges), match_search. */
+int b200sa_match_stats_dev(b200sa_ctx *ctx, const uint8_t *d_text, uint64_t n, const uint32_t *d_sa,
+                           const uint32_t *d_lcp, const uint8_t *d_queries, const uint64_t *d_q_off,
+                           uint32_t nq, uint64_t q_bytes, uint32_t *d_len, uint32_t *d_start,
+                           uint32_t *d_end, void *stream);
+int b200sa_docs_match_stats_dev(b200sa_ctx *ctx, const uint8_t *d_text, uint64_t n, const uint32_t *d_gsa,
+                                const uint32_t *d_glcp, const uint32_t *d_doc_starts, uint32_t ndocs,
+                                const uint8_t *d_queries, const uint64_t *d_q_off, uint32_t nq,
+                                uint64_t q_bytes, uint32_t *d_len, uint32_t *d_start, uint32_t *d_end,
+                                void *stream);
+/* Super-maximal exact matches (SMEMs) of query q at threshold min_len >= 1: the positions x of q with
+ * len[x] >= min_len and (x = q_off[q] or len[x-1] <= len[x]).  Dropping the first byte of a match leaves a
+ * match, so len[x+1] >= len[x] - 1 and x + len[x] never decreases inside a query; hence a match
+ * [x, x+len[x]) lies inside another match of the query exactly when x-1 is in the query and
+ * len[x-1] > len[x], and the SMEMs are the matches of at least min_len bytes contained in no other.
+ * d_len is what the calls above wrote for the same q_off.  Follows the listing's protocol: always writes
+ * d_offsets (nq + 1 x u64, exclusive: query q's SMEMs are [offsets[q], offsets[q+1])) and
+ * *total = offsets[nq]; writes d_qpos[0, total), the offset x - q_off[q] of each SMEM inside its query, in
+ * ascending x, only when total <= cap; cap = 0 (d_qpos may then be NULL) counts only.  The caller gathers
+ * len / start / end at q_off[q] + qpos.  min_len = 0 returns B200SA_ERR_BAD_ARG; q_off is checked as above;
+ * q_bytes above B200SA_MAX_N returns B200SA_ERR_TOO_LARGE; nq = 0 writes offsets[0] = 0.  Device workspace:
+ * 8 bytes per query byte.  Synchronises the stream (it reads the total back).  Phases: match_check,
+ * smem_flag, smem_scan, smem_emit. */
+int b200sa_smems_dev(b200sa_ctx *ctx, const uint64_t *d_q_off, uint32_t nq, uint64_t q_bytes,
+                     const uint32_t *d_len, uint32_t min_len, uint64_t *d_offsets, uint32_t *d_qpos,
+                     uint64_t cap, uint64_t *total, void *stream);
+
 /* ---- multi-GPU: communicator + sharded LMS-suffix sort (SURVEY.md 8e, config 5) ----
  * One process (or thread) and one context per GPU.  NCCL is resolved at run time
  * (the copy already loaded in the process, else libnccl.so.2); the single-GPU entry

@@ -90,6 +90,9 @@ def lib():
         "b200sa_docs_list_dev": ([vp, u64, vp, vp, u32, vp, vp, vp, vp, u32, vp, vp, vp, u64, ctypes.POINTER(u64), vp],
                                  ci),
         "b200sa_docs_topk_dev": ([vp, u64, vp, vp, u32, vp, vp, vp, vp, u32, u32, vp, vp, vp, vp], ci),
+        "b200sa_match_stats_dev": ([vp, vp, u64, vp, vp, vp, vp, u32, u64, vp, vp, vp, vp], ci),
+        "b200sa_docs_match_stats_dev": ([vp, vp, u64, vp, vp, vp, u32, vp, vp, u32, u64, vp, vp, vp, vp], ci),
+        "b200sa_smems_dev": ([vp, vp, u32, u64, vp, u32, vp, vp, u64, ctypes.POINTER(u64), vp], ci),
         "b200sa_last_stats": ([vp, ctypes.POINTER(Stats)], ci),
         "b200sa_set_timing": ([vp, ci], ci),
         "b200sa_last_phase_times": ([vp, ctypes.POINTER(ctypes.c_char_p), ctypes.POINTER(ctypes.c_float), ci], ci),
@@ -312,6 +315,27 @@ class Context:
         """b200sa_docs_topk_dev: count[q] = min(k, df(q)); docs / tf[q*k + j] for j < count[q], best first."""
         self._check(lib().b200sa_docs_topk_dev(self._h, n, d_gsa, d_doc_starts or None, ndocs, d_byd, d_prev, d_start,
                                                d_end, nq, k, d_count, d_docs, d_tf, stream))
+
+    def match_stats_dev(self, d_text, n, d_sa, d_lcp, d_q, d_qoff, nq, q_bytes, d_len, d_start=0, d_end=0,
+                        stream: int = 0):
+        """b200sa_match_stats_dev: len (and the table range, when d_start / d_end are given) of every pattern
+        position; d_lcp may be 0 without the ranges."""
+        self._check(lib().b200sa_match_stats_dev(self._h, d_text, n, d_sa, d_lcp or None, d_q, d_qoff, nq, q_bytes,
+                                                 d_len, d_start or None, d_end or None, stream))
+
+    def docs_match_stats_dev(self, d_text, n, d_gsa, d_glcp, d_doc_starts, ndocs, d_q, d_qoff, nq, q_bytes, d_len,
+                             d_start=0, d_end=0, stream: int = 0):
+        """b200sa_docs_match_stats_dev: the same over G, every suffix cut at its document's end."""
+        self._check(lib().b200sa_docs_match_stats_dev(self._h, d_text, n, d_gsa, d_glcp or None, d_doc_starts or None,
+                                                      ndocs, d_q, d_qoff, nq, q_bytes, d_len, d_start or None,
+                                                      d_end or None, stream))
+
+    def smems_dev(self, d_qoff, nq, q_bytes, d_len, min_len, d_offsets, d_qpos, cap, stream: int = 0) -> int:
+        """b200sa_smems_dev: writes the offsets, and qpos when the SMEMs fit in cap.  Returns the total."""
+        total = ctypes.c_uint64(0)
+        self._check(lib().b200sa_smems_dev(self._h, d_qoff, nq, q_bytes, d_len, min_len, d_offsets, d_qpos or None,
+                                           cap, ctypes.byref(total), stream))
+        return int(total.value)
 
     def lcp_sharded(self, d_text: int, n: int, d_sa: int, d_lcp: int, replicated: bool = False, stream: int = 0):
         self._check(lib().b200sa_lcp_sharded(self._h, d_text, n, d_sa, d_lcp, 1 if replicated else 0, stream))

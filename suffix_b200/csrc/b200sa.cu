@@ -31,6 +31,7 @@
 #include "docs_tree.cuh"
 #include "docs_list.cuh"
 #include "docs_topk.cuh"
+#include "match.cuh"
 #include "nccl_dyn.h"
 
 using namespace b200sa;
@@ -2355,6 +2356,178 @@ int b200sa_docs_topk_dev(b200sa_ctx *c, uint64_t n, const uint32_t *d_gsa, const
     if (nq == 0) return end_call(c);
     return tree_exit(c, docs_topk_core(c, (uint32_t)n, d_gsa, d_doc_starts, ndocs, d_byd, d_prev, d_start, d_end, nq,
                                        k, d_count, d_docs, d_tf));
+}
+
+// ------------------------------------------------------------ matching statistics and SMEMs (DESIGN 6b f-10)
+// q_off[0] = 0, ascending, q_off[nq] = q_bytes, checked on the device (one read-back).  nq >= 1.
+static int match_check(b200sa_ctx *c, const uint64_t *d_q_off, uint32_t nq, uint64_t q_bytes) {
+    TRY(ensure(c, c->small, 4096));
+    uint32_t *word = ptr<uint32_t>(c->small);
+    CU_TRY(c, cudaMemsetAsync(word, 0, 4, c->stream));
+    LAUNCH(c, k_match_check, cdiv((uint64_t)nq + 1, BLK), d_q_off, nq, q_bytes, word);
+    CU_TRY(c, cudaGetLastError());
+    TRY(read_words(c, word, 1));
+    if (const uint32_t bits = c->h_pin[0]) {
+        std::string m = "q_off rejected:";
+        if (bits & MATCH_BAD_FIRST) m += " q_off[0] != 0;";
+        if (bits & MATCH_BAD_ORDER) m += " not ascending;";
+        if (bits & MATCH_BAD_LAST) m += " q_off[nq] != q_bytes;";
+        c->last_error = m;
+        return B200SA_ERR_BAD_ARG;
+    }
+    return B200SA_OK;
+}
+
+static int match_args(b200sa_ctx *c, uint64_t n, const void *text, const void *sa, const void *queries,
+                      const void *q_off, uint32_t nq, uint64_t q_bytes, const void *len, const void *start,
+                      const void *end) {
+    if (!c) return B200SA_ERR_BAD_ARG;
+    if ((n > 0 && (!text || !sa)) || (nq > 0 && !q_off) || (q_bytes > 0 && (!queries || !len))) {
+        c->last_error = "null pointer";
+        return B200SA_ERR_BAD_ARG;
+    }
+    if ((start == nullptr) != (end == nullptr)) {
+        c->last_error = "match stats: d_start and d_end are both given or both NULL";
+        return B200SA_ERR_BAD_ARG;
+    }
+    if (n > B200SA_MAX_N || q_bytes > B200SA_MAX_N) {
+        c->last_error = "text or queries longer than 2^32-4096 bytes";
+        return B200SA_ERR_TOO_LARGE;
+    }
+    return B200SA_OK;
+}
+
+extern "C++" {
+// nq >= 1, q_bytes >= 1.  d_starts non-null (EndF = DocsEnd): doc_starts is verified with q_off.  Phases:
+// match_check, match_levels (with ranges), match_search.
+template <class EndF>
+static int match_stats_core(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const uint32_t *d_sa,
+                            const uint32_t *d_lcp, const uint8_t *d_queries, const uint64_t *d_q_off, uint32_t nq,
+                            uint64_t q_bytes, uint32_t *d_len, uint32_t *d_start, uint32_t *d_end, EndF end,
+                            const uint32_t *d_starts, uint32_t ndocs) {
+    TRY(mark(c, "match_check"));
+    TRY(match_check(c, d_q_off, nq, q_bytes));
+    if (n > 0 && d_starts) {
+        uint32_t *words = ptr<uint32_t>(c->small);
+        CU_TRY(c, cudaMemsetAsync(words, 0, 8, c->stream));
+        LAUNCH(c, k_docs_check, cdiv(ndocs, BLK), d_starts, ndocs, n, words);
+        CU_TRY(c, cudaGetLastError());
+        TRY(read_words(c, words, 1));
+        if (c->h_pin[0]) return docs_bad(c, c->h_pin[0]);
+    }
+    if (n == 0) {                                        // nothing occurs
+        CU_TRY(c, cudaMemsetAsync(d_len, 0, q_bytes * 4, c->stream));
+        if (d_start) {
+            CU_TRY(c, cudaMemsetAsync(d_start, 0, q_bytes * 4, c->stream));
+            CU_TRY(c, cudaMemsetAsync(d_end, 0, q_bytes * 4, c->stream));
+        }
+        TRY(mark(c, "end"));
+        return B200SA_OK;
+    }
+    const MatchBuf T(d_text, n), Q(d_queries, q_bytes);
+    const uint32_t grid = cdiv(q_bytes, BLK);
+    AnsvLevels L;
+    memset(&L, 0, sizeof L);
+    if (d_start) {
+        TRY(mark(c, "match_levels"));
+        TRY(ansv_levels(c, d_lcp, n, &L));
+        TRY(mark(c, "match_search"));
+        LAUNCH(c, (k_match_stats<EndF, true>), grid, T, n, d_sa, L, Q, d_q_off, nq, q_bytes, d_len, d_start, d_end, end);
+    } else {
+        TRY(mark(c, "match_search"));
+        LAUNCH(c, (k_match_stats<EndF, false>), grid, T, n, d_sa, L, Q, d_q_off, nq, q_bytes, d_len, d_start, d_end, end);
+    }
+    TRY(mark(c, "end"));
+    CU_TRY(c, cudaGetLastError());
+    return B200SA_OK;
+}
+}  // extern "C++"
+
+int b200sa_match_stats_dev(b200sa_ctx *c, const uint8_t *d_text, uint64_t n, const uint32_t *d_sa,
+                           const uint32_t *d_lcp, const uint8_t *d_queries, const uint64_t *d_q_off, uint32_t nq,
+                           uint64_t q_bytes, uint32_t *d_len, uint32_t *d_start, uint32_t *d_end, void *stream) {
+    TRY(match_args(c, n, d_text, d_sa, d_queries, d_q_off, nq, q_bytes, d_len, d_start, d_end));
+    if (n > 0 && d_start && !d_lcp) {
+        c->last_error = "null pointer";
+        return B200SA_ERR_BAD_ARG;
+    }
+    CU_TRY(c, cudaSetDevice(c->device));
+    begin_call(c, stream);
+    if (nq == 0 || q_bytes == 0) return end_call(c);
+    return tree_exit(c, match_stats_core(c, d_text, (uint32_t)n, d_sa, d_lcp, d_queries, d_q_off, nq, q_bytes, d_len,
+                                         d_start, d_end, TextEnd{(uint32_t)n}, nullptr, 0));
+}
+
+int b200sa_docs_match_stats_dev(b200sa_ctx *c, const uint8_t *d_text, uint64_t n, const uint32_t *d_gsa,
+                                const uint32_t *d_glcp, const uint32_t *d_doc_starts, uint32_t ndocs,
+                                const uint8_t *d_queries, const uint64_t *d_q_off, uint32_t nq, uint64_t q_bytes,
+                                uint32_t *d_len, uint32_t *d_start, uint32_t *d_end, void *stream) {
+    TRY(match_args(c, n, d_text, d_gsa, d_queries, d_q_off, nq, q_bytes, d_len, d_start, d_end));
+    if (n > 0 && ((d_start && !d_glcp) || !d_doc_starts)) {
+        c->last_error = "null pointer";
+        return B200SA_ERR_BAD_ARG;
+    }
+    if (ndocs == 0 && n > 0) {
+        c->last_error = "doc_starts rejected: ndocs == 0 with n > 0;";
+        return B200SA_ERR_BAD_ARG;
+    }
+    CU_TRY(c, cudaSetDevice(c->device));
+    begin_call(c, stream);
+    if (nq == 0 || q_bytes == 0) return end_call(c);
+    return tree_exit(c, match_stats_core(c, d_text, (uint32_t)n, d_gsa, d_glcp, d_queries, d_q_off, nq, q_bytes,
+                                         d_len, d_start, d_end, DocsEnd{d_doc_starts, ndocs, (uint32_t)n},
+                                         d_doc_starts, ndocs));
+}
+
+// nq >= 1.  Phases: match_check, smem_flag, smem_scan, smem_emit.
+static int smems_core(b200sa_ctx *c, const uint64_t *d_q_off, uint32_t nq, uint64_t q_bytes, const uint32_t *d_len,
+                      uint32_t min_len, uint64_t *d_offsets, uint32_t *d_qpos, uint64_t cap, uint64_t *total) {
+    TRY(mark(c, "match_check"));
+    TRY(match_check(c, d_q_off, nq, q_bytes));
+    TRY(mark(c, "smem_flag"));
+    TRY(ensure(c, c->p0, (q_bytes + 1) * 4));
+    TRY(ensure(c, c->p1, (q_bytes + 1) * 4));
+    uint32_t *flag = ptr<uint32_t>(c->p0), *exc = ptr<uint32_t>(c->p1), *d_total = ptr<uint32_t>(c->small) + 2;
+    LAUNCH(c, k_smem_flag, cdiv(q_bytes + 1, BLK), d_len, d_q_off, nq, q_bytes, min_len, flag);
+    TRY(mark(c, "smem_scan"));                          // q_bytes <= B200SA_MAX_N: a u32 sum
+    TRY((dev_scan<OpSum>(c, SmemIn{flag}, SmemOut{exc}, q_bytes + 1, d_total)));
+    TRY(read_words(c, d_total, 1));
+    *total = c->h_pin[0];
+    TRY(mark(c, "smem_emit"));
+    const uint64_t items = std::max<uint64_t>(q_bytes, (uint64_t)nq + 1);
+    LAUNCH(c, k_smem_emit, cdiv(items, BLK), flag, exc, d_q_off, nq, q_bytes,
+           reinterpret_cast<unsigned long long *>(d_offsets), *total <= cap ? d_qpos : (uint32_t *)nullptr);
+    TRY(mark(c, "end"));
+    CU_TRY(c, cudaGetLastError());
+    CU_TRY(c, cudaStreamSynchronize(c->stream));
+    return B200SA_OK;
+}
+
+int b200sa_smems_dev(b200sa_ctx *c, const uint64_t *d_q_off, uint32_t nq, uint64_t q_bytes, const uint32_t *d_len,
+                     uint32_t min_len, uint64_t *d_offsets, uint32_t *d_qpos, uint64_t cap, uint64_t *total,
+                     void *stream) {
+    if (!c) return B200SA_ERR_BAD_ARG;
+    if (!total || !d_offsets || (nq > 0 && !d_q_off) || (q_bytes > 0 && !d_len) || (cap > 0 && !d_qpos)) {
+        c->last_error = "null pointer";
+        return B200SA_ERR_BAD_ARG;
+    }
+    if (min_len == 0) {
+        c->last_error = "smems: min_len must be at least 1";
+        return B200SA_ERR_BAD_ARG;
+    }
+    if (q_bytes > B200SA_MAX_N) {
+        c->last_error = "queries longer than 2^32-4096 bytes";
+        return B200SA_ERR_TOO_LARGE;
+    }
+    CU_TRY(c, cudaSetDevice(c->device));
+    begin_call(c, stream);
+    *total = 0;
+    if (nq == 0) {
+        CU_TRY(c, cudaMemsetAsync(d_offsets, 0, 8, c->stream));
+        CU_TRY(c, cudaStreamSynchronize(c->stream));
+        return end_call(c);
+    }
+    return tree_exit(c, smems_core(c, d_q_off, nq, q_bytes, d_len, min_len, d_offsets, d_qpos, cap, total));
 }
 
 // ------------------------------------------------------------ multi-GPU: communicator + sharded LMS sort

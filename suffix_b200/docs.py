@@ -12,7 +12,7 @@ import bisect
 
 import numpy as np
 
-from . import _lib
+from . import _lib, _match
 from .table import _as_bytes, _lock      # the lock of the per-device default context, shared with SuffixTable
 
 MAX_N = 0xFFFFF000        # B200SA_MAX_N
@@ -35,6 +35,7 @@ class DocumentSuffixTable:
         self._starts = np.asarray(starts, dtype=np.uint32)
         self._ends = np.append(self._starts[1:], np.uint32(len(self._text))).astype(np.uint32) if docs else self._starts
         self._dev = None
+        self._dev_lcp = None
         self._dlist = None
         t = np.frombuffer(self._text, dtype=np.uint8)
         with _lock:                           # default context is not thread-safe
@@ -215,12 +216,16 @@ class DocumentSuffixTable:
         return self._dlist
 
     def _list_dev(self, queries, cap_guess, with_tf=True):
-        """b200sa_docs_list_dev over the ranges of positions_batch: (offsets, docs, tf) as device tensors
+        """_list_ranges_dev over the ranges of positions_batch."""
+        d_start, d_end = self._positions_dev(queries)
+        return self._list_ranges_dev(d_start, d_end, cap_guess, with_tf)
+
+    def _list_ranges_dev(self, d_start, d_end, cap_guess, with_tf=True):
+        """b200sa_docs_list_dev over ranges of table() on the device: (offsets, docs, tf) as device tensors
         (u64 offsets as int64, u32 entries as int32, tf None without with_tf).  cap_guess = 0 asks for the
         offsets alone; otherwise the buffers hold cap_guess entries and a larger listing is fetched by a
         second call sized to it."""
         import torch
-        d_start, d_end = self._positions_dev(queries)
         nq = len(d_start)
         dev = d_start.device
         d_off = torch.zeros(nq + 1, dtype=torch.int64, device=dev)
@@ -253,12 +258,33 @@ class DocumentSuffixTable:
         on the device (b200sa_docs_list_dev, Muthukrishnan's array over the ranges of positions_batch); its
         index, built on the first call and kept, holds 8 bytes per text byte of device memory.  b"" lists
         nothing."""
-        import torch
         qs = list(queries)
         if _cap_guess is None:
             _cap_guess = max(1, min(1 << 24, 64 * len(qs)))
-        d_off, docs, tf = self._list_dev(qs, _cap_guess)
-        nq = len(qs)
+        return self._documents_sorted(*self._list_dev(qs, _cap_guess))
+
+    def _ranges_dev(self, start, end):
+        """Two equally long arrays of u32 range bounds as int32 device tensors."""
+        import torch
+        start = np.ascontiguousarray(start, dtype=np.uint32)
+        end = np.ascontiguousarray(end, dtype=np.uint32)
+        if start.shape != end.shape or start.ndim != 1:
+            raise ValueError("start and end must be one-dimensional and equally long")
+        dev = torch.device("cuda", self._device)
+        return (torch.from_numpy(start.view(np.int32).copy()).to(dev),
+                torch.from_numpy(end.view(np.int32).copy()).to(dev))
+
+    def documents_for_ranges(self, start, end):
+        """documents_batch for ranges [start[q], end[q]) of table() instead of query strings: the ranges that
+        positions_batch, matching_statistics and smems return.  A range with start > end or end > len(self)
+        is an error."""
+        d_start, d_end = self._ranges_dev(start, end)
+        return self._documents_sorted(*self._list_ranges_dev(d_start, d_end, max(1, min(1 << 24, 64 * len(d_start)))))
+
+    def _documents_sorted(self, d_off, docs, tf):
+        """The listing of _list_ranges_dev by ascending document per query, on the host."""
+        import torch
+        nq = len(d_off) - 1
         if len(docs):
             # rank order -> document order per query: one sort of (query, document) keys
             q = torch.repeat_interleave(torch.arange(nq, device=docs.device, dtype=torch.int64), d_off.diff())
@@ -292,7 +318,19 @@ class DocumentSuffixTable:
         k = int(k)
         if not 1 <= k <= TOPK_MAX:
             raise ValueError("k must be in 1 .. %d, got %d" % (TOPK_MAX, k))
-        d_start, d_end = self._positions_dev(queries)
+        return self._top_ranges_dev(*self._positions_dev(queries), k)
+
+    def top_documents_for_ranges(self, start, end, k):
+        """top_documents_batch for ranges [start[q], end[q]) of table() instead of query strings (see
+        documents_for_ranges)."""
+        k = int(k)
+        if not 1 <= k <= TOPK_MAX:
+            raise ValueError("k must be in 1 .. %d, got %d" % (TOPK_MAX, k))
+        return self._top_ranges_dev(*self._ranges_dev(start, end), k)
+
+    def _top_ranges_dev(self, d_start, d_end, k):
+        """b200sa_docs_topk_dev over ranges of table() on the device, compacted to the host triple."""
+        import torch
         nq = len(d_start)
         if nq == 0:
             return np.zeros(1, dtype=np.uint64), np.zeros(0, dtype=np.uint32), np.zeros(0, dtype=np.uint32)
@@ -313,6 +351,32 @@ class DocumentSuffixTable:
         docs, tf = docs.view(nq, k)[keep], tf.view(nq, k)[keep]
         torch.cuda.synchronize(dev)
         return off.cpu().numpy().view(np.uint64), docs.cpu().numpy().view(np.uint32), tf.cpu().numpy().view(np.uint32)
+
+    # ---- matching statistics and SMEMs (DESIGN 6b f-10)
+    def _match_call(self, ctx, d_q, d_off, nq, q_bytes, d_len, d_start, d_end, stream):
+        import torch
+        d_t, d_g, d_s = self._device_arrays()
+        if self._dev_lcp is None:                 # glcp joins the device copies on first use: 4 bytes per text byte
+            self._dev_lcp = torch.from_numpy(self._lcp.view(np.int32).copy()).to(d_g.device)
+        ctx.docs_match_stats_dev(d_t.data_ptr(), len(self._table), d_g.data_ptr(), self._dev_lcp.data_ptr(),
+                                 d_s.data_ptr(), len(self._starts), d_q, d_off, nq, q_bytes, d_len, d_start, d_end,
+                                 stream)
+
+    def matching_statistics(self, queries):
+        """For every byte of every query, the longest piece starting there that occurs inside one document,
+        and where (b200sa_docs_match_stats_dev): (offsets u64[nq + 1], length u32[], start u32[], end u32[]),
+        the row of query q, offset j at offsets[q] + j.  table()[start:end] are the occurrences of
+        query[j:j + length], the range positions_batch returns for that string ((0, 0) when length = 0)."""
+        self._device_arrays()
+        return _match.matching_statistics(self, queries)
+
+    def smems(self, queries, min_len=1):
+        """The super-maximal exact matches of every query: its matches of at least min_len bytes that lie
+        inside no other match of the same query (b200sa_smems_dev).  (offsets u64[nq + 1], qpos u32[],
+        length u32[], start u32[], end u32[]): query q's rows are [offsets[q], offsets[q+1]) by ascending
+        qpos.  start / end feed documents_for_ranges and top_documents_for_ranges as they are."""
+        self._device_arrays()
+        return _match.smems(self, queries, min_len)
 
     def top_documents(self, query, k) -> np.ndarray:
         """(document, count) rows of the min(k, df) documents that contain `query` most often, by count

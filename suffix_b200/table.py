@@ -159,6 +159,44 @@ class SuffixTable:
         torch.cuda.synchronize()
         return lcp, d_p.cpu().numpy().view(np.uint32), d_n.cpu().numpy().view(np.uint32)
 
+    # ---- matching statistics and SMEMs (DESIGN 6b f-10)
+    def _device_arrays(self):
+        """Device copies of the text, the table and lcp_lens(), made on first use and kept while the table
+        lives: 9 bytes per text byte of device memory."""
+        if getattr(self, "_dev", None) is None:
+            import torch
+            dev = torch.device("cuda", self._device)
+            up = lambda a: torch.from_numpy(a.copy()).to(dev)
+            lcp = self.lcp_lens()
+            self._dev = (up(np.frombuffer(self._text or b"\0", dtype=np.uint8)),
+                         up(np.ascontiguousarray(self._table, dtype=np.uint32).view(np.int32)),
+                         up(lcp.view(np.int32)))
+        return self._dev
+
+    def _match_call(self, ctx, d_q, d_off, nq, q_bytes, d_len, d_start, d_end, stream):
+        d_t, d_sa, d_lcp = self._dev
+        ctx.match_stats_dev(d_t.data_ptr(), len(self._table), d_sa.data_ptr(), d_lcp.data_ptr(), d_q, d_off, nq,
+                            q_bytes, d_len, d_start, d_end, stream)
+
+    def matching_statistics(self, queries):
+        """For every byte of every query, the longest piece starting there that occurs in the text, and
+        where (b200sa_match_stats_dev): (offsets u64[nq + 1], length u32[], start u32[], end u32[]), the
+        row of query q, offset j at offsets[q] + j.  length is the longest l with query[j:j + l] in the
+        text; table()[start:end] are its occurrences, what positions(query[j:j + l]) returns ((0, 0) when
+        l = 0).  Uses _device_arrays()."""
+        from . import _match
+        self._device_arrays()
+        return _match.matching_statistics(self, queries)
+
+    def smems(self, queries, min_len=1):
+        """The super-maximal exact matches of every query: its matches of at least min_len bytes that lie
+        inside no other match of the same query (b200sa_smems_dev).  (offsets u64[nq + 1], qpos u32[],
+        length u32[], start u32[], end u32[]): query q's rows are [offsets[q], offsets[q+1]) by ascending
+        qpos, the match is query[qpos:qpos + length] and table()[start:end] are its occurrences."""
+        from . import _match
+        self._device_arrays()
+        return _match.smems(self, queries, min_len)
+
     # ---- persistence (SURVEY 8f-2): the only "wire format" the reference API implies is
     # from_parts/into_parts (src/table.rs:111-127): text bytes + little-endian u32 table.
     def save(self, path: str) -> None:

@@ -114,6 +114,22 @@ for k, docs in enumerate(doc_sets + [[b"ACGT"] * 9000 + [b""]]):
         got = dl.top_documents_batch(qs, kk)
         del os.environ["B200SA_TOPK_ROUND"]
         assert all(np.array_equal(x, y) for x, y in zip(want, got)), (k, kk)
+# matching statistics: both entry points, lengths only, SMEMs with cap too small then sufficient
+ms_qs = [dna[100:180], dna[:40] + b"N" + dna[41:90], b"", b"\x00\x01", b"banana" * 3, bytes(range(256))]
+single = SuffixTable(dna)
+for k, tab in enumerate([single] + [DocumentSuffixTable(docs) for docs in doc_sets]):
+    off, ln, s_, e_ = tab.matching_statistics(ms_qs)
+    assert all(int(a) <= int(b) for a, b in zip(s_, e_)), k
+    so, qpos, sl, _, _ = tab.smems(ms_qs, 2)                       # count call (cap = 0), then the fetch
+    assert len(qpos) == int(so[-1]) and (sl >= 2).all(), k
+blob = torch.from_numpy(np.frombuffer(b"".join(ms_qs), dtype=np.uint8).copy()).cuda()
+d_qo = torch.from_numpy(np.cumsum([0] + [len(q) for q in ms_qs]).astype(np.int64)).cuda()
+d_ln = torch.empty(len(blob), dtype=torch.int32, device="cuda")
+d_t_, d_sa_, _ = single._device_arrays()
+ctx.match_stats_dev(d_t_.data_ptr(), len(dna), d_sa_.data_ptr(), 0, blob.data_ptr(), d_qo.data_ptr(), len(ms_qs),
+                    len(blob), d_ln.data_ptr(), 0, 0, 0)                          # lengths only, no lcp
+torch.cuda.synchronize()
+assert np.array_equal(d_ln.cpu().numpy().view(np.uint32), single.matching_statistics(ms_qs)[1])
 print("sanitize workload ok")
 PY
 for tool in memcheck racecheck; do
