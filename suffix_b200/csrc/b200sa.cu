@@ -376,19 +376,20 @@ static int doubling_rounds(b200sa_ctx *c, uint32_t m, uint32_t na, uint32_t *asu
         uint32_t *Vsorted = nullptr;
         bool sorted_locally = false;
         bool use_local = !first && try_local;
+        const char *how = first ? "radix(kgram)" : (try_local ? "local" : "radix(off)");   // for B200SA_TRACE
         if (use_local) {                        // probe ~4096 elements: are large groups common?
             CU_TRY(c, cudaMemsetAsync(d_na + 24, 0, 16, c->stream));   // [24] overflow, [25] large count, [26] max size
             uint32_t stride = na / 4096u; if (stride < 1) stride = 1;
             uint32_t samples = cdiv(na, stride);
             LAUNCH(c, k_group_probe, cdiv(samples, BLK), KA, na, (uint32_t)b2, stride, d_na + 25);
             TRY(read_words(c, d_na + 25, 2));
-            if (c->h_pin[0] * 20u > samples) use_local = false;   // > 5 % of the elements in big groups: this round only
+            if (c->h_pin[0] * 20u > samples) { use_local = false; how = "radix(probe)"; }   // > 5 % in big groups: this round only
         }
         if (use_local) {                        // tiny groups: rank inside the group by counting
             LAUNCH(c, k_group_local_sort, cdiv(na, BLK), KA, asuf, na, (uint32_t)b2, KB, ascratch, d_na + 24);
             TRY(read_words(c, d_na + 24, 1));
             if (c->h_pin[0] == 0) { K2 = KB; Vsorted = ascratch; sorted_locally = true; }
-            else try_local = false;             // some group is large: radix sort from now on
+            else { try_local = false; how = "radix(overflow)"; }   // some group is large: radix sort from now on
         }
         if (!sorted_locally) TRY(sort_pairs<uint64_t>(c, KA, asuf, KB, ascratch, na, bits, &K2, &Vsorted));
         uint32_t *Vother = (Vsorted == asuf) ? ascratch : asuf;
@@ -398,7 +399,7 @@ static int doubling_rounds(b200sa_ctx *c, uint32_t m, uint32_t na, uint32_t *asu
                                 reinterpret_cast<unsigned long long *>(d_na + 16))));
         TRY(read_words(c, d_na + 16, 1));          // low word of the pair total = number of ambiguous suffixes
         na = c->h_pin[0];
-        if (getenv("B200SA_TRACE")) fprintf(stderr, "[b200sa] doubling round %u: h=%llu -> active %u of %u\n", rounds, (unsigned long long)h, na, m);
+        if (getenv("B200SA_TRACE")) fprintf(stderr, "[b200sa] doubling round %u: h=%llu -> active %u of %u, %s\n", rounds, (unsigned long long)h, na, m, how);
         asuf = Vother; ascratch = Vsorted;
         uint32_t *t = apos; apos = apos_next; apos_next = t;
         agrp = G0;
@@ -444,6 +445,8 @@ static int reduced_sa(b200sa_ctx *c, uint32_t *R, uint32_t m, uint32_t names, ui
         if ((int)k0 * bw > 64) k0 = 64 / bw;
     }
     if (const char *e = getenv("B200SA_K0")) { int v = atoi(e); if (v >= 1 && v * bw <= 64) k0 = (uint32_t)v; }
+    if (getenv("B200SA_TRACE")) fprintf(stderr, "[b200sa] reduced_sa: m=%u names=%u k0=%u bw=%d: %s round-0 keys\n", m, names, k0, bw,
+                                        (int)k0 * bw <= 32 ? "32-bit" : "64-bit");
     uint32_t *Vs;
     uint32_t na = 0;
     if ((int)k0 * bw <= 32) {
@@ -505,6 +508,12 @@ static uint32_t window_chars(uint32_t sigma, int bits, uint64_t *range_out) {
     while (k < cap && r * sigma <= (1ull << 32)) { r *= sigma; k++; }
     *range_out = r;
     return k;
+}
+
+// *done stays false: the caller takes the robust path.  B200SA_TRACE names the reason.
+static int direct_hand_over(const char *why) {
+    if (getenv("B200SA_TRACE")) fprintf(stderr, "[b200sa] direct LMS sort: hand over to the robust path: %s\n", why);
+    return B200SA_OK;
 }
 
 template <int BITS>
@@ -614,14 +623,14 @@ static int lms_direct_sort_t(b200sa_ctx *c, uint32_t n, uint32_t m, uint32_t **l
     const bool force = getenv("B200SA_DIRECT_FORCE") != nullptr;            // experiments: never bail out early
     // the window tells (almost) nothing apart: every suffix has a twin for kc characters -- repeats, not
     // a skewed alphabet (English leaves 99.5 % tied after 5 bytes and still converges in ~10 rounds)
-    if (!force && (uint64_t)na * 1000 > (uint64_t)m * 999 && m > 64) return B200SA_OK;
+    if (!force && (uint64_t)na * 1000 > (uint64_t)m * 999 && m > 64) return direct_hand_over("round1-tied");
     if (na > 0 && !bucketed)     // group id of every tied element = slot of its group's head (the bucket sort writes it)
         TRY((dev_scan<OpMax>(c, InArray{grpA}, OutMaxInPlace{grpA}, na, nullptr)));
     uint64_t h = kc;
     const bool allow_local = getenv("B200SA_NO_LOCAL_SORT") == nullptr;
     const int gbits = 32 + bit_length(m);
     while (na > 0) {
-        if (rounds >= max_rounds) return B200SA_OK;            // still tied: robust path
+        if (rounds >= max_rounds) return direct_hand_over("round-limit");   // still tied: robust path
         rounds++;
         {
             static const char *kNames[] = {"lms_refine2", "lms_refine3", "lms_refine4", "lms_refine5", "lms_refineN"};
@@ -636,6 +645,7 @@ static int lms_direct_sort_t(b200sa_ctx *c, uint32_t n, uint32_t m, uint32_t **l
         const uint32_t span = (uint32_t)(h + kc > 0xffffffffull ? 0xffffffffull : h + kc);
         bool local_ok = false;
         bool try_local = allow_local;
+        const char *how = allow_local ? "local" : "radix(off)";      // for B200SA_TRACE
         if (try_local && na >= (1u << 20)) {    // probe ~4096 elements: counting inside a group is quadratic in its size
                                                 // (a short list is cheap either way: no probe, no extra host round trip)
             CU_TRY(c, cudaMemsetAsync(sm + 24, 0, 16, c->stream));   // [24] overflow, [25] members of big groups, [26] max size
@@ -643,7 +653,7 @@ static int lms_direct_sort_t(b200sa_ctx *c, uint32_t n, uint32_t m, uint32_t **l
             uint32_t samples = cdiv(na, stride);
             LAUNCH(c, k_group_probe, cdiv(samples, BLK), KA, na, 32u, stride, sm + 25);
             TRY(read_words(c, sm + 25, 2));
-            if (c->h_pin[0] * 20u > samples) try_local = false;     // > 5 % of the elements sit in groups of >= 128
+            if (c->h_pin[0] * 20u > samples) { try_local = false; how = "radix(probe)"; }   // > 5 % sit in groups of >= 128
         }
         if (try_local) {                         // tiny groups: rank inside the group by counting
             CU_TRY(c, cudaMemsetAsync(sm + 24, 0, 4, c->stream));
@@ -652,6 +662,7 @@ static int lms_direct_sort_t(b200sa_ctx *c, uint32_t n, uint32_t m, uint32_t **l
                                     OutLmsCompactR{scratch, slotA, Ps, slotB, posB, grpB}, na, d_tot)));
             TRY(read_words(c, sm + 16, 9));          // [0] tied count ... [8] = sm[24] overflow flag
             local_ok = c->h_pin[8] == 0;             // some group larger than the limit: radix sort this round
+            if (!local_ok) how = "radix(overflow)";
         }
         if (!local_ok) {
             TRY(sort_pairs<uint64_t>(c, KA, posA, KB, scratch, na, gbits, &K2, &P2));
@@ -661,9 +672,9 @@ static int lms_direct_sort_t(b200sa_ctx *c, uint32_t n, uint32_t m, uint32_t **l
             TRY(read_words(c, sm + 16, 1));
         }
         uint32_t na_next = c->h_pin[0];
-        if (getenv("B200SA_TRACE")) fprintf(stderr, "[b200sa] direct LMS sort: round %u (h=%llu): %u -> %u tied\n", rounds, (unsigned long long)h, na, na_next);
+        if (getenv("B200SA_TRACE")) fprintf(stderr, "[b200sa] direct LMS sort: round %u (h=%llu): %u -> %u tied, %s\n", rounds, (unsigned long long)h, na, na_next, how);
         // slow convergence on a large residue means long repeats: stop early
-        if (!force && (uint64_t)na_next * 100 > (uint64_t)na * 85 && (uint64_t)na_next * 64 > m) return B200SA_OK;
+        if (!force && (uint64_t)na_next * 100 > (uint64_t)na * 85 && (uint64_t)na_next * 64 > m) return direct_hand_over("no-convergence");
         na = na_next;
         uint32_t *t;
         t = slotA; slotA = slotB; slotB = t;

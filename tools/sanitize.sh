@@ -1,7 +1,8 @@
 #!/bin/bash
 # compute-sanitizer on small builds: every path of round 2 (direct / robust LMS sort, the 2-bit bucket sort and its
 # overflow, both induce kernels with and without cascade steps,
-# fused classifier, sharded world-1 entry points, LCP paths, rows f, the suffix tree, the document suffix array)
+# fused classifier, sharded world-1 entry points, LCP paths, rows f, the suffix tree, the document suffix array,
+# the local-sort overflow, the direct path's probe and 64-bit round-0 keys)
 mkdir -p gpurun_out
 cat > /tmp/san.py <<'PY'
 import sys, os
@@ -130,6 +131,18 @@ ctx.match_stats_dev(d_t_.data_ptr(), len(dna), d_sa_.data_ptr(), 0, blob.data_pt
                     len(blob), d_ln.data_ptr(), 0, 0, 0)                          # lengths only, no lcp
 torch.cuda.synchronize()
 assert np.array_equal(d_ln.cpu().numpy().view(np.uint32), single.matching_statistics(ms_qs)[1])
+# refinement branches (tests/test_gpu_refine.py): a local-sort overflow in round 2 of the direct path, the direct
+# path's probe (2^20 tied after round 1, large groups), 64-bit round-0 keys of the reduced string
+import ctypes
+from tests.test_gpu_refine import motif_copies, probe_text
+from tests.model_u32_sa import u32_sa
+for name, t in (("local_overflow", motif_copies("bytes", 1026, seed=1026)), ("probe", probe_text(150, 7000, seed=150))):
+    assert np.array_equal(ctx.build(t), oracle.sais(t)), name
+R = np.random.default_rng(1).integers(0, 1 << 16, 1 << 20, dtype=np.uint32)
+R[0] = (1 << 16) - 1                             # names = 2^16: 17-bit symbols, two of them per 64-bit key
+out = np.empty(len(R), dtype=np.uint32)
+rc = _lib.lib().b200sa_test_reduced_sa(ctx._h, R.ctypes.data, len(R), 1 << 16, out.ctypes.data, ctypes.byref(ctypes.c_uint32()))
+assert rc == 0 and np.array_equal(out, u32_sa(R)), "reduced_sa 64-bit"
 print("sanitize workload ok")
 PY
 for tool in memcheck racecheck; do
