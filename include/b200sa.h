@@ -384,6 +384,59 @@ int b200sa_smems_dev(b200sa_ctx *ctx, const uint64_t *d_q_off, uint32_t nq, uint
                      const uint32_t *d_len, uint32_t min_len, uint64_t *d_offsets, uint32_t *d_qpos,
                      uint64_t cap, uint64_t *total, void *stream);
 
+/* ---- repeats: what in the text repeats itself (DESIGN.md 6b f-11) ----
+ * Index as for the matching statistics: a text T of n bytes with sa and lcp, or the concatenation C with G,
+ * glcp and doc_starts (pass G as d_sa and glcp as d_lcp).  R is the table, lam its LCP array with
+ * lam[n] := 0, S_p the suffix at p cut at the end of p's document, len(p) = |S_p|, ds(p) and de(p) the start
+ * and end of p's document (0 and n for a single text).  L = min_len >= 1.  The gram at p is S_p[0, L),
+ * defined when len(p) >= L; it never crosses a document end.
+ * 1. Repeat length.  rl[p] = max(lam[r], lam[r+1]) for the rank r with R[r] = p: the largest l such that
+ *    S_p[0, l) is a prefix of S_p' for some p' != p.  rl[p] >= L iff the gram at p occurs elsewhere.
+ * 2. Runs at L.  The maximal rank ranges [a, b), b - a >= 2, with lam[i] >= L for a < i < b.  They
+ *    correspond one to one to the distinct strings of L bytes that occur at least twice, and [a, b) is the
+ *    range b200sa_positions_dev / b200sa_docs_positions_dev return for that string.  first(run) = min R[a..b),
+ *    last(run) = max R[a..b).  Positions are ordered by document, so first lies in the run's lowest document
+ *    and last in its highest.
+ * 3. Flagged positions, by mode (a position outside every run is never flagged):
+ *      B200SA_REPEAT_ANY          p is in a run: the gram at p occurs at another position;
+ *      B200SA_REPEAT_EARLIER      p != first(run): it occurs at a smaller position;
+ *      B200SA_REPEAT_OTHER_DOC    first(run) < ds(p) or last(run) >= de(p): it occurs in a different document;
+ *      B200SA_REPEAT_EARLIER_DOC  first(run) < ds(p): it occurs in a document of smaller index.
+ *    For a single text the two document modes flag nothing by definition and are rejected.
+ * 4. Duplicate spans.  Byte x is covered iff some flagged p has p <= x < p + L.  The spans are the maximal
+ *    intervals [begin, end) of covered bytes with no document start strictly inside: touching intervals of
+ *    one document merge, those of adjacent documents do not.  Each span lies in one document and is at
+ *    least L bytes long.  Spans are reported by ascending begin, in coordinates of the concatenation;
+ *    covered = the number of covered bytes = the sum of end - begin.
+ * The two counting calls follow the listing's protocol: *total (and *covered) are always written; the arrays
+ * are written only when total <= cap, and never past total; cap = 0 (the arrays may then be NULL) counts only.
+ * min_len = 0, an unknown mode, a document mode without doc_starts or a required NULL pointer return
+ * B200SA_ERR_BAD_ARG with a b200sa_last_error detail; doc_starts is checked on the device; n above
+ * B200SA_MAX_N returns B200SA_ERR_TOO_LARGE; n = 0 gives totals 0 without launching; min_len > n is legal and
+ * gives nothing.  sa and lcp must be what the build returned; they are not verified.  The counting calls
+ * synchronise the stream (they read the totals back).  Device workspace per text byte: runs 0, with
+ * first / last 8 or 12; spans 4.25 for ANY, 8.25 for EARLIER and EARLIER_DOC, 12.25 for OTHER_DOC. */
+enum {
+    B200SA_REPEAT_ANY = 0,
+    B200SA_REPEAT_EARLIER = 1,
+    B200SA_REPEAT_OTHER_DOC = 2,
+    B200SA_REPEAT_EARLIER_DOC = 3
+};
+/* rl in text order: d_rl[p], n x u32.  Phase: rep_lens. */
+int b200sa_repeat_lens_dev(b200sa_ctx *ctx, uint64_t n, const uint32_t *d_sa, const uint32_t *d_lcp,
+                           uint32_t *d_rl, void *stream);
+/* The runs at min_len, ascending: d_start[i], d_end[i] and, where non-NULL, d_first[i], d_last[i].
+ * Phases: rep_count, rep_segments (with first / last), rep_emit. */
+int b200sa_repeat_runs_dev(b200sa_ctx *ctx, uint64_t n, const uint32_t *d_sa, const uint32_t *d_lcp,
+                           uint32_t min_len, uint32_t *d_start, uint32_t *d_end, uint32_t *d_first,
+                           uint32_t *d_last, uint64_t cap, uint64_t *total, void *stream);
+/* The spans for `mode`.  d_doc_starts = NULL with ndocs = 0: a single text.  Phases: rep_check (with
+ * documents), rep_segments (every mode but ANY), rep_flag, rep_cover, rep_count, rep_emit. */
+int b200sa_duplicate_spans_dev(b200sa_ctx *ctx, uint64_t n, const uint32_t *d_sa, const uint32_t *d_lcp,
+                               const uint32_t *d_doc_starts, uint32_t ndocs, uint32_t min_len, int mode,
+                               uint32_t *d_begin, uint32_t *d_end, uint64_t cap, uint64_t *total,
+                               uint64_t *covered, void *stream);
+
 /* ---- multi-GPU: communicator + sharded LMS-suffix sort (SURVEY.md 8e, config 5) ----
  * One process (or thread) and one context per GPU.  NCCL is resolved at run time
  * (the copy already loaded in the process, else libnccl.so.2); the single-GPU entry

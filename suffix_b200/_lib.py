@@ -93,6 +93,10 @@ def lib():
         "b200sa_match_stats_dev": ([vp, vp, u64, vp, vp, vp, vp, u32, u64, vp, vp, vp, vp], ci),
         "b200sa_docs_match_stats_dev": ([vp, vp, u64, vp, vp, vp, u32, vp, vp, u32, u64, vp, vp, vp, vp], ci),
         "b200sa_smems_dev": ([vp, vp, u32, u64, vp, u32, vp, vp, u64, ctypes.POINTER(u64), vp], ci),
+        "b200sa_repeat_lens_dev": ([vp, u64, vp, vp, vp, vp], ci),
+        "b200sa_repeat_runs_dev": ([vp, u64, vp, vp, u32, vp, vp, vp, vp, u64, ctypes.POINTER(u64), vp], ci),
+        "b200sa_duplicate_spans_dev": ([vp, u64, vp, vp, vp, u32, u32, ci, vp, vp, u64, ctypes.POINTER(u64),
+                                        ctypes.POINTER(u64), vp], ci),
         "b200sa_last_stats": ([vp, ctypes.POINTER(Stats)], ci),
         "b200sa_set_timing": ([vp, ci], ci),
         "b200sa_last_phase_times": ([vp, ctypes.POINTER(ctypes.c_char_p), ctypes.POINTER(ctypes.c_float), ci], ci),
@@ -336,6 +340,28 @@ class Context:
         self._check(lib().b200sa_smems_dev(self._h, d_qoff, nq, q_bytes, d_len, min_len, d_offsets, d_qpos or None,
                                            cap, ctypes.byref(total), stream))
         return int(total.value)
+
+    def repeat_lens_dev(self, n, d_sa, d_lcp, d_rl, stream: int = 0):
+        """b200sa_repeat_lens_dev: d_rl[p] = the longest prefix of the suffix at p that starts elsewhere too."""
+        self._check(lib().b200sa_repeat_lens_dev(self._h, n, d_sa or None, d_lcp or None, d_rl or None, stream))
+
+    def repeat_runs_dev(self, n, d_sa, d_lcp, min_len, d_start=0, d_end=0, d_first=0, d_last=0, cap=0,
+                        stream: int = 0) -> int:
+        """b200sa_repeat_runs_dev: writes the runs at min_len when they fit in cap.  Returns the total."""
+        total = ctypes.c_uint64(0)
+        self._check(lib().b200sa_repeat_runs_dev(self._h, n, d_sa or None, d_lcp or None, min_len, d_start or None,
+                                                 d_end or None, d_first or None, d_last or None, cap,
+                                                 ctypes.byref(total), stream))
+        return int(total.value)
+
+    def duplicate_spans_dev(self, n, d_sa, d_lcp, d_doc_starts, ndocs, min_len, mode, d_begin=0, d_end=0, cap=0,
+                            stream: int = 0):
+        """b200sa_duplicate_spans_dev: writes the spans when they fit in cap.  Returns (total, covered)."""
+        total, covered = ctypes.c_uint64(0), ctypes.c_uint64(0)
+        self._check(lib().b200sa_duplicate_spans_dev(self._h, n, d_sa or None, d_lcp or None, d_doc_starts or None,
+                                                     ndocs, min_len, mode, d_begin or None, d_end or None, cap,
+                                                     ctypes.byref(total), ctypes.byref(covered), stream))
+        return int(total.value), int(covered.value)
 
     def lcp_sharded(self, d_text: int, n: int, d_sa: int, d_lcp: int, replicated: bool = False, stream: int = 0):
         self._check(lib().b200sa_lcp_sharded(self._h, d_text, n, d_sa, d_lcp, 1 if replicated else 0, stream))

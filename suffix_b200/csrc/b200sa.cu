@@ -32,6 +32,7 @@
 #include "docs_list.cuh"
 #include "docs_topk.cuh"
 #include "match.cuh"
+#include "repeats.cuh"
 #include "nccl_dyn.h"
 
 using namespace b200sa;
@@ -2539,6 +2540,190 @@ int b200sa_smems_dev(b200sa_ctx *c, const uint64_t *d_q_off, uint32_t nq, uint64
         return end_call(c);
     }
     return tree_exit(c, smems_core(c, d_q_off, nq, q_bytes, d_len, min_len, d_offsets, d_qpos, cap, total));
+}
+
+// ------------------------------------------------------------ repeats (DESIGN 6b f-11)
+static int repeat_args(b200sa_ctx *c, uint64_t n, const void *sa, const void *lcp) {
+    if (!c) return B200SA_ERR_BAD_ARG;
+    if (n > 0 && (!sa || !lcp)) {
+        c->last_error = "null pointer";
+        return B200SA_ERR_BAD_ARG;
+    }
+    if (n > B200SA_MAX_N) {
+        c->last_error = "text longer than 2^32-4096 bytes";
+        return B200SA_ERR_TOO_LARGE;
+    }
+    return B200SA_OK;
+}
+
+int b200sa_repeat_lens_dev(b200sa_ctx *c, uint64_t n, const uint32_t *d_sa, const uint32_t *d_lcp, uint32_t *d_rl,
+                           void *stream) {
+    TRY(repeat_args(c, n, d_sa, d_lcp));
+    if (n > 0 && !d_rl) {
+        c->last_error = "null pointer";
+        return B200SA_ERR_BAD_ARG;
+    }
+    CU_TRY(c, cudaSetDevice(c->device));
+    begin_call(c, stream);
+    if (n == 0) return end_call(c);
+    TRY(mark(c, "rep_lens"));
+    LAUNCH(c, k_rep_lens, cdiv(n, BLK), d_sa, d_lcp, (uint32_t)n, d_rl);
+    TRY(mark(c, "end"));
+    CU_TRY(c, cudaGetLastError());
+    return end_call(c);
+}
+
+// seg (p0) and, on request, the smallest (p1) and largest (g0) position of every segment, at its head's slot
+static int repeat_segments(b200sa_ctx *c, uint32_t n, const uint32_t *d_sa, const uint32_t *d_lcp, uint32_t L,
+                           bool want_first, bool want_last) {
+    TRY(ensure(c, c->p0, (size_t)n * 4));
+    uint32_t *seg = ptr<uint32_t>(c->p0);
+    TRY((dev_scan<OpMax>(c, RepSegIn{d_lcp, L}, RepSegOut{seg}, n, nullptr)));
+    if (want_first) {
+        TRY(ensure(c, c->p1, (size_t)n * 4));
+        TRY((dev_scan<OpMax64>(c, RepExtIn<true>{d_sa, seg}, RepExtOut<true>{d_lcp, n, L, ptr<uint32_t>(c->p1)}, n,
+                               nullptr)));
+    }
+    if (want_last) {
+        TRY(ensure(c, c->g0, (size_t)n * 4));
+        TRY((dev_scan<OpMax64>(c, RepExtIn<false>{d_sa, seg}, RepExtOut<false>{d_lcp, n, L, ptr<uint32_t>(c->g0)}, n,
+                               nullptr)));
+    }
+    return B200SA_OK;
+}
+
+// n >= 1.  Phases: rep_count, rep_segments (with first / last), rep_emit.
+static int repeat_runs_core(b200sa_ctx *c, uint32_t n, const uint32_t *d_sa, const uint32_t *d_lcp, uint32_t L,
+                            uint32_t *d_start, uint32_t *d_end, uint32_t *d_first, uint32_t *d_last, uint64_t cap,
+                            uint64_t *total) {
+    TRY(ensure(c, c->small, 4096));
+    uint32_t *d_total = ptr<uint32_t>(c->small) + 2;
+    TRY(mark(c, "rep_count"));
+    TRY((dev_scan<OpSum>(c, RepRunIn{d_lcp, n, L}, RepNoOut{}, n, d_total)));
+    TRY(read_words(c, d_total, 1));
+    *total = c->h_pin[0];
+    if (*total > 0 && *total <= cap) {
+        if (d_first || d_last) {
+            TRY(mark(c, "rep_segments"));
+            TRY(repeat_segments(c, n, d_sa, d_lcp, L, d_first != nullptr, d_last != nullptr));
+        }
+        TRY(mark(c, "rep_emit"));
+        TRY((dev_scan<OpSum>(c, RepRunIn{d_lcp, n, L},
+                             RepRunOut{d_lcp, n, L, d_start, d_end, d_first, d_last, ptr<uint32_t>(c->p1),
+                                       ptr<uint32_t>(c->g0)},
+                             n, nullptr)));
+    }
+    TRY(mark(c, "end"));
+    CU_TRY(c, cudaStreamSynchronize(c->stream));
+    return B200SA_OK;
+}
+
+int b200sa_repeat_runs_dev(b200sa_ctx *c, uint64_t n, const uint32_t *d_sa, const uint32_t *d_lcp, uint32_t min_len,
+                           uint32_t *d_start, uint32_t *d_end, uint32_t *d_first, uint32_t *d_last, uint64_t cap,
+                           uint64_t *total, void *stream) {
+    TRY(repeat_args(c, n, d_sa, d_lcp));
+    if (!total || (cap > 0 && (!d_start || !d_end))) {
+        c->last_error = "null pointer";
+        return B200SA_ERR_BAD_ARG;
+    }
+    if (min_len == 0) {
+        c->last_error = "repeat runs: min_len must be at least 1";
+        return B200SA_ERR_BAD_ARG;
+    }
+    CU_TRY(c, cudaSetDevice(c->device));
+    begin_call(c, stream);
+    *total = 0;
+    if (n == 0) return end_call(c);
+    return tree_exit(c, repeat_runs_core(c, (uint32_t)n, d_sa, d_lcp, min_len, d_start, d_end, d_first, d_last, cap,
+                                         total));
+}
+
+// n >= 1.  Phases: rep_check (with documents), rep_segments (every mode but ANY), rep_flag, rep_cover,
+// rep_count, rep_emit.
+static int duplicate_spans_core(b200sa_ctx *c, uint32_t n, const uint32_t *d_sa, const uint32_t *d_lcp,
+                                const uint32_t *d_starts, uint32_t ndocs, uint32_t L, int mode, uint32_t *d_begin,
+                                uint32_t *d_end, uint64_t cap, uint64_t *total, uint64_t *covered) {
+    TRY(ensure(c, c->small, 4096));
+    uint32_t *words = ptr<uint32_t>(c->small);
+    unsigned long long *d_total = reinterpret_cast<unsigned long long *>(words + 4);
+    if (d_starts) {
+        TRY(mark(c, "rep_check"));
+        CU_TRY(c, cudaMemsetAsync(words, 0, 8, c->stream));
+        LAUNCH(c, k_docs_check, cdiv(ndocs, BLK), d_starts, ndocs, n, words);
+        CU_TRY(c, cudaGetLastError());
+        TRY(read_words(c, words, 1));
+        if (c->h_pin[0]) return docs_bad(c, c->h_pin[0]);
+    }
+    // two bitmaps of n bits, padded to whole words: flagged positions, document starts
+    const size_t bm_words = ((size_t)n + 31) / 32;
+    TRY(ensure(c, c->g1, bm_words * 8));
+    uint32_t *flagged = ptr<uint32_t>(c->g1), *doc_bits = flagged + bm_words;
+    CU_TRY(c, cudaMemsetAsync(flagged, 0, bm_words * 8, c->stream));
+    if (mode != REP_ANY) {
+        TRY(mark(c, "rep_segments"));
+        TRY(repeat_segments(c, n, d_sa, d_lcp, L, true, mode == REP_OTHER_DOC));
+    }
+    TRY(mark(c, "rep_flag"));
+    const uint32_t *seg = ptr<uint32_t>(c->p0), *sf = ptr<uint32_t>(c->p1), *sl = ptr<uint32_t>(c->g0);
+    const uint32_t grid = cdiv(n, BLK);
+    switch (mode) {
+        case REP_ANY: LAUNCH(c, k_rep_flag<REP_ANY>, grid, d_sa, d_lcp, n, L, seg, sf, sl, d_starts, ndocs, flagged); break;
+        case REP_EARLIER: LAUNCH(c, k_rep_flag<REP_EARLIER>, grid, d_sa, d_lcp, n, L, seg, sf, sl, d_starts, ndocs, flagged); break;
+        case REP_OTHER_DOC: LAUNCH(c, k_rep_flag<REP_OTHER_DOC>, grid, d_sa, d_lcp, n, L, seg, sf, sl, d_starts, ndocs, flagged); break;
+        default: LAUNCH(c, k_rep_flag<REP_EARLIER_DOC>, grid, d_sa, d_lcp, n, L, seg, sf, sl, d_starts, ndocs, flagged); break;
+    }
+    if (d_starts) LAUNCH(c, k_rep_doc_bits, cdiv(ndocs, BLK), d_starts, ndocs, n, doc_bits);
+    TRY(mark(c, "rep_cover"));                           // seg is dead: its buffer takes near
+    TRY(ensure(c, c->p0, (size_t)n * 4));
+    uint32_t *near = ptr<uint32_t>(c->p0);
+    TRY((dev_scan<OpMax>(c, RepNearIn{flagged}, RepNearOut{near}, n, nullptr)));
+    TRY(mark(c, "rep_count"));
+    const RepCover C{near, doc_bits, n, L};
+    TRY((dev_scan<OpSum64>(c, RepSpanIn{C}, RepSpanNoOut{}, n, d_total)));
+    TRY(read_words(c, reinterpret_cast<const uint32_t *>(d_total), 2));
+    *covered = c->h_pin[0];
+    *total = c->h_pin[1];
+    if (*total > 0 && *total <= cap) {
+        TRY(mark(c, "rep_emit"));
+        TRY((dev_scan<OpSum64>(c, RepSpanIn{C}, RepSpanOut{C, d_begin, d_end}, n, nullptr)));
+    }
+    TRY(mark(c, "end"));
+    CU_TRY(c, cudaStreamSynchronize(c->stream));
+    return B200SA_OK;
+}
+
+int b200sa_duplicate_spans_dev(b200sa_ctx *c, uint64_t n, const uint32_t *d_sa, const uint32_t *d_lcp,
+                               const uint32_t *d_doc_starts, uint32_t ndocs, uint32_t min_len, int mode,
+                               uint32_t *d_begin, uint32_t *d_end, uint64_t cap, uint64_t *total, uint64_t *covered,
+                               void *stream) {
+    TRY(repeat_args(c, n, d_sa, d_lcp));
+    if (!total || !covered || (cap > 0 && (!d_begin || !d_end)) || (ndocs > 0 && !d_doc_starts)) {
+        c->last_error = "null pointer";
+        return B200SA_ERR_BAD_ARG;
+    }
+    if (min_len == 0) {
+        c->last_error = "duplicate spans: min_len must be at least 1";
+        return B200SA_ERR_BAD_ARG;
+    }
+    if (mode < B200SA_REPEAT_ANY || mode > B200SA_REPEAT_EARLIER_DOC) {
+        c->last_error = "duplicate spans: unknown mode";
+        return B200SA_ERR_BAD_ARG;
+    }
+    if (!d_doc_starts && mode >= B200SA_REPEAT_OTHER_DOC) {
+        c->last_error = "duplicate spans: the document modes need doc_starts";
+        return B200SA_ERR_BAD_ARG;
+    }
+    if (d_doc_starts && ndocs == 0 && n > 0) {
+        c->last_error = "doc_starts rejected: ndocs == 0 with n > 0;";
+        return B200SA_ERR_BAD_ARG;
+    }
+    CU_TRY(c, cudaSetDevice(c->device));
+    begin_call(c, stream);
+    *total = 0;
+    *covered = 0;
+    if (n == 0) return end_call(c);
+    return tree_exit(c, duplicate_spans_core(c, (uint32_t)n, d_sa, d_lcp, d_doc_starts, ndocs, min_len, mode, d_begin,
+                                             d_end, cap, total, covered));
 }
 
 // ------------------------------------------------------------ multi-GPU: communicator + sharded LMS sort

@@ -12,7 +12,7 @@ import bisect
 
 import numpy as np
 
-from . import _lib, _match
+from . import _lib, _match, _repeats
 from .table import _as_bytes, _lock      # the lock of the per-device default context, shared with SuffixTable
 
 MAX_N = 0xFFFFF000        # B200SA_MAX_N
@@ -377,6 +377,42 @@ class DocumentSuffixTable:
         qpos.  start / end feed documents_for_ranges and top_documents_for_ranges as they are."""
         self._device_arrays()
         return _match.smems(self, queries, min_len)
+
+    # ---- repeats (DESIGN 6b f-11)
+    _REPEAT_MODES = ("any", "earlier", "other_document", "earlier_document")
+
+    def _repeat_arrays(self):
+        import torch
+        _, d_g, d_s = self._device_arrays()
+        if self._dev_lcp is None:                 # glcp joins the device copies on first use: 4 bytes per text byte
+            self._dev_lcp = torch.from_numpy(self._lcp.view(np.int32).copy()).to(d_g.device)
+        return d_g, self._dev_lcp, d_s, len(self._starts)
+
+    def repeat_lengths(self) -> np.ndarray:
+        """u32[n]: for every position p of the concatenation, the longest prefix of p's document suffix
+        that also starts at another position, in any document (b200sa_repeat_lens_dev)."""
+        return _repeats.repeat_lengths(self)
+
+    def repeated_substrings(self, min_len, with_ends=False):
+        """The distinct strings of min_len bytes that occur at least twice inside documents, as ranges of
+        the table (b200sa_repeat_runs_dev): (start u32[], end u32[]) in ascending order, or (start, end,
+        first, last) with the smallest and largest position of each.  The ranges feed documents_for_ranges
+        and top_documents_for_ranges as they are."""
+        return _repeats.repeated_substrings(self, min_len, with_ends)
+
+    def duplicate_spans(self, min_len, mode="any") -> np.ndarray:
+        """(document, begin_offset, end_offset) rows, by document and offset: the maximal spans of bytes
+        covered by a flagged position's next min_len bytes; a span never crosses a document end
+        (b200sa_duplicate_spans_dev).  mode: "any" flags every position whose next min_len bytes occur at
+        another position, "earlier" every such occurrence but the first, "other_document" those that
+        occur in a different document, "earlier_document" those that occur in a document of smaller index."""
+        begin, end = _repeats.duplicate_spans(self, min_len, mode, self._REPEAT_MODES)
+        at = self.locate(begin)
+        return np.concatenate([at, (at[:, 1] + (end - begin))[:, None]], axis=1).astype(np.uint32)
+
+    def duplicated_bytes(self, min_len, mode="any") -> int:
+        """The number of bytes duplicate_spans(min_len, mode) covers, without fetching the spans."""
+        return _repeats.duplicated_bytes(self, min_len, mode, self._REPEAT_MODES)
 
     def top_documents(self, query, k) -> np.ndarray:
         """(document, count) rows of the min(k, df) documents that contain `query` most often, by count

@@ -197,6 +197,40 @@ class SuffixTable:
         self._device_arrays()
         return _match.smems(self, queries, min_len)
 
+    # ---- repeats (DESIGN 6b f-11)
+    _REPEAT_MODES = ("any", "earlier")
+
+    def _repeat_arrays(self):
+        _, d_sa, d_lcp = self._device_arrays()
+        return d_sa, d_lcp, None, 0
+
+    def repeat_lengths(self) -> np.ndarray:
+        """u32[n]: for every position p, the longest prefix of text[p:] that also starts at another
+        position (b200sa_repeat_lens_dev).  Uses _device_arrays()."""
+        from . import _repeats
+        return _repeats.repeat_lengths(self)
+
+    def repeated_substrings(self, min_len, with_ends=False):
+        """The distinct strings of min_len bytes that occur at least twice, as ranges of the table
+        (b200sa_repeat_runs_dev): (start u32[], end u32[]) in ascending order, table()[start:end] the
+        occurrences of one string, what positions() returns for it.  with_ends adds (first u32[], last
+        u32[]), the smallest and largest of those positions."""
+        from . import _repeats
+        return _repeats.repeated_substrings(self, min_len, with_ends)
+
+    def duplicate_spans(self, min_len, mode="any"):
+        """(begin u32[], end u32[]): the maximal spans of bytes covered by a flagged position's next
+        min_len bytes, by ascending begin (b200sa_duplicate_spans_dev).  mode "any" flags every position
+        whose next min_len bytes occur at another position, "earlier" every such occurrence but the
+        first."""
+        from . import _repeats
+        return _repeats.duplicate_spans(self, min_len, mode, self._REPEAT_MODES)
+
+    def duplicated_bytes(self, min_len, mode="any") -> int:
+        """The number of bytes duplicate_spans(min_len, mode) covers, without fetching the spans."""
+        from . import _repeats
+        return _repeats.duplicated_bytes(self, min_len, mode, self._REPEAT_MODES)
+
     # ---- persistence (SURVEY 8f-2): the only "wire format" the reference API implies is
     # from_parts/into_parts (src/table.rs:111-127): text bytes + little-endian u32 table.
     def save(self, path: str) -> None:

@@ -131,6 +131,16 @@ ctx.match_stats_dev(d_t_.data_ptr(), len(dna), d_sa_.data_ptr(), 0, blob.data_pt
                     len(blob), d_ln.data_ptr(), 0, 0, 0)                          # lengths only, no lcp
 torch.cuda.synchronize()
 assert np.array_equal(d_ln.cpu().numpy().view(np.uint32), single.matching_statistics(ms_qs)[1])
+# repeats: the three entry points, every mode, count call (cap = 0) then the fetch
+for k, tab in enumerate([single] + [DocumentSuffixTable(docs) for docs in doc_sets]):
+    assert len(tab.repeat_lengths()) == len(tab), k
+    for L in (1, 4, 12):
+        rs, re_, rf, rl_ = tab.repeated_substrings(L, with_ends=True)
+        assert (re_ - rs >= 2).all() and (rf <= rl_).all(), (k, L)
+        for mode in tab._REPEAT_MODES:
+            sp = tab.duplicate_spans(L, mode)
+            width = (sp[1] - sp[0]) if isinstance(sp, tuple) else (sp[:, 2] - sp[:, 1])
+            assert int(width.astype(np.int64).sum()) == tab.duplicated_bytes(L, mode), (k, L, mode)
 # refinement branches (tests/test_gpu_refine.py): a local-sort overflow in round 2 of the direct path, the direct
 # path's probe (2^20 tied after round 1, large groups), 64-bit round-0 keys of the reduced string
 import ctypes
