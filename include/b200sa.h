@@ -437,6 +437,40 @@ int b200sa_duplicate_spans_dev(b200sa_ctx *ctx, uint64_t n, const uint32_t *d_sa
                                uint32_t *d_begin, uint32_t *d_end, uint64_t cap, uint64_t *total,
                                uint64_t *covered, void *stream);
 
+/* ---- longest previous factor and LZ77 factorization (DESIGN.md 6b f-12) ----
+ * Index as for the repeats: R the table (sa, or G for documents: pass G as d_sa and glcp as d_lcp), lam its
+ * LCP array, S_p the suffix at p cut at the end of p's document, positions in coordinates of the text or
+ * of the concatenation, R[r] = p.  No doc_starts is needed: glcp never crosses a document end.
+ * 1. Nearest smaller positions.  psv(r) = the largest r' < r with R[r'] < p, nsv(r) = the smallest r' > r
+ *    with R[r'] < p; either may be absent.  lcp(a, b) = min lam(a, b] for ranks a < b; lL = lcp(psv, r),
+ *    lR = lcp(r, nsv), a missing side counting 0.
+ * 2. LPF.  lpf[p] = max(lL, lR): the largest l such that S_p[0, l) is a prefix of S_q for some q < p;
+ *    the occurrence may overlap p (q + l > p).  (Crochemore & Ilie, IPL 2008.)
+ * 3. Source.  src[p] = R[psv] if lL >= lR and lL > 0, else R[nsv] if lR > 0, else B200SA_LZ_LITERAL.
+ *    The tie goes to the psv side.  src[p] is AN earlier occurrence of S_p[0, lpf[p]), not necessarily the
+ *    leftmost or the closest one.
+ * 4. Factorization.  next(p) = p + max(1, lpf[p]); the factor starts are f_0 = 0 and f_(i+1) = next(f_i)
+ *    while below n.  Factor i is (start = f_i, len = max(1, lpf[f_i]), src = src[f_i]); a literal has
+ *    len = 1 and src = B200SA_LZ_LITERAL, its byte is the text's byte at start.  z = the number of factors.
+ * Properties: lpf[p+1] >= lpf[p] - 1, so next never decreases and next(p) > p; with documents
+ * lpf[p] <= de(p) - p, so no factor crosses a document end and every non-empty document starts a factor:
+ * the document call is the single-text call applied to G and glcp.
+ * b200sa_lz77_dev follows the listing's protocol: *total = z is always written; the arrays are written only
+ * when z <= cap, and never past z; cap = 0 (the arrays may then be NULL) counts only.  A required NULL
+ * pointer returns B200SA_ERR_BAD_ARG; n above B200SA_MAX_N returns B200SA_ERR_TOO_LARGE; n = 0 gives z = 0
+ * without launching.  sa and lcp must be what the build returned; they are not verified.  The
+ * factorization synchronises the stream (it reads z back) and leaves the number of parse rounds,
+ * ceil(log2 z), in b200sa_last_stats().doubling_rounds.  Device workspace per text byte (computed, not
+ * measured): lpf 0.26 (two sets of 32-ary block minima); lz77 16.4 (lpf, src, two jump arrays, a 1-bit
+ * mark and the minima). */
+#define B200SA_LZ_LITERAL 0xFFFFFFFFu
+/* lpf and (when d_src != NULL) src in text order, n x u32 each.  Phases: lz_levels, lz_lpf. */
+int b200sa_lpf_dev(b200sa_ctx *ctx, uint64_t n, const uint32_t *d_sa, const uint32_t *d_lcp, uint32_t *d_lpf,
+                   uint32_t *d_src, void *stream);
+/* The factors by ascending start.  Phases: lz_levels, lz_lpf, lz_parse, lz_count, lz_emit. */
+int b200sa_lz77_dev(b200sa_ctx *ctx, uint64_t n, const uint32_t *d_sa, const uint32_t *d_lcp, uint32_t *d_start,
+                    uint32_t *d_len, uint32_t *d_src, uint64_t cap, uint64_t *total, void *stream);
+
 /* ---- multi-GPU: communicator + sharded LMS-suffix sort (SURVEY.md 8e, config 5) ----
  * One process (or thread) and one context per GPU.  NCCL is resolved at run time
  * (the copy already loaded in the process, else libnccl.so.2); the single-GPU entry

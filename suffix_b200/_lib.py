@@ -97,6 +97,8 @@ def lib():
         "b200sa_repeat_runs_dev": ([vp, u64, vp, vp, u32, vp, vp, vp, vp, u64, ctypes.POINTER(u64), vp], ci),
         "b200sa_duplicate_spans_dev": ([vp, u64, vp, vp, vp, u32, u32, ci, vp, vp, u64, ctypes.POINTER(u64),
                                         ctypes.POINTER(u64), vp], ci),
+        "b200sa_lpf_dev": ([vp, u64, vp, vp, vp, vp, vp], ci),
+        "b200sa_lz77_dev": ([vp, u64, vp, vp, vp, vp, vp, u64, ctypes.POINTER(u64), vp], ci),
         "b200sa_last_stats": ([vp, ctypes.POINTER(Stats)], ci),
         "b200sa_set_timing": ([vp, ci], ci),
         "b200sa_last_phase_times": ([vp, ctypes.POINTER(ctypes.c_char_p), ctypes.POINTER(ctypes.c_float), ci], ci),
@@ -362,6 +364,18 @@ class Context:
                                                      ndocs, min_len, mode, d_begin or None, d_end or None, cap,
                                                      ctypes.byref(total), ctypes.byref(covered), stream))
         return int(total.value), int(covered.value)
+
+    def lpf_dev(self, n, d_sa, d_lcp, d_lpf, d_src=0, stream: int = 0):
+        """b200sa_lpf_dev: d_lpf[p] = the longest previous factor at p, d_src[p] (if given) one earlier start."""
+        self._check(lib().b200sa_lpf_dev(self._h, n, d_sa or None, d_lcp or None, d_lpf or None, d_src or None,
+                                         stream))
+
+    def lz77_dev(self, n, d_sa, d_lcp, d_start=0, d_len=0, d_src=0, cap=0, stream: int = 0) -> int:
+        """b200sa_lz77_dev: writes the factors when they fit in cap.  Returns z."""
+        total = ctypes.c_uint64(0)
+        self._check(lib().b200sa_lz77_dev(self._h, n, d_sa or None, d_lcp or None, d_start or None, d_len or None,
+                                          d_src or None, cap, ctypes.byref(total), stream))
+        return int(total.value)
 
     def lcp_sharded(self, d_text: int, n: int, d_sa: int, d_lcp: int, replicated: bool = False, stream: int = 0):
         self._check(lib().b200sa_lcp_sharded(self._h, d_text, n, d_sa, d_lcp, 1 if replicated else 0, stream))

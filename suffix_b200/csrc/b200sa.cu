@@ -33,6 +33,7 @@
 #include "docs_topk.cuh"
 #include "match.cuh"
 #include "repeats.cuh"
+#include "lz.cuh"
 #include "nccl_dyn.h"
 
 using namespace b200sa;
@@ -1480,14 +1481,14 @@ int b200sa_doc_ids_dev(b200sa_ctx *c, const uint32_t *d_pos, uint64_t count, con
     return end_call(c);
 }
 
-// Block minima of the LCP array over 32^k entries (in c->qbuf) for the ANSV searches.
-static int ansv_levels(b200sa_ctx *c, const uint32_t *d_lcp, uint64_t n, AnsvLevels *L) {
+// Block minima of an array (the LCP array, or any other) over 32^k entries, in `buf`, for the ANSV searches.
+static int ansv_levels(b200sa_ctx *c, const uint32_t *d_lcp, uint64_t n, AnsvLevels *L, DevBuf &buf) {
     memset(L, 0, sizeof *L);
     L->lv[0] = d_lcp; L->cnt[0] = n; L->nlev = 1;
     uint64_t total = 0;
     for (uint64_t k = (n + 31) / 32; ; k = (k + 31) / 32) { total += k; if (k <= 32) break; }
-    TRY(ensure(c, c->qbuf, (total + 64) * 4));
-    uint32_t *lvbuf = ptr<uint32_t>(c->qbuf);
+    TRY(ensure(c, buf, (total + 64) * 4));
+    uint32_t *lvbuf = ptr<uint32_t>(buf);
     uint64_t cnt = n;
     while (cnt > 32 && L->nlev < 8) {
         uint64_t nxt = (cnt + 31) / 32;
@@ -1507,7 +1508,7 @@ int b200sa_lcp_intervals_dev(b200sa_ctx *c, const uint32_t *d_lcp, uint64_t n, u
     begin_call(c, stream);
     if (n == 0) return end_call(c);
     AnsvLevels L;
-    TRY(ansv_levels(c, d_lcp, n, &L));
+    TRY(ansv_levels(c, d_lcp, n, &L, c->qbuf));
     LAUNCH(c, k_ansv, cdiv(n, BLK), L, n, d_psv, d_nsv);
     CU_TRY(c, cudaGetLastError());
     return end_call(c);
@@ -1549,7 +1550,7 @@ static int suffix_tree_core(b200sa_ctx *c, uint32_t n, const uint32_t *d_sa, con
     uint32_t *words = ptr<uint32_t>(c->small);          // [0] nodes below the root, [1] check bits
     TRY(mark(c, "tree_ansv"));
     AnsvLevels L;
-    TRY(ansv_levels(c, d_lcp, n, &L));
+    TRY(ansv_levels(c, d_lcp, n, &L, c->qbuf));
     LAUNCH(c, k_tree_ansv, cdiv(n, BLK), L, (uint64_t)n, psv, nsv, rep);
     TRY(mark(c, "tree_emit"));
     CU_TRY(c, cudaMemsetAsync(words, 0, 8, c->stream));
@@ -1778,7 +1779,7 @@ static int docs_core(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const uin
     uint32_t *rem = ptr<uint32_t>(c->isa), *pre = ptr<uint32_t>(c->rank), *list = ptr<uint32_t>(c->p0);
     TRY((dev_scan<OpSum>(c, DocsSplitIn{sa, lcp, d_starts, ndocs, n, rem}, DocsSplitOut{pre, list, n}, n, words)));
     AnsvLevels L;
-    TRY(ansv_levels(c, lcp, n, &L));
+    TRY(ansv_levels(c, lcp, n, &L, c->qbuf));
     TRY(read_words(c, words, 1));
     const uint32_t na = c->h_pin[0];
 
@@ -1963,7 +1964,7 @@ static int docs_tree_core(b200sa_ctx *c, uint32_t n, const uint32_t *d_g, const 
     // terminals
     TRY(mark(c, "dtree_term"));
     AnsvLevels L;
-    TRY(ansv_levels(c, d_glcp, n, &L));
+    TRY(ansv_levels(c, d_glcp, n, &L, c->qbuf));
     CU_TRY(c, cudaMemsetAsync(words + 2, 0, 4, c->stream));
     CU_TRY(c, cudaMemcpyAsync(out->term_end, t.sa_lo, (size_t)N * 4, cudaMemcpyDeviceToDevice, c->stream));
     LAUNCH(c, k_dtree_term, cdiv(n, BLK), L, len, n, K, first, N, B, out->term_end, words + 2);
@@ -2162,7 +2163,7 @@ static int docs_list_front(b200sa_ctx *c, uint32_t n, const uint32_t *d_g, const
     u64 *d_items = reinterpret_cast<u64 *>(words + 2), *d_total = reinterpret_cast<u64 *>(words + 4);
     TRY(mark(c, "dlist_levels"));
     DListArgs A;
-    TRY(ansv_levels(c, d_prev, n, &A.L));
+    TRY(ansv_levels(c, d_prev, n, &A.L, c->qbuf));
     TRY(mark(c, "dlist_count"));
     CU_TRY(c, cudaMemsetAsync(words, 0, 24, c->stream));
     TRY(ensure(c, c->k64a, ((size_t)nq + 1) * 8));
@@ -2442,7 +2443,7 @@ static int match_stats_core(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, co
     memset(&L, 0, sizeof L);
     if (d_start) {
         TRY(mark(c, "match_levels"));
-        TRY(ansv_levels(c, d_lcp, n, &L));
+        TRY(ansv_levels(c, d_lcp, n, &L, c->qbuf));
         TRY(mark(c, "match_search"));
         LAUNCH(c, (k_match_stats<EndF, true>), grid, T, n, d_sa, L, Q, d_q_off, nq, q_bytes, d_len, d_start, d_end, end);
     } else {
@@ -2724,6 +2725,89 @@ int b200sa_duplicate_spans_dev(b200sa_ctx *c, uint64_t n, const uint32_t *d_sa, 
     if (n == 0) return end_call(c);
     return tree_exit(c, duplicate_spans_core(c, (uint32_t)n, d_sa, d_lcp, d_doc_starts, ndocs, min_len, mode, d_begin,
                                              d_end, cap, total, covered));
+}
+
+// ------------------------------------------------------------ longest previous factor and LZ77 (DESIGN 6b f-12)
+// n >= 1: the block minima of R (qbuf) and of lam (isa), then lpf / src.  Phases: lz_levels, lz_lpf.
+static int lz_lpf_core(b200sa_ctx *c, uint32_t n, const uint32_t *d_sa, const uint32_t *d_lcp, uint32_t *d_lpf,
+                       uint32_t *d_src) {
+    AnsvLevels LR, LL;
+    TRY(mark(c, "lz_levels"));
+    TRY(ansv_levels(c, d_sa, n, &LR, c->qbuf));
+    TRY(ansv_levels(c, d_lcp, n, &LL, c->isa));
+    TRY(mark(c, "lz_lpf"));
+    LAUNCH(c, k_lz_lpf, cdiv(n, BLK), LR, LL, n, d_lpf, d_src);
+    CU_TRY(c, cudaGetLastError());
+    return B200SA_OK;
+}
+
+int b200sa_lpf_dev(b200sa_ctx *c, uint64_t n, const uint32_t *d_sa, const uint32_t *d_lcp, uint32_t *d_lpf,
+                   uint32_t *d_src, void *stream) {
+    TRY(repeat_args(c, n, d_sa, d_lcp));
+    if (n > 0 && !d_lpf) {
+        c->last_error = "null pointer";
+        return B200SA_ERR_BAD_ARG;
+    }
+    CU_TRY(c, cudaSetDevice(c->device));
+    begin_call(c, stream);
+    if (n == 0) return end_call(c);
+    int rc = lz_lpf_core(c, (uint32_t)n, d_sa, d_lcp, d_lpf, d_src);
+    if (rc == B200SA_OK) rc = mark(c, "end");
+    return tree_exit(c, rc);
+}
+
+// n >= 1.  lpf (p0), src (p1), the jump arrays J (g0, g1: n + 1 each), the mark bitmap (v0).  Phases:
+// lz_levels, lz_lpf, lz_parse, lz_count, lz_emit.
+static int lz77_core(b200sa_ctx *c, uint32_t n, const uint32_t *d_sa, const uint32_t *d_lcp, uint32_t *d_start,
+                     uint32_t *d_len, uint32_t *d_src, uint64_t cap, uint64_t *total) {
+    const uint32_t nwords = (uint32_t)(((uint64_t)n + 31) / 32);
+    TRY(ensure(c, c->p0, (size_t)n * 4));
+    TRY(ensure(c, c->p1, (size_t)n * 4));
+    TRY(ensure(c, c->g0, ((size_t)n + 1) * 4));
+    TRY(ensure(c, c->g1, ((size_t)n + 1) * 4));
+    TRY(ensure(c, c->v0, (size_t)nwords * 4));
+    TRY(ensure(c, c->small, 4096));
+    uint32_t *lpf = ptr<uint32_t>(c->p0), *src = ptr<uint32_t>(c->p1), *marks = ptr<uint32_t>(c->v0);
+    uint32_t *J[2] = {ptr<uint32_t>(c->g0), ptr<uint32_t>(c->g1)};
+    uint32_t *state = ptr<uint32_t>(c->small) + 8, *d_total = state + 2;   // done, rounds, z
+    TRY(lz_lpf_core(c, n, d_sa, d_lcp, lpf, src));
+    TRY(mark(c, "lz_parse"));
+    CU_TRY(c, cudaMemsetAsync(marks, 0, (size_t)nwords * 4, c->stream));
+    CU_TRY(c, cudaMemsetAsync(state, 0, 8, c->stream));
+    LAUNCH(c, k_lz_next, cdiv((uint64_t)n + 1, BLK), lpf, n, J[0], marks);
+    int cur = 0;
+    for (uint32_t b = n; b; b >>= 1, cur ^= 1) {         // bit_length(n) >= ceil(log2 z) rounds
+        LAUNCH(c, k_lz_mark, cdiv(nwords, BLK), J[cur], n, marks, nwords, state);
+        LAUNCH(c, k_lz_square, cdiv((uint64_t)n + 1, BLK), J[cur], n, J[cur ^ 1], state);
+    }
+    TRY(mark(c, "lz_count"));
+    TRY((dev_scan<OpSum>(c, InPopcWords{marks}, LzNoOut{}, nwords, d_total)));
+    CU_TRY(c, cudaGetLastError());
+    TRY(read_words(c, state + 1, 2));
+    c->stats.doubling_rounds = c->h_pin[0];
+    *total = c->h_pin[1];
+    if (*total > 0 && *total <= cap) {
+        TRY(mark(c, "lz_emit"));
+        TRY((dev_scan<OpSum>(c, InPopcWords{marks}, LzEmitOut{marks, lpf, src, d_start, d_len, d_src}, nwords,
+                             nullptr)));
+    }
+    TRY(mark(c, "end"));
+    CU_TRY(c, cudaStreamSynchronize(c->stream));
+    return B200SA_OK;
+}
+
+int b200sa_lz77_dev(b200sa_ctx *c, uint64_t n, const uint32_t *d_sa, const uint32_t *d_lcp, uint32_t *d_start,
+                    uint32_t *d_len, uint32_t *d_src, uint64_t cap, uint64_t *total, void *stream) {
+    TRY(repeat_args(c, n, d_sa, d_lcp));
+    if (!total || (cap > 0 && (!d_start || !d_len || !d_src))) {
+        c->last_error = "null pointer";
+        return B200SA_ERR_BAD_ARG;
+    }
+    CU_TRY(c, cudaSetDevice(c->device));
+    begin_call(c, stream);
+    *total = 0;
+    if (n == 0) return end_call(c);
+    return tree_exit(c, lz77_core(c, (uint32_t)n, d_sa, d_lcp, d_start, d_len, d_src, cap, total));
 }
 
 // ------------------------------------------------------------ multi-GPU: communicator + sharded LMS sort

@@ -12,7 +12,7 @@ import bisect
 
 import numpy as np
 
-from . import _lib, _match, _repeats
+from . import _lib, _lz, _match, _repeats
 from .table import _as_bytes, _lock      # the lock of the per-device default context, shared with SuffixTable
 
 MAX_N = 0xFFFFF000        # B200SA_MAX_N
@@ -413,6 +413,25 @@ class DocumentSuffixTable:
     def duplicated_bytes(self, min_len, mode="any") -> int:
         """The number of bytes duplicate_spans(min_len, mode) covers, without fetching the spans."""
         return _repeats.duplicated_bytes(self, min_len, mode, self._REPEAT_MODES)
+
+    # ---- longest previous factor and LZ77 (DESIGN 6b f-12)
+    def longest_previous_factors(self):
+        """(lpf u32[n], src u32[n]) over the concatenation: lpf[p] is the longest prefix of p's document
+        suffix that also starts at some q < p, in p's document or an earlier one (the occurrence may
+        overlap p); src[p] is one such q, 0xFFFFFFFF where lpf[p] = 0 (b200sa_lpf_dev).  No factor
+        crosses a document end."""
+        return _lz.longest_previous_factors(self)
+
+    def lz77_factors(self, *, _cap_guess=None):
+        """(start u32[z], length u32[z], source u32[z]): the LZ77 factorization of the collection, with
+        sources in any earlier position (b200sa_lz77_dev).  Positions are in coordinates of the
+        concatenation, locate() maps them to (document, offset); every non-empty document starts a factor
+        and no factor crosses a document end.  A literal has length 1 and source 0xFFFFFFFF."""
+        return _lz.lz77_factors(self, _cap_guess)
+
+    def lz77_count(self) -> int:
+        """z, the number of LZ77 factors, without fetching them."""
+        return _lz.lz77_count(self)
 
     def top_documents(self, query, k) -> np.ndarray:
         """(document, count) rows of the min(k, df) documents that contain `query` most often, by count

@@ -231,6 +231,27 @@ class SuffixTable:
         from . import _repeats
         return _repeats.duplicated_bytes(self, min_len, mode, self._REPEAT_MODES)
 
+    # ---- longest previous factor and LZ77 (DESIGN 6b f-12)
+    def longest_previous_factors(self):
+        """(lpf u32[n], src u32[n]): lpf[p] is the longest prefix of text[p:] that also starts at some
+        q < p (the occurrence may overlap p); src[p] is one such q, 0xFFFFFFFF where lpf[p] = 0
+        (b200sa_lpf_dev).  src is an earlier occurrence, not necessarily the leftmost or the closest."""
+        from . import _lz
+        return _lz.longest_previous_factors(self)
+
+    def lz77_factors(self, *, _cap_guess=None):
+        """(start u32[z], length u32[z], source u32[z]): the LZ77 factorization of the text, the greedy
+        parse by longest previous factors (b200sa_lz77_dev).  A factor of length l at start copies
+        text[source:source + l] (source < start, the copy may overlap); a literal has length 1 and
+        source 0xFFFFFFFF and stands for the byte text[start]."""
+        from . import _lz
+        return _lz.lz77_factors(self, _cap_guess)
+
+    def lz77_count(self) -> int:
+        """z, the number of LZ77 factors, without fetching them."""
+        from . import _lz
+        return _lz.lz77_count(self)
+
     # ---- persistence (SURVEY 8f-2): the only "wire format" the reference API implies is
     # from_parts/into_parts (src/table.rs:111-127): text bytes + little-endian u32 table.
     def save(self, path: str) -> None:

@@ -141,6 +141,11 @@ for k, tab in enumerate([single] + [DocumentSuffixTable(docs) for docs in doc_se
             sp = tab.duplicate_spans(L, mode)
             width = (sp[1] - sp[0]) if isinstance(sp, tuple) else (sp[:, 2] - sp[:, 1])
             assert int(width.astype(np.int64).sum()) == tab.duplicated_bytes(L, mode), (k, L, mode)
+# LZ77: lpf, the count call (cap = 0) then the fetch, on the single text and every document set
+for k, tab in enumerate([single] + [DocumentSuffixTable(docs) for docs in doc_sets]):
+    lpf, src = tab.longest_previous_factors()
+    fs, fl, fq = tab.lz77_factors()
+    assert len(fs) == tab.lz77_count() and int(fl.astype(np.int64).sum()) == len(tab), k
 # refinement branches (tests/test_gpu_refine.py): a local-sort overflow in round 2 of the direct path, the direct
 # path's probe (2^20 tied after round 1, large groups), 64-bit round-0 keys of the reduced string
 import ctypes
