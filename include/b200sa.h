@@ -471,6 +471,47 @@ int b200sa_lpf_dev(b200sa_ctx *ctx, uint64_t n, const uint32_t *d_sa, const uint
 int b200sa_lz77_dev(b200sa_ctx *ctx, uint64_t n, const uint32_t *d_sa, const uint32_t *d_lcp, uint32_t *d_start,
                     uint32_t *d_len, uint32_t *d_src, uint64_t cap, uint64_t *total, void *stream);
 
+/* ---- Burrows-Wheeler transform and its inverse (DESIGN.md 6b f-13) ----
+ * Documents D_0 .. D_(k-1), k >= 1, with concatenation C (n bytes) and doc_starts as b200sa_docs_build takes
+ * them; empty documents are allowed.  A single text is k = 1, doc_starts = [0], G = SA.
+ * 1. Rows.  There are n + k rows.  Row d < k is the rotation $_d D_d.  Row k + r is the rotation that starts
+ *    at position G[r] of its document d: C[G[r], end_d) $_d D_d[0, G[r] - start_d).  The terminators order
+ *    as $_0 < $_1 < ... < every byte: G's order with the k terminator rows placed first.
+ * 2. L.  L[d] is the last byte of D_d, or $_d when D_d is empty.  L[k + r] is C[G[r] - 1], or $_d when G[r]
+ *    is the start of its document d (with several empty documents at one offset, the last one owns it).
+ * 3. Output.  bwt = the n bytes of L in row order with the k terminators removed; term_rows[d] = the row
+ *    whose L is $_d (distinct, not sorted by d).  For a single text term_rows[0] is the primary index,
+ *    1 + the rank of position 0.
+ * 4. Runs.  r = the number of maximal runs of equal symbols in the full L of n + k symbols; every
+ *    terminator is a symbol of its own.
+ * 5. Inverse.  psi(d) = term_rows[d] for d < k; the non-terminator rows of L, stably sorted by byte: the
+ *    j-th is psi(k + j) and its byte is F[k + j].  Document d is the bytes F along psi from row d, until the
+ *    walk returns to a row below k.
+ * 6. Validity.  (bwt, term_rows) is the image of some documents exactly when the term rows are in range
+ *    and distinct, and following psi from every row d < k returns to d without meeting another row below
+ *    k, these k cycles covering all n + k rows.
+ * A required NULL pointer, doc_starts that fails the b200sa_docs_build checks (checked on the device),
+ * d_doc_starts with ndocs = 0 and n > 0, and on the inverse ndocs = 0, term rows out of range or repeated or
+ * an input that breaks the validity rule return B200SA_ERR_BAD_ARG with a b200sa_last_error detail; the
+ * inverse then writes no byte and no start.  n + k above B200SA_MAX_N returns B200SA_ERR_TOO_LARGE before
+ * any launch.  n = 0 writes the k term rows and no bytes.  sa / G must be what the build returned; they are
+ * not verified.  The inverse ranks psi with rulers: the rows below k and rows picked by a hash of the row
+ * index, one in s (B200SA_BWT_RULER, default 64; a spacing above n leaves the terminator rows alone); it
+ * leaves its pointer-doubling rounds in b200sa_last_stats().doubling_rounds.  Device workspace per text
+ * byte (computed from the buffers, not measured): forward 1.13 (L bytes and a 1-bit terminator flag);
+ * inverse 20.25 + at most 28 / s (sorted bytes and indices and the sort's key copy 12, psi and F 8, the ruler bitmap
+ * and its prefix 0.25; per ruler its row, walk length and two list entries), plus 16 per document. */
+/* d_doc_starts = NULL with ndocs = 0: a single text (k = 1).  d_sa is SA, or G for documents.  runs may be
+ * NULL; if it is not, the call reads r back and synchronises.  Writes d_bwt (n bytes) and d_term_rows (k).
+ * Phases: bwt_check (with documents), bwt_gather, bwt_compact. */
+int b200sa_bwt_dev(b200sa_ctx *ctx, uint64_t n, const uint8_t *d_text, const uint32_t *d_sa,
+                   const uint32_t *d_doc_starts, uint32_t ndocs, uint8_t *d_bwt, uint32_t *d_term_rows,
+                   uint64_t *runs, void *stream);
+/* k = ndocs >= 1.  Writes C (n bytes) and, when d_doc_starts_out != NULL, doc_starts (k entries).
+ * Synchronises: it reads the validity word back.  Phases: unbwt_sort, unbwt_walk, unbwt_rank, unbwt_emit. */
+int b200sa_unbwt_dev(b200sa_ctx *ctx, uint64_t n, uint32_t ndocs, const uint8_t *d_bwt,
+                     const uint32_t *d_term_rows, uint8_t *d_text_out, uint32_t *d_doc_starts_out, void *stream);
+
 /* ---- multi-GPU: communicator + sharded LMS-suffix sort (SURVEY.md 8e, config 5) ----
  * One process (or thread) and one context per GPU.  NCCL is resolved at run time
  * (the copy already loaded in the process, else libnccl.so.2); the single-GPU entry

@@ -99,6 +99,8 @@ def lib():
                                         ctypes.POINTER(u64), vp], ci),
         "b200sa_lpf_dev": ([vp, u64, vp, vp, vp, vp, vp], ci),
         "b200sa_lz77_dev": ([vp, u64, vp, vp, vp, vp, vp, u64, ctypes.POINTER(u64), vp], ci),
+        "b200sa_bwt_dev": ([vp, u64, vp, vp, vp, u32, vp, vp, ctypes.POINTER(u64), vp], ci),
+        "b200sa_unbwt_dev": ([vp, u64, u32, vp, vp, vp, vp, vp], ci),
         "b200sa_last_stats": ([vp, ctypes.POINTER(Stats)], ci),
         "b200sa_set_timing": ([vp, ci], ci),
         "b200sa_last_phase_times": ([vp, ctypes.POINTER(ctypes.c_char_p), ctypes.POINTER(ctypes.c_float), ci], ci),
@@ -376,6 +378,20 @@ class Context:
         self._check(lib().b200sa_lz77_dev(self._h, n, d_sa or None, d_lcp or None, d_start or None, d_len or None,
                                           d_src or None, cap, ctypes.byref(total), stream))
         return int(total.value)
+
+    def bwt_dev(self, n, d_text, d_sa, d_doc_starts, ndocs, d_bwt, d_term_rows, runs=False, stream: int = 0):
+        """b200sa_bwt_dev: writes the bwt (n bytes) and the term rows; d_doc_starts = 0 with ndocs = 0 is a single
+        text.  Returns r when runs is true (the call then synchronises), else None."""
+        r = ctypes.c_uint64(0)
+        self._check(lib().b200sa_bwt_dev(self._h, n, d_text or None, d_sa or None, d_doc_starts or None, ndocs,
+                                         d_bwt or None, d_term_rows or None, ctypes.byref(r) if runs else None,
+                                         stream))
+        return int(r.value) if runs else None
+
+    def unbwt_dev(self, n, ndocs, d_bwt, d_term_rows, d_text, d_doc_starts=0, stream: int = 0):
+        """b200sa_unbwt_dev: writes the documents' concatenation (n bytes) and, if given, their starts (ndocs)."""
+        self._check(lib().b200sa_unbwt_dev(self._h, n, ndocs, d_bwt or None, d_term_rows or None, d_text or None,
+                                           d_doc_starts or None, stream))
 
     def lcp_sharded(self, d_text: int, n: int, d_sa: int, d_lcp: int, replicated: bool = False, stream: int = 0):
         self._check(lib().b200sa_lcp_sharded(self._h, d_text, n, d_sa, d_lcp, 1 if replicated else 0, stream))

@@ -34,6 +34,7 @@
 #include "match.cuh"
 #include "repeats.cuh"
 #include "lz.cuh"
+#include "bwt.cuh"
 #include "nccl_dyn.h"
 
 using namespace b200sa;
@@ -2808,6 +2809,188 @@ int b200sa_lz77_dev(b200sa_ctx *c, uint64_t n, const uint32_t *d_sa, const uint3
     *total = 0;
     if (n == 0) return end_call(c);
     return tree_exit(c, lz77_core(c, (uint32_t)n, d_sa, d_lcp, d_start, d_len, d_src, cap, total));
+}
+
+// ------------------------------------------------------------ Burrows-Wheeler transform (DESIGN 6b f-13)
+// nrows = n + k >= 1, k >= 1.  The gather (the L bytes in flag, the terminator bitmap in v0), then the
+// compaction.  Phases: bwt_check (with documents), bwt_gather, bwt_compact (n > 0).
+static int bwt_core(b200sa_ctx *c, uint32_t n, const uint8_t *d_text, const uint32_t *d_sa, const uint32_t *d_starts,
+                    uint32_t k, uint8_t *d_bwt, uint32_t *d_term_rows, uint64_t *runs) {
+    const uint32_t nrows = n + k, nwords = cdiv(nrows, 32);
+    TRY(ensure(c, c->small, 4096));
+    uint32_t *words = ptr<uint32_t>(c->small);
+    unsigned long long *d_runs = reinterpret_cast<unsigned long long *>(words + 4);
+    if (d_starts) {
+        TRY(mark(c, "bwt_check"));
+        CU_TRY(c, cudaMemsetAsync(words, 0, 8, c->stream));
+        LAUNCH(c, k_docs_check, cdiv(k, BLK), d_starts, k, n, words);
+        CU_TRY(c, cudaGetLastError());
+        TRY(read_words(c, words, 1));
+        if (c->h_pin[0]) return docs_bad(c, c->h_pin[0]);
+    }
+    TRY(ensure(c, c->flag, nrows));
+    TRY(ensure(c, c->v0, (size_t)nwords * 4));
+    uint8_t *lbyte = ptr<uint8_t>(c->flag);
+    uint32_t *term_bm = ptr<uint32_t>(c->v0);
+    TRY(mark(c, "bwt_gather"));
+    if (runs) CU_TRY(c, cudaMemsetAsync(d_runs, 0, 8, c->stream));
+    LAUNCH(c, k_bwt_gather, cdiv(nrows, BLK), BwtRows{d_text, d_sa, d_starts, n, k}, nrows, lbyte, term_bm, d_term_rows,
+           runs ? d_runs : (unsigned long long *)nullptr);
+    if (n > 0) {
+        TRY(mark(c, "bwt_compact"));
+        TRY((dev_scan<OpSum>(c, InPopcWords{term_bm}, BwtCompactOut{term_bm, lbyte, d_bwt, nrows}, nwords, nullptr)));
+    }
+    TRY(mark(c, "end"));
+    CU_TRY(c, cudaGetLastError());
+    if (runs) {
+        TRY(read_words(c, reinterpret_cast<const uint32_t *>(d_runs), 2));
+        *runs = c->h_pin[0] | ((uint64_t)c->h_pin[1] << 32);
+    }
+    return B200SA_OK;
+}
+
+int b200sa_bwt_dev(b200sa_ctx *c, uint64_t n, const uint8_t *d_text, const uint32_t *d_sa, const uint32_t *d_doc_starts,
+                   uint32_t ndocs, uint8_t *d_bwt, uint32_t *d_term_rows, uint64_t *runs, void *stream) {
+    if (!c) return B200SA_ERR_BAD_ARG;
+    const uint64_t k = d_doc_starts ? ndocs : 1;
+    if ((n > 0 && (!d_text || !d_sa || !d_bwt)) || (k > 0 && !d_term_rows) || (ndocs > 0 && !d_doc_starts)) {
+        c->last_error = "null pointer";
+        return B200SA_ERR_BAD_ARG;
+    }
+    if (k == 0 && n > 0) {
+        c->last_error = "doc_starts rejected: ndocs == 0 with n > 0;";
+        return B200SA_ERR_BAD_ARG;
+    }
+    if (n + k > B200SA_MAX_N) {
+        c->last_error = "bwt: text and terminators above 2^32-4096 rows";
+        return B200SA_ERR_TOO_LARGE;
+    }
+    CU_TRY(c, cudaSetDevice(c->device));
+    begin_call(c, stream);
+    if (runs) *runs = 0;
+    if (k == 0) return end_call(c);                      // no documents: no rows
+    return tree_exit(c, bwt_core(c, (uint32_t)n, d_text, d_sa, d_doc_starts, (uint32_t)k, d_bwt, d_term_rows, runs));
+}
+
+extern "C++" {
+// The stable sorts of the inverse: the term rows (bits wide) or the bwt bytes (8 bits), by index.
+template <class KeyF>
+static int unbwt_sort(b200sa_ctx *c, KeyF kf, DevBuf &ka, DevBuf &va, DevBuf &kb, DevBuf &vb, uint32_t cnt, int bits,
+                      uint32_t **kout, uint32_t **vout) {
+    TRY(ensure(c, ka, (size_t)cnt * 4));
+    TRY(ensure(c, va, (size_t)cnt * 4));
+    TRY(ensure(c, kb, (size_t)cnt * 4));
+    if (bits > 8) TRY(ensure(c, vb, (size_t)cnt * 4));    // one pass never writes vb
+    uint32_t *a = ptr<uint32_t>(ka), *v = ptr<uint32_t>(va), *b = ptr<uint32_t>(kb), *w = ptr<uint32_t>(vb);
+    if (cnt >= (1u << 20) && !getenv("B200SA_SORT_NARROW"))
+        return sort_pairs_from<uint32_t, KeyF, LoadIndex, 16>(c, kf, LoadIndex{}, a, v, b, w, cnt, bits, kout, vout);
+    return sort_pairs_from<uint32_t, KeyF, LoadIndex, ITEMS>(c, kf, LoadIndex{}, a, v, b, w, cnt, bits, kout, vout);
+}
+}  // extern "C++"
+
+constexpr uint32_t BWT_RULER_DEFAULT = 64;
+
+// k >= 1.  Buffers: the sorted term rows (g0, g1, p1, rank: k entries), the sorted bytes (v0, v1, p0: n
+// entries), psi / F (k64a: n + k u64), the ruler bitmap and its word prefix (isa), the ruler rows (qbuf),
+// walk lengths (p0), the list (k64b, v0: two u64 per ruler), document starts (g1).  Phases: unbwt_sort,
+// unbwt_walk, unbwt_rank, unbwt_emit.
+static int unbwt_core(b200sa_ctx *c, uint32_t n, uint32_t k, const uint8_t *d_bwt, const uint32_t *d_term_rows,
+                      uint8_t *d_text, uint32_t *d_starts_out) {
+    const uint32_t nrows = n + k, nwords = cdiv(nrows, 32);
+    TRY(ensure(c, c->small, 4096));
+    // [0] check bits, [1] longest walk, [2, 4) rows covered (u64), [4] rulers, [8, 41) rounds that moved
+    uint32_t *words = ptr<uint32_t>(c->small) + 16;
+    CU_TRY(c, cudaMemsetAsync(words, 0, 48 * 4, c->stream));
+
+    // 1. psi and F
+    TRY(mark(c, "unbwt_sort"));
+    uint32_t *ts, *tv, *fk = nullptr, *fu = nullptr;
+    TRY(unbwt_sort(c, LoadArr<uint32_t>{d_term_rows}, c->g0, c->g1, c->p1, c->rank, k, bit_length(nrows - 1), &ts,
+                   &tv));
+    LAUNCH(c, k_bwt_terms_check, cdiv(k, BLK), ts, k, nrows, words);
+    CU_TRY(c, cudaGetLastError());
+    TRY(read_words(c, words, 1));
+    if (c->h_pin[0]) {
+        c->last_error = "unbwt: term_rows out of range or repeated";
+        return B200SA_ERR_BAD_ARG;
+    }
+    if (n > 0) TRY(unbwt_sort(c, BwtByteKey{d_bwt}, c->v0, c->v1, c->p0, c->p0, n, 8, &fk, &fu));
+    TRY(ensure(c, c->k64a, (size_t)nrows * 8));
+    unsigned long long *pf = ptr<unsigned long long>(c->k64a);
+    LAUNCH(c, k_bwt_psi, cdiv(nrows, BLK), d_term_rows, ts, k, fk, fu, nrows, pf);
+
+    // 2. rulers and their walks
+    TRY(mark(c, "unbwt_walk"));
+    uint32_t s = BWT_RULER_DEFAULT;
+    if (const char *e = getenv("B200SA_BWT_RULER")) { long v = atol(e); if (v >= 1) s = v > 0xffffffffL ? 0xffffffffu : (uint32_t)v; }
+    const BwtRuler isr{k, s, s <= n};
+    TRY(ensure(c, c->isa, (size_t)nwords * 8));
+    uint32_t *rbm = ptr<uint32_t>(c->isa), *wpre = rbm + nwords;
+    LAUNCH(c, k_bwt_ruler_bits, cdiv(nrows, BLK), isr, nrows, rbm);
+    TRY((dev_scan<OpSum>(c, InPopcWords{rbm}, OutStoreExcl{wpre}, nwords, words + 4)));
+    TRY(read_words(c, words + 4, 1));
+    const uint32_t m = c->h_pin[0];
+    TRY(ensure(c, c->qbuf, (size_t)m * 4));
+    TRY(ensure(c, c->p0, (size_t)m * 4));
+    TRY(ensure(c, c->k64b, (size_t)m * 8));
+    TRY(ensure(c, c->v0, (size_t)m * 8));
+    uint32_t *rrow = ptr<uint32_t>(c->qbuf), *steps = ptr<uint32_t>(c->p0);
+    unsigned long long *nv = ptr<unsigned long long>(c->k64b), *nv2 = ptr<unsigned long long>(c->v0);
+    LAUNCH(c, k_bwt_ruler_list, cdiv(nwords, BLK), rbm, wpre, nwords, rrow);
+    LAUNCH(c, k_bwt_walk, cdiv(m, BLK), pf, isr, rrow, rbm, wpre, m, nv, steps, words);
+
+    // 3. ranking and the validity check
+    TRY(mark(c, "unbwt_rank"));
+    const int R = bit_length(m);                          // >= ceil(log2 m): every list of rulers is ranked
+    for (int r = 0; r < R; r++) {
+        LAUNCH(c, k_bwt_jump, cdiv(m, BLK), nv, m, k, nv2, words + 8, (uint32_t)r);
+        std::swap(nv, nv2);
+    }
+    LAUNCH(c, k_bwt_valid, cdiv(m, BLK), nv, steps, m, k, reinterpret_cast<unsigned long long *>(words + 2), words);
+    CU_TRY(c, cudaGetLastError());
+    TRY(read_words(c, words, 8 + R));
+    const uint64_t covered = c->h_pin[2] | ((uint64_t)c->h_pin[3] << 32);
+    uint32_t rounds = 0;
+    for (int r = 0; r < R; r++) rounds += c->h_pin[8 + r] ? 1u : 0u;
+    c->stats.doubling_rounds = rounds;
+    if (getenv("B200SA_TRACE"))
+        fprintf(stderr, "[b200sa] unbwt: n=%u k=%u spacing=%u rulers=%u longest walk=%u rank rounds=%u\n", n, k, s, m,
+                c->h_pin[1], rounds);
+    if (c->h_pin[0] || covered != nrows) {
+        c->last_error = "unbwt: (bwt, term_rows) is not the transform of any documents";
+        return B200SA_ERR_BAD_ARG;
+    }
+
+    // 4. document starts, then every ruler writes its segment
+    TRY(mark(c, "unbwt_emit"));
+    TRY(ensure(c, c->g1, (size_t)k * 4));
+    uint32_t *starts = ptr<uint32_t>(c->g1);
+    TRY((dev_scan<OpSum>(c, BwtLenIn{nv}, BwtStartsOut{starts, d_starts_out}, k, nullptr)));
+    if (n > 0) LAUNCH(c, k_bwt_emit, cdiv(m, BLK), pf, rrow, steps, nv, starts, m, k, d_text);
+    TRY(mark(c, "end"));
+    CU_TRY(c, cudaGetLastError());
+    CU_TRY(c, cudaStreamSynchronize(c->stream));
+    return B200SA_OK;
+}
+
+int b200sa_unbwt_dev(b200sa_ctx *c, uint64_t n, uint32_t ndocs, const uint8_t *d_bwt, const uint32_t *d_term_rows,
+                     uint8_t *d_text_out, uint32_t *d_doc_starts_out, void *stream) {
+    if (!c) return B200SA_ERR_BAD_ARG;
+    if (!d_term_rows || (n > 0 && (!d_bwt || !d_text_out))) {
+        c->last_error = "null pointer";
+        return B200SA_ERR_BAD_ARG;
+    }
+    if (ndocs == 0) {
+        c->last_error = "unbwt: ndocs must be at least 1";
+        return B200SA_ERR_BAD_ARG;
+    }
+    if (n + ndocs > B200SA_MAX_N) {
+        c->last_error = "unbwt: text and terminators above 2^32-4096 rows";
+        return B200SA_ERR_TOO_LARGE;
+    }
+    CU_TRY(c, cudaSetDevice(c->device));
+    begin_call(c, stream);
+    return tree_exit(c, unbwt_core(c, (uint32_t)n, ndocs, d_bwt, d_term_rows, d_text_out, d_doc_starts_out));
 }
 
 // ------------------------------------------------------------ multi-GPU: communicator + sharded LMS sort

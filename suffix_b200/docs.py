@@ -12,7 +12,7 @@ import bisect
 
 import numpy as np
 
-from . import _lib, _lz, _match, _repeats
+from . import _bwt, _lib, _lz, _match, _repeats
 from .table import _as_bytes, _lock      # the lock of the per-device default context, shared with SuffixTable
 
 MAX_N = 0xFFFFF000        # B200SA_MAX_N
@@ -432,6 +432,24 @@ class DocumentSuffixTable:
     def lz77_count(self) -> int:
         """z, the number of LZ77 factors, without fetching them."""
         return _lz.lz77_count(self)
+
+    # ---- Burrows-Wheeler transform (DESIGN 6b f-13)
+    def _bwt_arrays(self):
+        d_t, d_g, d_s = self._device_arrays()
+        return d_t, d_g, d_s, len(self._starts)
+
+    def bwt(self):
+        """(bwt bytes[n], term_rows u32[k]): the multi-string Burrows-Wheeler transform of the documents, each
+        ended by a terminator of its own, $_0 < $_1 < ... < every byte (b200sa_bwt_dev).  The rows are the k
+        terminator rows followed by table()'s order; bwt holds the n bytes of L with the terminators left
+        out, term_rows[d] the row whose L is $_d.  suffix_b200.inverse_bwt_documents(bwt, term_rows) gives
+        the documents back."""
+        return _bwt.bwt(self)
+
+    def bwt_runs(self) -> int:
+        """r, the number of maximal runs of equal symbols in the transform's n + k symbols; every terminator
+        is a symbol of its own."""
+        return _bwt.bwt_runs(self)
 
     def top_documents(self, query, k) -> np.ndarray:
         """(document, count) rows of the min(k, df) documents that contain `query` most often, by count

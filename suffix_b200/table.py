@@ -252,6 +252,33 @@ class SuffixTable:
         from . import _lz
         return _lz.lz77_count(self)
 
+    # ---- Burrows-Wheeler transform (DESIGN 6b f-13)
+    def _bwt_arrays(self):
+        """Device copies of the text and the table: those of _device_arrays() when they exist, else made
+        on first use without the LCP array and kept while the table lives (5 bytes per text byte)."""
+        if getattr(self, "_dev", None) is not None:
+            return self._dev[0], self._dev[1], None, 0
+        if getattr(self, "_dev_bwt", None) is None:
+            import torch
+            dev = torch.device("cuda", self._device)
+            up = lambda a: torch.from_numpy(a.copy()).to(dev)
+            self._dev_bwt = (up(np.frombuffer(self._text or b"\0", dtype=np.uint8)),
+                             up(np.ascontiguousarray(self._table, dtype=np.uint32).view(np.int32)))
+        return self._dev_bwt[0], self._dev_bwt[1], None, 0
+
+    def bwt(self):
+        """(bwt bytes[n], primary): the Burrows-Wheeler transform of text + $, with $ below every byte and
+        left out of the bytes; primary is the row of $, 1 + the rank of position 0 (b200sa_bwt_dev).
+        suffix_b200.inverse_bwt(bwt, primary) gives the text back."""
+        from . import _bwt
+        b, term = _bwt.bwt(self)
+        return b, int(term[0])
+
+    def bwt_runs(self) -> int:
+        """r, the number of maximal runs of equal symbols in the transform's n + 1 symbols, $ included."""
+        from . import _bwt
+        return _bwt.bwt_runs(self)
+
     # ---- persistence (SURVEY 8f-2): the only "wire format" the reference API implies is
     # from_parts/into_parts (src/table.rs:111-127): text bytes + little-endian u32 table.
     def save(self, path: str) -> None:

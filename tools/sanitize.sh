@@ -146,6 +146,16 @@ for k, tab in enumerate([single] + [DocumentSuffixTable(docs) for docs in doc_se
     lpf, src = tab.longest_previous_factors()
     fs, fl, fq = tab.lz77_factors()
     assert len(fs) == tab.lz77_count() and int(fl.astype(np.int64).sum()) == len(tab), k
+# BWT: the forward (with r) and the inverse on the single text and every document set, at the default ruler
+# spacing and at forced ones (every row a ruler, one in three, the terminator rows alone)
+from suffix_b200 import inverse_bwt_documents
+for k, tab in enumerate([single] + [DocumentSuffixTable(docs) for docs in doc_sets]):
+    b, t = tab.bwt()
+    assert tab.bwt_runs() >= 1, k
+    for sp in (None, 1, 3, len(tab) + 1):
+        if sp: os.environ["B200SA_BWT_RULER"] = str(sp)
+        assert b"".join(inverse_bwt_documents(b, t)) == tab.text(), (k, sp)
+        os.environ.pop("B200SA_BWT_RULER", None)
 # refinement branches (tests/test_gpu_refine.py): a local-sort overflow in round 2 of the direct path, the direct
 # path's probe (2^20 tied after round 1, large groups), 64-bit round-0 keys of the reduced string
 import ctypes
