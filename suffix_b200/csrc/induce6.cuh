@@ -27,6 +27,7 @@ namespace b200sa {
 struct Ind6Shared {
     unsigned long long wtot[2][NWARP];   // per-warp packed totals, double buffered over tiles
     uint32_t cbase[4];                   // running destination position per code (inside the bucket part)
+    uint32_t sbase[2][4];                // per tile and code: SA slot of staged item 0, double buffered over tiles
     uint32_t ctot[4];                    // step totals per code
     uint32_t code_of[256];
     uint32_t nsig;
@@ -499,11 +500,10 @@ __device__ __noinline__ void induce6_big_step(const InduceArgs &A, IndShared &sh
     __syncthreads();
     IND_MARK(3)
     if (tb0 < tb1) {
-        uint32_t rb0 = s4.cbase[0], rb1 = s4.cbase[1], rb2 = s4.cbase[2], rb3 = s4.cbase[3];
-        const uint32_t bs0 = SPASS ? sh.bstart[sh.alpha[0] + 1] - 1u : sh.bstart[sh.alpha[0]];
-        const uint32_t bs1 = SPASS ? sh.bstart[sh.alpha[1] + 1] - 1u : sh.bstart[sh.alpha[1]];
-        const uint32_t bs2 = SPASS ? sh.bstart[sh.alpha[2] + 1] - 1u : sh.bstart[sh.alpha[2]];
-        const uint32_t bs3 = SPASS ? sh.bstart[sh.alpha[3] + 1] - 1u : sh.bstart[sh.alpha[3]];
+        // the running position of code q lives in s4.cbase[q] (thread q alone advances it); per tile thread
+        // q leaves the slot of staged item 0 of its code in s4.sbase, so the store loop keeps no bases in
+        // registers
+        const uint32_t bsq = tid < 4 ? (SPASS ? sh.bstart[sh.alpha[tid] + 1] - 1u : sh.bstart[sh.alpha[tid]]) : 0u;
         uint32_t s_cur[ITEMS], s_nxt[ITEMS], p_cur[4], p_nxt[4] = {0, 0, 0, 0};
         ind6_load8(src, chunk_of(tb0), limit, s_cur);
         load_carry8(pc, chunk_of(tb0), limit, p_cur);
@@ -554,6 +554,12 @@ __device__ __noinline__ void induce6_big_step(const InduceArgs &A, IndShared &sh
             const uint32_t o1 = t0c, o2 = t0c + t1c, o3 = o2 + t2c, oall = o3 + t3c;
             uint32_t e0 = (uint32_t)(exc & 0xffffu), e1 = o1 + (uint32_t)((exc >> 16) & 0xffffu);
             uint32_t e2 = o2 + (uint32_t)((exc >> 32) & 0xffffu), e3 = o3 + (uint32_t)((exc >> 48) & 0xffffu);
+            if (tid < 4) {      // item j of code q (staged at o_q + i) goes to position cbase[q] + i
+                const uint32_t oq = tid == 0 ? 0u : tid == 1 ? o1 : tid == 2 ? o2 : o3;
+                const uint32_t rb = s4.cbase[tid];
+                s4.sbase[par][tid] = SPASS ? bsq - rb + oq : bsq + rb - oq;
+                s4.cbase[tid] = rb + (uint32_t)((ttot >> (16 * tid)) & 0xffffu);
+            }
             uint16_t *stage_c = reinterpret_cast<uint16_t *>(sh.rl);
 #pragma unroll
             for (int ii = 0; ii < ITEMS; ii++) {
@@ -571,17 +577,12 @@ __device__ __noinline__ void induce6_big_step(const InduceArgs &A, IndShared &sh
             }
             __syncthreads();
             for (uint32_t j = tid; j < oall; j += BLK) {
-                uint32_t pos, bs;
-                if (j < o1) { pos = rb0 + j; bs = bs0; }
-                else if (j < o2) { pos = rb1 + (j - o1); bs = bs1; }
-                else if (j < o3) { pos = rb2 + (j - o2); bs = bs2; }
-                else { pos = rb3 + (j - o3); bs = bs3; }
-                uint32_t slot = SPASS ? bs - pos : bs + pos;
+                const uint32_t q = (j >= o1) + (j >= o2) + (j >= o3);
+                const uint32_t sb = s4.sbase[par][q];
+                uint32_t slot = SPASS ? sb - j : sb + j;
                 A.sa[slot] = sh.ent[j];
                 pc_sa[slot] = stage_c[j];
             }
-            rb0 += (uint32_t)(ttot & 0xffffu); rb1 += (uint32_t)((ttot >> 16) & 0xffffu);
-            rb2 += (uint32_t)((ttot >> 32) & 0xffffu); rb3 += (uint32_t)((ttot >> 48) & 0xffffu);
             par ^= 1u;
 #pragma unroll
             for (int i = 0; i < ITEMS; i++) s_cur[i] = s_nxt[i];
