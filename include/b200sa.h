@@ -512,6 +512,49 @@ int b200sa_bwt_dev(b200sa_ctx *ctx, uint64_t n, const uint8_t *d_text, const uin
 int b200sa_unbwt_dev(b200sa_ctx *ctx, uint64_t n, uint32_t ndocs, const uint8_t *d_bwt,
                      const uint32_t *d_term_rows, uint8_t *d_text_out, uint32_t *d_doc_starts_out, void *stream);
 
+/* ---- approximate positions: occurrences with at most k mismatches (DESIGN.md 6b f-14) ----
+ * Index: a text T of n bytes with its sa, or the documents' concatenation C with G and doc_starts as
+ * b200sa_docs_build_dev takes and returns them.  No LCP array is needed.  end(p) = n for a single text, or
+ * the end of p's document.  Query q is bytes [q_off[q], q_off[q+1]) of d_queries, m bytes of any values.
+ * One threshold k, 0 <= k <= B200SA_APPROX_MAX_K, holds for the whole call.
+ * An occurrence of q is a position p with
+ *   1. p + m <= end(p): the window never crosses the text end or a document end;
+ *   2. mis(p) = #{x < m : T[p+x] != q[x]} <= k.
+ * m = 0 has no occurrences (b"" matches nothing, as for b200sa_positions_dev).  When 0 < m <= k every window
+ * of m bytes is an occurrence.  For k = 0 the occurrences are the positions of table[start, end) that
+ * b200sa_positions_dev / b200sa_docs_positions_dev return, in ascending order.
+ * Output follows the listing's protocol: d_offsets (nq + 1 x u64, exclusive) and *total = offsets[nq] are
+ * always written; d_pos[offsets[q], offsets[q+1]) holds query q's occurrences in ascending p, and
+ * d_mismatches (may be NULL) mis(p) beside them, written only when total <= cap and never past total.
+ * cap = 0 (d_pos may then be NULL) counts only.
+ * Method: pigeonhole filter and verification.  When m > k the query is cut into k + 1 pieces,
+ * piece j = [j*m/(k+1), (j+1)*m/(k+1)); a window with at most k mismatches matches some piece exactly.  Each
+ * rank of the table range of piece j is a candidate, verified against the other pieces; it is reported only
+ * when no piece before j matches exactly, so every occurrence is reported once, by its first exact piece.
+ * A required NULL pointer, k > B200SA_APPROX_MAX_K, a bad q_off (q_off[0] != 0 or not ascending; checked on
+ * the device, q_off[nq] is read back as the queries' length) and, for documents, doc_starts that fails the
+ * b200sa_docs_build checks (on the device) or ndocs = 0 with n > 0 return B200SA_ERR_BAD_ARG with a
+ * b200sa_last_error detail.  n or q_off[nq] above B200SA_MAX_N, or nq * (k + 1) >= 2^32 - 1, return
+ * B200SA_ERR_TOO_LARGE.  nq = 0 writes offsets[0] = 0 and total = 0; n = 0 gives empty lists without launching
+ * a search kernel.  sa / G must be what the build returned; they are not verified.  No byte outside
+ * [d_text, d_text + n) and [d_queries, d_queries + q_off[nq]) is read: the buffers need no padding and no
+ * alignment.  Synchronises the stream (it reads the total back).  Device workspace (computed from the
+ * buffers, not measured): 16 bytes per piece (nq * (k + 1) pieces), 12 bytes per candidate chunk (1024 ranks
+ * of a piece's range, or of the whole table for a query of 0 < m <= k), and, when the occurrences are
+ * fetched, 24 bytes per output entry plus the radix sort's tile status (at most 1 byte per entry).
+ * B200SA_ERR_OOM when that cannot be allocated.  Phases: approx_check, approx_pieces, approx_scan,
+ * approx_count, approx_emit, approx_sort (the last two only when total <= cap and total > 0). */
+#define B200SA_APPROX_MAX_K 31
+int b200sa_approx_positions_dev(b200sa_ctx *ctx, const uint8_t *d_text, uint64_t n, const uint32_t *d_sa,
+                                const uint8_t *d_queries, const uint64_t *d_q_off, uint32_t nq, uint32_t k,
+                                uint64_t *d_offsets, uint32_t *d_pos, uint32_t *d_mismatches, uint64_t cap,
+                                uint64_t *total, void *stream);
+int b200sa_docs_approx_positions_dev(b200sa_ctx *ctx, const uint8_t *d_text, uint64_t n, const uint32_t *d_gsa,
+                                     const uint32_t *d_doc_starts, uint32_t ndocs, const uint8_t *d_queries,
+                                     const uint64_t *d_q_off, uint32_t nq, uint32_t k, uint64_t *d_offsets,
+                                     uint32_t *d_pos, uint32_t *d_mismatches, uint64_t cap, uint64_t *total,
+                                     void *stream);
+
 /* ---- multi-GPU: communicator + sharded LMS-suffix sort (SURVEY.md 8e, config 5) ----
  * One process (or thread) and one context per GPU.  NCCL is resolved at run time
  * (the copy already loaded in the process, else libnccl.so.2); the single-GPU entry

@@ -1,0 +1,65 @@
+"""Approximate positions (occurrences with at most k mismatches) over a device-resident table: the part
+SuffixTable and DocumentSuffixTable share.  A table supplies `_device` and `_bwt_arrays()` -> (d_text,
+d_table, d_doc_starts or None, ndocs), its text and table on the device; the LCP array is not needed."""
+import numpy as np
+
+from . import _lib
+from .table import _as_bytes, _lock
+
+MAX_K = 31                # B200SA_APPROX_MAX_K
+
+
+def _call(table, queries, k, fetch):
+    """(offsets u64[nq + 1], positions u32[], mismatches u32[]); positions and mismatches are None without
+    fetch (the cap = 0 call)."""
+    import torch
+    k = int(k)
+    if not 0 <= k <= MAX_K:
+        raise ValueError("k must be in 0 .. %d, got %d" % (MAX_K, k))
+    qs = [_as_bytes(q) for q in queries]
+    nq, n = len(qs), len(table)
+    d_t, d_r, d_s, ndocs = table._bwt_arrays()
+    dev = torch.device("cuda", table._device)
+    off = np.zeros(nq + 1, dtype=np.uint64)
+    off[1:] = np.cumsum([len(q) for q in qs])
+    d_q = torch.from_numpy(np.frombuffer(b"".join(qs) or b"\0", dtype=np.uint8).copy()).to(dev)
+    d_off = torch.from_numpy(off.view(np.int64)).to(dev)
+    d_o = torch.zeros(nq + 1, dtype=torch.int64, device=dev)
+    ctx = _lib.default_context(table._device)
+    stream = torch.cuda.current_stream(dev).cuda_stream
+
+    def call(cap, d_pos=0, d_mis=0):
+        if d_s is None:
+            return ctx.approx_positions_dev(d_t.data_ptr(), n, d_r.data_ptr(), d_q.data_ptr(), d_off.data_ptr(), nq,
+                                            k, d_o.data_ptr(), d_pos, d_mis, cap, stream)
+        return ctx.docs_approx_positions_dev(d_t.data_ptr(), n, d_r.data_ptr(), d_s.data_ptr(), ndocs,
+                                             d_q.data_ptr(), d_off.data_ptr(), nq, k, d_o.data_ptr(), d_pos, d_mis,
+                                             cap, stream)
+
+    pos = mis = None
+    with _lock:                                   # count, then fetch into buffers of that size
+        total = call(0)
+        if fetch:
+            pos = torch.empty(max(total, 1), dtype=torch.int32, device=dev)
+            mis = torch.empty(max(total, 1), dtype=torch.int32, device=dev)
+            if total:
+                call(total, pos.data_ptr(), mis.data_ptr())
+    torch.cuda.synchronize(dev)
+    offsets = d_o.cpu().numpy().view(np.uint64)
+    if not fetch:
+        return offsets, None, None
+    return offsets, pos[:total].cpu().numpy().view(np.uint32), mis[:total].cpu().numpy().view(np.uint32)
+
+
+def positions_batch(table, queries, k):
+    return _call(table, queries, k, True)
+
+
+def positions(table, query, k):
+    _, pos, mis = _call(table, [query], k, True)
+    return pos, mis
+
+
+def counts(table, queries, k):
+    off, _, _ = _call(table, queries, k, False)
+    return np.diff(off.astype(np.int64)).astype(np.uint64)

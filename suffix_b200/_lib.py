@@ -101,6 +101,10 @@ def lib():
         "b200sa_lz77_dev": ([vp, u64, vp, vp, vp, vp, vp, u64, ctypes.POINTER(u64), vp], ci),
         "b200sa_bwt_dev": ([vp, u64, vp, vp, vp, u32, vp, vp, ctypes.POINTER(u64), vp], ci),
         "b200sa_unbwt_dev": ([vp, u64, u32, vp, vp, vp, vp, vp], ci),
+        "b200sa_approx_positions_dev": ([vp, vp, u64, vp, vp, vp, u32, u32, vp, vp, vp, u64, ctypes.POINTER(u64), vp],
+                                        ci),
+        "b200sa_docs_approx_positions_dev": ([vp, vp, u64, vp, vp, u32, vp, vp, u32, u32, vp, vp, vp, u64,
+                                              ctypes.POINTER(u64), vp], ci),
         "b200sa_last_stats": ([vp, ctypes.POINTER(Stats)], ci),
         "b200sa_set_timing": ([vp, ci], ci),
         "b200sa_last_phase_times": ([vp, ctypes.POINTER(ctypes.c_char_p), ctypes.POINTER(ctypes.c_float), ci], ci),
@@ -392,6 +396,26 @@ class Context:
         """b200sa_unbwt_dev: writes the documents' concatenation (n bytes) and, if given, their starts (ndocs)."""
         self._check(lib().b200sa_unbwt_dev(self._h, n, ndocs, d_bwt or None, d_term_rows or None, d_text or None,
                                            d_doc_starts or None, stream))
+
+    def approx_positions_dev(self, d_text, n, d_sa, d_q, d_qoff, nq, k, d_offsets, d_pos=0, d_mis=0, cap=0,
+                             stream: int = 0) -> int:
+        """b200sa_approx_positions_dev: writes the offsets, and the positions (and mismatches, if given) of the
+        occurrences with at most k mismatches when they fit in cap.  Returns the total."""
+        total = ctypes.c_uint64(0)
+        self._check(lib().b200sa_approx_positions_dev(self._h, d_text or None, n, d_sa or None, d_q or None,
+                                                      d_qoff or None, nq, k, d_offsets or None, d_pos or None,
+                                                      d_mis or None, cap, ctypes.byref(total), stream))
+        return int(total.value)
+
+    def docs_approx_positions_dev(self, d_text, n, d_gsa, d_doc_starts, ndocs, d_q, d_qoff, nq, k, d_offsets,
+                                  d_pos=0, d_mis=0, cap=0, stream: int = 0) -> int:
+        """b200sa_docs_approx_positions_dev: the same over G, no window crossing a document end."""
+        total = ctypes.c_uint64(0)
+        self._check(lib().b200sa_docs_approx_positions_dev(self._h, d_text or None, n, d_gsa or None,
+                                                           d_doc_starts or None, ndocs, d_q or None, d_qoff or None,
+                                                           nq, k, d_offsets or None, d_pos or None, d_mis or None,
+                                                           cap, ctypes.byref(total), stream))
+        return int(total.value)
 
     def lcp_sharded(self, d_text: int, n: int, d_sa: int, d_lcp: int, replicated: bool = False, stream: int = 0):
         self._check(lib().b200sa_lcp_sharded(self._h, d_text, n, d_sa, d_lcp, 1 if replicated else 0, stream))

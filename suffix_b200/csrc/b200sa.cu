@@ -35,6 +35,7 @@
 #include "repeats.cuh"
 #include "lz.cuh"
 #include "bwt.cuh"
+#include "approx.cuh"
 #include "nccl_dyn.h"
 
 using namespace b200sa;
@@ -2991,6 +2992,166 @@ int b200sa_unbwt_dev(b200sa_ctx *c, uint64_t n, uint32_t ndocs, const uint8_t *d
     CU_TRY(c, cudaSetDevice(c->device));
     begin_call(c, stream);
     return tree_exit(c, unbwt_core(c, (uint32_t)n, ndocs, d_bwt, d_term_rows, d_text_out, d_doc_starts_out));
+}
+
+// ------------------------------------------------------------ approximate positions (DESIGN 6b f-14)
+extern "C++" {
+// nq >= 1, k <= B200SA_APPROX_MAX_K; d_starts non-null for documents (EndF = DocsEnd).  Phases: approx_check,
+// approx_pieces, approx_scan, approx_count, and approx_emit, approx_sort when the occurrences fit in cap.
+template <class EndF>
+static int approx_core(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const uint32_t *d_sa,
+                       const uint32_t *d_starts, uint32_t ndocs, const uint8_t *d_queries, const uint64_t *d_q_off,
+                       uint32_t nq, uint32_t k, uint64_t *d_offsets, uint32_t *d_pos, uint32_t *d_mis, uint64_t cap,
+                       uint64_t *total, EndF end) {
+    typedef unsigned long long u64;
+    TRY(mark(c, "approx_check"));
+    TRY(ensure(c, c->small, 4096));
+    uint32_t *words = ptr<uint32_t>(c->small);           // [0] check bits, [2, 4) items, [4, 6) total
+    CU_TRY(c, cudaMemcpyAsync(c->h_pin, d_q_off + nq, 8, cudaMemcpyDeviceToHost, c->stream));
+    CU_TRY(c, cudaStreamSynchronize(c->stream));
+    const uint64_t q_bytes = c->h_pin[0] | ((uint64_t)c->h_pin[1] << 32);
+    TRY(match_check(c, d_q_off, nq, q_bytes));           // q_off[0] = 0 and ascending
+    if (d_starts && ndocs > 0) {
+        CU_TRY(c, cudaMemsetAsync(words, 0, 8, c->stream));
+        LAUNCH(c, k_docs_check, cdiv(ndocs, BLK), d_starts, ndocs, n, words);
+        CU_TRY(c, cudaGetLastError());
+        TRY(read_words(c, words, 1));
+        if (c->h_pin[0]) return docs_bad(c, c->h_pin[0]);
+    }
+    if (q_bytes > B200SA_MAX_N) {
+        c->last_error = "queries longer than 2^32-4096 bytes";
+        return B200SA_ERR_TOO_LARGE;
+    }
+    if (q_bytes > 0 && !d_queries) {
+        c->last_error = "null pointer";
+        return B200SA_ERR_BAD_ARG;
+    }
+    const uint32_t P = k + 1;
+    const uint64_t nslots = (uint64_t)nq * P;
+    if (nslots >= 0xFFFFFFFFull) {
+        c->last_error = "approx positions: nq * (k + 1) of 2^32 - 1 or more slots";
+        return B200SA_ERR_TOO_LARGE;
+    }
+    if (n == 0) {                                        // nothing occurs
+        CU_TRY(c, cudaMemsetAsync(d_offsets, 0, ((size_t)nq + 1) * 8, c->stream));
+        TRY(mark(c, "end"));
+        CU_TRY(c, cudaStreamSynchronize(c->stream));
+        return B200SA_OK;
+    }
+    TRY(mark(c, "approx_pieces"));
+    TRY(ensure(c, c->p1, (size_t)nslots * 8));
+    uint32_t *ps = ptr<uint32_t>(c->p1), *pe = ps + nslots;
+    LAUNCH(c, (k_approx_pieces<EndF>), cdiv(nslots, BLK), d_text, n, d_sa, d_queries, d_q_off, nq, P, ps, pe, end);
+    TRY(mark(c, "approx_scan"));
+    CU_TRY(c, cudaMemsetAsync(words, 0, 24, c->stream));
+    TRY(ensure(c, c->k64a, ((size_t)nslots + 1) * 8));
+    u64 *item_start = ptr<u64>(c->k64a), *d_items = reinterpret_cast<u64 *>(words + 2),
+        *d_total = reinterpret_cast<u64 *>(words + 4);
+    TRY((dev_scan<OpSum64>(c, DListChunks{ps, pe, (uint32_t)nslots, n, words}, OutStoreExcl64{item_start},
+                           nslots + 1, d_items)));
+    TRY(read_words(c, words + 2, 2));
+    const uint64_t items = c->h_pin[0] | ((uint64_t)c->h_pin[1] << 32);
+    if (items > (uint64_t)0x7fffffff * NWARP) {
+        c->last_error = "approx positions: more than 2^31 * 8 chunks of 1024 candidates in one batch";
+        return B200SA_ERR_TOO_LARGE;
+    }
+    TRY(mark(c, "approx_count"));
+    TRY(ensure(c, c->p0, (size_t)items * 4));
+    TRY(ensure(c, c->k64b, ((size_t)items + 1) * 8));
+    uint32_t *cnt = ptr<uint32_t>(c->p0);
+    u64 *item_off = ptr<u64>(c->k64b);
+    const ApproxArgs A{d_text, d_sa, d_starts, ndocs, n, d_queries, d_q_off, (uint32_t)nslots, P, k, ps, pe,
+                       item_start, items};
+    const int pbits = bit_length(n - 1);
+    if (items) LAUNCH(c, k_approx<false>, cdiv(items, NWARP), A, cnt, (const u64 *)nullptr, pbits, (u64 *)nullptr,
+                      (uint32_t *)nullptr);
+    TRY((dev_scan<OpSum64>(c, InCount64{cnt, items}, OutStoreExcl64{item_off}, items + 1, d_total)));
+    LAUNCH(c, k_approx_qoff, cdiv((uint64_t)nq + 1, BLK), item_start, item_off, nq, P,
+           reinterpret_cast<u64 *>(d_offsets));
+    TRY(read_words(c, words + 4, 2));
+    *total = c->h_pin[0] | ((uint64_t)c->h_pin[1] << 32);
+    if (*total > 0 && *total <= cap) {
+        TRY(mark(c, "approx_emit"));
+        TRY(ensure(c, c->g0, (size_t)*total * 8));
+        TRY(ensure(c, c->g1, (size_t)*total * 8));
+        TRY(ensure(c, c->v0, (size_t)*total * 4));
+        TRY(ensure(c, c->v1, (size_t)*total * 4));
+        LAUNCH(c, k_approx<true>, cdiv(items, NWARP), A, cnt, (const u64 *)item_off, pbits, ptr<u64>(c->g0),
+               ptr<uint32_t>(c->v0));
+        TRY(mark(c, "approx_sort"));                     // by (q, p)
+        uint64_t *ko;
+        uint32_t *vo;
+        TRY(sort_pairs<uint64_t>(c, ptr<uint64_t>(c->g0), ptr<uint32_t>(c->v0), ptr<uint64_t>(c->g1),
+                                 ptr<uint32_t>(c->v1), *total, bit_length(nq - 1) + pbits, &ko, &vo));
+        LAUNCH(c, k_approx_gather, cdiv(*total, BLK), (const u64 *)ko, (const uint32_t *)vo, *total,
+               (u64)((1ull << pbits) - 1), d_pos, d_mis);
+    }
+    TRY(mark(c, "end"));
+    CU_TRY(c, cudaGetLastError());
+    CU_TRY(c, cudaStreamSynchronize(c->stream));
+    return B200SA_OK;
+}
+}  // extern "C++"
+
+static int approx_args(b200sa_ctx *c, uint64_t n, const void *text, const void *sa, const void *q_off, uint32_t nq,
+                       uint32_t k, const void *offsets, const void *pos, uint64_t cap, const void *total) {
+    if (!c) return B200SA_ERR_BAD_ARG;
+    if (!total || !offsets || (nq > 0 && !q_off) || (cap > 0 && !pos) || (n > 0 && (!text || !sa))) {
+        c->last_error = "null pointer";
+        return B200SA_ERR_BAD_ARG;
+    }
+    if (k > B200SA_APPROX_MAX_K) {
+        c->last_error = "approx positions: k above B200SA_APPROX_MAX_K";
+        return B200SA_ERR_BAD_ARG;
+    }
+    if (n > B200SA_MAX_N) {
+        c->last_error = "text longer than 2^32-4096 bytes";
+        return B200SA_ERR_TOO_LARGE;
+    }
+    return B200SA_OK;
+}
+
+// nq = 0: offsets[0] = 0, *total = 0.
+static int approx_none(b200sa_ctx *c, uint64_t *d_offsets) {
+    CU_TRY(c, cudaMemsetAsync(d_offsets, 0, 8, c->stream));
+    CU_TRY(c, cudaStreamSynchronize(c->stream));
+    return B200SA_OK;
+}
+
+int b200sa_approx_positions_dev(b200sa_ctx *c, const uint8_t *d_text, uint64_t n, const uint32_t *d_sa,
+                                const uint8_t *d_queries, const uint64_t *d_q_off, uint32_t nq, uint32_t k,
+                                uint64_t *d_offsets, uint32_t *d_pos, uint32_t *d_mismatches, uint64_t cap,
+                                uint64_t *total, void *stream) {
+    TRY(approx_args(c, n, d_text, d_sa, d_q_off, nq, k, d_offsets, d_pos, cap, total));
+    CU_TRY(c, cudaSetDevice(c->device));
+    begin_call(c, stream);
+    *total = 0;
+    if (nq == 0) return tree_exit(c, approx_none(c, d_offsets));
+    return tree_exit(c, approx_core(c, d_text, (uint32_t)n, d_sa, nullptr, 0, d_queries, d_q_off, nq, k, d_offsets,
+                                    d_pos, d_mismatches, cap, total, TextEnd{(uint32_t)n}));
+}
+
+int b200sa_docs_approx_positions_dev(b200sa_ctx *c, const uint8_t *d_text, uint64_t n, const uint32_t *d_gsa,
+                                     const uint32_t *d_doc_starts, uint32_t ndocs, const uint8_t *d_queries,
+                                     const uint64_t *d_q_off, uint32_t nq, uint32_t k, uint64_t *d_offsets,
+                                     uint32_t *d_pos, uint32_t *d_mismatches, uint64_t cap, uint64_t *total,
+                                     void *stream) {
+    TRY(approx_args(c, n, d_text, d_gsa, d_q_off, nq, k, d_offsets, d_pos, cap, total));
+    if ((n > 0 || ndocs > 0) && !d_doc_starts) {
+        c->last_error = "null pointer";
+        return B200SA_ERR_BAD_ARG;
+    }
+    if (ndocs == 0 && n > 0) {
+        c->last_error = "doc_starts rejected: ndocs == 0 with n > 0;";
+        return B200SA_ERR_BAD_ARG;
+    }
+    CU_TRY(c, cudaSetDevice(c->device));
+    begin_call(c, stream);
+    *total = 0;
+    if (nq == 0) return tree_exit(c, approx_none(c, d_offsets));
+    return tree_exit(c, approx_core(c, d_text, (uint32_t)n, d_gsa, d_doc_starts, ndocs, d_queries, d_q_off, nq, k,
+                                    d_offsets, d_pos, d_mismatches, cap, total,
+                                    DocsEnd{d_doc_starts, ndocs, (uint32_t)n}));
 }
 
 // ------------------------------------------------------------ multi-GPU: communicator + sharded LMS sort

@@ -544,17 +544,13 @@ struct TextEnd {
     uint32_t n;
     __device__ __forceinline__ uint32_t operator()(uint32_t) const { return n; }
 };
-// One thread per query: reference early-outs (src/table.rs:228-235), then the
-// two binary searches (:244-250), every suffix cut at end(p).
+// The range [*out_start, *out_end) of the table whose suffixes, cut at end(p), start with q[0, m):
+// reference early-outs (src/table.rs:228-235), then the two binary searches (:244-250).  (0, 0) when
+// n = 0 or m = 0.
 template <class EndF>
-__global__ void __launch_bounds__(BLK) k_positions(const uint8_t *__restrict__ text, uint32_t n,
-                                                   const uint32_t *__restrict__ sa, const uint8_t *__restrict__ qs,
-                                                   const uint64_t *__restrict__ qoff, uint32_t nq,
-                                                   uint32_t *out_start, uint32_t *out_end, EndF end) {
-    uint32_t qi = blockIdx.x * BLK + threadIdx.x;
-    if (qi >= nq) return;
-    const uint8_t *q = qs + qoff[qi];
-    uint32_t m = (uint32_t)(qoff[qi + 1] - qoff[qi]);
+__device__ __forceinline__ void positions_range(const uint8_t *__restrict__ text, uint32_t n,
+                                                const uint32_t *__restrict__ sa, const uint8_t *__restrict__ q,
+                                                uint32_t m, EndF end, uint32_t *out_start, uint32_t *out_end) {
     uint32_t start = 0, finish = 0;
     auto cmp = [&](uint32_t p, bool *pre) { return cmp_query_suffix(text, end(p), p, q, m, pre); };
     if (n > 0 && m > 0) {
@@ -581,8 +577,19 @@ __global__ void __launch_bounds__(BLK) k_positions(const uint8_t *__restrict__ t
             finish = start + lo2;
         }
     }
-    out_start[qi] = start;
-    out_end[qi] = finish;
+    *out_start = start;
+    *out_end = finish;
+}
+// One thread per query.
+template <class EndF>
+__global__ void __launch_bounds__(BLK) k_positions(const uint8_t *__restrict__ text, uint32_t n,
+                                                   const uint32_t *__restrict__ sa, const uint8_t *__restrict__ qs,
+                                                   const uint64_t *__restrict__ qoff, uint32_t nq,
+                                                   uint32_t *out_start, uint32_t *out_end, EndF end) {
+    uint32_t qi = blockIdx.x * BLK + threadIdx.x;
+    if (qi >= nq) return;
+    positions_range(text, n, sa, qs + qoff[qi], (uint32_t)(qoff[qi + 1] - qoff[qi]), end, out_start + qi,
+                    out_end + qi);
 }
 
 // ------------------------------------------------------------ generalized suffix array (SURVEY 8f-3)

@@ -12,7 +12,7 @@ import bisect
 
 import numpy as np
 
-from . import _bwt, _lib, _lz, _match, _repeats
+from . import _approx, _bwt, _lib, _lz, _match, _repeats
 from .table import _as_bytes, _lock      # the lock of the per-device default context, shared with SuffixTable
 
 MAX_N = 0xFFFFF000        # B200SA_MAX_N
@@ -450,6 +450,24 @@ class DocumentSuffixTable:
         """r, the number of maximal runs of equal symbols in the transform's n + k symbols; every terminator
         is a symbol of its own."""
         return _bwt.bwt_runs(self)
+
+    # ---- approximate positions (DESIGN 6b f-14)
+    def approximate_positions(self, query, k):
+        """(positions u32[], mismatches u32[]): every position p of the concatenation whose window of m bytes
+        lies inside p's document and differs from the query (m bytes) in at most k bytes, 0 <= k <= 31, by
+        ascending p, with that number of mismatches beside it (b200sa_docs_approx_positions_dev).  locate()
+        maps the positions to (document, offset).  b"" matches nothing."""
+        return _approx.positions(self, query, k)
+
+    def approximate_positions_batch(self, queries, k):
+        """(offsets u64[nq + 1], positions u32[], mismatches u32[]): query q's occurrences with at most k
+        mismatches are positions[offsets[q]:offsets[q + 1]], as approximate_positions returns them."""
+        return _approx.positions_batch(self, queries, k)
+
+    def approximate_counts(self, queries, k):
+        """u64[nq]: the number of occurrences with at most k mismatches of every query, without fetching
+        them."""
+        return _approx.counts(self, queries, k)
 
     def top_documents(self, query, k) -> np.ndarray:
         """(document, count) rows of the min(k, df) documents that contain `query` most often, by count

@@ -279,6 +279,27 @@ class SuffixTable:
         from . import _bwt
         return _bwt.bwt_runs(self)
 
+    # ---- approximate positions (DESIGN 6b f-14)
+    def approximate_positions(self, query, k):
+        """(positions u32[], mismatches u32[]): every p with p + m <= n where text[p:p + m] differs from
+        the query (m bytes) in at most k bytes, 0 <= k <= 31, by ascending p, with that number of
+        mismatches beside it (b200sa_approx_positions_dev).  b"" matches nothing; for k = 0 the positions
+        are those of positions(query), sorted.  Uses the device copies of _bwt_arrays()."""
+        from . import _approx
+        return _approx.positions(self, query, k)
+
+    def approximate_positions_batch(self, queries, k):
+        """(offsets u64[nq + 1], positions u32[], mismatches u32[]): query q's occurrences with at most k
+        mismatches are positions[offsets[q]:offsets[q + 1]], as approximate_positions returns them."""
+        from . import _approx
+        return _approx.positions_batch(self, queries, k)
+
+    def approximate_counts(self, queries, k):
+        """u64[nq]: the number of occurrences with at most k mismatches of every query, without fetching
+        them."""
+        from . import _approx
+        return _approx.counts(self, queries, k)
+
     # ---- persistence (SURVEY 8f-2): the only "wire format" the reference API implies is
     # from_parts/into_parts (src/table.rs:111-127): text bytes + little-endian u32 table.
     def save(self, path: str) -> None:

@@ -156,6 +156,14 @@ for k, tab in enumerate([single] + [DocumentSuffixTable(docs) for docs in doc_se
         if sp: os.environ["B200SA_BWT_RULER"] = str(sp)
         assert b"".join(inverse_bwt_documents(b, t)) == tab.text(), (k, sp)
         os.environ.pop("B200SA_BWT_RULER", None)
+# approximate positions: the count call (cap = 0) then the fetch, on the single text, every document set, a
+# repetitive text whose slots span many chunks, and queries of m <= k on documents with empty ones
+ap_qs = [dna[a:a + 25] for a in range(0, 4000, 97)] + [b"", b"A", b"ACG", b"ACGTACGT"]
+for k, tab in enumerate([single] + [DocumentSuffixTable(docs) for docs in doc_sets] +
+                        [SuffixTable(b"a" * 5000), DocumentSuffixTable([b"", b"ab", b"", b"c"])]):
+    for kk in (0, 3, 31):
+        off, pos, mis = tab.approximate_positions_batch(ap_qs + [b"a" * 9], kk)
+        assert len(pos) == int(off[-1]) and (mis <= kk).all(), (k, kk)
 # refinement branches (tests/test_gpu_refine.py): a local-sort overflow in round 2 of the direct path, the direct
 # path's probe (2^20 tied after round 1, large groups), 64-bit round-0 keys of the reduced string
 import ctypes
