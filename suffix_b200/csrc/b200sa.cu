@@ -148,14 +148,35 @@ static int mark(b200sa_ctx *c, const char *name) {
     c->marks.push_back({name, e});
     return B200SA_OK;
 }
-static void begin_call(b200sa_ctx *c, void *stream) {
+// Every argument error of an entry point leaves its own message, so that b200sa_last_error never
+// reports an earlier call's failure.
+static int fail(b200sa_ctx *c, int code, const char *msg) {
+    c->last_error = msg;
+    return code;
+}
+static int null_ptr(b200sa_ctx *c) { return fail(c, B200SA_ERR_BAD_ARG, "null pointer"); }
+static int too_long(b200sa_ctx *c) { return fail(c, B200SA_ERR_TOO_LARGE, "text longer than 2^32-4096 bytes"); }
+static int no_docs(b200sa_ctx *c) { return fail(c, B200SA_ERR_BAD_ARG, "doc_starts rejected: ndocs == 0 with n > 0;"); }
+
+// The start of every entry point once its arguments are checked; each one then returns through leave().
+static int enter(b200sa_ctx *c, void *stream) {
+    CU_TRY(c, cudaSetDevice(c->device));
     c->stream = stream ? (cudaStream_t)stream : c->own_stream;
     c->marks.clear();
     c->events_used = 0;
     c->launches = 0;
     c->last_error.clear();
+    return B200SA_OK;
 }
-static int end_call(b200sa_ctx *c) {
+// On failure, work of the call may still be in flight on its stream, writing into the caller's
+// buffers, which the caller is free to release as soon as we return: wait for it, and clear the
+// sticky error.  On success nothing waits beyond what the call did itself.
+static int leave(b200sa_ctx *c, int rc) {
+    if (rc != B200SA_OK) {
+        if (c->stream) cudaStreamSynchronize(c->stream);
+        cudaGetLastError();
+        return rc;
+    }
     c->stats.kernel_launches = c->launches;
     c->stats.workspace_bytes = c->ws_bytes;
     c->phase_names.clear();
@@ -184,6 +205,8 @@ static int read_words(b200sa_ctx *c, const uint32_t *dsrc, int count) {
     CU_TRY(c, cudaStreamSynchronize(c->stream));
     return B200SA_OK;
 }
+// Words i and i + 1 of the last read_words as one u64 (low word first).
+static uint64_t pin_u64(const b200sa_ctx *c, int i) { return c->h_pin[i] | ((uint64_t)c->h_pin[i + 1] << 32); }
 
 // ------------------------------------------------------- generic primitives
 // Single-pass scan (k_scan_lb, common.cuh): one launch, the input functor is evaluated once
@@ -895,7 +918,7 @@ static int build_dev(b200sa_ctx *c, const uint8_t *d_text, uint64_t n, uint32_t 
     c->stats.sm_count = c->sm_count;
     c->stats.induce_blocks = c->induce_blocks;   // updated after classification
     c->last_n = n; c->last_m = 0;
-    if (n > B200SA_MAX_N) { c->last_error = "text longer than 2^32-4096 bytes"; return B200SA_ERR_TOO_LARGE; }
+    if (n > B200SA_MAX_N) return too_long(c);
     if (n == 0) return B200SA_OK;
     if (n == 1) { CU_TRY(c, cudaMemsetAsync(d_sa, 0, 4, c->stream)); return B200SA_OK; }
     const uint8_t *text = d_text;
@@ -1047,10 +1070,8 @@ static int lcp_dev(b200sa_ctx *c, const uint8_t *d_text, uint64_t n, const uint3
         LAUNCH(c, k_sa_validate_count, (uint32_t)c->sm_count * 4u, seen, n32, bad + 1);
         LAUNCH(c, k_sa_validate_verdict, 1u, bad + 1, n32, bad);
         TRY(read_words(c, bad, 1));
-        if (c->h_pin[0] != 0) {
-            c->last_error = "table is not a permutation of 0..n-1 (index out of range or repeated)";
-            return B200SA_ERR_BAD_ARG;
-        }
+        if (c->h_pin[0] != 0)
+            return fail(c, B200SA_ERR_BAD_ARG, "table is not a permutation of 0..n-1 (index out of range or repeated)");
     }
     if (!reuse_pack) {
         // stand-alone call: byte histogram -> alphabet -> packed text
@@ -1139,10 +1160,7 @@ static int lcp_dev(b200sa_ctx *c, const uint8_t *d_text, uint64_t n, const uint3
 }
 
 template <class K>
-static int test_sort(b200sa_ctx *c, K *keys, uint32_t *vals, uint64_t n, int bits) {
-    if (!c || (n > 0 && (!keys || !vals))) return B200SA_ERR_BAD_ARG;
-    CU_TRY(c, cudaSetDevice(c->device));
-    begin_call(c, nullptr);
+static int test_sort_core(b200sa_ctx *c, K *keys, uint32_t *vals, uint64_t n, int bits) {
     TRY(ensure(c, c->k64a, n * sizeof(K)));
     TRY(ensure(c, c->k64b, n * sizeof(K)));
     TRY(ensure(c, c->v0, n * 4));
@@ -1156,7 +1174,15 @@ static int test_sort(b200sa_ctx *c, K *keys, uint32_t *vals, uint64_t n, int bit
         CU_TRY(c, cudaMemcpyAsync(vals, vo, n * 4, cudaMemcpyDeviceToHost, c->stream));
     }
     CU_TRY(c, cudaStreamSynchronize(c->stream));
-    return end_call(c);
+    return B200SA_OK;
+}
+
+template <class K>
+static int test_sort(b200sa_ctx *c, K *keys, uint32_t *vals, uint64_t n, int bits) {
+    if (!c) return B200SA_ERR_BAD_ARG;
+    if (n > 0 && (!keys || !vals)) return null_ptr(c);
+    TRY(enter(c, nullptr));
+    return leave(c, test_sort_core(c, keys, vals, n, bits));
 }
 
 // SA + LCP of one text, device-resident (b200sa_build_lcp_dev, and step 1 of b200sa_docs_build).
@@ -1185,7 +1211,8 @@ static int docs_sort(b200sa_ctx *c, KeyF kf, const uint32_t *vals, K *ka, uint32
 }
 
 // ================================================================= C ABI
-extern "C" {
+// include/b200sa.h and include/b200sa_internal.h give every entry point C linkage, which the
+// definitions below keep.
 
 const char *b200sa_version(void) { return kVersion; }
 
@@ -1287,49 +1314,41 @@ int b200sa_last_phase_times(b200sa_ctx *c, const char **names, float *ms, int ca
 }
 
 int b200sa_last_stats(b200sa_ctx *c, b200sa_stats *out) {
-    if (!c || !out) return B200SA_ERR_BAD_ARG;
+    if (!c) return B200SA_ERR_BAD_ARG;
+    if (!out) return null_ptr(c);
     *out = c->stats;
     out->workspace_bytes = c->ws_bytes;
     return B200SA_OK;
 }
 
 int b200sa_build_dev(b200sa_ctx *c, const uint8_t *d_text, uint64_t n, uint32_t *d_sa, void *stream) {
-    if (!c || (n > 0 && (!d_text || !d_sa))) return B200SA_ERR_BAD_ARG;
-    CU_TRY(c, cudaSetDevice(c->device));
-    begin_call(c, stream);
-    int rc = build_dev(c, d_text, n, d_sa);
-    if (rc == B200SA_OK) rc = end_call(c);
-    return rc;
+    if (!c) return B200SA_ERR_BAD_ARG;
+    if (n > 0 && (!d_text || !d_sa)) return null_ptr(c);
+    TRY(enter(c, stream));
+    return leave(c, build_dev(c, d_text, n, d_sa));
 }
 
 int b200sa_lcp_dev(b200sa_ctx *c, const uint8_t *d_text, uint64_t n, const uint32_t *d_sa, uint32_t *d_lcp,
                    void *stream) {
-    if (!c || (n > 0 && (!d_text || !d_sa || !d_lcp))) return B200SA_ERR_BAD_ARG;
-    CU_TRY(c, cudaSetDevice(c->device));
-    begin_call(c, stream);
-    int rc = lcp_dev(c, d_text, n, d_sa, d_lcp, false);
-    if (rc == B200SA_OK) rc = end_call(c);
-    return rc;
+    if (!c) return B200SA_ERR_BAD_ARG;
+    if (n > 0 && (!d_text || !d_sa || !d_lcp)) return null_ptr(c);
+    TRY(enter(c, stream));
+    return leave(c, lcp_dev(c, d_text, n, d_sa, d_lcp, false));
 }
 
 int b200sa_build_lcp_dev(b200sa_ctx *c, const uint8_t *d_text, uint64_t n, uint32_t *d_sa, uint32_t *d_lcp,
                          void *stream) {
-    if (!c || (n > 0 && (!d_text || !d_sa || !d_lcp))) return B200SA_ERR_BAD_ARG;
-    CU_TRY(c, cudaSetDevice(c->device));
-    begin_call(c, stream);
-    int rc = build_lcp_dev(c, d_text, n, d_sa, d_lcp);
-    if (rc == B200SA_OK) rc = end_call(c);
-    return rc;
+    if (!c) return B200SA_ERR_BAD_ARG;
+    if (n > 0 && (!d_text || !d_sa || !d_lcp)) return null_ptr(c);
+    TRY(enter(c, stream));
+    return leave(c, build_lcp_dev(c, d_text, n, d_sa, d_lcp));
 }
 
 static int host_build_inner(b200sa_ctx *c, const uint8_t *text, uint64_t n, uint32_t *sa_out, uint32_t *lcp_out,
                             const uint32_t *sa_in) {
-    if (n > B200SA_MAX_N) { c->last_error = "text longer than 2^32-4096 bytes"; return B200SA_ERR_TOO_LARGE; }
-    CU_TRY(c, cudaSetDevice(c->device));
-    begin_call(c, nullptr);
     memset(&c->stats, 0, sizeof c->stats);
     c->stats.n = n;
-    if (n == 0) return end_call(c);
+    if (n == 0) return B200SA_OK;
     TRY(ensure(c, c->text, n));
     TRY(ensure(c, c->sa, (size_t)n * 4));
     TRY(mark(c, "h2d"));
@@ -1371,60 +1390,73 @@ static int host_build_inner(b200sa_ctx *c, const uint8_t *text, uint64_t n, uint
     TRY(mark(c, "end"));
     CU_TRY(c, cudaStreamSynchronize(c->stream));
     CU_TRY(c, cudaStreamSynchronize(c->copy_stream));
-    return end_call(c);
+    return B200SA_OK;
 }
 
-// Every exit of the host API passes through here: on failure, D2H copies into the caller's
-// buffers may still be in flight on either stream, and the caller is free to release the
-// buffers as soon as we return.
+// The host API: a failed build may also have D2H copies into the caller's buffers in flight on
+// the copy stream.
 static int host_build(b200sa_ctx *c, const uint8_t *text, uint64_t n, uint32_t *sa_out, uint32_t *lcp_out,
                       const uint32_t *sa_in) {
+    if (n > B200SA_MAX_N) return too_long(c);
+    TRY(enter(c, nullptr));
     int rc = host_build_inner(c, text, n, sa_out, lcp_out, sa_in);
     if (rc != B200SA_OK) {
         c->early_sa_out = nullptr;
-        if (c->stream) cudaStreamSynchronize(c->stream);
         if (c->copy_stream) cudaStreamSynchronize(c->copy_stream);
-        cudaGetLastError();
     }
-    return rc;
+    return leave(c, rc);
 }
 
 int b200sa_build(b200sa_ctx *c, const uint8_t *text, uint64_t n, uint32_t *sa_out) {
-    if (!c || (n > 0 && (!text || !sa_out))) return B200SA_ERR_BAD_ARG;
+    if (!c) return B200SA_ERR_BAD_ARG;
+    if (n > 0 && (!text || !sa_out)) return null_ptr(c);
     return host_build(c, text, n, sa_out, nullptr, nullptr);
 }
 
 int b200sa_lcp(b200sa_ctx *c, const uint8_t *text, uint64_t n, const uint32_t *sa, uint32_t *lcp_out) {
-    if (!c || (n > 0 && (!text || !sa || !lcp_out))) return B200SA_ERR_BAD_ARG;
+    if (!c) return B200SA_ERR_BAD_ARG;
+    if (n > 0 && (!text || !sa || !lcp_out)) return null_ptr(c);
     return host_build(c, text, n, nullptr, lcp_out, sa);
 }
 
 int b200sa_build_lcp(b200sa_ctx *c, const uint8_t *text, uint64_t n, uint32_t *sa_out, uint32_t *lcp_out) {
-    if (!c || (n > 0 && (!text || !sa_out || !lcp_out))) return B200SA_ERR_BAD_ARG;
+    if (!c) return B200SA_ERR_BAD_ARG;
+    if (n > 0 && (!text || !sa_out || !lcp_out)) return null_ptr(c);
     return host_build(c, text, n, sa_out, lcp_out, nullptr);
 }
 
-int b200sa_positions_dev(b200sa_ctx *c, const uint8_t *d_text, uint64_t n, const uint32_t *d_sa,
-                         const uint8_t *d_queries, const uint64_t *d_q_off, uint32_t nq, uint32_t *d_start,
-                         uint32_t *d_end, void *stream) {
-    if (!c || (nq > 0 && (!d_q_off || !d_start || !d_end)) || (n > 0 && (!d_text || !d_sa))) return B200SA_ERR_BAD_ARG;
-    if (n > B200SA_MAX_N) return B200SA_ERR_TOO_LARGE;
-    CU_TRY(c, cudaSetDevice(c->device));
-    begin_call(c, stream);
+static int positions_core(b200sa_ctx *c, const uint8_t *d_text, uint64_t n, const uint32_t *d_sa,
+                          const uint8_t *d_queries, const uint64_t *d_q_off, uint32_t nq, uint32_t *d_start,
+                          uint32_t *d_end) {
     if (nq > 0) {
         LAUNCH(c, k_positions<TextEnd>, cdiv(nq, BLK), d_text, (uint32_t)n, d_sa, d_queries, d_q_off, nq, d_start, d_end,
                TextEnd{(uint32_t)n});
         CU_TRY(c, cudaGetLastError());
     }
-    return end_call(c);
+    return B200SA_OK;
+}
+
+int b200sa_positions_dev(b200sa_ctx *c, const uint8_t *d_text, uint64_t n, const uint32_t *d_sa,
+                         const uint8_t *d_queries, const uint64_t *d_q_off, uint32_t nq, uint32_t *d_start,
+                         uint32_t *d_end, void *stream) {
+    if (!c) return B200SA_ERR_BAD_ARG;
+    if ((nq > 0 && (!d_q_off || !d_start || !d_end)) || (n > 0 && (!d_text || !d_sa))) return null_ptr(c);
+    if (n > B200SA_MAX_N) return too_long(c);
+    TRY(enter(c, stream));
+    return leave(c, positions_core(c, d_text, n, d_sa, d_queries, d_q_off, nq, d_start, d_end));
 }
 
 // ------------------------------------------------------------ multi-GPU shards (SURVEY 8e)
-int b200sa_shard_summary(b200sa_ctx *c, const uint8_t *d_shard, uint64_t len, int next_char, int *state_out, void *stream) {
-    if (!c || !d_shard || len < 1 || len > B200SA_MAX_N || !state_out || next_char > 255) return B200SA_ERR_BAD_ARG;
-    if (((uintptr_t)d_shard & 15) != 0) { c->last_error = "shard pointer must be 16-byte aligned"; return B200SA_ERR_BAD_ARG; }
-    CU_TRY(c, cudaSetDevice(c->device));
-    begin_call(c, stream);
+// The checks of both shard entry points on the shard and the next character.
+static int shard_args(b200sa_ctx *c, const uint8_t *d_shard, uint64_t len, int next_char) {
+    if (!d_shard) return null_ptr(c);
+    if (len < 1 || len > B200SA_MAX_N) return fail(c, B200SA_ERR_BAD_ARG, "shard: len must be in [1, 2^32-4096]");
+    if (next_char > 255) return fail(c, B200SA_ERR_BAD_ARG, "shard: next_char above 255");
+    if (((uintptr_t)d_shard & 15) != 0) return fail(c, B200SA_ERR_BAD_ARG, "shard pointer must be 16-byte aligned");
+    return B200SA_OK;
+}
+
+static int shard_summary_core(b200sa_ctx *c, const uint8_t *d_shard, uint64_t len, int next_char, int *state_out) {
     uint64_t nw = (len + 31) / 32;
     uint32_t nbc = cdiv(nw, CLS_WORDS);
     TRY(ensure(c, c->blkstate, nbc));
@@ -1439,17 +1471,20 @@ int b200sa_shard_summary(b200sa_ctx *c, const uint8_t *d_shard, uint64_t len, in
     CU_TRY(c, cudaMemcpyAsync(&h[1], c->carry.p, 1, cudaMemcpyDeviceToHost, c->stream));
     CU_TRY(c, cudaStreamSynchronize(c->stream));
     *state_out = (h[0] != ST_P) ? h[0] : h[1];
-    return end_call(c);
+    return B200SA_OK;
 }
 
-int b200sa_shard_classify(b200sa_ctx *c, const uint8_t *d_shard, uint64_t len, int prev_char, int next_char,
-                          int tail_carry, uint32_t *d_stype_words, uint32_t *d_lms_words, uint32_t *d_lmspos,
-                          uint64_t cap_lms, uint64_t *hist768, uint64_t *m_out, void *stream) {
-    if (!c || !d_shard || len < 1 || len > B200SA_MAX_N || prev_char > 255 || next_char > 255) return B200SA_ERR_BAD_ARG;
-    if (next_char >= 0 && tail_carry != (int)ST_L && tail_carry != (int)ST_S) return B200SA_ERR_BAD_ARG;
-    if (((uintptr_t)d_shard & 15) != 0) { c->last_error = "shard pointer must be 16-byte aligned"; return B200SA_ERR_BAD_ARG; }
-    CU_TRY(c, cudaSetDevice(c->device));
-    begin_call(c, stream);
+int b200sa_shard_summary(b200sa_ctx *c, const uint8_t *d_shard, uint64_t len, int next_char, int *state_out, void *stream) {
+    if (!c) return B200SA_ERR_BAD_ARG;
+    if (!state_out) return null_ptr(c);
+    TRY(shard_args(c, d_shard, len, next_char));
+    TRY(enter(c, stream));
+    return leave(c, shard_summary_core(c, d_shard, len, next_char, state_out));
+}
+
+static int shard_classify_core(b200sa_ctx *c, const uint8_t *d_shard, uint64_t len, int prev_char, int next_char,
+                               int tail_carry, uint32_t *d_stype_words, uint32_t *d_lms_words, uint32_t *d_lmspos,
+                               uint64_t cap_lms, uint64_t *hist768, uint64_t *m_out) {
     uint32_t m = 0;
     ShardEdge edge{next_char, prev_char, next_char >= 0 ? (uint32_t)tail_carry : ST_L};
     TRY(classify_dev(c, d_shard, len, &m, edge));
@@ -1469,18 +1504,37 @@ int b200sa_shard_classify(b200sa_ctx *c, const uint8_t *d_shard, uint64_t len, i
         CU_TRY(c, cudaStreamSynchronize(c->stream));
     }
     if (m_out) *m_out = m;
-    return end_call(c);
+    return B200SA_OK;
+}
+
+int b200sa_shard_classify(b200sa_ctx *c, const uint8_t *d_shard, uint64_t len, int prev_char, int next_char,
+                          int tail_carry, uint32_t *d_stype_words, uint32_t *d_lms_words, uint32_t *d_lmspos,
+                          uint64_t cap_lms, uint64_t *hist768, uint64_t *m_out, void *stream) {
+    if (!c) return B200SA_ERR_BAD_ARG;
+    if (prev_char > 255) return fail(c, B200SA_ERR_BAD_ARG, "shard: prev_char above 255");
+    TRY(shard_args(c, d_shard, len, next_char));
+    if (next_char >= 0 && tail_carry != (int)ST_L && tail_carry != (int)ST_S)
+        return fail(c, B200SA_ERR_BAD_ARG, "shard: tail_carry must be L or S when next_char >= 0");
+    TRY(enter(c, stream));
+    return leave(c, shard_classify_core(c, d_shard, len, prev_char, next_char, tail_carry, d_stype_words, d_lms_words,
+                                        d_lmspos, cap_lms, hist768, m_out));
 }
 
 // ------------------------------------------------------------ generalized SA / LCP intervals (SURVEY 8f-3, 8f-4)
-int b200sa_doc_ids_dev(b200sa_ctx *c, const uint32_t *d_pos, uint64_t count, const uint32_t *d_doc_starts,
-                       uint32_t ndocs, uint32_t *d_doc, uint32_t *d_off, void *stream) {
-    if (!c || ndocs < 1 || !d_doc_starts || (count > 0 && (!d_pos || !d_doc || !d_off))) return B200SA_ERR_BAD_ARG;
-    CU_TRY(c, cudaSetDevice(c->device));
-    begin_call(c, stream);
+static int doc_ids_core(b200sa_ctx *c, const uint32_t *d_pos, uint64_t count, const uint32_t *d_doc_starts,
+                        uint32_t ndocs, uint32_t *d_doc, uint32_t *d_off) {
     if (count) LAUNCH(c, k_doc_ids, cdiv(count, BLK), d_pos, count, d_doc_starts, ndocs, d_doc, d_off);
     CU_TRY(c, cudaGetLastError());
-    return end_call(c);
+    return B200SA_OK;
+}
+
+int b200sa_doc_ids_dev(b200sa_ctx *c, const uint32_t *d_pos, uint64_t count, const uint32_t *d_doc_starts,
+                       uint32_t ndocs, uint32_t *d_doc, uint32_t *d_off, void *stream) {
+    if (!c) return B200SA_ERR_BAD_ARG;
+    if (!d_doc_starts || (count > 0 && (!d_pos || !d_doc || !d_off))) return null_ptr(c);
+    if (ndocs < 1) return fail(c, B200SA_ERR_BAD_ARG, "doc ids: ndocs must be at least 1");
+    TRY(enter(c, stream));
+    return leave(c, doc_ids_core(c, d_pos, count, d_doc_starts, ndocs, d_doc, d_off));
 }
 
 // Block minima of an array (the LCP array, or any other) over 32^k entries, in `buf`, for the ANSV searches.
@@ -1502,18 +1556,22 @@ static int ansv_levels(b200sa_ctx *c, const uint32_t *d_lcp, uint64_t n, AnsvLev
     return B200SA_OK;
 }
 
-int b200sa_lcp_intervals_dev(b200sa_ctx *c, const uint32_t *d_lcp, uint64_t n, uint32_t *d_psv, uint32_t *d_nsv,
-                             void *stream) {
-    if (!c || (n > 0 && (!d_lcp || !d_psv || !d_nsv))) return B200SA_ERR_BAD_ARG;
-    if (n > B200SA_MAX_N) return B200SA_ERR_TOO_LARGE;
-    CU_TRY(c, cudaSetDevice(c->device));
-    begin_call(c, stream);
-    if (n == 0) return end_call(c);
+static int lcp_intervals_core(b200sa_ctx *c, const uint32_t *d_lcp, uint64_t n, uint32_t *d_psv, uint32_t *d_nsv) {
+    if (n == 0) return B200SA_OK;
     AnsvLevels L;
     TRY(ansv_levels(c, d_lcp, n, &L, c->qbuf));
     LAUNCH(c, k_ansv, cdiv(n, BLK), L, n, d_psv, d_nsv);
     CU_TRY(c, cudaGetLastError());
-    return end_call(c);
+    return B200SA_OK;
+}
+
+int b200sa_lcp_intervals_dev(b200sa_ctx *c, const uint32_t *d_lcp, uint64_t n, uint32_t *d_psv, uint32_t *d_nsv,
+                             void *stream) {
+    if (!c) return B200SA_ERR_BAD_ARG;
+    if (n > 0 && (!d_lcp || !d_psv || !d_nsv)) return null_ptr(c);
+    if (n > B200SA_MAX_N) return too_long(c);
+    TRY(enter(c, stream));
+    return leave(c, lcp_intervals_core(c, d_lcp, n, d_psv, d_nsv));
 }
 
 // ------------------------------------------------------------ suffix tree from SA + LCP (SURVEY 8f-5)
@@ -1532,7 +1590,6 @@ static int tree_bad(b200sa_ctx *c, uint32_t bits) {
 // n >= 1, device inputs and outputs (capacity >= 2n each).  Phases: tree_ansv, tree_emit, tree_sort,
 // tree_first, tree_nodes.  len gives the suffix length of a rank (TextLen: one text; DocsLen: the
 // generalized tree, whose sorted keys and first[] b200sa_docs_tree reads afterwards in k64a/k64b and g0).
-extern "C++" {   // templates inside the C-ABI block
 template <class LenF>
 static int suffix_tree_core(b200sa_ctx *c, uint32_t n, const uint32_t *d_sa, const uint32_t *d_lcp, const TreeOut &o,
                             uint64_t *num_nodes, LenF len, uint64_t **keys_out = nullptr) {
@@ -1587,63 +1644,59 @@ static int suffix_tree_core(b200sa_ctx *c, uint32_t n, const uint32_t *d_sa, con
     if (keys_out) *keys_out = K;
     return B200SA_OK;
 }
-}  // extern "C++"
 
 static int tree_args(b200sa_ctx *c, uint64_t n, const void *sa, const void *lcp, const b200sa_tree *out,
                      uint64_t cap, uint64_t *num_nodes) {
-    if (!c || !out || !num_nodes) return B200SA_ERR_BAD_ARG;
-    if (!out->parent || !out->depth || !out->sa_lo || !out->sa_hi || !out->label_start || !out->subtree_end ||
-        (n > 0 && (!sa || !lcp))) {
-        c->last_error = "null pointer";
-        return B200SA_ERR_BAD_ARG;
-    }
-    if (n > B200SA_TREE_MAX_N) {
-        c->last_error = "suffix tree: n >= 2^31 (node ids are u32 with 0xFFFFFFFF reserved)";
-        return B200SA_ERR_TOO_LARGE;
-    }
-    if (cap < (n ? 2 * n : 1)) {
-        c->last_error = "suffix tree: cap < max(1, 2n)";
-        return B200SA_ERR_BAD_ARG;
-    }
+    if (!c) return B200SA_ERR_BAD_ARG;
+    if (!out || !num_nodes || !out->parent || !out->depth || !out->sa_lo || !out->sa_hi || !out->label_start ||
+        !out->subtree_end || (n > 0 && (!sa || !lcp)))
+        return null_ptr(c);
+    if (n > B200SA_TREE_MAX_N)
+        return fail(c, B200SA_ERR_TOO_LARGE, "suffix tree: n >= 2^31 (node ids are u32 with 0xFFFFFFFF reserved)");
+    if (cap < (n ? 2 * n : 1)) return fail(c, B200SA_ERR_BAD_ARG, "suffix tree: cap < max(1, 2n)");
     return B200SA_OK;
 }
 
-// Every failing exit of the tree and docs entry points passes through here (like host_build).
-static int tree_exit(b200sa_ctx *c, int rc) {
-    if (rc != B200SA_OK) {
-        if (c->stream) cudaStreamSynchronize(c->stream);
-        cudaGetLastError();
-        return rc;
+// The root alone, in the first entry of the device arrays dst[0, count): its values in root.
+static int root_dev(b200sa_ctx *c, uint32_t *const *dst, const uint32_t *root, int count, uint64_t *num_nodes) {
+    for (int k = 0; k < count; k++) {
+        cudaError_t e = cudaMemcpyAsync(dst[k], &root[k], 4, cudaMemcpyHostToDevice, c->stream);
+        if (e != cudaSuccess) return fail(c, B200SA_ERR_CUDA, cudaGetErrorString(e));
     }
-    return end_call(c);
+    CU_TRY(c, cudaStreamSynchronize(c->stream));
+    *num_nodes = 1;
+    return B200SA_OK;
+}
+
+static int suffix_tree_dev_core(b200sa_ctx *c, uint64_t n, const uint32_t *d_sa, const uint32_t *d_lcp,
+                                const b200sa_tree *out, uint64_t *num_nodes) {
+    if (n == 0) {
+        // the root alone: parent none, depth 0, range [0, 0), empty label, subtree [0, 1)
+        const uint32_t root[6] = {TREE_NONE, 0, 0, 0, 0, 1};
+        uint32_t *dst[6] = {out->parent, out->depth, out->sa_lo, out->sa_hi, out->label_start, out->subtree_end};
+        return root_dev(c, dst, root, 6, num_nodes);
+    }
+    TreeOut o{out->parent, out->depth, out->sa_lo, out->sa_hi, out->label_start, out->subtree_end};
+    return suffix_tree_core(c, (uint32_t)n, d_sa, d_lcp, o, num_nodes, TextLen{});
 }
 
 int b200sa_suffix_tree_dev(b200sa_ctx *c, uint64_t n, const uint32_t *d_sa, const uint32_t *d_lcp,
                            const b200sa_tree *out, uint64_t cap, uint64_t *num_nodes, void *stream) {
     TRY(tree_args(c, n, d_sa, d_lcp, out, cap, num_nodes));
-    CU_TRY(c, cudaSetDevice(c->device));
-    begin_call(c, stream);
+    TRY(enter(c, stream));
     *num_nodes = 0;
-    int rc = B200SA_OK;
-    if (n == 0) {
-        // the root alone: parent none, depth 0, range [0, 0), empty label, subtree [0, 1)
-        const uint32_t root[6] = {TREE_NONE, 0, 0, 0, 0, 1};
-        uint32_t *dst[6] = {out->parent, out->depth, out->sa_lo, out->sa_hi, out->label_start, out->subtree_end};
-        for (int k = 0; k < 6 && rc == B200SA_OK; k++) {
-            cudaError_t e = cudaMemcpyAsync(dst[k], &root[k], 4, cudaMemcpyHostToDevice, c->stream);
-            if (e != cudaSuccess) { c->last_error = cudaGetErrorString(e); rc = B200SA_ERR_CUDA; }
-        }
-        if (rc == B200SA_OK && cudaStreamSynchronize(c->stream) != cudaSuccess) rc = B200SA_ERR_CUDA;
-        if (rc == B200SA_OK) *num_nodes = 1;
-        return tree_exit(c, rc);
-    }
-    TreeOut o{out->parent, out->depth, out->sa_lo, out->sa_hi, out->label_start, out->subtree_end};
-    rc = suffix_tree_core(c, (uint32_t)n, d_sa, d_lcp, o, num_nodes, TextLen{});
-    return tree_exit(c, rc);
+    return leave(c, suffix_tree_dev_core(c, n, d_sa, d_lcp, out, num_nodes));
 }
 
 static int suffix_tree_host(b200sa_ctx *c, uint64_t n, const uint32_t *sa, const uint32_t *lcp, const b200sa_tree *out,
                             uint64_t *num_nodes) {
+    if (n == 0) {
+        out->parent[0] = TREE_NONE;
+        out->depth[0] = out->sa_lo[0] = out->sa_hi[0] = out->label_start[0] = 0;
+        out->subtree_end[0] = 1;
+        *num_nodes = 1;
+        return B200SA_OK;
+    }
     const uint64_t cap = 2 * n;
     TRY(ensure(c, c->sa, n * 4));
     TRY(ensure(c, c->lcp, n * 4));
@@ -1670,17 +1723,9 @@ static int suffix_tree_host(b200sa_ctx *c, uint64_t n, const uint32_t *sa, const
 int b200sa_suffix_tree(b200sa_ctx *c, uint64_t n, const uint32_t *sa, const uint32_t *lcp, const b200sa_tree *out,
                        uint64_t cap, uint64_t *num_nodes) {
     TRY(tree_args(c, n, sa, lcp, out, cap, num_nodes));
-    CU_TRY(c, cudaSetDevice(c->device));
-    begin_call(c, nullptr);
+    TRY(enter(c, nullptr));
     *num_nodes = 0;
-    if (n == 0) {
-        out->parent[0] = TREE_NONE;
-        out->depth[0] = out->sa_lo[0] = out->sa_hi[0] = out->label_start[0] = 0;
-        out->subtree_end[0] = 1;
-        *num_nodes = 1;
-        return end_call(c);
-    }
-    return tree_exit(c, suffix_tree_host(c, n, sa, lcp, out, num_nodes));
+    return leave(c, suffix_tree_host(c, n, sa, lcp, out, num_nodes));
 }
 
 // ------------------------------------------------------------ generalized suffix array without separators (SURVEY 8f-6)
@@ -1691,6 +1736,20 @@ static int docs_bad(b200sa_ctx *c, uint32_t bits) {
     if (bits & DOCS_BAD_RANGE) m += " an entry above n;";
     c->last_error = m;
     return B200SA_ERR_BAD_ARG;
+}
+
+// k_docs_check on the device doc_starts (ndocs >= 1), one read-back; *maxlen gets the longest document.
+static int docs_check_dev(b200sa_ctx *c, const uint32_t *d_starts, uint32_t ndocs, uint32_t n,
+                          uint32_t *maxlen = nullptr) {
+    TRY(ensure(c, c->small, 4096));
+    uint32_t *words = ptr<uint32_t>(c->small);           // [0] check bits, [1] longest document
+    CU_TRY(c, cudaMemsetAsync(words, 0, 8, c->stream));
+    LAUNCH(c, k_docs_check, cdiv(ndocs, BLK), d_starts, ndocs, n, words);
+    CU_TRY(c, cudaGetLastError());
+    TRY(read_words(c, words, maxlen ? 2 : 1));
+    if (c->h_pin[0]) return docs_bad(c, c->h_pin[0]);
+    if (maxlen) *maxlen = c->h_pin[1];
+    return B200SA_OK;
 }
 
 // The checks of k_docs_check on host entries doc_starts[first, first + count); *prev holds
@@ -1737,18 +1796,9 @@ static int docs_check_dev_copy(b200sa_ctx *c, uint64_t n, const uint32_t *d_star
 
 static int docs_args(b200sa_ctx *c, uint64_t n, const void *text, const void *starts, uint32_t ndocs, const void *gsa) {
     if (!c) return B200SA_ERR_BAD_ARG;
-    if ((n > 0 && (!text || !gsa)) || (ndocs > 0 && !starts)) {
-        c->last_error = "null pointer";
-        return B200SA_ERR_BAD_ARG;
-    }
-    if (n > B200SA_MAX_N) {
-        c->last_error = "text longer than 2^32-4096 bytes";
-        return B200SA_ERR_TOO_LARGE;
-    }
-    if (ndocs == 0 && n > 0) {
-        c->last_error = "doc_starts rejected: ndocs == 0 with n > 0;";
-        return B200SA_ERR_BAD_ARG;
-    }
+    if ((n > 0 && (!text || !gsa)) || (ndocs > 0 && !starts)) return null_ptr(c);
+    if (n > B200SA_MAX_N) return too_long(c);
+    if (ndocs == 0 && n > 0) return no_docs(c);
     return B200SA_OK;
 }
 
@@ -1756,15 +1806,10 @@ static int docs_args(b200sa_ctx *c, uint64_t n, const void *text, const void *st
 // build's own, docs_split, docs_sort, docs_place, docs_fill, docs_out.
 static int docs_core(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const uint32_t *d_starts, uint32_t ndocs,
                      uint32_t *d_gsa, uint32_t *d_glcp) {
-    TRY(ensure(c, c->small, 4096));
-    uint32_t *words = ptr<uint32_t>(c->small);           // [0] check bits / |A|, [1] longest document
     TRY(mark(c, "docs_check"));
-    CU_TRY(c, cudaMemsetAsync(words, 0, 8, c->stream));
-    LAUNCH(c, k_docs_check, cdiv(ndocs, BLK), d_starts, ndocs, n, words);
-    CU_TRY(c, cudaGetLastError());
-    TRY(read_words(c, words, 2));
-    if (c->h_pin[0]) return docs_bad(c, c->h_pin[0]);
-    const uint32_t maxlen = c->h_pin[1];
+    uint32_t maxlen;
+    TRY(docs_check_dev(c, d_starts, ndocs, n, &maxlen));
+    uint32_t *words = ptr<uint32_t>(c->small);           // [0] |A|
 
     // 1. SA and LCP of the concatenation
     TRY(ensure(c, c->sa, (size_t)n * 4));
@@ -1835,29 +1880,33 @@ static int docs_core(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const uin
     return B200SA_OK;
 }
 
+static int docs_build_dev_core(b200sa_ctx *c, const uint8_t *d_text, uint64_t n, const uint32_t *d_doc_starts,
+                               uint32_t ndocs, uint32_t *d_gsa, uint32_t *d_glcp) {
+    if (n >= 2) return docs_core(c, d_text, (uint32_t)n, d_doc_starts, ndocs, d_gsa, d_glcp);
+    // nothing to launch: doc_starts is checked from host copies, G = [0] and glcp = [0] for n = 1
+    TRY(docs_check_dev_copy(c, n, d_doc_starts, ndocs));
+    if (n == 1 && (cudaMemsetAsync(d_gsa, 0, 4, c->stream) != cudaSuccess ||
+                   (d_glcp && cudaMemsetAsync(d_glcp, 0, 4, c->stream) != cudaSuccess)))
+        return fail(c, B200SA_ERR_CUDA, "output write failed");
+    return B200SA_OK;
+}
+
 int b200sa_docs_build_dev(b200sa_ctx *c, const uint8_t *d_text, uint64_t n, const uint32_t *d_doc_starts,
                           uint32_t ndocs, uint32_t *d_gsa, uint32_t *d_glcp, void *stream) {
     TRY(docs_args(c, n, d_text, d_doc_starts, ndocs, d_gsa));
-    CU_TRY(c, cudaSetDevice(c->device));
-    begin_call(c, stream);
-    int rc = B200SA_OK;
-    if (n <= 1) {
-        // nothing to launch: doc_starts is checked from host copies, G = [0] and glcp = [0] for n = 1
-        rc = docs_check_dev_copy(c, n, d_doc_starts, ndocs);
-        if (rc == B200SA_OK && n == 1) {
-            if (cudaMemsetAsync(d_gsa, 0, 4, c->stream) != cudaSuccess ||
-                (d_glcp && cudaMemsetAsync(d_glcp, 0, 4, c->stream) != cudaSuccess)) {
-                c->last_error = "output write failed";
-                rc = B200SA_ERR_CUDA;
-            }
-        }
-        return tree_exit(c, rc);
-    }
-    return tree_exit(c, docs_core(c, d_text, (uint32_t)n, d_doc_starts, ndocs, d_gsa, d_glcp));
+    TRY(enter(c, stream));
+    return leave(c, docs_build_dev_core(c, d_text, n, d_doc_starts, ndocs, d_gsa, d_glcp));
 }
 
 static int docs_host(b200sa_ctx *c, const uint8_t *text, uint32_t n, const uint32_t *starts, uint32_t ndocs,
                      uint32_t *gsa_out, uint32_t *glcp_out) {
+    if (n <= 1) {
+        if (n == 1) {
+            gsa_out[0] = 0;
+            if (glcp_out) glcp_out[0] = 0;
+        }
+        return B200SA_OK;
+    }
     TRY(ensure(c, c->text, n));
     TRY(ensure(c, c->docs_starts, (size_t)ndocs * 4));
     TRY(ensure(c, c->docs_out, (size_t)n * 4 * (glcp_out ? 2 : 1)));
@@ -1879,52 +1928,45 @@ int b200sa_docs_build(b200sa_ctx *c, const uint8_t *text, uint64_t n, const uint
                       uint32_t *gsa_out, uint32_t *glcp_out) {
     TRY(docs_args(c, n, text, doc_starts, ndocs, gsa_out));
     TRY(docs_check_host(c, n, doc_starts, ndocs));
-    CU_TRY(c, cudaSetDevice(c->device));
-    begin_call(c, nullptr);
-    if (n <= 1) {
-        if (n == 1) {
-            gsa_out[0] = 0;
-            if (glcp_out) glcp_out[0] = 0;
-        }
-        return end_call(c);
-    }
-    return tree_exit(c, docs_host(c, text, (uint32_t)n, doc_starts, ndocs, gsa_out, glcp_out));
+    TRY(enter(c, nullptr));
+    return leave(c, docs_host(c, text, (uint32_t)n, doc_starts, ndocs, gsa_out, glcp_out));
 }
 
-int b200sa_docs_positions_dev(b200sa_ctx *c, const uint8_t *d_text, uint64_t n, const uint32_t *d_gsa,
-                              const uint32_t *d_doc_starts, uint32_t ndocs, const uint8_t *d_queries,
-                              const uint64_t *d_q_off, uint32_t nq, uint32_t *d_start, uint32_t *d_end, void *stream) {
-    if (!c || (nq > 0 && (!d_q_off || !d_start || !d_end)) ||
-        (n > 0 && (!d_text || !d_gsa || !d_doc_starts || ndocs == 0)))
-        return B200SA_ERR_BAD_ARG;
-    if (n > B200SA_MAX_N) return B200SA_ERR_TOO_LARGE;
-    CU_TRY(c, cudaSetDevice(c->device));
-    begin_call(c, stream);
+static int docs_positions_core(b200sa_ctx *c, const uint8_t *d_text, uint64_t n, const uint32_t *d_gsa,
+                               const uint32_t *d_doc_starts, uint32_t ndocs, const uint8_t *d_queries,
+                               const uint64_t *d_q_off, uint32_t nq, uint32_t *d_start, uint32_t *d_end) {
     if (nq > 0) {
         LAUNCH(c, k_positions<DocsEnd>, cdiv(nq, BLK), d_text, (uint32_t)n, d_gsa, d_queries, d_q_off, nq, d_start,
                d_end, DocsEnd{d_doc_starts, ndocs, (uint32_t)n});
         CU_TRY(c, cudaGetLastError());
     }
-    return end_call(c);
+    return B200SA_OK;
+}
+
+int b200sa_docs_positions_dev(b200sa_ctx *c, const uint8_t *d_text, uint64_t n, const uint32_t *d_gsa,
+                              const uint32_t *d_doc_starts, uint32_t ndocs, const uint8_t *d_queries,
+                              const uint64_t *d_q_off, uint32_t nq, uint32_t *d_start, uint32_t *d_end, void *stream) {
+    if (!c) return B200SA_ERR_BAD_ARG;
+    if ((nq > 0 && (!d_q_off || !d_start || !d_end)) || (n > 0 && (!d_text || !d_gsa || !d_doc_starts)))
+        return null_ptr(c);
+    if (ndocs == 0 && n > 0) return no_docs(c);
+    if (n > B200SA_MAX_N) return too_long(c);
+    TRY(enter(c, stream));
+    return leave(c, docs_positions_core(c, d_text, n, d_gsa, d_doc_starts, ndocs, d_queries, d_q_off, nq, d_start,
+                                        d_end));
 }
 
 // ------------------------------------------------------------ generalized suffix tree with document counts (SURVEY 8f-7)
 static int docs_tree_args(b200sa_ctx *c, uint64_t n, const void *gsa, const void *glcp, const void *starts,
                           uint32_t ndocs, const b200sa_docs_tree_out *out, uint64_t cap, uint64_t *num_nodes) {
-    if (!c || !out || !num_nodes) return B200SA_ERR_BAD_ARG;
+    if (!c) return B200SA_ERR_BAD_ARG;
+    if (!out) return null_ptr(c);
     TRY(tree_args(c, n, gsa, glcp, &out->tree, cap, num_nodes));
-    if (!out->term_end || !out->doc_count || (ndocs > 0 && !starts)) {
-        c->last_error = "null pointer";
-        return B200SA_ERR_BAD_ARG;
-    }
-    if (ndocs == 0 && n > 0) {
-        c->last_error = "doc_starts rejected: ndocs == 0 with n > 0;";
-        return B200SA_ERR_BAD_ARG;
-    }
+    if (!out->term_end || !out->doc_count || (ndocs > 0 && !starts)) return null_ptr(c);
+    if (ndocs == 0 && n > 0) return no_docs(c);
     return B200SA_OK;
 }
 
-extern "C++" {
 // The tree's document-sort key: the document of a rank.
 template <int OSI>
 static int dtree_sort(b200sa_ctx *c, const uint32_t *doc, uint32_t n, int bits, uint32_t **kout, uint32_t **vout) {
@@ -1932,7 +1974,6 @@ static int dtree_sort(b200sa_ctx *c, const uint32_t *doc, uint32_t n, int bits, 
         c, LoadArr<uint32_t>{doc}, LoadIndex{}, ptr<uint32_t>(c->p0), ptr<uint32_t>(c->p1), ptr<uint32_t>(c->v0),
         ptr<uint32_t>(c->v1), n, bits, kout, vout);
 }
-}  // extern "C++"
 
 // n >= 1, ndocs >= 1, device inputs and outputs (capacity >= 2n each).  Phases: docs_check (when
 // check_starts), dtree_len, the tree's five, dtree_term, dtree_sort, dtree_pairs, dtree_count.
@@ -1943,11 +1984,7 @@ static int docs_tree_core(b200sa_ctx *c, uint32_t n, const uint32_t *d_g, const 
     uint32_t *words = ptr<uint32_t>(c->small);           // [0, 2) the tree's, [2] the check bits of the stages after it
     if (check_starts) {
         TRY(mark(c, "docs_check"));
-        CU_TRY(c, cudaMemsetAsync(words, 0, 8, c->stream));
-        LAUNCH(c, k_docs_check, cdiv(ndocs, BLK), d_starts, ndocs, n, words);
-        CU_TRY(c, cudaGetLastError());
-        TRY(read_words(c, words, 1));
-        if (c->h_pin[0]) return docs_bad(c, c->h_pin[0]);
+        TRY(docs_check_dev(c, d_starts, ndocs, n));
     }
     // document and suffix length of every rank, then the tree with rule 3'
     TRY(mark(c, "dtree_len"));
@@ -1995,33 +2032,38 @@ static int docs_tree_core(b200sa_ctx *c, uint32_t n, const uint32_t *d_g, const 
     return B200SA_OK;
 }
 
+// n = 0: doc_starts checked from host copies; the root alone, without terminals or documents.
+static int docs_tree_root_dev(b200sa_ctx *c, const uint32_t *d_starts, uint32_t ndocs, const b200sa_docs_tree_out *out,
+                              uint64_t *num_nodes) {
+    TRY(docs_check_dev_copy(c, 0, d_starts, ndocs));
+    const uint32_t root[8] = {TREE_NONE, 0, 0, 0, 0, 1, 0, 0};
+    const b200sa_tree &t = out->tree;
+    uint32_t *dst[8] = {t.parent, t.depth, t.sa_lo, t.sa_hi, t.label_start, t.subtree_end, out->term_end,
+                        out->doc_count};
+    return root_dev(c, dst, root, 8, num_nodes);
+}
+
 int b200sa_docs_tree_dev(b200sa_ctx *c, uint64_t n, const uint32_t *d_gsa, const uint32_t *d_glcp,
                          const uint32_t *d_doc_starts, uint32_t ndocs, const b200sa_docs_tree_out *out, uint64_t cap,
                          uint64_t *num_nodes, void *stream) {
     TRY(docs_tree_args(c, n, d_gsa, d_glcp, d_doc_starts, ndocs, out, cap, num_nodes));
-    CU_TRY(c, cudaSetDevice(c->device));
-    begin_call(c, stream);
+    TRY(enter(c, stream));
     *num_nodes = 0;
-    if (n == 0) {
-        // doc_starts checked from host copies; the root alone, without terminals or documents
-        int rc = docs_check_dev_copy(c, 0, d_doc_starts, ndocs);
-        const uint32_t root[8] = {TREE_NONE, 0, 0, 0, 0, 1, 0, 0};
-        const b200sa_tree &t = out->tree;
-        uint32_t *dst[8] = {t.parent, t.depth, t.sa_lo, t.sa_hi, t.label_start, t.subtree_end, out->term_end,
-                            out->doc_count};
-        for (int k = 0; k < 8 && rc == B200SA_OK; k++) {
-            cudaError_t e = cudaMemcpyAsync(dst[k], &root[k], 4, cudaMemcpyHostToDevice, c->stream);
-            if (e != cudaSuccess) { c->last_error = cudaGetErrorString(e); rc = B200SA_ERR_CUDA; }
-        }
-        if (rc == B200SA_OK && cudaStreamSynchronize(c->stream) != cudaSuccess) rc = B200SA_ERR_CUDA;
-        if (rc == B200SA_OK) *num_nodes = 1;
-        return tree_exit(c, rc);
-    }
-    return tree_exit(c, docs_tree_core(c, (uint32_t)n, d_gsa, d_glcp, d_doc_starts, ndocs, true, out, num_nodes));
+    if (n == 0) return leave(c, docs_tree_root_dev(c, d_doc_starts, ndocs, out, num_nodes));
+    return leave(c, docs_tree_core(c, (uint32_t)n, d_gsa, d_glcp, d_doc_starts, ndocs, true, out, num_nodes));
 }
 
 static int docs_tree_host(b200sa_ctx *c, uint32_t n, const uint32_t *gsa, const uint32_t *glcp, const uint32_t *starts,
                           uint32_t ndocs, const b200sa_docs_tree_out *out, uint64_t *num_nodes) {
+    if (n == 0) {
+        const b200sa_tree &t = out->tree;
+        t.parent[0] = TREE_NONE;
+        t.depth[0] = t.sa_lo[0] = t.sa_hi[0] = t.label_start[0] = 0;
+        t.subtree_end[0] = 1;
+        out->term_end[0] = out->doc_count[0] = 0;
+        *num_nodes = 1;
+        return B200SA_OK;
+    }
     const uint64_t cap = 2 * (uint64_t)n;
     TRY(ensure(c, c->sa, (size_t)n * 4));
     TRY(ensure(c, c->lcp, (size_t)n * 4));
@@ -2054,65 +2096,43 @@ int b200sa_docs_tree(b200sa_ctx *c, uint64_t n, const uint32_t *gsa, const uint3
                      uint32_t ndocs, const b200sa_docs_tree_out *out, uint64_t cap, uint64_t *num_nodes) {
     TRY(docs_tree_args(c, n, gsa, glcp, doc_starts, ndocs, out, cap, num_nodes));
     TRY(docs_check_host(c, n, doc_starts, ndocs));
-    CU_TRY(c, cudaSetDevice(c->device));
-    begin_call(c, nullptr);
+    TRY(enter(c, nullptr));
     *num_nodes = 0;
-    if (n == 0) {
-        const b200sa_tree &t = out->tree;
-        t.parent[0] = TREE_NONE;
-        t.depth[0] = t.sa_lo[0] = t.sa_hi[0] = t.label_start[0] = 0;
-        t.subtree_end[0] = 1;
-        out->term_end[0] = out->doc_count[0] = 0;
-        *num_nodes = 1;
-        return end_call(c);
-    }
-    return tree_exit(c, docs_tree_host(c, (uint32_t)n, gsa, glcp, doc_starts, ndocs, out, num_nodes));
+    return leave(c, docs_tree_host(c, (uint32_t)n, gsa, glcp, doc_starts, ndocs, out, num_nodes));
+}
+
+static int docs_tree_counts_core(b200sa_ctx *c, const uint32_t *d_sa_lo, const uint32_t *d_sa_hi,
+                                 const uint32_t *d_doc_count, uint64_t num_nodes, const uint32_t *d_start,
+                                 const uint32_t *d_end, uint32_t nq, uint32_t *d_count) {
+    if (nq == 0) return B200SA_OK;
+    TRY(ensure(c, c->small, 4096));
+    uint32_t *flag = ptr<uint32_t>(c->small);
+    CU_TRY(c, cudaMemsetAsync(flag, 0, 4, c->stream));
+    LAUNCH(c, k_dtree_counts, cdiv(nq, BLK), d_sa_lo, d_sa_hi, d_doc_count, (uint32_t)num_nodes, d_start, d_end, nq,
+           d_count, flag);
+    CU_TRY(c, cudaGetLastError());
+    TRY(read_words(c, flag, 1));
+    if (c->h_pin[0]) return fail(c, B200SA_ERR_BAD_ARG, "docs tree counts: a range [start, end) is the range of no node");
+    return B200SA_OK;
 }
 
 int b200sa_docs_tree_counts_dev(b200sa_ctx *c, const uint32_t *d_sa_lo, const uint32_t *d_sa_hi,
                                 const uint32_t *d_doc_count, uint64_t num_nodes, const uint32_t *d_start,
                                 const uint32_t *d_end, uint32_t nq, uint32_t *d_count, void *stream) {
     if (!c) return B200SA_ERR_BAD_ARG;
-    if (nq > 0 && (!d_sa_lo || !d_sa_hi || !d_doc_count || !d_start || !d_end || !d_count)) {
-        c->last_error = "null pointer";
-        return B200SA_ERR_BAD_ARG;
-    }
-    if (nq > 0 && (num_nodes == 0 || num_nodes > 2 * B200SA_TREE_MAX_N)) {
-        c->last_error = "docs tree counts: num_nodes must be in [1, 2 * B200SA_TREE_MAX_N]";
-        return B200SA_ERR_BAD_ARG;
-    }
-    CU_TRY(c, cudaSetDevice(c->device));
-    begin_call(c, stream);
-    if (nq == 0) return end_call(c);
-    int rc = ensure(c, c->small, 4096);
-    uint32_t *flag = ptr<uint32_t>(c->small);
-    if (rc == B200SA_OK && cudaMemsetAsync(flag, 0, 4, c->stream) != cudaSuccess) rc = B200SA_ERR_CUDA;
-    if (rc == B200SA_OK) {
-        LAUNCH(c, k_dtree_counts, cdiv(nq, BLK), d_sa_lo, d_sa_hi, d_doc_count, (uint32_t)num_nodes, d_start, d_end, nq,
-               d_count, flag);
-        if (cudaGetLastError() != cudaSuccess) rc = B200SA_ERR_CUDA;
-    }
-    if (rc == B200SA_OK) rc = read_words(c, flag, 1);
-    if (rc == B200SA_OK && c->h_pin[0]) {
-        c->last_error = "docs tree counts: a range [start, end) is the range of no node";
-        rc = B200SA_ERR_BAD_ARG;
-    }
-    if (rc == B200SA_ERR_CUDA && c->last_error.empty()) c->last_error = "kernel launch failed";
-    return tree_exit(c, rc);
+    if (nq > 0 && (!d_sa_lo || !d_sa_hi || !d_doc_count || !d_start || !d_end || !d_count)) return null_ptr(c);
+    if (nq > 0 && (num_nodes == 0 || num_nodes > 2 * B200SA_TREE_MAX_N))
+        return fail(c, B200SA_ERR_BAD_ARG, "docs tree counts: num_nodes must be in [1, 2 * B200SA_TREE_MAX_N]");
+    TRY(enter(c, stream));
+    return leave(c, docs_tree_counts_core(c, d_sa_lo, d_sa_hi, d_doc_count, num_nodes, d_start, d_end, nq, d_count));
 }
 
 // ------------------------------------------------------------ document listing (SURVEY 8f-8)
 // n >= 1, ndocs >= 1.  Phases: docs_check, dlist_len, dlist_sort, dlist_prev.
 static int docs_list_index_core(b200sa_ctx *c, uint32_t n, const uint32_t *d_g, const uint32_t *d_starts,
                                 uint32_t ndocs, uint32_t *d_byd, uint32_t *d_prev) {
-    TRY(ensure(c, c->small, 4096));
-    uint32_t *words = ptr<uint32_t>(c->small);
     TRY(mark(c, "docs_check"));
-    CU_TRY(c, cudaMemsetAsync(words, 0, 8, c->stream));
-    LAUNCH(c, k_docs_check, cdiv(ndocs, BLK), d_starts, ndocs, n, words);
-    CU_TRY(c, cudaGetLastError());
-    TRY(read_words(c, words, 1));
-    if (c->h_pin[0]) return docs_bad(c, c->h_pin[0]);
+    TRY(docs_check_dev(c, d_starts, ndocs, n));
     TRY(mark(c, "dlist_len"));                          // the document of every rank (its length is not used)
     TRY(ensure(c, c->isa, (size_t)n * 4));
     TRY(ensure(c, c->rank, (size_t)n * 4));
@@ -2137,19 +2157,12 @@ static int docs_list_index_core(b200sa_ctx *c, uint32_t n, const uint32_t *d_g, 
 int b200sa_docs_list_index_dev(b200sa_ctx *c, uint64_t n, const uint32_t *d_gsa, const uint32_t *d_doc_starts,
                                uint32_t ndocs, uint32_t *d_byd, uint32_t *d_prev, void *stream) {
     if (!c) return B200SA_ERR_BAD_ARG;
-    if ((n > 0 && (!d_gsa || !d_byd || !d_prev)) || (ndocs > 0 && !d_doc_starts)) {
-        c->last_error = "null pointer";
-        return B200SA_ERR_BAD_ARG;
-    }
-    if (ndocs == 0 && n > 0) {
-        c->last_error = "doc_starts rejected: ndocs == 0 with n > 0;";
-        return B200SA_ERR_BAD_ARG;
-    }
-    if (n > B200SA_MAX_N) return B200SA_ERR_TOO_LARGE;
-    CU_TRY(c, cudaSetDevice(c->device));
-    begin_call(c, stream);
-    if (n == 0) return tree_exit(c, docs_check_dev_copy(c, 0, d_doc_starts, ndocs));
-    return tree_exit(c, docs_list_index_core(c, (uint32_t)n, d_gsa, d_doc_starts, ndocs, d_byd, d_prev));
+    if ((n > 0 && (!d_gsa || !d_byd || !d_prev)) || (ndocs > 0 && !d_doc_starts)) return null_ptr(c);
+    if (ndocs == 0 && n > 0) return no_docs(c);
+    if (n > B200SA_MAX_N) return too_long(c);
+    TRY(enter(c, stream));
+    if (n == 0) return leave(c, docs_check_dev_copy(c, 0, d_doc_starts, ndocs));
+    return leave(c, docs_list_index_core(c, (uint32_t)n, d_gsa, d_doc_starts, ndocs, d_byd, d_prev));
 }
 
 // The listing's front half, shared by the listing and top-k: nq >= 1.  Writes the offsets (nq + 1) and
@@ -2173,15 +2186,11 @@ static int docs_list_front(b200sa_ctx *c, uint32_t n, const uint32_t *d_g, const
     TRY((dev_scan<OpSum64>(c, DListChunks{d_start, d_end, nq, n, words}, OutStoreExcl64{item_start}, (uint64_t)nq + 1,
                            d_items)));
     TRY(read_words(c, words, 4));
-    if (c->h_pin[0] & DLIST_BAD_RANGE) {
-        c->last_error = "docs list: a range [start, end) has start > end or end > n";
-        return B200SA_ERR_BAD_ARG;
-    }
-    const uint64_t items = c->h_pin[2] | ((uint64_t)c->h_pin[3] << 32);
-    if (items > (uint64_t)0x7fffffff * NWARP) {
-        c->last_error = "docs list: more than 2^31 * 8 chunks of 1024 ranks in one batch";
-        return B200SA_ERR_TOO_LARGE;
-    }
+    if (c->h_pin[0] & DLIST_BAD_RANGE)
+        return fail(c, B200SA_ERR_BAD_ARG, "docs list: a range [start, end) has start > end or end > n");
+    const uint64_t items = pin_u64(c, 2);
+    if (items > (uint64_t)0x7fffffff * NWARP)
+        return fail(c, B200SA_ERR_TOO_LARGE, "docs list: more than 2^31 * 8 chunks of 1024 ranks in one batch");
     A.qs = d_start; A.qe = d_end; A.item_start = item_start; A.nq = nq; A.items = items;
     TRY(ensure(c, c->p0, (size_t)items * 4));
     TRY(ensure(c, c->k64b, ((size_t)items + 1) * 8));
@@ -2194,7 +2203,7 @@ static int docs_list_front(b200sa_ctx *c, uint32_t n, const uint32_t *d_g, const
     TRY((dev_scan<OpSum64>(c, InCount64{cnt, items}, OutStoreExcl64{item_off}, items + 1, d_total)));
     LAUNCH(c, k_dlist_qoff, cdiv((uint64_t)nq + 1, BLK), item_start, item_off, nq, reinterpret_cast<u64 *>(d_offsets));
     TRY(read_words(c, words + 4, 2));
-    *total = c->h_pin[0] | ((uint64_t)c->h_pin[1] << 32);
+    *total = pin_u64(c, 0);
     *Aout = A;
     *item_off_out = item_off;
     return B200SA_OK;
@@ -2220,31 +2229,29 @@ static int docs_list_core(b200sa_ctx *c, uint32_t n, const uint32_t *d_g, const 
     return B200SA_OK;
 }
 
+// The answer of the count-then-fetch entry points to a batch of no queries: offsets = [0] (the
+// caller sets *total = 0).
+static int empty_batch(b200sa_ctx *c, uint64_t *d_offsets) {
+    CU_TRY(c, cudaMemsetAsync(d_offsets, 0, 8, c->stream));
+    CU_TRY(c, cudaStreamSynchronize(c->stream));
+    return B200SA_OK;
+}
+
 int b200sa_docs_list_dev(b200sa_ctx *c, uint64_t n, const uint32_t *d_gsa, const uint32_t *d_doc_starts,
                          uint32_t ndocs, const uint32_t *d_byd, const uint32_t *d_prev, const uint32_t *d_start,
                          const uint32_t *d_end, uint32_t nq, uint64_t *d_offsets, uint32_t *d_docs, uint32_t *d_tf,
                          uint64_t cap, uint64_t *total, void *stream) {
     if (!c) return B200SA_ERR_BAD_ARG;
     if (!total || !d_offsets || (nq > 0 && (!d_start || !d_end)) || (cap > 0 && !d_docs) ||
-        (n > 0 && (!d_gsa || !d_doc_starts || !d_byd || !d_prev))) {
-        c->last_error = "null pointer";
-        return B200SA_ERR_BAD_ARG;
-    }
-    if (ndocs == 0 && n > 0) {
-        c->last_error = "doc_starts rejected: ndocs == 0 with n > 0;";
-        return B200SA_ERR_BAD_ARG;
-    }
-    if (n > B200SA_MAX_N) return B200SA_ERR_TOO_LARGE;
-    CU_TRY(c, cudaSetDevice(c->device));
-    begin_call(c, stream);
+        (n > 0 && (!d_gsa || !d_doc_starts || !d_byd || !d_prev)))
+        return null_ptr(c);
+    if (ndocs == 0 && n > 0) return no_docs(c);
+    if (n > B200SA_MAX_N) return too_long(c);
+    TRY(enter(c, stream));
     *total = 0;
-    if (nq == 0) {
-        CU_TRY(c, cudaMemsetAsync(d_offsets, 0, 8, c->stream));
-        CU_TRY(c, cudaStreamSynchronize(c->stream));
-        return end_call(c);
-    }
-    return tree_exit(c, docs_list_core(c, (uint32_t)n, d_gsa, d_doc_starts, ndocs, d_byd, d_prev, d_start, d_end, nq,
-                                       d_offsets, d_docs, d_tf, cap, total));
+    if (nq == 0) return leave(c, empty_batch(c, d_offsets));
+    return leave(c, docs_list_core(c, (uint32_t)n, d_gsa, d_doc_starts, ndocs, d_byd, d_prev, d_start, d_end, nq,
+                                   d_offsets, d_docs, d_tf, cap, total));
 }
 
 // ------------------------------------------------------------ top-k document retrieval (SURVEY 8f-9)
@@ -2353,24 +2360,15 @@ int b200sa_docs_topk_dev(b200sa_ctx *c, uint64_t n, const uint32_t *d_gsa, const
                          uint32_t *d_tf, void *stream) {
     if (!c) return B200SA_ERR_BAD_ARG;
     if (!d_count || !d_docs || !d_tf || (nq > 0 && (!d_start || !d_end)) ||
-        (n > 0 && (!d_gsa || !d_doc_starts || !d_byd || !d_prev))) {
-        c->last_error = "null pointer";
-        return B200SA_ERR_BAD_ARG;
-    }
-    if (ndocs == 0 && n > 0) {
-        c->last_error = "doc_starts rejected: ndocs == 0 with n > 0;";
-        return B200SA_ERR_BAD_ARG;
-    }
-    if (k == 0 || k > B200SA_TOPK_MAX) {
-        c->last_error = "docs topk: k must be in 1 .. B200SA_TOPK_MAX";
-        return B200SA_ERR_BAD_ARG;
-    }
-    if (n > B200SA_MAX_N) return B200SA_ERR_TOO_LARGE;
-    CU_TRY(c, cudaSetDevice(c->device));
-    begin_call(c, stream);
-    if (nq == 0) return end_call(c);
-    return tree_exit(c, docs_topk_core(c, (uint32_t)n, d_gsa, d_doc_starts, ndocs, d_byd, d_prev, d_start, d_end, nq,
-                                       k, d_count, d_docs, d_tf));
+        (n > 0 && (!d_gsa || !d_doc_starts || !d_byd || !d_prev)))
+        return null_ptr(c);
+    if (ndocs == 0 && n > 0) return no_docs(c);
+    if (k == 0 || k > B200SA_TOPK_MAX) return fail(c, B200SA_ERR_BAD_ARG, "docs topk: k must be in 1 .. B200SA_TOPK_MAX");
+    if (n > B200SA_MAX_N) return too_long(c);
+    TRY(enter(c, stream));
+    if (nq == 0) return leave(c, B200SA_OK);
+    return leave(c, docs_topk_core(c, (uint32_t)n, d_gsa, d_doc_starts, ndocs, d_byd, d_prev, d_start, d_end, nq, k,
+                                   d_count, d_docs, d_tf));
 }
 
 // ------------------------------------------------------------ matching statistics and SMEMs (DESIGN 6b f-10)
@@ -2397,22 +2395,14 @@ static int match_args(b200sa_ctx *c, uint64_t n, const void *text, const void *s
                       const void *q_off, uint32_t nq, uint64_t q_bytes, const void *len, const void *start,
                       const void *end) {
     if (!c) return B200SA_ERR_BAD_ARG;
-    if ((n > 0 && (!text || !sa)) || (nq > 0 && !q_off) || (q_bytes > 0 && (!queries || !len))) {
-        c->last_error = "null pointer";
-        return B200SA_ERR_BAD_ARG;
-    }
-    if ((start == nullptr) != (end == nullptr)) {
-        c->last_error = "match stats: d_start and d_end are both given or both NULL";
-        return B200SA_ERR_BAD_ARG;
-    }
-    if (n > B200SA_MAX_N || q_bytes > B200SA_MAX_N) {
-        c->last_error = "text or queries longer than 2^32-4096 bytes";
-        return B200SA_ERR_TOO_LARGE;
-    }
+    if ((n > 0 && (!text || !sa)) || (nq > 0 && !q_off) || (q_bytes > 0 && (!queries || !len))) return null_ptr(c);
+    if ((start == nullptr) != (end == nullptr))
+        return fail(c, B200SA_ERR_BAD_ARG, "match stats: d_start and d_end are both given or both NULL");
+    if (n > B200SA_MAX_N || q_bytes > B200SA_MAX_N)
+        return fail(c, B200SA_ERR_TOO_LARGE, "text or queries longer than 2^32-4096 bytes");
     return B200SA_OK;
 }
 
-extern "C++" {
 // nq >= 1, q_bytes >= 1.  d_starts non-null (EndF = DocsEnd): doc_starts is verified with q_off.  Phases:
 // match_check, match_levels (with ranges), match_search.
 template <class EndF>
@@ -2422,14 +2412,7 @@ static int match_stats_core(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, co
                             const uint32_t *d_starts, uint32_t ndocs) {
     TRY(mark(c, "match_check"));
     TRY(match_check(c, d_q_off, nq, q_bytes));
-    if (n > 0 && d_starts) {
-        uint32_t *words = ptr<uint32_t>(c->small);
-        CU_TRY(c, cudaMemsetAsync(words, 0, 8, c->stream));
-        LAUNCH(c, k_docs_check, cdiv(ndocs, BLK), d_starts, ndocs, n, words);
-        CU_TRY(c, cudaGetLastError());
-        TRY(read_words(c, words, 1));
-        if (c->h_pin[0]) return docs_bad(c, c->h_pin[0]);
-    }
+    if (n > 0 && d_starts) TRY(docs_check_dev(c, d_starts, ndocs, n));
     if (n == 0) {                                        // nothing occurs
         CU_TRY(c, cudaMemsetAsync(d_len, 0, q_bytes * 4, c->stream));
         if (d_start) {
@@ -2456,21 +2439,16 @@ static int match_stats_core(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, co
     CU_TRY(c, cudaGetLastError());
     return B200SA_OK;
 }
-}  // extern "C++"
 
 int b200sa_match_stats_dev(b200sa_ctx *c, const uint8_t *d_text, uint64_t n, const uint32_t *d_sa,
                            const uint32_t *d_lcp, const uint8_t *d_queries, const uint64_t *d_q_off, uint32_t nq,
                            uint64_t q_bytes, uint32_t *d_len, uint32_t *d_start, uint32_t *d_end, void *stream) {
     TRY(match_args(c, n, d_text, d_sa, d_queries, d_q_off, nq, q_bytes, d_len, d_start, d_end));
-    if (n > 0 && d_start && !d_lcp) {
-        c->last_error = "null pointer";
-        return B200SA_ERR_BAD_ARG;
-    }
-    CU_TRY(c, cudaSetDevice(c->device));
-    begin_call(c, stream);
-    if (nq == 0 || q_bytes == 0) return end_call(c);
-    return tree_exit(c, match_stats_core(c, d_text, (uint32_t)n, d_sa, d_lcp, d_queries, d_q_off, nq, q_bytes, d_len,
-                                         d_start, d_end, TextEnd{(uint32_t)n}, nullptr, 0));
+    if (n > 0 && d_start && !d_lcp) return null_ptr(c);
+    TRY(enter(c, stream));
+    if (nq == 0 || q_bytes == 0) return leave(c, B200SA_OK);
+    return leave(c, match_stats_core(c, d_text, (uint32_t)n, d_sa, d_lcp, d_queries, d_q_off, nq, q_bytes, d_len,
+                                     d_start, d_end, TextEnd{(uint32_t)n}, nullptr, 0));
 }
 
 int b200sa_docs_match_stats_dev(b200sa_ctx *c, const uint8_t *d_text, uint64_t n, const uint32_t *d_gsa,
@@ -2478,20 +2456,12 @@ int b200sa_docs_match_stats_dev(b200sa_ctx *c, const uint8_t *d_text, uint64_t n
                                 const uint8_t *d_queries, const uint64_t *d_q_off, uint32_t nq, uint64_t q_bytes,
                                 uint32_t *d_len, uint32_t *d_start, uint32_t *d_end, void *stream) {
     TRY(match_args(c, n, d_text, d_gsa, d_queries, d_q_off, nq, q_bytes, d_len, d_start, d_end));
-    if (n > 0 && ((d_start && !d_glcp) || !d_doc_starts)) {
-        c->last_error = "null pointer";
-        return B200SA_ERR_BAD_ARG;
-    }
-    if (ndocs == 0 && n > 0) {
-        c->last_error = "doc_starts rejected: ndocs == 0 with n > 0;";
-        return B200SA_ERR_BAD_ARG;
-    }
-    CU_TRY(c, cudaSetDevice(c->device));
-    begin_call(c, stream);
-    if (nq == 0 || q_bytes == 0) return end_call(c);
-    return tree_exit(c, match_stats_core(c, d_text, (uint32_t)n, d_gsa, d_glcp, d_queries, d_q_off, nq, q_bytes,
-                                         d_len, d_start, d_end, DocsEnd{d_doc_starts, ndocs, (uint32_t)n},
-                                         d_doc_starts, ndocs));
+    if (n > 0 && ((d_start && !d_glcp) || !d_doc_starts)) return null_ptr(c);
+    if (ndocs == 0 && n > 0) return no_docs(c);
+    TRY(enter(c, stream));
+    if (nq == 0 || q_bytes == 0) return leave(c, B200SA_OK);
+    return leave(c, match_stats_core(c, d_text, (uint32_t)n, d_gsa, d_glcp, d_queries, d_q_off, nq, q_bytes, d_len,
+                                     d_start, d_end, DocsEnd{d_doc_starts, ndocs, (uint32_t)n}, d_doc_starts, ndocs));
 }
 
 // nq >= 1.  Phases: match_check, smem_flag, smem_scan, smem_emit.
@@ -2522,58 +2492,40 @@ int b200sa_smems_dev(b200sa_ctx *c, const uint64_t *d_q_off, uint32_t nq, uint64
                      uint32_t min_len, uint64_t *d_offsets, uint32_t *d_qpos, uint64_t cap, uint64_t *total,
                      void *stream) {
     if (!c) return B200SA_ERR_BAD_ARG;
-    if (!total || !d_offsets || (nq > 0 && !d_q_off) || (q_bytes > 0 && !d_len) || (cap > 0 && !d_qpos)) {
-        c->last_error = "null pointer";
-        return B200SA_ERR_BAD_ARG;
-    }
-    if (min_len == 0) {
-        c->last_error = "smems: min_len must be at least 1";
-        return B200SA_ERR_BAD_ARG;
-    }
-    if (q_bytes > B200SA_MAX_N) {
-        c->last_error = "queries longer than 2^32-4096 bytes";
-        return B200SA_ERR_TOO_LARGE;
-    }
-    CU_TRY(c, cudaSetDevice(c->device));
-    begin_call(c, stream);
+    if (!total || !d_offsets || (nq > 0 && !d_q_off) || (q_bytes > 0 && !d_len) || (cap > 0 && !d_qpos))
+        return null_ptr(c);
+    if (min_len == 0) return fail(c, B200SA_ERR_BAD_ARG, "smems: min_len must be at least 1");
+    if (q_bytes > B200SA_MAX_N) return fail(c, B200SA_ERR_TOO_LARGE, "queries longer than 2^32-4096 bytes");
+    TRY(enter(c, stream));
     *total = 0;
-    if (nq == 0) {
-        CU_TRY(c, cudaMemsetAsync(d_offsets, 0, 8, c->stream));
-        CU_TRY(c, cudaStreamSynchronize(c->stream));
-        return end_call(c);
-    }
-    return tree_exit(c, smems_core(c, d_q_off, nq, q_bytes, d_len, min_len, d_offsets, d_qpos, cap, total));
+    if (nq == 0) return leave(c, empty_batch(c, d_offsets));
+    return leave(c, smems_core(c, d_q_off, nq, q_bytes, d_len, min_len, d_offsets, d_qpos, cap, total));
 }
 
 // ------------------------------------------------------------ repeats (DESIGN 6b f-11)
 static int repeat_args(b200sa_ctx *c, uint64_t n, const void *sa, const void *lcp) {
     if (!c) return B200SA_ERR_BAD_ARG;
-    if (n > 0 && (!sa || !lcp)) {
-        c->last_error = "null pointer";
-        return B200SA_ERR_BAD_ARG;
-    }
-    if (n > B200SA_MAX_N) {
-        c->last_error = "text longer than 2^32-4096 bytes";
-        return B200SA_ERR_TOO_LARGE;
-    }
+    if (n > 0 && (!sa || !lcp)) return null_ptr(c);
+    if (n > B200SA_MAX_N) return too_long(c);
+    return B200SA_OK;
+}
+
+// n >= 1.  Phases: rep_lens.
+static int repeat_lens_core(b200sa_ctx *c, uint32_t n, const uint32_t *d_sa, const uint32_t *d_lcp, uint32_t *d_rl) {
+    TRY(mark(c, "rep_lens"));
+    LAUNCH(c, k_rep_lens, cdiv(n, BLK), d_sa, d_lcp, n, d_rl);
+    TRY(mark(c, "end"));
+    CU_TRY(c, cudaGetLastError());
     return B200SA_OK;
 }
 
 int b200sa_repeat_lens_dev(b200sa_ctx *c, uint64_t n, const uint32_t *d_sa, const uint32_t *d_lcp, uint32_t *d_rl,
                            void *stream) {
     TRY(repeat_args(c, n, d_sa, d_lcp));
-    if (n > 0 && !d_rl) {
-        c->last_error = "null pointer";
-        return B200SA_ERR_BAD_ARG;
-    }
-    CU_TRY(c, cudaSetDevice(c->device));
-    begin_call(c, stream);
-    if (n == 0) return end_call(c);
-    TRY(mark(c, "rep_lens"));
-    LAUNCH(c, k_rep_lens, cdiv(n, BLK), d_sa, d_lcp, (uint32_t)n, d_rl);
-    TRY(mark(c, "end"));
-    CU_TRY(c, cudaGetLastError());
-    return end_call(c);
+    if (n > 0 && !d_rl) return null_ptr(c);
+    TRY(enter(c, stream));
+    if (n == 0) return leave(c, B200SA_OK);
+    return leave(c, repeat_lens_core(c, (uint32_t)n, d_sa, d_lcp, d_rl));
 }
 
 // seg (p0) and, on request, the smallest (p1) and largest (g0) position of every segment, at its head's slot
@@ -2625,20 +2577,12 @@ int b200sa_repeat_runs_dev(b200sa_ctx *c, uint64_t n, const uint32_t *d_sa, cons
                            uint32_t *d_start, uint32_t *d_end, uint32_t *d_first, uint32_t *d_last, uint64_t cap,
                            uint64_t *total, void *stream) {
     TRY(repeat_args(c, n, d_sa, d_lcp));
-    if (!total || (cap > 0 && (!d_start || !d_end))) {
-        c->last_error = "null pointer";
-        return B200SA_ERR_BAD_ARG;
-    }
-    if (min_len == 0) {
-        c->last_error = "repeat runs: min_len must be at least 1";
-        return B200SA_ERR_BAD_ARG;
-    }
-    CU_TRY(c, cudaSetDevice(c->device));
-    begin_call(c, stream);
+    if (!total || (cap > 0 && (!d_start || !d_end))) return null_ptr(c);
+    if (min_len == 0) return fail(c, B200SA_ERR_BAD_ARG, "repeat runs: min_len must be at least 1");
+    TRY(enter(c, stream));
     *total = 0;
-    if (n == 0) return end_call(c);
-    return tree_exit(c, repeat_runs_core(c, (uint32_t)n, d_sa, d_lcp, min_len, d_start, d_end, d_first, d_last, cap,
-                                         total));
+    if (n == 0) return leave(c, B200SA_OK);
+    return leave(c, repeat_runs_core(c, (uint32_t)n, d_sa, d_lcp, min_len, d_start, d_end, d_first, d_last, cap, total));
 }
 
 // n >= 1.  Phases: rep_check (with documents), rep_segments (every mode but ANY), rep_flag, rep_cover,
@@ -2651,11 +2595,7 @@ static int duplicate_spans_core(b200sa_ctx *c, uint32_t n, const uint32_t *d_sa,
     unsigned long long *d_total = reinterpret_cast<unsigned long long *>(words + 4);
     if (d_starts) {
         TRY(mark(c, "rep_check"));
-        CU_TRY(c, cudaMemsetAsync(words, 0, 8, c->stream));
-        LAUNCH(c, k_docs_check, cdiv(ndocs, BLK), d_starts, ndocs, n, words);
-        CU_TRY(c, cudaGetLastError());
-        TRY(read_words(c, words, 1));
-        if (c->h_pin[0]) return docs_bad(c, c->h_pin[0]);
+        TRY(docs_check_dev(c, d_starts, ndocs, n));
     }
     // two bitmaps of n bits, padded to whole words: flagged positions, document starts
     const size_t bm_words = ((size_t)n + 31) / 32;
@@ -2700,33 +2640,19 @@ int b200sa_duplicate_spans_dev(b200sa_ctx *c, uint64_t n, const uint32_t *d_sa, 
                                uint32_t *d_begin, uint32_t *d_end, uint64_t cap, uint64_t *total, uint64_t *covered,
                                void *stream) {
     TRY(repeat_args(c, n, d_sa, d_lcp));
-    if (!total || !covered || (cap > 0 && (!d_begin || !d_end)) || (ndocs > 0 && !d_doc_starts)) {
-        c->last_error = "null pointer";
-        return B200SA_ERR_BAD_ARG;
-    }
-    if (min_len == 0) {
-        c->last_error = "duplicate spans: min_len must be at least 1";
-        return B200SA_ERR_BAD_ARG;
-    }
-    if (mode < B200SA_REPEAT_ANY || mode > B200SA_REPEAT_EARLIER_DOC) {
-        c->last_error = "duplicate spans: unknown mode";
-        return B200SA_ERR_BAD_ARG;
-    }
-    if (!d_doc_starts && mode >= B200SA_REPEAT_OTHER_DOC) {
-        c->last_error = "duplicate spans: the document modes need doc_starts";
-        return B200SA_ERR_BAD_ARG;
-    }
-    if (d_doc_starts && ndocs == 0 && n > 0) {
-        c->last_error = "doc_starts rejected: ndocs == 0 with n > 0;";
-        return B200SA_ERR_BAD_ARG;
-    }
-    CU_TRY(c, cudaSetDevice(c->device));
-    begin_call(c, stream);
+    if (!total || !covered || (cap > 0 && (!d_begin || !d_end)) || (ndocs > 0 && !d_doc_starts)) return null_ptr(c);
+    if (min_len == 0) return fail(c, B200SA_ERR_BAD_ARG, "duplicate spans: min_len must be at least 1");
+    if (mode < B200SA_REPEAT_ANY || mode > B200SA_REPEAT_EARLIER_DOC)
+        return fail(c, B200SA_ERR_BAD_ARG, "duplicate spans: unknown mode");
+    if (!d_doc_starts && mode >= B200SA_REPEAT_OTHER_DOC)
+        return fail(c, B200SA_ERR_BAD_ARG, "duplicate spans: the document modes need doc_starts");
+    if (d_doc_starts && ndocs == 0 && n > 0) return no_docs(c);
+    TRY(enter(c, stream));
     *total = 0;
     *covered = 0;
-    if (n == 0) return end_call(c);
-    return tree_exit(c, duplicate_spans_core(c, (uint32_t)n, d_sa, d_lcp, d_doc_starts, ndocs, min_len, mode, d_begin,
-                                             d_end, cap, total, covered));
+    if (n == 0) return leave(c, B200SA_OK);
+    return leave(c, duplicate_spans_core(c, (uint32_t)n, d_sa, d_lcp, d_doc_starts, ndocs, min_len, mode, d_begin, d_end,
+                                         cap, total, covered));
 }
 
 // ------------------------------------------------------------ longest previous factor and LZ77 (DESIGN 6b f-12)
@@ -2746,16 +2672,12 @@ static int lz_lpf_core(b200sa_ctx *c, uint32_t n, const uint32_t *d_sa, const ui
 int b200sa_lpf_dev(b200sa_ctx *c, uint64_t n, const uint32_t *d_sa, const uint32_t *d_lcp, uint32_t *d_lpf,
                    uint32_t *d_src, void *stream) {
     TRY(repeat_args(c, n, d_sa, d_lcp));
-    if (n > 0 && !d_lpf) {
-        c->last_error = "null pointer";
-        return B200SA_ERR_BAD_ARG;
-    }
-    CU_TRY(c, cudaSetDevice(c->device));
-    begin_call(c, stream);
-    if (n == 0) return end_call(c);
+    if (n > 0 && !d_lpf) return null_ptr(c);
+    TRY(enter(c, stream));
+    if (n == 0) return leave(c, B200SA_OK);
     int rc = lz_lpf_core(c, (uint32_t)n, d_sa, d_lcp, d_lpf, d_src);
     if (rc == B200SA_OK) rc = mark(c, "end");
-    return tree_exit(c, rc);
+    return leave(c, rc);
 }
 
 // n >= 1.  lpf (p0), src (p1), the jump arrays J (g0, g1: n + 1 each), the mark bitmap (v0).  Phases:
@@ -2801,15 +2723,11 @@ static int lz77_core(b200sa_ctx *c, uint32_t n, const uint32_t *d_sa, const uint
 int b200sa_lz77_dev(b200sa_ctx *c, uint64_t n, const uint32_t *d_sa, const uint32_t *d_lcp, uint32_t *d_start,
                     uint32_t *d_len, uint32_t *d_src, uint64_t cap, uint64_t *total, void *stream) {
     TRY(repeat_args(c, n, d_sa, d_lcp));
-    if (!total || (cap > 0 && (!d_start || !d_len || !d_src))) {
-        c->last_error = "null pointer";
-        return B200SA_ERR_BAD_ARG;
-    }
-    CU_TRY(c, cudaSetDevice(c->device));
-    begin_call(c, stream);
+    if (!total || (cap > 0 && (!d_start || !d_len || !d_src))) return null_ptr(c);
+    TRY(enter(c, stream));
     *total = 0;
-    if (n == 0) return end_call(c);
-    return tree_exit(c, lz77_core(c, (uint32_t)n, d_sa, d_lcp, d_start, d_len, d_src, cap, total));
+    if (n == 0) return leave(c, B200SA_OK);
+    return leave(c, lz77_core(c, (uint32_t)n, d_sa, d_lcp, d_start, d_len, d_src, cap, total));
 }
 
 // ------------------------------------------------------------ Burrows-Wheeler transform (DESIGN 6b f-13)
@@ -2823,11 +2741,7 @@ static int bwt_core(b200sa_ctx *c, uint32_t n, const uint8_t *d_text, const uint
     unsigned long long *d_runs = reinterpret_cast<unsigned long long *>(words + 4);
     if (d_starts) {
         TRY(mark(c, "bwt_check"));
-        CU_TRY(c, cudaMemsetAsync(words, 0, 8, c->stream));
-        LAUNCH(c, k_docs_check, cdiv(k, BLK), d_starts, k, n, words);
-        CU_TRY(c, cudaGetLastError());
-        TRY(read_words(c, words, 1));
-        if (c->h_pin[0]) return docs_bad(c, c->h_pin[0]);
+        TRY(docs_check_dev(c, d_starts, k, n));
     }
     TRY(ensure(c, c->flag, nrows));
     TRY(ensure(c, c->v0, (size_t)nwords * 4));
@@ -2845,7 +2759,7 @@ static int bwt_core(b200sa_ctx *c, uint32_t n, const uint8_t *d_text, const uint
     CU_TRY(c, cudaGetLastError());
     if (runs) {
         TRY(read_words(c, reinterpret_cast<const uint32_t *>(d_runs), 2));
-        *runs = c->h_pin[0] | ((uint64_t)c->h_pin[1] << 32);
+        *runs = pin_u64(c, 0);
     }
     return B200SA_OK;
 }
@@ -2854,26 +2768,16 @@ int b200sa_bwt_dev(b200sa_ctx *c, uint64_t n, const uint8_t *d_text, const uint3
                    uint32_t ndocs, uint8_t *d_bwt, uint32_t *d_term_rows, uint64_t *runs, void *stream) {
     if (!c) return B200SA_ERR_BAD_ARG;
     const uint64_t k = d_doc_starts ? ndocs : 1;
-    if ((n > 0 && (!d_text || !d_sa || !d_bwt)) || (k > 0 && !d_term_rows) || (ndocs > 0 && !d_doc_starts)) {
-        c->last_error = "null pointer";
-        return B200SA_ERR_BAD_ARG;
-    }
-    if (k == 0 && n > 0) {
-        c->last_error = "doc_starts rejected: ndocs == 0 with n > 0;";
-        return B200SA_ERR_BAD_ARG;
-    }
-    if (n + k > B200SA_MAX_N) {
-        c->last_error = "bwt: text and terminators above 2^32-4096 rows";
-        return B200SA_ERR_TOO_LARGE;
-    }
-    CU_TRY(c, cudaSetDevice(c->device));
-    begin_call(c, stream);
+    if ((n > 0 && (!d_text || !d_sa || !d_bwt)) || (k > 0 && !d_term_rows) || (ndocs > 0 && !d_doc_starts))
+        return null_ptr(c);
+    if (k == 0 && n > 0) return no_docs(c);
+    if (n + k > B200SA_MAX_N) return fail(c, B200SA_ERR_TOO_LARGE, "bwt: text and terminators above 2^32-4096 rows");
+    TRY(enter(c, stream));
     if (runs) *runs = 0;
-    if (k == 0) return end_call(c);                      // no documents: no rows
-    return tree_exit(c, bwt_core(c, (uint32_t)n, d_text, d_sa, d_doc_starts, (uint32_t)k, d_bwt, d_term_rows, runs));
+    if (k == 0) return leave(c, B200SA_OK);              // no documents: no rows
+    return leave(c, bwt_core(c, (uint32_t)n, d_text, d_sa, d_doc_starts, (uint32_t)k, d_bwt, d_term_rows, runs));
 }
 
-extern "C++" {
 // The stable sorts of the inverse: the term rows (bits wide) or the bwt bytes (8 bits), by index.
 template <class KeyF>
 static int unbwt_sort(b200sa_ctx *c, KeyF kf, DevBuf &ka, DevBuf &va, DevBuf &kb, DevBuf &vb, uint32_t cnt, int bits,
@@ -2887,7 +2791,6 @@ static int unbwt_sort(b200sa_ctx *c, KeyF kf, DevBuf &ka, DevBuf &va, DevBuf &kb
         return sort_pairs_from<uint32_t, KeyF, LoadIndex, 16>(c, kf, LoadIndex{}, a, v, b, w, cnt, bits, kout, vout);
     return sort_pairs_from<uint32_t, KeyF, LoadIndex, ITEMS>(c, kf, LoadIndex{}, a, v, b, w, cnt, bits, kout, vout);
 }
-}  // extern "C++"
 
 constexpr uint32_t BWT_RULER_DEFAULT = 64;
 
@@ -2911,10 +2814,7 @@ static int unbwt_core(b200sa_ctx *c, uint32_t n, uint32_t k, const uint8_t *d_bw
     LAUNCH(c, k_bwt_terms_check, cdiv(k, BLK), ts, k, nrows, words);
     CU_TRY(c, cudaGetLastError());
     TRY(read_words(c, words, 1));
-    if (c->h_pin[0]) {
-        c->last_error = "unbwt: term_rows out of range or repeated";
-        return B200SA_ERR_BAD_ARG;
-    }
+    if (c->h_pin[0]) return fail(c, B200SA_ERR_BAD_ARG, "unbwt: term_rows out of range or repeated");
     if (n > 0) TRY(unbwt_sort(c, BwtByteKey{d_bwt}, c->v0, c->v1, c->p0, c->p0, n, 8, &fk, &fu));
     TRY(ensure(c, c->k64a, (size_t)nrows * 8));
     unsigned long long *pf = ptr<unsigned long long>(c->k64a);
@@ -2950,17 +2850,15 @@ static int unbwt_core(b200sa_ctx *c, uint32_t n, uint32_t k, const uint8_t *d_bw
     LAUNCH(c, k_bwt_valid, cdiv(m, BLK), nv, steps, m, k, reinterpret_cast<unsigned long long *>(words + 2), words);
     CU_TRY(c, cudaGetLastError());
     TRY(read_words(c, words, 8 + R));
-    const uint64_t covered = c->h_pin[2] | ((uint64_t)c->h_pin[3] << 32);
+    const uint64_t covered = pin_u64(c, 2);
     uint32_t rounds = 0;
     for (int r = 0; r < R; r++) rounds += c->h_pin[8 + r] ? 1u : 0u;
     c->stats.doubling_rounds = rounds;
     if (getenv("B200SA_TRACE"))
         fprintf(stderr, "[b200sa] unbwt: n=%u k=%u spacing=%u rulers=%u longest walk=%u rank rounds=%u\n", n, k, s, m,
                 c->h_pin[1], rounds);
-    if (c->h_pin[0] || covered != nrows) {
-        c->last_error = "unbwt: (bwt, term_rows) is not the transform of any documents";
-        return B200SA_ERR_BAD_ARG;
-    }
+    if (c->h_pin[0] || covered != nrows)
+        return fail(c, B200SA_ERR_BAD_ARG, "unbwt: (bwt, term_rows) is not the transform of any documents");
 
     // 4. document starts, then every ruler writes its segment
     TRY(mark(c, "unbwt_emit"));
@@ -2977,25 +2875,14 @@ static int unbwt_core(b200sa_ctx *c, uint32_t n, uint32_t k, const uint8_t *d_bw
 int b200sa_unbwt_dev(b200sa_ctx *c, uint64_t n, uint32_t ndocs, const uint8_t *d_bwt, const uint32_t *d_term_rows,
                      uint8_t *d_text_out, uint32_t *d_doc_starts_out, void *stream) {
     if (!c) return B200SA_ERR_BAD_ARG;
-    if (!d_term_rows || (n > 0 && (!d_bwt || !d_text_out))) {
-        c->last_error = "null pointer";
-        return B200SA_ERR_BAD_ARG;
-    }
-    if (ndocs == 0) {
-        c->last_error = "unbwt: ndocs must be at least 1";
-        return B200SA_ERR_BAD_ARG;
-    }
-    if (n + ndocs > B200SA_MAX_N) {
-        c->last_error = "unbwt: text and terminators above 2^32-4096 rows";
-        return B200SA_ERR_TOO_LARGE;
-    }
-    CU_TRY(c, cudaSetDevice(c->device));
-    begin_call(c, stream);
-    return tree_exit(c, unbwt_core(c, (uint32_t)n, ndocs, d_bwt, d_term_rows, d_text_out, d_doc_starts_out));
+    if (!d_term_rows || (n > 0 && (!d_bwt || !d_text_out))) return null_ptr(c);
+    if (ndocs == 0) return fail(c, B200SA_ERR_BAD_ARG, "unbwt: ndocs must be at least 1");
+    if (n + ndocs > B200SA_MAX_N) return fail(c, B200SA_ERR_TOO_LARGE, "unbwt: text and terminators above 2^32-4096 rows");
+    TRY(enter(c, stream));
+    return leave(c, unbwt_core(c, (uint32_t)n, ndocs, d_bwt, d_term_rows, d_text_out, d_doc_starts_out));
 }
 
 // ------------------------------------------------------------ approximate positions (DESIGN 6b f-14)
-extern "C++" {
 // nq >= 1, k <= B200SA_APPROX_MAX_K; d_starts non-null for documents (EndF = DocsEnd).  Phases: approx_check,
 // approx_pieces, approx_scan, approx_count, and approx_emit, approx_sort when the occurrences fit in cap.
 template <class EndF>
@@ -3009,29 +2896,15 @@ static int approx_core(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const u
     uint32_t *words = ptr<uint32_t>(c->small);           // [0] check bits, [2, 4) items, [4, 6) total
     CU_TRY(c, cudaMemcpyAsync(c->h_pin, d_q_off + nq, 8, cudaMemcpyDeviceToHost, c->stream));
     CU_TRY(c, cudaStreamSynchronize(c->stream));
-    const uint64_t q_bytes = c->h_pin[0] | ((uint64_t)c->h_pin[1] << 32);
+    const uint64_t q_bytes = pin_u64(c, 0);
     TRY(match_check(c, d_q_off, nq, q_bytes));           // q_off[0] = 0 and ascending
-    if (d_starts && ndocs > 0) {
-        CU_TRY(c, cudaMemsetAsync(words, 0, 8, c->stream));
-        LAUNCH(c, k_docs_check, cdiv(ndocs, BLK), d_starts, ndocs, n, words);
-        CU_TRY(c, cudaGetLastError());
-        TRY(read_words(c, words, 1));
-        if (c->h_pin[0]) return docs_bad(c, c->h_pin[0]);
-    }
-    if (q_bytes > B200SA_MAX_N) {
-        c->last_error = "queries longer than 2^32-4096 bytes";
-        return B200SA_ERR_TOO_LARGE;
-    }
-    if (q_bytes > 0 && !d_queries) {
-        c->last_error = "null pointer";
-        return B200SA_ERR_BAD_ARG;
-    }
+    if (d_starts && ndocs > 0) TRY(docs_check_dev(c, d_starts, ndocs, n));
+    if (q_bytes > B200SA_MAX_N) return fail(c, B200SA_ERR_TOO_LARGE, "queries longer than 2^32-4096 bytes");
+    if (q_bytes > 0 && !d_queries) return null_ptr(c);
     const uint32_t P = k + 1;
     const uint64_t nslots = (uint64_t)nq * P;
-    if (nslots >= 0xFFFFFFFFull) {
-        c->last_error = "approx positions: nq * (k + 1) of 2^32 - 1 or more slots";
-        return B200SA_ERR_TOO_LARGE;
-    }
+    if (nslots >= 0xFFFFFFFFull)
+        return fail(c, B200SA_ERR_TOO_LARGE, "approx positions: nq * (k + 1) of 2^32 - 1 or more slots");
     if (n == 0) {                                        // nothing occurs
         CU_TRY(c, cudaMemsetAsync(d_offsets, 0, ((size_t)nq + 1) * 8, c->stream));
         TRY(mark(c, "end"));
@@ -3050,11 +2923,9 @@ static int approx_core(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const u
     TRY((dev_scan<OpSum64>(c, DListChunks{ps, pe, (uint32_t)nslots, n, words}, OutStoreExcl64{item_start},
                            nslots + 1, d_items)));
     TRY(read_words(c, words + 2, 2));
-    const uint64_t items = c->h_pin[0] | ((uint64_t)c->h_pin[1] << 32);
-    if (items > (uint64_t)0x7fffffff * NWARP) {
-        c->last_error = "approx positions: more than 2^31 * 8 chunks of 1024 candidates in one batch";
-        return B200SA_ERR_TOO_LARGE;
-    }
+    const uint64_t items = pin_u64(c, 0);
+    if (items > (uint64_t)0x7fffffff * NWARP)
+        return fail(c, B200SA_ERR_TOO_LARGE, "approx positions: more than 2^31 * 8 chunks of 1024 candidates in one batch");
     TRY(mark(c, "approx_count"));
     TRY(ensure(c, c->p0, (size_t)items * 4));
     TRY(ensure(c, c->k64b, ((size_t)items + 1) * 8));
@@ -3069,7 +2940,7 @@ static int approx_core(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const u
     LAUNCH(c, k_approx_qoff, cdiv((uint64_t)nq + 1, BLK), item_start, item_off, nq, P,
            reinterpret_cast<u64 *>(d_offsets));
     TRY(read_words(c, words + 4, 2));
-    *total = c->h_pin[0] | ((uint64_t)c->h_pin[1] << 32);
+    *total = pin_u64(c, 0);
     if (*total > 0 && *total <= cap) {
         TRY(mark(c, "approx_emit"));
         TRY(ensure(c, c->g0, (size_t)*total * 8));
@@ -3091,30 +2962,13 @@ static int approx_core(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const u
     CU_TRY(c, cudaStreamSynchronize(c->stream));
     return B200SA_OK;
 }
-}  // extern "C++"
 
 static int approx_args(b200sa_ctx *c, uint64_t n, const void *text, const void *sa, const void *q_off, uint32_t nq,
                        uint32_t k, const void *offsets, const void *pos, uint64_t cap, const void *total) {
     if (!c) return B200SA_ERR_BAD_ARG;
-    if (!total || !offsets || (nq > 0 && !q_off) || (cap > 0 && !pos) || (n > 0 && (!text || !sa))) {
-        c->last_error = "null pointer";
-        return B200SA_ERR_BAD_ARG;
-    }
-    if (k > B200SA_APPROX_MAX_K) {
-        c->last_error = "approx positions: k above B200SA_APPROX_MAX_K";
-        return B200SA_ERR_BAD_ARG;
-    }
-    if (n > B200SA_MAX_N) {
-        c->last_error = "text longer than 2^32-4096 bytes";
-        return B200SA_ERR_TOO_LARGE;
-    }
-    return B200SA_OK;
-}
-
-// nq = 0: offsets[0] = 0, *total = 0.
-static int approx_none(b200sa_ctx *c, uint64_t *d_offsets) {
-    CU_TRY(c, cudaMemsetAsync(d_offsets, 0, 8, c->stream));
-    CU_TRY(c, cudaStreamSynchronize(c->stream));
+    if (!total || !offsets || (nq > 0 && !q_off) || (cap > 0 && !pos) || (n > 0 && (!text || !sa))) return null_ptr(c);
+    if (k > B200SA_APPROX_MAX_K) return fail(c, B200SA_ERR_BAD_ARG, "approx positions: k above B200SA_APPROX_MAX_K");
+    if (n > B200SA_MAX_N) return too_long(c);
     return B200SA_OK;
 }
 
@@ -3123,12 +2977,11 @@ int b200sa_approx_positions_dev(b200sa_ctx *c, const uint8_t *d_text, uint64_t n
                                 uint64_t *d_offsets, uint32_t *d_pos, uint32_t *d_mismatches, uint64_t cap,
                                 uint64_t *total, void *stream) {
     TRY(approx_args(c, n, d_text, d_sa, d_q_off, nq, k, d_offsets, d_pos, cap, total));
-    CU_TRY(c, cudaSetDevice(c->device));
-    begin_call(c, stream);
+    TRY(enter(c, stream));
     *total = 0;
-    if (nq == 0) return tree_exit(c, approx_none(c, d_offsets));
-    return tree_exit(c, approx_core(c, d_text, (uint32_t)n, d_sa, nullptr, 0, d_queries, d_q_off, nq, k, d_offsets,
-                                    d_pos, d_mismatches, cap, total, TextEnd{(uint32_t)n}));
+    if (nq == 0) return leave(c, empty_batch(c, d_offsets));
+    return leave(c, approx_core(c, d_text, (uint32_t)n, d_sa, nullptr, 0, d_queries, d_q_off, nq, k, d_offsets, d_pos,
+                                d_mismatches, cap, total, TextEnd{(uint32_t)n}));
 }
 
 int b200sa_docs_approx_positions_dev(b200sa_ctx *c, const uint8_t *d_text, uint64_t n, const uint32_t *d_gsa,
@@ -3137,21 +2990,13 @@ int b200sa_docs_approx_positions_dev(b200sa_ctx *c, const uint8_t *d_text, uint6
                                      uint32_t *d_pos, uint32_t *d_mismatches, uint64_t cap, uint64_t *total,
                                      void *stream) {
     TRY(approx_args(c, n, d_text, d_gsa, d_q_off, nq, k, d_offsets, d_pos, cap, total));
-    if ((n > 0 || ndocs > 0) && !d_doc_starts) {
-        c->last_error = "null pointer";
-        return B200SA_ERR_BAD_ARG;
-    }
-    if (ndocs == 0 && n > 0) {
-        c->last_error = "doc_starts rejected: ndocs == 0 with n > 0;";
-        return B200SA_ERR_BAD_ARG;
-    }
-    CU_TRY(c, cudaSetDevice(c->device));
-    begin_call(c, stream);
+    if ((n > 0 || ndocs > 0) && !d_doc_starts) return null_ptr(c);
+    if (ndocs == 0 && n > 0) return no_docs(c);
+    TRY(enter(c, stream));
     *total = 0;
-    if (nq == 0) return tree_exit(c, approx_none(c, d_offsets));
-    return tree_exit(c, approx_core(c, d_text, (uint32_t)n, d_gsa, d_doc_starts, ndocs, d_queries, d_q_off, nq, k,
-                                    d_offsets, d_pos, d_mismatches, cap, total,
-                                    DocsEnd{d_doc_starts, ndocs, (uint32_t)n}));
+    if (nq == 0) return leave(c, empty_batch(c, d_offsets));
+    return leave(c, approx_core(c, d_text, (uint32_t)n, d_gsa, d_doc_starts, ndocs, d_queries, d_q_off, nq, k, d_offsets,
+                                d_pos, d_mismatches, cap, total, DocsEnd{d_doc_starts, ndocs, (uint32_t)n}));
 }
 
 // ------------------------------------------------------------ multi-GPU: communicator + sharded LMS sort
@@ -3178,9 +3023,12 @@ int b200sa_comm_unique_id(uint8_t *id_out) {
 }
 
 int b200sa_comm_init(b200sa_ctx *c, int nranks, int rank, const uint8_t *id128) {
-    if (!c || !id128 || nranks < 1 || rank < 0 || rank >= nranks || nranks > 16) return B200SA_ERR_BAD_ARG;
+    if (!c) return B200SA_ERR_BAD_ARG;
+    if (!id128) return null_ptr(c);
+    if (nranks < 1 || nranks > 16 || rank < 0 || rank >= nranks)
+        return fail(c, B200SA_ERR_BAD_ARG, "comm init: nranks must be in [1, 16] and rank in [0, nranks)");
     NcclApi &N = nccl_api();
-    if (!N.ok) { c->last_error = N.err; return B200SA_ERR_COMM; }
+    if (!N.ok) return fail(c, B200SA_ERR_COMM, N.err);
     CU_TRY(c, cudaSetDevice(c->device));
     if (c->comm && c->comm_owned) N.CommDestroy(c->comm);
     c->comm = nullptr;
@@ -3192,15 +3040,16 @@ int b200sa_comm_init(b200sa_ctx *c, int nranks, int rank, const uint8_t *id128) 
 }
 
 int b200sa_comm_attach(b200sa_ctx *c, void *nccl_comm) {
-    if (!c || !nccl_comm) return B200SA_ERR_BAD_ARG;
+    if (!c) return B200SA_ERR_BAD_ARG;
+    if (!nccl_comm) return null_ptr(c);
     NcclApi &N = nccl_api();
-    if (!N.ok) { c->last_error = N.err; return B200SA_ERR_COMM; }
+    if (!N.ok) return fail(c, B200SA_ERR_COMM, N.err);
     if (c->comm && c->comm_owned) N.CommDestroy(c->comm);
     c->comm = (ncclComm_t)nccl_comm;
     c->comm_owned = false;
     NCCL_TRY(c, N.CommCount(c->comm, &c->nranks));
     NCCL_TRY(c, N.CommUserRank(c->comm, &c->comm_rank));
-    if (c->nranks > 16) return B200SA_ERR_BAD_ARG;
+    if (c->nranks > 16) return fail(c, B200SA_ERR_BAD_ARG, "comm attach: more than 16 ranks");
     return B200SA_OK;
 }
 
@@ -3212,15 +3061,10 @@ int b200sa_comm_destroy(b200sa_ctx *c) {
 }
 
 // Collective over the context's communicator (a context without one is a world of 1).
-int b200sa_shard_lms_sort(b200sa_ctx *c, const uint8_t *d_shard, uint64_t len, unsigned long long *d_sorted_gpos,
-                          uint32_t *d_names, uint64_t cap, b200sa_shard_stats *out, void *stream) {
-    if (!c || !d_shard || len < 1 || len > B200SA_MAX_N || !out) return B200SA_ERR_BAD_ARG;
-    if (((uintptr_t)d_shard & 15) != 0) { c->last_error = "shard pointer must be 16-byte aligned"; return B200SA_ERR_BAD_ARG; }
+static int shard_lms_sort_core(b200sa_ctx *c, const uint8_t *d_shard, uint64_t len, unsigned long long *d_sorted_gpos,
+                               uint32_t *d_names, uint64_t cap, b200sa_shard_stats *out) {
     NcclApi &N = nccl_api();
     const int W = c->comm ? c->nranks : 1, R = c->comm ? c->comm_rank : 0;
-    if (W > 1 && !N.ok) { c->last_error = N.err; return B200SA_ERR_COMM; }
-    CU_TRY(c, cudaSetDevice(c->device));
-    begin_call(c, stream);
     memset(out, 0, sizeof *out);
     constexpr int HEAD = 64;                                   // bytes of every shard's head that travel (halo source)
     // ---- small exchange area: per rank {len, first byte, last byte, state, m, distinct} + head bytes
@@ -3361,7 +3205,7 @@ int b200sa_shard_lms_sort(b200sa_ctx *c, const uint8_t *d_shard, uint64_t len, u
     for (int r = 0; r < W; r++) {                  // the same verdict on every rank: nobody enters the exchange alone
         uint64_t slice = 0;
         for (int q = 0; q < W; q++) slice += hcnt[(size_t)q * W + r];
-        if (slice > 0xfffffff0ull) { c->last_error = "more than 2^32 LMS suffixes on one rank"; return B200SA_ERR_TOO_LARGE; }
+        if (slice > 0xfffffff0ull) return fail(c, B200SA_ERR_TOO_LARGE, "more than 2^32 LMS suffixes on one rank");
         if (slice > hrec[r * REC + 7]) {
             char b[160]; snprintf(b, sizeof b, "output capacity of rank %d too small for its slice (%llu entries)", r, (unsigned long long)slice);
             c->last_error = b; return B200SA_ERR_BAD_ARG;
@@ -3441,24 +3285,35 @@ int b200sa_shard_lms_sort(b200sa_ctx *c, const uint8_t *d_shard, uint64_t len, u
     out->bytes_recv = 0;
     for (int k = 0; k < W; k++) { int src = W - 1 - k; if (src != R) out->bytes_recv += (double)(roff[k + 1] - roff[k]) * 12.0; }
     CU_TRY(c, cudaStreamSynchronize(c->stream));
-    return end_call(c);
+    return B200SA_OK;
+}
+
+// A collective call needs NCCL when the context's communicator has more than one rank.
+static int comm_ready(b200sa_ctx *c) {
+    if (c->comm && c->nranks > 1 && !nccl_api().ok) return fail(c, B200SA_ERR_COMM, nccl_api().err);
+    return B200SA_OK;
+}
+
+int b200sa_shard_lms_sort(b200sa_ctx *c, const uint8_t *d_shard, uint64_t len, unsigned long long *d_sorted_gpos,
+                          uint32_t *d_names, uint64_t cap, b200sa_shard_stats *out, void *stream) {
+    if (!c) return B200SA_ERR_BAD_ARG;
+    if (!out) return null_ptr(c);
+    TRY(shard_args(c, d_shard, len, -1));
+    TRY(comm_ready(c));
+    TRY(enter(c, stream));
+    return leave(c, shard_lms_sort_core(c, d_shard, len, d_sorted_gpos, d_names, cap, out));
 }
 
 // Sharded LCP (SURVEY 8e row 5): text and SA are replicated (broadcast from rank 0 unless the caller
 // says they already are), every rank computes Phi and PLCP for ITS text range only, the PLCP ranges
 // are all-gathered, every rank turns its rank range into LCP values and the slices are all-gathered.
 // Same values as lcp_lens_quadratic (src/table.rs:348-361).
-int b200sa_lcp_sharded(b200sa_ctx *c, uint8_t *d_text, uint64_t n, uint32_t *d_sa, uint32_t *d_lcp, int replicated,
-                       void *stream) {
-    if (!c || (n > 0 && (!d_text || !d_sa || !d_lcp))) return B200SA_ERR_BAD_ARG;
-    if (n > B200SA_MAX_N) return B200SA_ERR_TOO_LARGE;
+static int lcp_sharded_core(b200sa_ctx *c, uint8_t *d_text, uint64_t n, uint32_t *d_sa, uint32_t *d_lcp,
+                            int replicated) {
     NcclApi &N = nccl_api();
     const int W = c->comm ? c->nranks : 1, R = c->comm ? c->comm_rank : 0;
-    if (W > 1 && !N.ok) { c->last_error = N.err; return B200SA_ERR_COMM; }
-    CU_TRY(c, cudaSetDevice(c->device));
-    begin_call(c, stream);
-    if (n == 0) return end_call(c);
-    if (((uintptr_t)d_text & 15) != 0) { c->last_error = "text pointer must be 16-byte aligned"; return B200SA_ERR_BAD_ARG; }
+    if (n == 0) return B200SA_OK;
+    if (((uintptr_t)d_text & 15) != 0) return fail(c, B200SA_ERR_BAD_ARG, "text pointer must be 16-byte aligned");
     const uint32_t n32 = (uint32_t)n;
     TRY(mark(c, "lcps_bcast"));
     if (W > 1 && !replicated) {
@@ -3487,10 +3342,8 @@ int b200sa_lcp_sharded(b200sa_ctx *c, uint8_t *d_text, uint64_t n, uint32_t *d_s
         LAUNCH(c, k_byte_hist, hb, d_text, n, tab + T_HIST);
         LAUNCH(c, k_alpha_from_hist, 1, tab + T_HIST, tab + T_CODE, tab + T_ALPHA, sm + 3);
         TRY(read_words(c, sm, 16));
-        if (c->h_pin[12] != 0) {      // identical on every rank: all fail together
-            c->last_error = "table is not a permutation of 0..n-1 (index out of range or repeated)";
-            return B200SA_ERR_BAD_ARG;
-        }
+        if (c->h_pin[12] != 0)        // identical on every rank: all fail together
+            return fail(c, B200SA_ERR_BAD_ARG, "table is not a permutation of 0..n-1 (index out of range or repeated)");
         TRY(pack_text(c, d_text, n, c->h_pin[3]));
     }
     // ---- Phi and PLCP of this rank's text range
@@ -3526,58 +3379,62 @@ int b200sa_lcp_sharded(b200sa_ctx *c, uint8_t *d_text, uint64_t n, uint32_t *d_s
     TRY(mark(c, "end"));
     CU_TRY(c, cudaGetLastError());
     CU_TRY(c, cudaStreamSynchronize(c->stream));
-    return end_call(c);
+    return B200SA_OK;
+}
+
+int b200sa_lcp_sharded(b200sa_ctx *c, uint8_t *d_text, uint64_t n, uint32_t *d_sa, uint32_t *d_lcp, int replicated,
+                       void *stream) {
+    if (!c) return B200SA_ERR_BAD_ARG;
+    if (n > 0 && (!d_text || !d_sa || !d_lcp)) return null_ptr(c);
+    if (n > B200SA_MAX_N) return too_long(c);
+    TRY(comm_ready(c));
+    TRY(enter(c, stream));
+    return leave(c, lcp_sharded_core(c, d_text, n, d_sa, d_lcp, replicated));
 }
 
 // ------------------------------------------------------------ test hooks
-int b200sa_test_classify(b200sa_ctx *c, const uint8_t *text, uint64_t n, uint32_t *stype_words, uint32_t *lms_words,
-                         uint32_t *hist768, uint32_t *lmspos, uint64_t cap_lms, uint64_t *m_out) {
-    if (!c || !text || n < 1 || n > B200SA_MAX_N) return B200SA_ERR_BAD_ARG;
-    CU_TRY(c, cudaSetDevice(c->device));
-    begin_call(c, nullptr);
+// The classification of a host text by the two-pass (fused = false) or the fused kernels, copied back.
+static int test_classify_core(b200sa_ctx *c, bool fused, const uint8_t *text, uint64_t n, uint32_t *stype_words,
+                              uint32_t *lms_words, uint32_t *hist768, uint32_t *lmspos, uint64_t cap_lms,
+                              uint64_t *m_out) {
     TRY(ensure(c, c->text, n));
     CU_TRY(c, cudaMemcpyAsync(c->text.p, text, n, cudaMemcpyHostToDevice, c->stream));
     uint32_t m = 0;
-    TRY(classify_dev(c, ptr<uint8_t>(c->text), n, &m));
+    if (fused) TRY(classify_fused_dev(c, ptr<uint8_t>(c->text), n, &m));
+    else TRY(classify_dev(c, ptr<uint8_t>(c->text), n, &m));
     uint64_t nw = (n + 31) / 32;
     if (stype_words) CU_TRY(c, cudaMemcpyAsync(stype_words, c->stype.p, nw * 4, cudaMemcpyDeviceToHost, c->stream));
     if (lms_words) CU_TRY(c, cudaMemcpyAsync(lms_words, c->lmsb.p, nw * 4, cudaMemcpyDeviceToHost, c->stream));
     if (hist768) CU_TRY(c, cudaMemcpyAsync(hist768, ptr<uint32_t>(c->tables) + T_HIST, 768 * 4, cudaMemcpyDeviceToHost, c->stream));
     if (lmspos && m > 0) {
         uint64_t k = m < cap_lms ? m : cap_lms;
-        CU_TRY(c, cudaMemcpyAsync(lmspos, c->lmspos.p, k * 4, cudaMemcpyDeviceToHost, c->stream));
+        CU_TRY(c, cudaMemcpyAsync(lmspos, (fused ? c->lmsdesc : c->lmspos).p, k * 4, cudaMemcpyDeviceToHost, c->stream));
     }
     CU_TRY(c, cudaStreamSynchronize(c->stream));
     if (m_out) *m_out = m;
-    return end_call(c);
+    return B200SA_OK;
+}
+
+static int test_classify(b200sa_ctx *c, bool fused, const uint8_t *text, uint64_t n, uint32_t *stype_words,
+                         uint32_t *lms_words, uint32_t *hist768, uint32_t *lmspos, uint64_t cap_lms, uint64_t *m_out) {
+    if (!c) return B200SA_ERR_BAD_ARG;
+    if (!text) return null_ptr(c);
+    if (n < 1 || n > B200SA_MAX_N) return fail(c, B200SA_ERR_BAD_ARG, "test classify: n must be in [1, 2^32-4096]");
+    TRY(enter(c, nullptr));
+    return leave(c, test_classify_core(c, fused, text, n, stype_words, lms_words, hist768, lmspos, cap_lms, m_out));
+}
+
+int b200sa_test_classify(b200sa_ctx *c, const uint8_t *text, uint64_t n, uint32_t *stype_words, uint32_t *lms_words,
+                         uint32_t *hist768, uint32_t *lmspos, uint64_t cap_lms, uint64_t *m_out) {
+    return test_classify(c, false, text, n, stype_words, lms_words, hist768, lmspos, cap_lms, m_out);
 }
 
 int b200sa_test_classify_fused(b200sa_ctx *c, const uint8_t *text, uint64_t n, uint32_t *stype_words, uint32_t *lms_words,
                                uint32_t *hist768, uint32_t *lmspos_desc, uint64_t cap_lms, uint64_t *m_out) {
-    if (!c || !text || n < 1 || n > B200SA_MAX_N) return B200SA_ERR_BAD_ARG;
-    CU_TRY(c, cudaSetDevice(c->device));
-    begin_call(c, nullptr);
-    TRY(ensure(c, c->text, n));
-    CU_TRY(c, cudaMemcpyAsync(c->text.p, text, n, cudaMemcpyHostToDevice, c->stream));
-    uint32_t m = 0;
-    TRY(classify_fused_dev(c, ptr<uint8_t>(c->text), n, &m));
-    uint64_t nw = (n + 31) / 32;
-    if (stype_words) CU_TRY(c, cudaMemcpyAsync(stype_words, c->stype.p, nw * 4, cudaMemcpyDeviceToHost, c->stream));
-    if (lms_words) CU_TRY(c, cudaMemcpyAsync(lms_words, c->lmsb.p, nw * 4, cudaMemcpyDeviceToHost, c->stream));
-    if (hist768) CU_TRY(c, cudaMemcpyAsync(hist768, ptr<uint32_t>(c->tables) + T_HIST, 768 * 4, cudaMemcpyDeviceToHost, c->stream));
-    if (lmspos_desc && m > 0) {
-        uint64_t k = m < cap_lms ? m : cap_lms;
-        CU_TRY(c, cudaMemcpyAsync(lmspos_desc, c->lmsdesc.p, k * 4, cudaMemcpyDeviceToHost, c->stream));
-    }
-    CU_TRY(c, cudaStreamSynchronize(c->stream));
-    if (m_out) *m_out = m;
-    return end_call(c);
+    return test_classify(c, true, text, n, stype_words, lms_words, hist768, lmspos_desc, cap_lms, m_out);
 }
 
-int b200sa_test_scan(b200sa_ctx *c, const uint32_t *in, uint64_t n, int op, uint32_t *out_excl, uint32_t *total) {
-    if (!c || (n > 0 && (!in || !out_excl))) return B200SA_ERR_BAD_ARG;
-    CU_TRY(c, cudaSetDevice(c->device));
-    begin_call(c, nullptr);
+static int test_scan_core(b200sa_ctx *c, const uint32_t *in, uint64_t n, int op, uint32_t *out_excl, uint32_t *total) {
     TRY(ensure(c, c->v0, n * 4));
     TRY(ensure(c, c->v1, n * 4));
     TRY(ensure(c, c->small, 4096));
@@ -3588,7 +3445,14 @@ int b200sa_test_scan(b200sa_ctx *c, const uint32_t *in, uint64_t n, int op, uint
     if (n) CU_TRY(c, cudaMemcpyAsync(out_excl, c->v1.p, n * 4, cudaMemcpyDeviceToHost, c->stream));
     TRY(read_words(c, d_tot, 1));
     if (total) *total = c->h_pin[0];
-    return end_call(c);
+    return B200SA_OK;
+}
+
+int b200sa_test_scan(b200sa_ctx *c, const uint32_t *in, uint64_t n, int op, uint32_t *out_excl, uint32_t *total) {
+    if (!c) return B200SA_ERR_BAD_ARG;
+    if (n > 0 && (!in || !out_excl)) return null_ptr(c);
+    TRY(enter(c, nullptr));
+    return leave(c, test_scan_core(c, in, n, op, out_excl, total));
 }
 
 int b200sa_test_sort_pairs32(b200sa_ctx *c, uint32_t *keys, uint32_t *vals, uint64_t n, int bits) {
@@ -3598,11 +3462,8 @@ int b200sa_test_sort_pairs64(b200sa_ctx *c, uint64_t *keys, uint32_t *vals, uint
     return test_sort<uint64_t>(c, keys, vals, n, bits);
 }
 
-int b200sa_test_reduced_sa(b200sa_ctx *c, const uint32_t *R, uint64_t m, uint32_t names, uint32_t *sa_out,
-                           uint32_t *rounds_out) {
-    if (!c || m < 1 || m > 0x7FFFFFFFull || !R || !sa_out) return B200SA_ERR_BAD_ARG;
-    CU_TRY(c, cudaSetDevice(c->device));
-    begin_call(c, nullptr);
+static int test_reduced_sa_core(b200sa_ctx *c, const uint32_t *R, uint64_t m, uint32_t names, uint32_t *sa_out,
+                                uint32_t *rounds_out) {
     TRY(ensure(c, c->reduced, m * 4));
     CU_TRY(c, cudaMemcpyAsync(c->reduced.p, R, m * 4, cudaMemcpyHostToDevice, c->stream));
     uint32_t rounds = 0;
@@ -3610,11 +3471,21 @@ int b200sa_test_reduced_sa(b200sa_ctx *c, const uint32_t *R, uint64_t m, uint32_
     CU_TRY(c, cudaMemcpyAsync(sa_out, c->sa_r.p, m * 4, cudaMemcpyDeviceToHost, c->stream));
     CU_TRY(c, cudaStreamSynchronize(c->stream));
     if (rounds_out) *rounds_out = rounds;
-    return end_call(c);
+    return B200SA_OK;
+}
+
+int b200sa_test_reduced_sa(b200sa_ctx *c, const uint32_t *R, uint64_t m, uint32_t names, uint32_t *sa_out,
+                           uint32_t *rounds_out) {
+    if (!c) return B200SA_ERR_BAD_ARG;
+    if (!R || !sa_out) return null_ptr(c);
+    if (m < 1 || m > 0x7FFFFFFFull) return fail(c, B200SA_ERR_BAD_ARG, "test reduced sa: m must be in [1, 2^31)");
+    TRY(enter(c, nullptr));
+    return leave(c, test_reduced_sa_core(c, R, m, names, sa_out, rounds_out));
 }
 
 int64_t b200sa_debug_fetch(b200sa_ctx *c, int which, void *out, uint64_t cap) {
-    if (!c || !out) return B200SA_ERR_BAD_ARG;
+    if (!c) return B200SA_ERR_BAD_ARG;
+    if (!out) return null_ptr(c);
     if (cudaSetDevice(c->device) != cudaSuccess) return B200SA_ERR_CUDA;
     const void *src = nullptr;
     uint64_t count = 0;
@@ -3627,12 +3498,10 @@ int64_t b200sa_debug_fetch(b200sa_ctx *c, int which, void *out, uint64_t cap) {
         case 5: src = c->small.p ? (const void *)(ptr<uint32_t>(c->small) + 32) : nullptr; count = 10; break;
         case 6: src = c->tables.p; count = T_HIST; break;
         case 7: src = c->steplog.p; count = c->steplog.p ? 16384 : 0; break;     // u64 records viewed as u32 pairs
-        default: return B200SA_ERR_BAD_ARG;
+        default: return fail(c, B200SA_ERR_BAD_ARG, "debug fetch: unknown buffer");
     }
     if (!src) return 0;
     uint64_t k = count < cap ? count : cap;
     if (k && cudaMemcpy(out, src, k * 4, cudaMemcpyDeviceToHost) != cudaSuccess) return B200SA_ERR_CUDA;
     return (int64_t)count;
 }
-
-}  // extern "C"
