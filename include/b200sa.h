@@ -543,8 +543,31 @@ int b200sa_unbwt_dev(b200sa_ctx *ctx, uint64_t n, uint32_t ndocs, const uint8_t 
  * of a piece's range, or of the whole table for a query of 0 < m <= k), and, when the occurrences are
  * fetched, 24 bytes per output entry plus the radix sort's tile status (at most 1 byte per entry).
  * B200SA_ERR_OOM when that cannot be allocated.  Phases: approx_check, approx_pieces, approx_scan,
- * approx_count, approx_emit, approx_sort (the last two only when total <= cap and total > 0). */
+ * approx_count, approx_emit, approx_sort (the last two only when total <= cap and total > 0).
+ *
+ * ---- the edit metric: occurrences within k insertions, deletions and substitutions (DESIGN.md 6b f-15) ----
+ * The k argument is threshold | flags: threshold = k & 0xFFFF, 0 <= threshold <= B200SA_APPROX_MAX_K, and the
+ * only flag is B200SA_APPROX_EDIT.  Without the flag the call is the Hamming search above, bit for bit.  Other
+ * flag bits, or a threshold above B200SA_APPROX_MAX_K, return B200SA_ERR_BAD_ARG with a b200sa_last_error detail
+ * that names B200SA_APPROX_MAX_K; the TOO_LARGE slot check counts nq * (threshold + 1).
+ * With B200SA_APPROX_EDIT (k below meaning the threshold): index, queries and end(p) are as above.  ED is the
+ * Levenshtein distance, unit cost for each substitution, insertion and deletion.  For a position p in [0, n):
+ *   dist(p) = min over e with p <= e <= end(p) of ED(q, T[p, e)),
+ * the best alignment of the whole query that starts at p and crosses neither the text end nor a document end;
+ * the empty substring (e = p) counts.  p is an occurrence iff dist(p) <= k.  Occurrences are listed by ascending
+ * p with dist(p) in d_mismatches (may be NULL) beside them; offsets, total, cap, ordering, workspace and phase
+ * names are as above.  m = 0 has no occurrences; 0 < m <= k makes every position an occurrence (dist <= m).
+ * k = 0 gives exactly the set b200sa_positions_dev returns.  For every k the Hamming occurrences are a subset of
+ * the edit occurrences, with dist(p) <= mis(p) on them.  One locus yields a run of neighbouring starts (an exact
+ * hit at p also puts p - 1 and p + 1 at distance 1, when they lie in p's document); no filtering is applied.
+ * Method: the same pieces and slots.  A candidate s of piece j (offset o_j) considers the starts p of s's
+ * document with |p - (s - o_j)| <= k and computes their dist(p) by one banded reversed Sellers DP over the
+ * diagonals [s - o_j - 2k, s - o_j + 2k].  It emits p iff dist(p) <= k and it is the least (i, s'') such that
+ * piece i occurs exactly at s'' inside p's document with |s'' - o_i - p| <= k; every occurrence has one such
+ * least pair (the partition lemma), so each is emitted once.  A query of 0 < m <= k keeps the whole-table slot
+ * and each rank s reports itself. */
 #define B200SA_APPROX_MAX_K 31
+#define B200SA_APPROX_EDIT 0x10000u
 int b200sa_approx_positions_dev(b200sa_ctx *ctx, const uint8_t *d_text, uint64_t n, const uint32_t *d_sa,
                                 const uint8_t *d_queries, const uint64_t *d_q_off, uint32_t nq, uint32_t k,
                                 uint64_t *d_offsets, uint32_t *d_pos, uint32_t *d_mismatches, uint64_t cap,

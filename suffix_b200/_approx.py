@@ -1,21 +1,27 @@
-"""Approximate positions (occurrences with at most k mismatches) over a device-resident table: the part
-SuffixTable and DocumentSuffixTable share.  A table supplies `_device` and `_bwt_arrays()` -> (d_text,
-d_table, d_doc_starts or None, ndocs), its text and table on the device; the LCP array is not needed."""
+"""Approximate positions (occurrences with at most k mismatches, or within k edits with metric="edit") over a
+device-resident table: the part SuffixTable and DocumentSuffixTable share.  A table supplies `_device` and
+`_bwt_arrays()` -> (d_text, d_table, d_doc_starts or None, ndocs), its text and table on the device; the LCP
+array is not needed."""
 import numpy as np
 
 from . import _lib
 from .table import _as_bytes, _lock
 
 MAX_K = 31                # B200SA_APPROX_MAX_K
+EDIT = 0x10000            # B200SA_APPROX_EDIT
+METRICS = {"hamming": 0, "edit": EDIT}
 
 
-def _call(table, queries, k, fetch):
-    """(offsets u64[nq + 1], positions u32[], mismatches u32[]); positions and mismatches are None without
-    fetch (the cap = 0 call)."""
+def _call(table, queries, k, fetch, metric="hamming"):
+    """(offsets u64[nq + 1], positions u32[], distances u32[]); positions and distances are None without
+    fetch (the cap = 0 call).  metric "hamming" counts mismatches, "edit" the Levenshtein distance."""
     import torch
     k = int(k)
     if not 0 <= k <= MAX_K:
         raise ValueError("k must be in 0 .. %d, got %d" % (MAX_K, k))
+    if metric not in METRICS:
+        raise ValueError("metric must be 'hamming' or 'edit', got %r" % (metric,))
+    kf = k | METRICS[metric]
     qs = [_as_bytes(q) for q in queries]
     nq, n = len(qs), len(table)
     d_t, d_r, d_s, ndocs = table._bwt_arrays()
@@ -31,9 +37,9 @@ def _call(table, queries, k, fetch):
     def call(cap, d_pos=0, d_mis=0):
         if d_s is None:
             return ctx.approx_positions_dev(d_t.data_ptr(), n, d_r.data_ptr(), d_q.data_ptr(), d_off.data_ptr(), nq,
-                                            k, d_o.data_ptr(), d_pos, d_mis, cap, stream)
+                                            kf, d_o.data_ptr(), d_pos, d_mis, cap, stream)
         return ctx.docs_approx_positions_dev(d_t.data_ptr(), n, d_r.data_ptr(), d_s.data_ptr(), ndocs,
-                                             d_q.data_ptr(), d_off.data_ptr(), nq, k, d_o.data_ptr(), d_pos, d_mis,
+                                             d_q.data_ptr(), d_off.data_ptr(), nq, kf, d_o.data_ptr(), d_pos, d_mis,
                                              cap, stream)
 
     pos = mis = None
@@ -51,15 +57,15 @@ def _call(table, queries, k, fetch):
     return offsets, pos[:total].cpu().numpy().view(np.uint32), mis[:total].cpu().numpy().view(np.uint32)
 
 
-def positions_batch(table, queries, k):
-    return _call(table, queries, k, True)
+def positions_batch(table, queries, k, metric="hamming"):
+    return _call(table, queries, k, True, metric)
 
 
-def positions(table, query, k):
-    _, pos, mis = _call(table, [query], k, True)
+def positions(table, query, k, metric="hamming"):
+    _, pos, mis = _call(table, [query], k, True, metric)
     return pos, mis
 
 
-def counts(table, queries, k):
-    off, _, _ = _call(table, queries, k, False)
+def counts(table, queries, k, metric="hamming"):
+    off, _, _ = _call(table, queries, k, False, metric)
     return np.diff(off.astype(np.int64)).astype(np.uint64)

@@ -36,6 +36,7 @@
 #include "lz.cuh"
 #include "bwt.cuh"
 #include "approx.cuh"
+#include "edit.cuh"
 #include "nccl_dyn.h"
 
 using namespace b200sa;
@@ -2882,15 +2883,18 @@ int b200sa_unbwt_dev(b200sa_ctx *c, uint64_t n, uint32_t ndocs, const uint8_t *d
     return leave(c, unbwt_core(c, (uint32_t)n, ndocs, d_bwt, d_term_rows, d_text_out, d_doc_starts_out));
 }
 
-// ------------------------------------------------------------ approximate positions (DESIGN 6b f-14)
-// nq >= 1, k <= B200SA_APPROX_MAX_K; d_starts non-null for documents (EndF = DocsEnd).  Phases: approx_check,
-// approx_pieces, approx_scan, approx_count, and approx_emit, approx_sort when the occurrences fit in cap.
+// ------------------------------------------------------------ approximate positions (DESIGN 6b f-14, f-15)
+// nq >= 1, k = threshold | flags as approx_args accepts it; d_starts non-null for documents (EndF = DocsEnd).
+// Phases: approx_check, approx_pieces, approx_scan, approx_count, and approx_emit, approx_sort when the
+// occurrences fit in cap.  B200SA_APPROX_EDIT picks k_approx_edit over k_approx; everything else is shared.
 template <class EndF>
 static int approx_core(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const uint32_t *d_sa,
                        const uint32_t *d_starts, uint32_t ndocs, const uint8_t *d_queries, const uint64_t *d_q_off,
-                       uint32_t nq, uint32_t k, uint64_t *d_offsets, uint32_t *d_pos, uint32_t *d_mis, uint64_t cap,
+                       uint32_t nq, uint32_t kf, uint64_t *d_offsets, uint32_t *d_pos, uint32_t *d_mis, uint64_t cap,
                        uint64_t *total, EndF end) {
     typedef unsigned long long u64;
+    const uint32_t k = kf & 0xFFFFu;
+    const bool edit = (kf & B200SA_APPROX_EDIT) != 0;
     TRY(mark(c, "approx_check"));
     TRY(ensure(c, c->small, 4096));
     uint32_t *words = ptr<uint32_t>(c->small);           // [0] check bits, [2, 4) items, [4, 6) total
@@ -2934,8 +2938,12 @@ static int approx_core(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const u
     const ApproxArgs A{d_text, d_sa, d_starts, ndocs, n, d_queries, d_q_off, (uint32_t)nslots, P, k, ps, pe,
                        item_start, items};
     const int pbits = bit_length(n - 1);
-    if (items) LAUNCH(c, k_approx<false>, cdiv(items, NWARP), A, cnt, (const u64 *)nullptr, pbits, (u64 *)nullptr,
-                      (uint32_t *)nullptr);
+    if (items && edit)
+        LAUNCH(c, k_approx_edit<false>, cdiv(items, NWARP), A, cnt, (const u64 *)nullptr, pbits, (u64 *)nullptr,
+               (uint32_t *)nullptr);
+    else if (items)
+        LAUNCH(c, k_approx<false>, cdiv(items, NWARP), A, cnt, (const u64 *)nullptr, pbits, (u64 *)nullptr,
+               (uint32_t *)nullptr);
     TRY((dev_scan<OpSum64>(c, InCount64{cnt, items}, OutStoreExcl64{item_off}, items + 1, d_total)));
     LAUNCH(c, k_approx_qoff, cdiv((uint64_t)nq + 1, BLK), item_start, item_off, nq, P,
            reinterpret_cast<u64 *>(d_offsets));
@@ -2947,8 +2955,12 @@ static int approx_core(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const u
         TRY(ensure(c, c->g1, (size_t)*total * 8));
         TRY(ensure(c, c->v0, (size_t)*total * 4));
         TRY(ensure(c, c->v1, (size_t)*total * 4));
-        LAUNCH(c, k_approx<true>, cdiv(items, NWARP), A, cnt, (const u64 *)item_off, pbits, ptr<u64>(c->g0),
-               ptr<uint32_t>(c->v0));
+        if (edit)
+            LAUNCH(c, k_approx_edit<true>, cdiv(items, NWARP), A, cnt, (const u64 *)item_off, pbits, ptr<u64>(c->g0),
+                   ptr<uint32_t>(c->v0));
+        else
+            LAUNCH(c, k_approx<true>, cdiv(items, NWARP), A, cnt, (const u64 *)item_off, pbits, ptr<u64>(c->g0),
+                   ptr<uint32_t>(c->v0));
         TRY(mark(c, "approx_sort"));                     // by (q, p)
         uint64_t *ko;
         uint32_t *vo;
@@ -2967,7 +2979,11 @@ static int approx_args(b200sa_ctx *c, uint64_t n, const void *text, const void *
                        uint32_t k, const void *offsets, const void *pos, uint64_t cap, const void *total) {
     if (!c) return B200SA_ERR_BAD_ARG;
     if (!total || !offsets || (nq > 0 && !q_off) || (cap > 0 && !pos) || (n > 0 && (!text || !sa))) return null_ptr(c);
-    if (k > B200SA_APPROX_MAX_K) return fail(c, B200SA_ERR_BAD_ARG, "approx positions: k above B200SA_APPROX_MAX_K");
+    if (k & ~(0xFFFFu | B200SA_APPROX_EDIT))
+        return fail(c, B200SA_ERR_BAD_ARG,
+                    "approx positions: k must be a threshold up to B200SA_APPROX_MAX_K, optionally | B200SA_APPROX_EDIT");
+    if ((k & 0xFFFFu) > B200SA_APPROX_MAX_K)
+        return fail(c, B200SA_ERR_BAD_ARG, "approx positions: k above B200SA_APPROX_MAX_K");
     if (n > B200SA_MAX_N) return too_long(c);
     return B200SA_OK;
 }

@@ -452,22 +452,26 @@ class DocumentSuffixTable:
         return _bwt.bwt_runs(self)
 
     # ---- approximate positions (DESIGN 6b f-14)
-    def approximate_positions(self, query, k):
+    def approximate_positions(self, query, k, *, metric="hamming"):
         """(positions u32[], mismatches u32[]): every position p of the concatenation whose window of m bytes
         lies inside p's document and differs from the query (m bytes) in at most k bytes, 0 <= k <= 31, by
         ascending p, with that number of mismatches beside it (b200sa_docs_approx_positions_dev).  locate()
-        maps the positions to (document, offset).  b"" matches nothing."""
-        return _approx.positions(self, query, k)
+        maps the positions to (document, offset).  b"" matches nothing.  metric="edit": every p with
+        dist(p) <= k instead, dist(p) the least Levenshtein distance between the query and a substring that
+        starts at p and ends inside p's document, listed beside p.  Any other metric than "hamming" or "edit"
+        raises ValueError."""
+        return _approx.positions(self, query, k, metric)
 
-    def approximate_positions_batch(self, queries, k):
+    def approximate_positions_batch(self, queries, k, *, metric="hamming"):
         """(offsets u64[nq + 1], positions u32[], mismatches u32[]): query q's occurrences with at most k
-        mismatches are positions[offsets[q]:offsets[q + 1]], as approximate_positions returns them."""
-        return _approx.positions_batch(self, queries, k)
+        mismatches (or within k edits, metric="edit") are positions[offsets[q]:offsets[q + 1]], as
+        approximate_positions returns them."""
+        return _approx.positions_batch(self, queries, k, metric)
 
-    def approximate_counts(self, queries, k):
-        """u64[nq]: the number of occurrences with at most k mismatches of every query, without fetching
-        them."""
-        return _approx.counts(self, queries, k)
+    def approximate_counts(self, queries, k, *, metric="hamming"):
+        """u64[nq]: the number of occurrences with at most k mismatches (or within k edits, metric="edit") of
+        every query, without fetching them."""
+        return _approx.counts(self, queries, k, metric)
 
     def top_documents(self, query, k) -> np.ndarray:
         """(document, count) rows of the min(k, df) documents that contain `query` most often, by count

@@ -280,25 +280,30 @@ class SuffixTable:
         return _bwt.bwt_runs(self)
 
     # ---- approximate positions (DESIGN 6b f-14)
-    def approximate_positions(self, query, k):
+    def approximate_positions(self, query, k, *, metric="hamming"):
         """(positions u32[], mismatches u32[]): every p with p + m <= n where text[p:p + m] differs from
         the query (m bytes) in at most k bytes, 0 <= k <= 31, by ascending p, with that number of
         mismatches beside it (b200sa_approx_positions_dev).  b"" matches nothing; for k = 0 the positions
-        are those of positions(query), sorted.  Uses the device copies of _bwt_arrays()."""
+        are those of positions(query), sorted.  Uses the device copies of _bwt_arrays().
+        metric="edit": every p in [0, n) with dist(p) <= k instead, dist(p) the least Levenshtein distance
+        between the query and a text[p:e], e <= n, listed beside p; an exact hit at p also puts its neighbours
+        at distance 1 (include/b200sa.h, B200SA_APPROX_EDIT).  Any other metric than "hamming" or "edit" raises
+        ValueError."""
         from . import _approx
-        return _approx.positions(self, query, k)
+        return _approx.positions(self, query, k, metric)
 
-    def approximate_positions_batch(self, queries, k):
+    def approximate_positions_batch(self, queries, k, *, metric="hamming"):
         """(offsets u64[nq + 1], positions u32[], mismatches u32[]): query q's occurrences with at most k
-        mismatches are positions[offsets[q]:offsets[q + 1]], as approximate_positions returns them."""
+        mismatches (or within k edits, metric="edit") are positions[offsets[q]:offsets[q + 1]], as
+        approximate_positions returns them."""
         from . import _approx
-        return _approx.positions_batch(self, queries, k)
+        return _approx.positions_batch(self, queries, k, metric)
 
-    def approximate_counts(self, queries, k):
-        """u64[nq]: the number of occurrences with at most k mismatches of every query, without fetching
-        them."""
+    def approximate_counts(self, queries, k, *, metric="hamming"):
+        """u64[nq]: the number of occurrences with at most k mismatches (or within k edits, metric="edit") of
+        every query, without fetching them."""
         from . import _approx
-        return _approx.counts(self, queries, k)
+        return _approx.counts(self, queries, k, metric)
 
     # ---- persistence (SURVEY 8f-2): the only "wire format" the reference API implies is
     # from_parts/into_parts (src/table.rs:111-127): text bytes + little-endian u32 table.

@@ -164,6 +164,13 @@ for k, tab in enumerate([single] + [DocumentSuffixTable(docs) for docs in doc_se
     for kk in (0, 3, 31):
         off, pos, mis = tab.approximate_positions_batch(ap_qs + [b"a" * 9], kk)
         assert len(pos) == int(off[-1]) and (mis <= kk).all(), (k, kk)
+# approximate positions within k edits: the same tables and queries with the edit metric, whose windows reach k
+# past both sides of every candidate and whose band reaches 2k past them, near document ends included
+for k, tab in enumerate([single] + [DocumentSuffixTable(docs) for docs in doc_sets] +
+                        [SuffixTable(b"a" * 5000), DocumentSuffixTable([b"", b"ab", b"", b"c"])]):
+    for kk in (0, 3, 31):
+        off, pos, dist = tab.approximate_positions_batch(ap_qs + [b"a" * 9, b"A" * 40], kk, metric="edit")
+        assert len(pos) == int(off[-1]) and (dist <= kk).all(), (k, kk)
 # refinement branches (tests/test_gpu_refine.py): a local-sort overflow in round 2 of the direct path, the direct
 # path's probe (2^20 tied after round 1, large groups), 64-bit round-0 keys of the reduced string
 import ctypes
