@@ -565,9 +565,36 @@ int b200sa_unbwt_dev(b200sa_ctx *ctx, uint64_t n, uint32_t ndocs, const uint8_t 
  * diagonals [s - o_j - 2k, s - o_j + 2k].  It emits p iff dist(p) <= k and it is the least (i, s'') such that
  * piece i occurs exactly at s'' inside p's document with |s'' - o_i - p| <= k; every occurrence has one such
  * least pair (the partition lemma), so each is emitted once.  A query of 0 < m <= k keeps the whole-table slot
- * and each rank s reports itself. */
+ * and each rank s reports itself.
+ *
+ * ---- best hits: each query's occurrences at its least distance, plus a slack (DESIGN.md 6b f-16) ----
+ * With B200SA_APPROX_BEST the k argument is threshold | B200SA_APPROX_SLACK(s) | B200SA_APPROX_BEST, optionally
+ * | B200SA_APPROX_EDIT: threshold = k & 0xFF and s = (k >> 8) & 0xFF, both at most B200SA_APPROX_MAX_K; any other
+ * bit, or a threshold or s above it, returns B200SA_ERR_BAD_ARG with a detail that names B200SA_APPROX_MAX_K.
+ * Without B200SA_APPROX_BEST, k is decoded as above (bits 8-15 are threshold bits) and nothing changes.
+ * d(p) is mis(p), or dist(p) with B200SA_APPROX_EDIT.  The occurrences of q at a threshold t are what the call
+ * without B200SA_APPROX_BEST returns at t; best(q) is the least d(p) over q's occurrences at the threshold,
+ * undefined when it has none.  Query q lists its occurrences with d(p) <= t(q), t(q) = min(threshold,
+ * best(q) + s): q's list is exactly what the call without the flag returns for q at threshold t(q), by ascending
+ * p with d(p) in d_mismatches.  A query with no occurrence within the threshold lists nothing.  So s = 0 lists
+ * the best stratum (every listed d equals best(q)); s >= threshold gives the call without the flag at threshold,
+ * bit for bit; threshold = 0 gives the exact call.  Offsets, total, cap, the nq * (threshold + 1) TOO_LARGE
+ * check, nq = 0, n = 0, m = 0 and the bytes read are as above.
+ * Method: rounds t = 0, 1, .., threshold.  Round t searches, with the pieces and verification above at
+ * threshold t, the live queries: those with no occurrence in an earlier round, and those whose first round
+ * with an occurrence, best(q), has t <= best(q) + s.  The search runs on the live queries compacted into a
+ * batch of their own.  The rounds stop when no query is live; b200sa_last_stats().doubling_rounds holds the
+ * number run.  q's count is its count in its last live round.  When total <= cap, one emission at each distinct
+ * t(q) over the queries that end there writes their lists into place.  Device workspace (computed, not
+ * measured): 25 bytes per query and 1 per query byte for the batches, plus what the search above takes per
+ * round for its batch at threshold t (16 bytes per piece, 12 per candidate chunk), and, when fetched, 24 bytes
+ * per entry of the largest group plus the sort's tile status.  Phases: approx_check; per round best_compact,
+ * approx_pieces, approx_scan, approx_count, best_update; per emitted group best_compact, approx_pieces,
+ * approx_scan, approx_count, approx_emit, approx_sort, best_scatter. */
 #define B200SA_APPROX_MAX_K 31
 #define B200SA_APPROX_EDIT 0x10000u
+#define B200SA_APPROX_BEST 0x100000u                      /* bit 20 */
+#define B200SA_APPROX_SLACK(s) ((uint32_t)(s) << 8)       /* 0 <= s <= 31, only with B200SA_APPROX_BEST */
 int b200sa_approx_positions_dev(b200sa_ctx *ctx, const uint8_t *d_text, uint64_t n, const uint32_t *d_sa,
                                 const uint8_t *d_queries, const uint64_t *d_q_off, uint32_t nq, uint32_t k,
                                 uint64_t *d_offsets, uint32_t *d_pos, uint32_t *d_mismatches, uint64_t cap,

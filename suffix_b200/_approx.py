@@ -1,5 +1,5 @@
-"""Approximate positions (occurrences with at most k mismatches, or within k edits with metric="edit") over a
-device-resident table: the part SuffixTable and DocumentSuffixTable share.  A table supplies `_device` and
+"""Approximate positions (occurrences with at most k mismatches, or within k edits with metric="edit", and with
+best=s only each query's best hits) over a device-resident table: the part SuffixTable and DocumentSuffixTable share.  A table supplies `_device` and
 `_bwt_arrays()` -> (d_text, d_table, d_doc_starts or None, ndocs), its text and table on the device; the LCP
 array is not needed."""
 import numpy as np
@@ -9,19 +9,30 @@ from .table import _as_bytes, _lock
 
 MAX_K = 31                # B200SA_APPROX_MAX_K
 EDIT = 0x10000            # B200SA_APPROX_EDIT
+BEST = 0x100000           # B200SA_APPROX_BEST
 METRICS = {"hamming": 0, "edit": EDIT}
 
 
-def _call(table, queries, k, fetch, metric="hamming"):
+def _flags(best):
+    """The k bits of best=: 0 for None, B200SA_APPROX_SLACK(s) | B200SA_APPROX_BEST for an int s in 0 .. 31."""
+    if best is None:
+        return 0
+    if isinstance(best, (bool, np.bool_)) or not isinstance(best, (int, np.integer)) or not 0 <= best <= MAX_K:
+        raise ValueError("best must be None or an int slack in 0 .. %d, got %r" % (MAX_K, best))
+    return (int(best) << 8) | BEST
+
+
+def _call(table, queries, k, fetch, metric="hamming", best=None):
     """(offsets u64[nq + 1], positions u32[], distances u32[]); positions and distances are None without
-    fetch (the cap = 0 call).  metric "hamming" counts mismatches, "edit" the Levenshtein distance."""
+    fetch (the cap = 0 call).  metric "hamming" counts mismatches, "edit" the Levenshtein distance; best=s keeps
+    each query's occurrences within s of its least distance (include/b200sa.h, B200SA_APPROX_BEST)."""
     import torch
     k = int(k)
     if not 0 <= k <= MAX_K:
         raise ValueError("k must be in 0 .. %d, got %d" % (MAX_K, k))
     if metric not in METRICS:
         raise ValueError("metric must be 'hamming' or 'edit', got %r" % (metric,))
-    kf = k | METRICS[metric]
+    kf = k | METRICS[metric] | _flags(best)
     qs = [_as_bytes(q) for q in queries]
     nq, n = len(qs), len(table)
     d_t, d_r, d_s, ndocs = table._bwt_arrays()
@@ -57,15 +68,15 @@ def _call(table, queries, k, fetch, metric="hamming"):
     return offsets, pos[:total].cpu().numpy().view(np.uint32), mis[:total].cpu().numpy().view(np.uint32)
 
 
-def positions_batch(table, queries, k, metric="hamming"):
-    return _call(table, queries, k, True, metric)
+def positions_batch(table, queries, k, metric="hamming", best=None):
+    return _call(table, queries, k, True, metric, best)
 
 
-def positions(table, query, k, metric="hamming"):
-    _, pos, mis = _call(table, [query], k, True, metric)
+def positions(table, query, k, metric="hamming", best=None):
+    _, pos, mis = _call(table, [query], k, True, metric, best)
     return pos, mis
 
 
-def counts(table, queries, k, metric="hamming"):
-    off, _, _ = _call(table, queries, k, False, metric)
+def counts(table, queries, k, metric="hamming", best=None):
+    off, _, _ = _call(table, queries, k, False, metric, best)
     return np.diff(off.astype(np.int64)).astype(np.uint64)

@@ -37,6 +37,7 @@
 #include "bwt.cuh"
 #include "approx.cuh"
 #include "edit.cuh"
+#include "best.cuh"
 #include "nccl_dyn.h"
 
 using namespace b200sa;
@@ -2883,38 +2884,46 @@ int b200sa_unbwt_dev(b200sa_ctx *c, uint64_t n, uint32_t ndocs, const uint8_t *d
     return leave(c, unbwt_core(c, (uint32_t)n, ndocs, d_bwt, d_term_rows, d_text_out, d_doc_starts_out));
 }
 
-// ------------------------------------------------------------ approximate positions (DESIGN 6b f-14, f-15)
-// nq >= 1, k = threshold | flags as approx_args accepts it; d_starts non-null for documents (EndF = DocsEnd).
-// Phases: approx_check, approx_pieces, approx_scan, approx_count, and approx_emit, approx_sort when the
-// occurrences fit in cap.  B200SA_APPROX_EDIT picks k_approx_edit over k_approx; everything else is shared.
-template <class EndF>
-static int approx_core(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const uint32_t *d_sa,
-                       const uint32_t *d_starts, uint32_t ndocs, const uint8_t *d_queries, const uint64_t *d_q_off,
-                       uint32_t nq, uint32_t kf, uint64_t *d_offsets, uint32_t *d_pos, uint32_t *d_mis, uint64_t cap,
-                       uint64_t *total, EndF end) {
-    typedef unsigned long long u64;
-    const uint32_t k = kf & 0xFFFFu;
-    const bool edit = (kf & B200SA_APPROX_EDIT) != 0;
+// ------------------------------------------------------------ approximate positions (DESIGN 6b f-14, f-15, f-16)
+// The checks of a call (nq >= 1, k its threshold): q_off on the device with q_off[nq] read back as *q_bytes,
+// doc_starts (d_starts non-null for documents), and the sizes.  Phase approx_check.
+static int approx_prep(b200sa_ctx *c, uint32_t n, const uint32_t *d_starts, uint32_t ndocs, const uint8_t *d_queries,
+                       const uint64_t *d_q_off, uint32_t nq, uint32_t k, uint64_t *q_bytes) {
     TRY(mark(c, "approx_check"));
     TRY(ensure(c, c->small, 4096));
-    uint32_t *words = ptr<uint32_t>(c->small);           // [0] check bits, [2, 4) items, [4, 6) total
     CU_TRY(c, cudaMemcpyAsync(c->h_pin, d_q_off + nq, 8, cudaMemcpyDeviceToHost, c->stream));
     CU_TRY(c, cudaStreamSynchronize(c->stream));
-    const uint64_t q_bytes = pin_u64(c, 0);
-    TRY(match_check(c, d_q_off, nq, q_bytes));           // q_off[0] = 0 and ascending
+    *q_bytes = pin_u64(c, 0);
+    TRY(match_check(c, d_q_off, nq, *q_bytes));          // q_off[0] = 0 and ascending
     if (d_starts && ndocs > 0) TRY(docs_check_dev(c, d_starts, ndocs, n));
-    if (q_bytes > B200SA_MAX_N) return fail(c, B200SA_ERR_TOO_LARGE, "queries longer than 2^32-4096 bytes");
-    if (q_bytes > 0 && !d_queries) return null_ptr(c);
+    if (*q_bytes > B200SA_MAX_N) return fail(c, B200SA_ERR_TOO_LARGE, "queries longer than 2^32-4096 bytes");
+    if (*q_bytes > 0 && !d_queries) return null_ptr(c);
+    if ((uint64_t)nq * (k + 1) >= 0xFFFFFFFFull)
+        return fail(c, B200SA_ERR_TOO_LARGE, "approx positions: nq * (k + 1) of 2^32 - 1 or more slots");
+    return B200SA_OK;
+}
+
+// n = 0: every list is empty.
+static int approx_nothing(b200sa_ctx *c, uint64_t *d_offsets, uint32_t nq) {
+    CU_TRY(c, cudaMemsetAsync(d_offsets, 0, ((size_t)nq + 1) * 8, c->stream));
+    TRY(mark(c, "end"));
+    CU_TRY(c, cudaStreamSynchronize(c->stream));
+    return B200SA_OK;
+}
+
+// One search of nq >= 1 queries at threshold k on n >= 1 bytes: d_offsets (nq + 1) and *total, read back.  When
+// 0 < total <= cap it also emits and sorts: *ko / *vo then hold the keys (q << *pbits) | p in (q, p) order and
+// their distances.  Phases: approx_pieces, approx_scan, approx_count, and approx_emit, approx_sort when it
+// emits.  B200SA_APPROX_EDIT picks k_approx_edit over k_approx; everything else is shared.
+template <class EndF>
+static int approx_search(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const uint32_t *d_sa,
+                         const uint32_t *d_starts, uint32_t ndocs, const uint8_t *d_queries, const uint64_t *d_q_off,
+                         uint32_t nq, uint32_t k, bool edit, uint64_t *d_offsets, uint64_t cap, uint64_t *total,
+                         EndF end, uint64_t **ko, uint32_t **vo, int *pbits_out) {
+    typedef unsigned long long u64;
+    uint32_t *words = ptr<uint32_t>(c->small);           // [0] check bits, [2, 4) items, [4, 6) total
     const uint32_t P = k + 1;
     const uint64_t nslots = (uint64_t)nq * P;
-    if (nslots >= 0xFFFFFFFFull)
-        return fail(c, B200SA_ERR_TOO_LARGE, "approx positions: nq * (k + 1) of 2^32 - 1 or more slots");
-    if (n == 0) {                                        // nothing occurs
-        CU_TRY(c, cudaMemsetAsync(d_offsets, 0, ((size_t)nq + 1) * 8, c->stream));
-        TRY(mark(c, "end"));
-        CU_TRY(c, cudaStreamSynchronize(c->stream));
-        return B200SA_OK;
-    }
     TRY(mark(c, "approx_pieces"));
     TRY(ensure(c, c->p1, (size_t)nslots * 8));
     uint32_t *ps = ptr<uint32_t>(c->p1), *pe = ps + nslots;
@@ -2949,6 +2958,7 @@ static int approx_core(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const u
            reinterpret_cast<u64 *>(d_offsets));
     TRY(read_words(c, words + 4, 2));
     *total = pin_u64(c, 0);
+    *pbits_out = pbits;
     if (*total > 0 && *total <= cap) {
         TRY(mark(c, "approx_emit"));
         TRY(ensure(c, c->g0, (size_t)*total * 8));
@@ -2962,12 +2972,117 @@ static int approx_core(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const u
             LAUNCH(c, k_approx<true>, cdiv(items, NWARP), A, cnt, (const u64 *)item_off, pbits, ptr<u64>(c->g0),
                    ptr<uint32_t>(c->v0));
         TRY(mark(c, "approx_sort"));                     // by (q, p)
-        uint64_t *ko;
-        uint32_t *vo;
         TRY(sort_pairs<uint64_t>(c, ptr<uint64_t>(c->g0), ptr<uint32_t>(c->v0), ptr<uint64_t>(c->g1),
-                                 ptr<uint32_t>(c->v1), *total, bit_length(nq - 1) + pbits, &ko, &vo));
+                                 ptr<uint32_t>(c->v1), *total, bit_length(nq - 1) + pbits, ko, vo));
+    }
+    return B200SA_OK;
+}
+
+// nq >= 1, k = threshold | flags as approx_args accepts it, without B200SA_APPROX_BEST.
+template <class EndF>
+static int approx_core(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const uint32_t *d_sa,
+                       const uint32_t *d_starts, uint32_t ndocs, const uint8_t *d_queries, const uint64_t *d_q_off,
+                       uint32_t nq, uint32_t kf, uint64_t *d_offsets, uint32_t *d_pos, uint32_t *d_mis, uint64_t cap,
+                       uint64_t *total, EndF end) {
+    typedef unsigned long long u64;
+    const uint32_t k = kf & 0xFFFFu;
+    uint64_t q_bytes;
+    TRY(approx_prep(c, n, d_starts, ndocs, d_queries, d_q_off, nq, k, &q_bytes));
+    if (n == 0) return approx_nothing(c, d_offsets, nq);
+    uint64_t *ko = nullptr;
+    uint32_t *vo = nullptr;
+    int pbits = 0;
+    TRY(approx_search(c, d_text, n, d_sa, d_starts, ndocs, d_queries, d_q_off, nq, k, (kf & B200SA_APPROX_EDIT) != 0,
+                      d_offsets, cap, total, end, &ko, &vo, &pbits));
+    if (*total > 0 && *total <= cap)
         LAUNCH(c, k_approx_gather, cdiv(*total, BLK), (const u64 *)ko, (const uint32_t *)vo, *total,
                (u64)((1ull << pbits) - 1), d_pos, d_mis);
+    TRY(mark(c, "end"));
+    CU_TRY(c, cudaGetLastError());
+    CU_TRY(c, cudaStreamSynchronize(c->stream));
+    return B200SA_OK;
+}
+
+// The batch a BestPick selects: *nb queries, map[i] the query of entry i; their bytes and offsets at *bq / *boff,
+// the call's own arrays when every query is picked, else gathered into c->qbuf and coff.
+static int best_batch(b200sa_ctx *c, const uint8_t *d_queries, const uint64_t *d_q_off, uint32_t nq, BestPick pick,
+                      uint32_t *map, uint64_t *coff, uint32_t *nb, const uint8_t **bq, const uint64_t **boff) {
+    typedef unsigned long long u64;
+    uint32_t *words = ptr<uint32_t>(c->small);           // [8, 10) (batch size << 32) | batch bytes
+    TRY((dev_scan<OpSum64>(c, pick, BestPickOut{nq, map, coff}, (uint64_t)nq + 1, reinterpret_cast<u64 *>(words + 8))));
+    TRY(read_words(c, words + 8, 2));
+    *nb = (uint32_t)(pin_u64(c, 0) >> 32);
+    *bq = d_queries;
+    *boff = d_q_off;
+    if (*nb == nq || *nb == 0) return B200SA_OK;
+    LAUNCH(c, k_best_gather, cdiv((uint64_t)*nb * 32, BLK), d_queries, d_q_off, (const uint32_t *)map,
+           (const uint64_t *)coff, *nb, ptr<uint8_t>(c->qbuf));
+    *bq = ptr<uint8_t>(c->qbuf);
+    *boff = coff;
+    return B200SA_OK;
+}
+
+// nq >= 1, k = threshold | B200SA_APPROX_SLACK(s) | B200SA_APPROX_BEST, optionally | B200SA_APPROX_EDIT.
+// Rounds t = 0 .. threshold over the live queries (best.cuh), then one emission per distinct final threshold.
+// Phases: approx_check; per round best_compact, the search's phases, best_update; per emitted group
+// best_compact, the search's phases, best_scatter.
+template <class EndF>
+static int approx_best_core(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const uint32_t *d_sa,
+                            const uint32_t *d_starts, uint32_t ndocs, const uint8_t *d_queries,
+                            const uint64_t *d_q_off, uint32_t nq, uint32_t kf, uint64_t *d_offsets, uint32_t *d_pos,
+                            uint32_t *d_mis, uint64_t cap, uint64_t *total, EndF end) {
+    typedef unsigned long long u64;
+    const uint32_t k = kf & 0xFFu, s = (kf >> 8) & 0xFFu;
+    const bool edit = (kf & B200SA_APPROX_EDIT) != 0;
+    uint64_t q_bytes;
+    c->stats.doubling_rounds = 0;
+    TRY(approx_prep(c, n, d_starts, ndocs, d_queries, d_q_off, nq, k, &q_bytes));
+    if (n == 0) return approx_nothing(c, d_offsets, nq);
+    TRY(ensure(c, c->k32b, (size_t)nq * 9));             // cnt, map (u32), best (u8) per query
+    TRY(ensure(c, c->rank, ((size_t)nq + 1) * 16));      // the batch's q_off, the search's offsets
+    TRY(ensure(c, c->qbuf, (size_t)q_bytes));
+    uint32_t *cnt = ptr<uint32_t>(c->k32b), *map = cnt + nq;
+    uint8_t *best = reinterpret_cast<uint8_t *>(map + nq);
+    uint64_t *coff = ptr<uint64_t>(c->rank), *soff = coff + nq + 1;
+    uint32_t *words = ptr<uint32_t>(c->small);           // [10] rounds where a query ended, [12, 14) total
+    CU_TRY(c, cudaMemsetAsync(cnt, 0, (size_t)nq * 4, c->stream));
+    CU_TRY(c, cudaMemsetAsync(best, BEST_NONE, nq, c->stream));
+    CU_TRY(c, cudaMemsetAsync(words + 8, 0, 24, c->stream));
+    uint64_t *ko = nullptr, rtotal = 0;
+    uint32_t *vo = nullptr, nb = 0, rounds = 0;
+    int pbits = 0;
+    const uint8_t *bq;
+    const uint64_t *boff;
+    for (uint32_t t = 0; t <= k; t++) {
+        TRY(mark(c, "best_compact"));
+        TRY(best_batch(c, d_queries, d_q_off, nq, BestPick{d_q_off, best, nq, t, s, k, false}, map, coff, &nb, &bq,
+                       &boff));
+        if (nb == 0) break;
+        rounds++;
+        TRY(approx_search(c, d_text, n, d_sa, d_starts, ndocs, bq, boff, nb, t, edit, soff, 0, &rtotal, end, &ko, &vo,
+                          &pbits));
+        TRY(mark(c, "best_update"));
+        LAUNCH(c, k_best_update, cdiv(nb, BLK), (const uint32_t *)map, (const u64 *)soff, nb, t, s, k, best, cnt,
+               words + 10);
+    }
+    c->stats.doubling_rounds = rounds;
+    TRY((dev_scan<OpSum64>(c, InCount64{cnt, nq}, OutStoreExcl64{reinterpret_cast<u64 *>(d_offsets)}, (uint64_t)nq + 1,
+                           reinterpret_cast<u64 *>(words + 12))));
+    TRY(read_words(c, words + 10, 4));
+    const uint32_t ended = c->h_pin[0];
+    *total = pin_u64(c, 2);
+    if (*total > 0 && *total <= cap) {
+        for (uint32_t t = 0; t <= k; t++) {
+            if (!(ended >> t & 1u)) continue;
+            TRY(mark(c, "best_compact"));
+            TRY(best_batch(c, d_queries, d_q_off, nq, BestPick{d_q_off, best, nq, t, s, k, true}, map, coff, &nb, &bq,
+                           &boff));
+            TRY(approx_search(c, d_text, n, d_sa, d_starts, ndocs, bq, boff, nb, t, edit, soff, ~0ull, &rtotal, end,
+                              &ko, &vo, &pbits));
+            TRY(mark(c, "best_scatter"));
+            LAUNCH(c, k_best_scatter, cdiv(rtotal, BLK), (const u64 *)ko, (const uint32_t *)vo, rtotal, pbits,
+                   (const u64 *)soff, (const uint32_t *)map, (const u64 *)d_offsets, d_pos, d_mis);
+        }
     }
     TRY(mark(c, "end"));
     CU_TRY(c, cudaGetLastError());
@@ -2979,11 +3094,19 @@ static int approx_args(b200sa_ctx *c, uint64_t n, const void *text, const void *
                        uint32_t k, const void *offsets, const void *pos, uint64_t cap, const void *total) {
     if (!c) return B200SA_ERR_BAD_ARG;
     if (!total || !offsets || (nq > 0 && !q_off) || (cap > 0 && !pos) || (n > 0 && (!text || !sa))) return null_ptr(c);
-    if (k & ~(0xFFFFu | B200SA_APPROX_EDIT))
-        return fail(c, B200SA_ERR_BAD_ARG,
-                    "approx positions: k must be a threshold up to B200SA_APPROX_MAX_K, optionally | B200SA_APPROX_EDIT");
-    if ((k & 0xFFFFu) > B200SA_APPROX_MAX_K)
-        return fail(c, B200SA_ERR_BAD_ARG, "approx positions: k above B200SA_APPROX_MAX_K");
+    if (k & B200SA_APPROX_BEST) {
+        if (k & ~(0xFFFFu | B200SA_APPROX_EDIT | B200SA_APPROX_BEST) || (k & 0xFFu) > B200SA_APPROX_MAX_K ||
+            ((k >> 8) & 0xFFu) > B200SA_APPROX_MAX_K)
+            return fail(c, B200SA_ERR_BAD_ARG,
+                        "approx positions: with B200SA_APPROX_BEST, k must be a threshold up to B200SA_APPROX_MAX_K | "
+                        "B200SA_APPROX_SLACK(s) with s up to B200SA_APPROX_MAX_K, optionally | B200SA_APPROX_EDIT");
+    } else {
+        if (k & ~(0xFFFFu | B200SA_APPROX_EDIT))
+            return fail(c, B200SA_ERR_BAD_ARG,
+                        "approx positions: k must be a threshold up to B200SA_APPROX_MAX_K, optionally | B200SA_APPROX_EDIT");
+        if ((k & 0xFFFFu) > B200SA_APPROX_MAX_K)
+            return fail(c, B200SA_ERR_BAD_ARG, "approx positions: k above B200SA_APPROX_MAX_K");
+    }
     if (n > B200SA_MAX_N) return too_long(c);
     return B200SA_OK;
 }
@@ -2996,6 +3119,9 @@ int b200sa_approx_positions_dev(b200sa_ctx *c, const uint8_t *d_text, uint64_t n
     TRY(enter(c, stream));
     *total = 0;
     if (nq == 0) return leave(c, empty_batch(c, d_offsets));
+    if (k & B200SA_APPROX_BEST)
+        return leave(c, approx_best_core(c, d_text, (uint32_t)n, d_sa, nullptr, 0, d_queries, d_q_off, nq, k, d_offsets,
+                                         d_pos, d_mismatches, cap, total, TextEnd{(uint32_t)n}));
     return leave(c, approx_core(c, d_text, (uint32_t)n, d_sa, nullptr, 0, d_queries, d_q_off, nq, k, d_offsets, d_pos,
                                 d_mismatches, cap, total, TextEnd{(uint32_t)n}));
 }
@@ -3011,6 +3137,10 @@ int b200sa_docs_approx_positions_dev(b200sa_ctx *c, const uint8_t *d_text, uint6
     TRY(enter(c, stream));
     *total = 0;
     if (nq == 0) return leave(c, empty_batch(c, d_offsets));
+    if (k & B200SA_APPROX_BEST)
+        return leave(c, approx_best_core(c, d_text, (uint32_t)n, d_gsa, d_doc_starts, ndocs, d_queries, d_q_off, nq, k,
+                                         d_offsets, d_pos, d_mismatches, cap, total,
+                                         DocsEnd{d_doc_starts, ndocs, (uint32_t)n}));
     return leave(c, approx_core(c, d_text, (uint32_t)n, d_gsa, d_doc_starts, ndocs, d_queries, d_q_off, nq, k, d_offsets,
                                 d_pos, d_mismatches, cap, total, DocsEnd{d_doc_starts, ndocs, (uint32_t)n}));
 }

@@ -451,27 +451,34 @@ class DocumentSuffixTable:
         is a symbol of its own."""
         return _bwt.bwt_runs(self)
 
-    # ---- approximate positions (DESIGN 6b f-14)
-    def approximate_positions(self, query, k, *, metric="hamming"):
+    # ---- approximate positions (DESIGN 6b f-14, f-15, f-16)
+    def approximate_positions(self, query, k, *, metric="hamming", best=None):
         """(positions u32[], mismatches u32[]): every position p of the concatenation whose window of m bytes
         lies inside p's document and differs from the query (m bytes) in at most k bytes, 0 <= k <= 31, by
         ascending p, with that number of mismatches beside it (b200sa_docs_approx_positions_dev).  locate()
         maps the positions to (document, offset).  b"" matches nothing.  metric="edit": every p with
         dist(p) <= k instead, dist(p) the least Levenshtein distance between the query and a substring that
         starts at p and ends inside p's document, listed beside p.  Any other metric than "hamming" or "edit"
+        raises ValueError.
+        best=s (an int, 0 <= s <= 31) lists only each query's best hits: with best(q) its least distance within
+        k, the occurrences at distance <= min(k, best(q) + s), exactly what the call returns at that threshold
+        (B200SA_APPROX_BEST).  best=0 gives each query's best hits, and the distance column then holds best(q)
+        on every one.  best=None (the default) lists every occurrence within k; any other value, True included,
         raises ValueError."""
-        return _approx.positions(self, query, k, metric)
+        return _approx.positions(self, query, k, metric, best)
 
-    def approximate_positions_batch(self, queries, k, *, metric="hamming"):
+    def approximate_positions_batch(self, queries, k, *, metric="hamming", best=None):
         """(offsets u64[nq + 1], positions u32[], mismatches u32[]): query q's occurrences with at most k
         mismatches (or within k edits, metric="edit") are positions[offsets[q]:offsets[q + 1]], as
-        approximate_positions returns them."""
-        return _approx.positions_batch(self, queries, k, metric)
+        approximate_positions returns them; best=0 gives each query's best hits, with best(q) in the
+        distance column (best= as in approximate_positions)."""
+        return _approx.positions_batch(self, queries, k, metric, best)
 
-    def approximate_counts(self, queries, k, *, metric="hamming"):
+    def approximate_counts(self, queries, k, *, metric="hamming", best=None):
         """u64[nq]: the number of occurrences with at most k mismatches (or within k edits, metric="edit") of
-        every query, without fetching them."""
-        return _approx.counts(self, queries, k, metric)
+        every query, without fetching them; best=0 counts each query's best hits, those at distance best(q)
+        (best= as in approximate_positions)."""
+        return _approx.counts(self, queries, k, metric, best)
 
     def top_documents(self, query, k) -> np.ndarray:
         """(document, count) rows of the min(k, df) documents that contain `query` most often, by count

@@ -279,8 +279,8 @@ class SuffixTable:
         from . import _bwt
         return _bwt.bwt_runs(self)
 
-    # ---- approximate positions (DESIGN 6b f-14)
-    def approximate_positions(self, query, k, *, metric="hamming"):
+    # ---- approximate positions (DESIGN 6b f-14, f-15, f-16)
+    def approximate_positions(self, query, k, *, metric="hamming", best=None):
         """(positions u32[], mismatches u32[]): every p with p + m <= n where text[p:p + m] differs from
         the query (m bytes) in at most k bytes, 0 <= k <= 31, by ascending p, with that number of
         mismatches beside it (b200sa_approx_positions_dev).  b"" matches nothing; for k = 0 the positions
@@ -288,22 +288,29 @@ class SuffixTable:
         metric="edit": every p in [0, n) with dist(p) <= k instead, dist(p) the least Levenshtein distance
         between the query and a text[p:e], e <= n, listed beside p; an exact hit at p also puts its neighbours
         at distance 1 (include/b200sa.h, B200SA_APPROX_EDIT).  Any other metric than "hamming" or "edit" raises
-        ValueError."""
+        ValueError.
+        best=s (an int, 0 <= s <= 31) lists only each query's best hits: with best(q) its least distance within
+        k, the occurrences at distance <= min(k, best(q) + s), exactly what the call returns at that threshold
+        (B200SA_APPROX_BEST).  best=0 gives each query's best hits, and the distance column then holds best(q)
+        on every one.  best=None (the default) lists every occurrence within k; any other value, True included,
+        raises ValueError."""
         from . import _approx
-        return _approx.positions(self, query, k, metric)
+        return _approx.positions(self, query, k, metric, best)
 
-    def approximate_positions_batch(self, queries, k, *, metric="hamming"):
+    def approximate_positions_batch(self, queries, k, *, metric="hamming", best=None):
         """(offsets u64[nq + 1], positions u32[], mismatches u32[]): query q's occurrences with at most k
         mismatches (or within k edits, metric="edit") are positions[offsets[q]:offsets[q + 1]], as
-        approximate_positions returns them."""
+        approximate_positions returns them; best=0 gives each query's best hits, with best(q) in the
+        distance column (best= as in approximate_positions)."""
         from . import _approx
-        return _approx.positions_batch(self, queries, k, metric)
+        return _approx.positions_batch(self, queries, k, metric, best)
 
-    def approximate_counts(self, queries, k, *, metric="hamming"):
+    def approximate_counts(self, queries, k, *, metric="hamming", best=None):
         """u64[nq]: the number of occurrences with at most k mismatches (or within k edits, metric="edit") of
-        every query, without fetching them."""
+        every query, without fetching them; best=0 counts each query's best hits, those at distance best(q)
+        (best= as in approximate_positions)."""
         from . import _approx
-        return _approx.counts(self, queries, k, metric)
+        return _approx.counts(self, queries, k, metric, best)
 
     # ---- persistence (SURVEY 8f-2): the only "wire format" the reference API implies is
     # from_parts/into_parts (src/table.rs:111-127): text bytes + little-endian u32 table.

@@ -171,6 +171,14 @@ for k, tab in enumerate([single] + [DocumentSuffixTable(docs) for docs in doc_se
     for kk in (0, 3, 31):
         off, pos, dist = tab.approximate_positions_batch(ap_qs + [b"a" * 9, b"A" * 40], kk, metric="edit")
         assert len(pos) == int(off[-1]) and (dist <= kk).all(), (k, kk)
+# best hits: the same tables and queries in rounds over compacted batches (every query live, some, none), with
+# one emission and scatter per final threshold, for both metrics
+for k, tab in enumerate([single] + [DocumentSuffixTable(docs) for docs in doc_sets] +
+                        [SuffixTable(b"a" * 5000), DocumentSuffixTable([b"", b"ab", b"", b"c"])]):
+    for kk, sl in ((0, 0), (3, 0), (3, 1), (31, 2)):
+        for metric in ("hamming", "edit"):
+            off, pos, dist = tab.approximate_positions_batch(ap_qs + [b"a" * 9, b"A" * 40], kk, metric=metric, best=sl)
+            assert len(pos) == int(off[-1]) and (dist <= kk).all(), (k, kk, sl, metric)
 # refinement branches (tests/test_gpu_refine.py): a local-sort overflow in round 2 of the direct path, the direct
 # path's probe (2^20 tied after round 1, large groups), 64-bit round-0 keys of the reduced string
 import ctypes
