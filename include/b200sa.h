@@ -590,11 +590,40 @@ int b200sa_unbwt_dev(b200sa_ctx *ctx, uint64_t n, uint32_t ndocs, const uint8_t 
  * round for its batch at threshold t (16 bytes per piece, 12 per candidate chunk), and, when fetched, 24 bytes
  * per entry of the largest group plus the sort's tile status.  Phases: approx_check; per round best_compact,
  * approx_pieces, approx_scan, approx_count, best_update; per emitted group best_compact, approx_pieces,
- * approx_scan, approx_count, approx_emit, approx_sort, best_scatter. */
+ * approx_scan, approx_count, approx_emit, approx_sort, best_scatter.
+ *
+ * ---- IUPAC nucleotide codes in the queries (DESIGN.md 6b f-17) ----
+ * With B200SA_APPROX_IUPAC (bit 24) in k, each query byte is an IUPAC code that stands for a class of text bytes:
+ * A C G T for themselves, U for T, R = AG, Y = CT, S = CG, W = AT, K = GT, M = AC, B = CGT, D = AGT, H = ACT,
+ * V = ACG, N = ACGT, in either case.  Any other query byte ('-' and '.' included) returns B200SA_ERR_BAD_ARG,
+ * checked on the device in phase approx_check, with a detail that names the byte and its offset in d_queries.
+ * The flag combines with B200SA_APPROX_EDIT, with B200SA_APPROX_BEST | B200SA_APPROX_SLACK(s), or with both;
+ * the threshold is decoded as above (k & 0xFFFF, or k & 0xFF with B200SA_APPROX_BEST).  Without it nothing changes.
+ * Text side: only the uppercase bytes A C G T are in any class, and nothing is folded.  Lowercase (soft-masked)
+ * bases, N, U and every other text byte match no query symbol and count as a mismatch; uppercase a soft-masked
+ * text before building the table.  (The filter looks up exact pieces in the table, so a case-insensitive or
+ * U = T text would need 2^len variants of each piece.)
+ * Definitions: those above with "T[p + x] != q[x]" read as "T[p + x] is not in the class of q[x]": mis(p) counts
+ * such positions, and in dist(p) a substitution costs 0 iff the text byte is in the class.  best(q), t(q), the
+ * window and document-end rules, offsets, ordering, cap, the nq * (threshold + 1) TOO_LARGE check, m = 0 and
+ * n = 0 are as above.  So a query of uppercase A C G T alone gives exactly the call without the flag (positions
+ * and distances, either metric, with or without best); lowercase letters act as their uppercase, U as T; and at
+ * threshold 0 the Hamming list is the sorted union of b200sa_positions_dev over the query's concrete expansions.
+ * Method: A C G T U are the concrete symbols (classes of one base); the maximal runs of concrete symbols are the
+ * query's stretches, of lengths L_i, and P = threshold + 1.  t is the largest length with sum floor(L_i / t) >= P;
+ * stretch i, left to right, gives c_i = min(floor(L_i / t), pieces still needed) pieces, piece j of the stretch
+ * being [j*L_i/c_i, (j+1)*L_i/c_i) from its start.  The pieces are disjoint, concrete and at least t long, so
+ * each is one exact range of the table; for a concrete query they are the pieces above.  If sum L_i < P (m <=
+ * threshold included) the query keeps the whole-table slot: every rank is a candidate, verified in full.  The
+ * reporter rules above carry over with each piece's offset and length from a per-slot table: the partition lemma
+ * needs only threshold + 1 disjoint pieces, not a cover, so each occurrence is still reported once.  Device
+ * workspace (computed, not measured): what the call takes without the flag, plus 1 byte per query byte for the
+ * canonical copy and 8 bytes per slot for the piece table. */
 #define B200SA_APPROX_MAX_K 31
 #define B200SA_APPROX_EDIT 0x10000u
 #define B200SA_APPROX_BEST 0x100000u                      /* bit 20 */
 #define B200SA_APPROX_SLACK(s) ((uint32_t)(s) << 8)       /* 0 <= s <= 31, only with B200SA_APPROX_BEST */
+#define B200SA_APPROX_IUPAC 0x1000000u                    /* bit 24 */
 int b200sa_approx_positions_dev(b200sa_ctx *ctx, const uint8_t *d_text, uint64_t n, const uint32_t *d_sa,
                                 const uint8_t *d_queries, const uint64_t *d_q_off, uint32_t nq, uint32_t k,
                                 uint64_t *d_offsets, uint32_t *d_pos, uint32_t *d_mismatches, uint64_t cap,

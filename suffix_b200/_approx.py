@@ -1,5 +1,6 @@
-"""Approximate positions (occurrences with at most k mismatches, or within k edits with metric="edit", and with
-best=s only each query's best hits) over a device-resident table: the part SuffixTable and DocumentSuffixTable share.  A table supplies `_device` and
+"""Approximate positions (occurrences with at most k mismatches, or within k edits with metric="edit", with
+best=s only each query's best hits, and with iupac=True queries in IUPAC nucleotide codes) over a device-resident
+table: the part SuffixTable and DocumentSuffixTable share.  A table supplies `_device` and
 `_bwt_arrays()` -> (d_text, d_table, d_doc_starts or None, ndocs), its text and table on the device; the LCP
 array is not needed."""
 import numpy as np
@@ -10,6 +11,7 @@ from .table import _as_bytes, _lock
 MAX_K = 31                # B200SA_APPROX_MAX_K
 EDIT = 0x10000            # B200SA_APPROX_EDIT
 BEST = 0x100000           # B200SA_APPROX_BEST
+IUPAC = 0x1000000         # B200SA_APPROX_IUPAC
 METRICS = {"hamming": 0, "edit": EDIT}
 
 
@@ -22,17 +24,26 @@ def _flags(best):
     return (int(best) << 8) | BEST
 
 
-def _call(table, queries, k, fetch, metric="hamming", best=None):
+def _iupac(iupac):
+    """The k bit of iupac=: B200SA_APPROX_IUPAC for True, 0 for False."""
+    if not isinstance(iupac, (bool, np.bool_)):
+        raise ValueError("iupac must be True or False, got %r" % (iupac,))
+    return IUPAC if iupac else 0
+
+
+def _call(table, queries, k, fetch, metric="hamming", best=None, iupac=False):
     """(offsets u64[nq + 1], positions u32[], distances u32[]); positions and distances are None without
     fetch (the cap = 0 call).  metric "hamming" counts mismatches, "edit" the Levenshtein distance; best=s keeps
-    each query's occurrences within s of its least distance (include/b200sa.h, B200SA_APPROX_BEST)."""
+    each query's occurrences within s of its least distance (include/b200sa.h, B200SA_APPROX_BEST); iupac=True reads
+    the queries as IUPAC nucleotide codes, matched against the uppercase text bytes A C G T only
+    (B200SA_APPROX_IUPAC)."""
     import torch
     k = int(k)
     if not 0 <= k <= MAX_K:
         raise ValueError("k must be in 0 .. %d, got %d" % (MAX_K, k))
     if metric not in METRICS:
         raise ValueError("metric must be 'hamming' or 'edit', got %r" % (metric,))
-    kf = k | METRICS[metric] | _flags(best)
+    kf = k | METRICS[metric] | _flags(best) | _iupac(iupac)
     qs = [_as_bytes(q) for q in queries]
     nq, n = len(qs), len(table)
     d_t, d_r, d_s, ndocs = table._bwt_arrays()
@@ -68,15 +79,15 @@ def _call(table, queries, k, fetch, metric="hamming", best=None):
     return offsets, pos[:total].cpu().numpy().view(np.uint32), mis[:total].cpu().numpy().view(np.uint32)
 
 
-def positions_batch(table, queries, k, metric="hamming", best=None):
-    return _call(table, queries, k, True, metric, best)
+def positions_batch(table, queries, k, metric="hamming", best=None, iupac=False):
+    return _call(table, queries, k, True, metric, best, iupac)
 
 
-def positions(table, query, k, metric="hamming", best=None):
-    _, pos, mis = _call(table, [query], k, True, metric, best)
+def positions(table, query, k, metric="hamming", best=None, iupac=False):
+    _, pos, mis = _call(table, [query], k, True, metric, best, iupac)
     return pos, mis
 
 
-def counts(table, queries, k, metric="hamming", best=None):
-    off, _, _ = _call(table, queries, k, False, metric, best)
+def counts(table, queries, k, metric="hamming", best=None, iupac=False):
+    off, _, _ = _call(table, queries, k, False, metric, best, iupac)
     return np.diff(off.astype(np.int64)).astype(np.uint64)

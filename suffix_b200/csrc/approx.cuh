@@ -99,11 +99,26 @@ __device__ __forceinline__ bool approx_verify(const ApproxArgs &A, uint32_t s, c
     return true;
 }
 
+// f-14's pieces: piece j = [j*m/P, (j+1)*m/P), a whole-table slot for m <= k, and approx_verify.  The walks
+// of k_approx and k_approx_edit take the pieces as a policy, so that B200SA_APPROX_IUPAC (iupac.cuh) reuses them.
+struct CutPieces {
+    __device__ __forceinline__ bool whole(const ApproxArgs &A, uint32_t, uint32_t m) const { return m <= A.k; }
+    __device__ __forceinline__ uint32_t off(const ApproxArgs &A, uint32_t, uint32_t m, uint32_t j) const {
+        return approx_cut(m, A.P, j);
+    }
+    __device__ __forceinline__ bool verify(const ApproxArgs &A, uint32_t s, const uint8_t *__restrict__ qq, uint32_t m,
+                                           uint32_t, uint32_t j, uint32_t oj, bool whole, uint32_t *p_out,
+                                           uint32_t *mis_out) const {
+        return approx_verify(A, s, qq, m, j, oj, whole, p_out, mis_out);
+    }
+};
+
 // EMIT = false: cnt[item] = the occurrences the item reports.  EMIT = true: the same walk writes them from
 // item_off[item] on, in rank order: key = (q << pbits) | p, val = mis(p).
-template <bool EMIT>
-__global__ void __launch_bounds__(BLK) k_approx(ApproxArgs A, uint32_t *cnt, const unsigned long long *item_off,
-                                                int pbits, unsigned long long *key, uint32_t *val) {
+template <bool EMIT, class Pieces>
+__device__ __forceinline__ void approx_walk(ApproxArgs A, Pieces pc, uint32_t *cnt,
+                                            const unsigned long long *item_off, int pbits, unsigned long long *key,
+                                            uint32_t *val) {
     const uint64_t item = ((uint64_t)blockIdx.x * BLK + threadIdx.x) >> 5;
     if (item >= A.items) return;                                  // whole warps
     const uint32_t l = lane_id();
@@ -119,14 +134,14 @@ __global__ void __launch_bounds__(BLK) k_approx(ApproxArgs A, uint32_t *cnt, con
     const uint64_t hi = blk * DLIST_CHUNK + DLIST_CHUNK < e0 ? blk * DLIST_CHUNK + DLIST_CHUNK : e0;
     const uint64_t qo = A.qoff[q];
     const uint32_t m = (uint32_t)(A.qoff[q + 1] - qo);
-    const bool whole = m <= A.k;
-    const uint32_t oj = whole ? 0u : approx_cut(m, A.P, j);
+    const bool whole = pc.whole(A, a, m);
+    const uint32_t oj = whole ? 0u : pc.off(A, a, m, j);
     const uint64_t base = EMIT ? item_off[item] : 0;
     uint32_t count = 0;
     for (uint64_t i0 = lo; i0 < hi; i0 += 32) {                   // the same trip count on every lane
         const uint64_t i = i0 + l;
         uint32_t p = 0, mis = 0;
-        const bool hit = i < hi && approx_verify(A, A.sa[i], A.qs + qo, m, j, oj, whole, &p, &mis);
+        const bool hit = i < hi && pc.verify(A, A.sa[i], A.qs + qo, m, q, j, oj, whole, &p, &mis);
         const uint32_t m0 = __ballot_sync(FULL, hit);
         if (EMIT && hit) {
             const uint64_t slot = base + count + __popc(m0 & lanemask_lt());
@@ -136,6 +151,12 @@ __global__ void __launch_bounds__(BLK) k_approx(ApproxArgs A, uint32_t *cnt, con
         count += __popc(m0);
     }
     if (!EMIT && l == 0) cnt[item] = count;
+}
+
+template <bool EMIT>
+__global__ void __launch_bounds__(BLK) k_approx(ApproxArgs A, uint32_t *cnt, const unsigned long long *item_off,
+                                                int pbits, unsigned long long *key, uint32_t *val) {
+    approx_walk<EMIT>(A, CutPieces{}, cnt, item_off, pbits, key, val);
 }
 
 // offsets[q] = the output offset of query q's first item (its slots are q*P .. q*P + P - 1)

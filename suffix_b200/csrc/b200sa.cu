@@ -38,6 +38,7 @@
 #include "approx.cuh"
 #include "edit.cuh"
 #include "best.cuh"
+#include "iupac.cuh"
 #include "nccl_dyn.h"
 
 using namespace b200sa;
@@ -84,6 +85,7 @@ struct b200sa_ctx {
     DevBuf packed, scan_state, cls_state, lmsdesc, steplog, hist_copies;
     DevBuf tree_out;                           // output staging of b200sa_suffix_tree
     DevBuf docs_starts, docs_out;              // doc_starts and output staging of b200sa_docs_build
+    DevBuf icode;                              // approx positions with B200SA_APPROX_IUPAC: the canonical queries
     uint32_t cls_calls = 0;
     // multi-GPU (SURVEY 8e): communicator owned or attached, NCCL resolved at run time
     ncclComm_t comm = nullptr;
@@ -1288,7 +1290,7 @@ void b200sa_ctx_destroy(b200sa_ctx *c) {
     DevBuf *bufs[] = {&c->text, &c->sa, &c->lcp, &c->pred, &c->stype, &c->lmsb, &c->lmsrank, &c->lmspos, &c->lmslist,
                       &c->lmspred, &c->sorted, &c->flag, &c->reduced, &c->sa_r, &c->blkstate, &c->carry, &c->tables,
                       &c->small, &c->scan_partial, &c->radix_cnt, &c->blkcnt, &c->k32b, &c->k64a, &c->k64b, &c->v0,
-                      &c->v1, &c->p0, &c->p1, &c->g0, &c->g1, &c->rank, &c->isa, &c->qbuf, &c->os_hist, &c->os_status, &c->packed, &c->phik, &c->phiv, &c->runscr, &c->plcp_samp, &c->scan_state, &c->cls_state, &c->lmsdesc, &c->steplog, &c->hist_copies, &c->tree_out, &c->docs_starts, &c->docs_out, &c->sh_a, &c->sh_b, &c->sh_c, &c->sh_d, &c->sh_e, &c->sh_f, &c->sh_small};
+                      &c->v1, &c->p0, &c->p1, &c->g0, &c->g1, &c->rank, &c->isa, &c->qbuf, &c->os_hist, &c->os_status, &c->packed, &c->phik, &c->phiv, &c->runscr, &c->plcp_samp, &c->scan_state, &c->cls_state, &c->lmsdesc, &c->steplog, &c->hist_copies, &c->tree_out, &c->docs_starts, &c->docs_out, &c->icode, &c->sh_a, &c->sh_b, &c->sh_c, &c->sh_d, &c->sh_e, &c->sh_f, &c->sh_small};
     for (DevBuf *b : bufs) if (b->p) cudaFree(b->p);
     for (cudaEvent_t e : c->event_pool) cudaEventDestroy(e);
     if (c->h_pin) cudaFreeHost(c->h_pin);
@@ -2884,7 +2886,7 @@ int b200sa_unbwt_dev(b200sa_ctx *c, uint64_t n, uint32_t ndocs, const uint8_t *d
     return leave(c, unbwt_core(c, (uint32_t)n, ndocs, d_bwt, d_term_rows, d_text_out, d_doc_starts_out));
 }
 
-// ------------------------------------------------------------ approximate positions (DESIGN 6b f-14, f-15, f-16)
+// ------------------------------------------------------------ approximate positions (DESIGN 6b f-14 .. f-17)
 // The checks of a call (nq >= 1, k its threshold): q_off on the device with q_off[nq] read back as *q_bytes,
 // doc_starts (d_starts non-null for documents), and the sizes.  Phase approx_check.
 static int approx_prep(b200sa_ctx *c, uint32_t n, const uint32_t *d_starts, uint32_t ndocs, const uint8_t *d_queries,
@@ -2911,23 +2913,54 @@ static int approx_nothing(b200sa_ctx *c, uint64_t *d_offsets, uint32_t nq) {
     return B200SA_OK;
 }
 
+// B200SA_APPROX_IUPAC: the canonical copy of the q_bytes query bytes into c->icode (*out), or BAD_ARG naming the
+// first byte that is not an IUPAC letter.  Phase approx_check.
+static int iupac_canon(b200sa_ctx *c, const uint8_t *d_queries, uint64_t q_bytes, const uint8_t **out) {
+    typedef unsigned long long u64;
+    uint32_t *words = ptr<uint32_t>(c->small);           // [16, 18) the least (offset << 8) | byte rejected
+    TRY(ensure(c, c->icode, (size_t)q_bytes));
+    CU_TRY(c, cudaMemsetAsync(words + 16, 0xFF, 8, c->stream));
+    if (q_bytes > 0)
+        LAUNCH(c, k_iupac_code, cdiv(q_bytes, BLK), d_queries, q_bytes, ptr<uint8_t>(c->icode),
+               reinterpret_cast<u64 *>(words + 16));
+    CU_TRY(c, cudaGetLastError());
+    TRY(read_words(c, words + 16, 2));
+    const uint64_t bad = pin_u64(c, 0);
+    if (bad != ~0ull) {
+        char m[200];
+        snprintf(m, sizeof m,
+                 "approx positions: with B200SA_APPROX_IUPAC, query byte 0x%02x at offset %llu of the queries is not "
+                 "an IUPAC nucleotide code",
+                 (unsigned)(bad & 0xFF), (unsigned long long)(bad >> 8));
+        return fail(c, B200SA_ERR_BAD_ARG, m);
+    }
+    *out = ptr<uint8_t>(c->icode);
+    return B200SA_OK;
+}
+
 // One search of nq >= 1 queries at threshold k on n >= 1 bytes: d_offsets (nq + 1) and *total, read back.  When
 // 0 < total <= cap it also emits and sorts: *ko / *vo then hold the keys (q << *pbits) | p in (q, p) order and
 // their distances.  Phases: approx_pieces, approx_scan, approx_count, and approx_emit, approx_sort when it
-// emits.  B200SA_APPROX_EDIT picks k_approx_edit over k_approx; everything else is shared.
+// emits.  B200SA_APPROX_EDIT picks k_approx_edit over k_approx; iupac (d_queries then the canonical copy) picks
+// the pieces of k_iupac_pieces and the kernels' IUPAC instantiations; everything else is shared.
 template <class EndF>
 static int approx_search(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const uint32_t *d_sa,
                          const uint32_t *d_starts, uint32_t ndocs, const uint8_t *d_queries, const uint64_t *d_q_off,
-                         uint32_t nq, uint32_t k, bool edit, uint64_t *d_offsets, uint64_t cap, uint64_t *total,
-                         EndF end, uint64_t **ko, uint32_t **vo, int *pbits_out) {
+                         uint32_t nq, uint32_t k, bool edit, bool iupac, uint64_t *d_offsets, uint64_t cap,
+                         uint64_t *total, EndF end, uint64_t **ko, uint32_t **vo, int *pbits_out) {
     typedef unsigned long long u64;
     uint32_t *words = ptr<uint32_t>(c->small);           // [0] check bits, [2, 4) items, [4, 6) total
     const uint32_t P = k + 1;
     const uint64_t nslots = (uint64_t)nq * P;
     TRY(mark(c, "approx_pieces"));
-    TRY(ensure(c, c->p1, (size_t)nslots * 8));
+    TRY(ensure(c, c->p1, (size_t)nslots * (iupac ? 16 : 8)));   // with iupac, the piece table follows pe
     uint32_t *ps = ptr<uint32_t>(c->p1), *pe = ps + nslots;
-    LAUNCH(c, (k_approx_pieces<EndF>), cdiv(nslots, BLK), d_text, n, d_sa, d_queries, d_q_off, nq, P, ps, pe, end);
+    if (iupac) {
+        LAUNCH(c, (k_iupac_pieces<EndF>), cdiv(nq, BLK), d_text, n, d_sa, d_queries, d_q_off, nq, P, ps, pe,
+               reinterpret_cast<uint2 *>(pe + nslots), end);
+    } else {
+        LAUNCH(c, (k_approx_pieces<EndF>), cdiv(nslots, BLK), d_text, n, d_sa, d_queries, d_q_off, nq, P, ps, pe, end);
+    }
     TRY(mark(c, "approx_scan"));
     CU_TRY(c, cudaMemsetAsync(words, 0, 24, c->stream));
     TRY(ensure(c, c->k64a, ((size_t)nslots + 1) * 8));
@@ -2947,7 +2980,13 @@ static int approx_search(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const
     const ApproxArgs A{d_text, d_sa, d_starts, ndocs, n, d_queries, d_q_off, (uint32_t)nslots, P, k, ps, pe,
                        item_start, items};
     const int pbits = bit_length(n - 1);
-    if (items && edit)
+    if (items && iupac && edit)
+        LAUNCH(c, k_approx_edit_iupac<false>, cdiv(items, NWARP), A, cnt, (const u64 *)nullptr, pbits, (u64 *)nullptr,
+               (uint32_t *)nullptr);
+    else if (items && iupac)
+        LAUNCH(c, k_approx_iupac<false>, cdiv(items, NWARP), A, cnt, (const u64 *)nullptr, pbits, (u64 *)nullptr,
+               (uint32_t *)nullptr);
+    else if (items && edit)
         LAUNCH(c, k_approx_edit<false>, cdiv(items, NWARP), A, cnt, (const u64 *)nullptr, pbits, (u64 *)nullptr,
                (uint32_t *)nullptr);
     else if (items)
@@ -2965,7 +3004,13 @@ static int approx_search(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const
         TRY(ensure(c, c->g1, (size_t)*total * 8));
         TRY(ensure(c, c->v0, (size_t)*total * 4));
         TRY(ensure(c, c->v1, (size_t)*total * 4));
-        if (edit)
+        if (iupac && edit)
+            LAUNCH(c, k_approx_edit_iupac<true>, cdiv(items, NWARP), A, cnt, (const u64 *)item_off, pbits,
+                   ptr<u64>(c->g0), ptr<uint32_t>(c->v0));
+        else if (iupac)
+            LAUNCH(c, k_approx_iupac<true>, cdiv(items, NWARP), A, cnt, (const u64 *)item_off, pbits, ptr<u64>(c->g0),
+                   ptr<uint32_t>(c->v0));
+        else if (edit)
             LAUNCH(c, k_approx_edit<true>, cdiv(items, NWARP), A, cnt, (const u64 *)item_off, pbits, ptr<u64>(c->g0),
                    ptr<uint32_t>(c->v0));
         else
@@ -2988,12 +3033,14 @@ static int approx_core(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const u
     const uint32_t k = kf & 0xFFFFu;
     uint64_t q_bytes;
     TRY(approx_prep(c, n, d_starts, ndocs, d_queries, d_q_off, nq, k, &q_bytes));
+    const bool iupac = (kf & B200SA_APPROX_IUPAC) != 0;
+    if (iupac) TRY(iupac_canon(c, d_queries, q_bytes, &d_queries));
     if (n == 0) return approx_nothing(c, d_offsets, nq);
     uint64_t *ko = nullptr;
     uint32_t *vo = nullptr;
     int pbits = 0;
     TRY(approx_search(c, d_text, n, d_sa, d_starts, ndocs, d_queries, d_q_off, nq, k, (kf & B200SA_APPROX_EDIT) != 0,
-                      d_offsets, cap, total, end, &ko, &vo, &pbits));
+                      iupac, d_offsets, cap, total, end, &ko, &vo, &pbits));
     if (*total > 0 && *total <= cap)
         LAUNCH(c, k_approx_gather, cdiv(*total, BLK), (const u64 *)ko, (const uint32_t *)vo, *total,
                (u64)((1ull << pbits) - 1), d_pos, d_mis);
@@ -3022,7 +3069,8 @@ static int best_batch(b200sa_ctx *c, const uint8_t *d_queries, const uint64_t *d
     return B200SA_OK;
 }
 
-// nq >= 1, k = threshold | B200SA_APPROX_SLACK(s) | B200SA_APPROX_BEST, optionally | B200SA_APPROX_EDIT.
+// nq >= 1, k = threshold | B200SA_APPROX_SLACK(s) | B200SA_APPROX_BEST, optionally | B200SA_APPROX_EDIT and
+// | B200SA_APPROX_IUPAC (the batches are then gathered from the canonical copy).
 // Rounds t = 0 .. threshold over the live queries (best.cuh), then one emission per distinct final threshold.
 // Phases: approx_check; per round best_compact, the search's phases, best_update; per emitted group
 // best_compact, the search's phases, best_scatter.
@@ -3033,10 +3081,11 @@ static int approx_best_core(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, co
                             uint32_t *d_mis, uint64_t cap, uint64_t *total, EndF end) {
     typedef unsigned long long u64;
     const uint32_t k = kf & 0xFFu, s = (kf >> 8) & 0xFFu;
-    const bool edit = (kf & B200SA_APPROX_EDIT) != 0;
+    const bool edit = (kf & B200SA_APPROX_EDIT) != 0, iupac = (kf & B200SA_APPROX_IUPAC) != 0;
     uint64_t q_bytes;
     c->stats.doubling_rounds = 0;
     TRY(approx_prep(c, n, d_starts, ndocs, d_queries, d_q_off, nq, k, &q_bytes));
+    if (iupac) TRY(iupac_canon(c, d_queries, q_bytes, &d_queries));
     if (n == 0) return approx_nothing(c, d_offsets, nq);
     TRY(ensure(c, c->k32b, (size_t)nq * 9));             // cnt, map (u32), best (u8) per query
     TRY(ensure(c, c->rank, ((size_t)nq + 1) * 16));      // the batch's q_off, the search's offsets
@@ -3059,7 +3108,7 @@ static int approx_best_core(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, co
                        &boff));
         if (nb == 0) break;
         rounds++;
-        TRY(approx_search(c, d_text, n, d_sa, d_starts, ndocs, bq, boff, nb, t, edit, soff, 0, &rtotal, end, &ko, &vo,
+        TRY(approx_search(c, d_text, n, d_sa, d_starts, ndocs, bq, boff, nb, t, edit, iupac, soff, 0, &rtotal, end, &ko, &vo,
                           &pbits));
         TRY(mark(c, "best_update"));
         LAUNCH(c, k_best_update, cdiv(nb, BLK), (const uint32_t *)map, (const u64 *)soff, nb, t, s, k, best, cnt,
@@ -3077,7 +3126,7 @@ static int approx_best_core(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, co
             TRY(mark(c, "best_compact"));
             TRY(best_batch(c, d_queries, d_q_off, nq, BestPick{d_q_off, best, nq, t, s, k, true}, map, coff, &nb, &bq,
                            &boff));
-            TRY(approx_search(c, d_text, n, d_sa, d_starts, ndocs, bq, boff, nb, t, edit, soff, ~0ull, &rtotal, end,
+            TRY(approx_search(c, d_text, n, d_sa, d_starts, ndocs, bq, boff, nb, t, edit, iupac, soff, ~0ull, &rtotal, end,
                               &ko, &vo, &pbits));
             TRY(mark(c, "best_scatter"));
             LAUNCH(c, k_best_scatter, cdiv(rtotal, BLK), (const u64 *)ko, (const uint32_t *)vo, rtotal, pbits,
@@ -3095,15 +3144,18 @@ static int approx_args(b200sa_ctx *c, uint64_t n, const void *text, const void *
     if (!c) return B200SA_ERR_BAD_ARG;
     if (!total || !offsets || (nq > 0 && !q_off) || (cap > 0 && !pos) || (n > 0 && (!text || !sa))) return null_ptr(c);
     if (k & B200SA_APPROX_BEST) {
-        if (k & ~(0xFFFFu | B200SA_APPROX_EDIT | B200SA_APPROX_BEST) || (k & 0xFFu) > B200SA_APPROX_MAX_K ||
+        if (k & ~(0xFFFFu | B200SA_APPROX_EDIT | B200SA_APPROX_BEST | B200SA_APPROX_IUPAC) ||
+            (k & 0xFFu) > B200SA_APPROX_MAX_K ||
             ((k >> 8) & 0xFFu) > B200SA_APPROX_MAX_K)
             return fail(c, B200SA_ERR_BAD_ARG,
                         "approx positions: with B200SA_APPROX_BEST, k must be a threshold up to B200SA_APPROX_MAX_K | "
-                        "B200SA_APPROX_SLACK(s) with s up to B200SA_APPROX_MAX_K, optionally | B200SA_APPROX_EDIT");
+                        "B200SA_APPROX_SLACK(s) with s up to B200SA_APPROX_MAX_K, optionally | B200SA_APPROX_EDIT "
+                        "and | B200SA_APPROX_IUPAC");
     } else {
-        if (k & ~(0xFFFFu | B200SA_APPROX_EDIT))
+        if (k & ~(0xFFFFu | B200SA_APPROX_EDIT | B200SA_APPROX_IUPAC))
             return fail(c, B200SA_ERR_BAD_ARG,
-                        "approx positions: k must be a threshold up to B200SA_APPROX_MAX_K, optionally | B200SA_APPROX_EDIT");
+                        "approx positions: k must be a threshold up to B200SA_APPROX_MAX_K, optionally | B200SA_APPROX_EDIT "
+                        "and | B200SA_APPROX_IUPAC");
         if ((k & 0xFFFFu) > B200SA_APPROX_MAX_K)
             return fail(c, B200SA_ERR_BAD_ARG, "approx positions: k above B200SA_APPROX_MAX_K");
     }

@@ -52,12 +52,24 @@ __device__ __noinline__ bool edit_reports(const ApproxArgs &A, int64_t p, uint32
     return true;
 }
 
+// f-14's pieces and byte equality for the edit walk; whole: dist(s) <= m <= k.
+struct EditCut : CutPieces {
+    static constexpr bool CLASSES = false;          // byte equality
+    __device__ __forceinline__ uint64_t whole_hits(const uint8_t *, int32_t k) const { return 1ull << k; }
+    __device__ __forceinline__ bool reports(const ApproxArgs &A, int64_t p, uint32_t s, const uint8_t *__restrict__ qq,
+                                            uint32_t m, uint32_t, uint32_t j, uint32_t oj, uint32_t ds,
+                                            uint32_t de) const {
+        return edit_reports(A, p, s, qq, m, j, oj, ds, de);
+    }
+};
+
 // The starts this candidate reports, bit b for p = c - k + b, with *c_out = c and v[k + b] = dist(p).  v holds
 // one band row: v[d] = D(x, t) at t = c - 2k + x + d, D(x, t) = min over e of ED(q[x, m), T[t, e)), e <= de,
-// saturated at k + 1.  whole: m <= k, only p = s (o_j = 0).
-__device__ __forceinline__ uint64_t edit_verify(const ApproxArgs &A, uint32_t s, const uint8_t *__restrict__ qq,
-                                                uint32_t m, uint32_t j, uint32_t oj, bool whole, uint8_t *v,
-                                                int64_t *c_out) {
+// saturated at k + 1.  whole: the whole-table slot, only p = s (o_j = 0).  Pieces: EditCut or IupacPieces.
+template <class Pieces>
+__device__ __forceinline__ uint64_t edit_verify(const ApproxArgs &A, const Pieces &pc, uint32_t s,
+                                                const uint8_t *__restrict__ qq, uint32_t m, uint32_t q, uint32_t j,
+                                                uint32_t oj, bool whole, uint8_t *v, int64_t *c_out) {
     const int32_t k = (int32_t)A.k, W = 4 * k + 1;
     const uint32_t INF = (uint32_t)k + 1;
     uint32_t ds = 0, de = A.n;
@@ -79,10 +91,14 @@ __device__ __forceinline__ uint64_t edit_verify(const ApproxArgs &A, uint32_t s,
             const uint32_t up = d > 0 ? v[d - 1] : INF;    // D(x + 1, t)
             const int64_t t = base + x + d;
             uint32_t y = INF;
-            if (t >= (int64_t)ds && t < (int64_t)de)
-                y = min(min(right, up) + 1, old + (__ldg(A.text + t) != qc));
-            else if (t == (int64_t)de)
+            if (t >= (int64_t)ds && t < (int64_t)de) {
+                if constexpr (Pieces::CLASSES)                 // the byte test written inline, as before
+                    y = min(min(right, up) + 1, old + pc.miss(__ldg(A.text + t), qc));
+                else
+                    y = min(min(right, up) + 1, old + (__ldg(A.text + t) != qc));
+            } else if (t == (int64_t)de) {
                 y = up + 1;                                // no text left: delete q[x]
+            }
             y = min(y, INF);
             v[d] = (uint8_t)y;
             right = y;
@@ -91,21 +107,22 @@ __device__ __forceinline__ uint64_t edit_verify(const ApproxArgs &A, uint32_t s,
         }
         if (low > (uint32_t)k) return 0;                   // every path to row 0 passes this row
     }
-    if (whole) return 1ull << k;                           // dist(s) <= m <= k
+    if (whole) return pc.whole_hits(v, k);
     const int64_t lo = max((int64_t)ds, c - k), hi = min((int64_t)de - 1, c + k);
     uint64_t hits = 0;
     for (int64_t p = lo; p <= hi; p++) {
         const uint32_t b = (uint32_t)(p - (c - k));
-        if (v[k + b] <= (uint32_t)k && edit_reports(A, p, s, qq, m, j, oj, ds, de)) hits |= 1ull << b;
+        if (v[k + b] <= (uint32_t)k && pc.reports(A, p, s, qq, m, q, j, oj, ds, de)) hits |= 1ull << b;
     }
     return hits;
 }
 
 // EMIT = false: cnt[item] = the occurrences the item reports.  EMIT = true: the same walk writes them from
-// item_off[item] on: key = (q << pbits) | p, val = dist(p).
-template <bool EMIT>
-__global__ void __launch_bounds__(BLK) k_approx_edit(ApproxArgs A, uint32_t *cnt, const unsigned long long *item_off,
-                                                     int pbits, unsigned long long *key, uint32_t *val) {
+// item_off[item] on: key = (q << pbits) | p, val = dist(p).  v: the kernel's band row of EDIT_BAND bytes.
+template <bool EMIT, class Pieces>
+__device__ __forceinline__ void edit_walk(ApproxArgs A, Pieces pc, uint8_t *v, uint32_t *cnt,
+                                          const unsigned long long *item_off, int pbits, unsigned long long *key,
+                                          uint32_t *val) {
     const uint64_t item = ((uint64_t)blockIdx.x * BLK + threadIdx.x) >> 5;
     if (item >= A.items) return;                                  // whole warps
     const uint32_t l = lane_id();
@@ -121,15 +138,14 @@ __global__ void __launch_bounds__(BLK) k_approx_edit(ApproxArgs A, uint32_t *cnt
     const uint64_t hi = blk * DLIST_CHUNK + DLIST_CHUNK < e0 ? blk * DLIST_CHUNK + DLIST_CHUNK : e0;
     const uint64_t qo = A.qoff[q];
     const uint32_t m = (uint32_t)(A.qoff[q + 1] - qo);
-    const bool whole = m <= A.k;
-    const uint32_t oj = whole ? 0u : approx_cut(m, A.P, j);
+    const bool whole = pc.whole(A, a, m);
+    const uint32_t oj = whole ? 0u : pc.off(A, a, m, j);
     const uint64_t base = EMIT ? item_off[item] : 0;
-    uint8_t v[EDIT_BAND];
     uint32_t count = 0;
     for (uint64_t i0 = lo; i0 < hi; i0 += 32) {                   // the same trip count on every lane
         const uint64_t i = i0 + l;
         int64_t c = 0;
-        const uint64_t hits = i < hi ? edit_verify(A, A.sa[i], A.qs + qo, m, j, oj, whole, v, &c) : 0;
+        const uint64_t hits = i < hi ? edit_verify(A, pc, A.sa[i], A.qs + qo, m, q, j, oj, whole, v, &c) : 0;
         const uint32_t h = __popcll(hits);
         uint32_t incl = h;                                        // inclusive warp scan of the lanes' hits
         for (int o = 1; o < 32; o <<= 1) {
@@ -150,6 +166,13 @@ __global__ void __launch_bounds__(BLK) k_approx_edit(ApproxArgs A, uint32_t *cnt
         count += __shfl_sync(FULL, incl, 31);
     }
     if (!EMIT && l == 0) cnt[item] = count;
+}
+
+template <bool EMIT>
+__global__ void __launch_bounds__(BLK) k_approx_edit(ApproxArgs A, uint32_t *cnt, const unsigned long long *item_off,
+                                                     int pbits, unsigned long long *key, uint32_t *val) {
+    uint8_t v[EDIT_BAND];
+    edit_walk<EMIT>(A, EditCut{}, v, cnt, item_off, pbits, key, val);
 }
 
 }  // namespace b200sa

@@ -279,8 +279,8 @@ class SuffixTable:
         from . import _bwt
         return _bwt.bwt_runs(self)
 
-    # ---- approximate positions (DESIGN 6b f-14, f-15, f-16)
-    def approximate_positions(self, query, k, *, metric="hamming", best=None):
+    # ---- approximate positions (DESIGN 6b f-14 .. f-17)
+    def approximate_positions(self, query, k, *, metric="hamming", best=None, iupac=False):
         """(positions u32[], mismatches u32[]): every p with p + m <= n where text[p:p + m] differs from
         the query (m bytes) in at most k bytes, 0 <= k <= 31, by ascending p, with that number of
         mismatches beside it (b200sa_approx_positions_dev).  b"" matches nothing; for k = 0 the positions
@@ -293,24 +293,29 @@ class SuffixTable:
         k, the occurrences at distance <= min(k, best(q) + s), exactly what the call returns at that threshold
         (B200SA_APPROX_BEST).  best=0 gives each query's best hits, and the distance column then holds best(q)
         on every one.  best=None (the default) lists every occurrence within k; any other value, True included,
-        raises ValueError."""
+        raises ValueError.
+        iupac=True reads each query byte as an IUPAC nucleotide code (A C G T, U = T, R Y S W K M B D H V N, in
+        either case), which matches the uppercase text bytes A C G T of its class (B200SA_APPROX_IUPAC); any
+        other query byte raises B200SA_ERR_BAD_ARG.  Lowercase (soft-masked) text bases, N, U and every other
+        text byte match no code and count as a mismatch: uppercase a soft-masked text before building the
+        table.  Combines with metric= and best=; a non-bool value raises ValueError."""
         from . import _approx
-        return _approx.positions(self, query, k, metric, best)
+        return _approx.positions(self, query, k, metric, best, iupac)
 
-    def approximate_positions_batch(self, queries, k, *, metric="hamming", best=None):
+    def approximate_positions_batch(self, queries, k, *, metric="hamming", best=None, iupac=False):
         """(offsets u64[nq + 1], positions u32[], mismatches u32[]): query q's occurrences with at most k
         mismatches (or within k edits, metric="edit") are positions[offsets[q]:offsets[q + 1]], as
         approximate_positions returns them; best=0 gives each query's best hits, with best(q) in the
-        distance column (best= as in approximate_positions)."""
+        distance column (best= and iupac= as in approximate_positions)."""
         from . import _approx
-        return _approx.positions_batch(self, queries, k, metric, best)
+        return _approx.positions_batch(self, queries, k, metric, best, iupac)
 
-    def approximate_counts(self, queries, k, *, metric="hamming", best=None):
+    def approximate_counts(self, queries, k, *, metric="hamming", best=None, iupac=False):
         """u64[nq]: the number of occurrences with at most k mismatches (or within k edits, metric="edit") of
         every query, without fetching them; best=0 counts each query's best hits, those at distance best(q)
-        (best= as in approximate_positions)."""
+        (best= and iupac= as in approximate_positions)."""
         from . import _approx
-        return _approx.counts(self, queries, k, metric, best)
+        return _approx.counts(self, queries, k, metric, best, iupac)
 
     # ---- persistence (SURVEY 8f-2): the only "wire format" the reference API implies is
     # from_parts/into_parts (src/table.rs:111-127): text bytes + little-endian u32 table.

@@ -179,6 +179,15 @@ for k, tab in enumerate([single] + [DocumentSuffixTable(docs) for docs in doc_se
         for metric in ("hamming", "edit"):
             off, pos, dist = tab.approximate_positions_batch(ap_qs + [b"a" * 9, b"A" * 40], kk, metric=metric, best=sl)
             assert len(pos) == int(off[-1]) and (dist <= kk).all(), (k, kk, sl, metric)
+# IUPAC queries: the canonical copy, the stretch pieces (a whole-table query among them) and the piece table read
+# by both verifications, with and without best hits
+iu_qs = [q[:20] + b"NGG" for q in ap_qs if len(q) >= 20] + [b"N" * 21 + b"GG", b"RYACGTNNacgu", b"", b"n"]
+for k, tab in enumerate([single] + [DocumentSuffixTable(docs) for docs in doc_sets] +
+                        [SuffixTable(b"A" * 5000), DocumentSuffixTable([b"", b"AC", b"", b"G"])]):
+    for kk, sl in ((0, None), (3, None), (31, None), (3, 1)):
+        for metric in ("hamming", "edit"):
+            off, pos, dist = tab.approximate_positions_batch(iu_qs, kk, metric=metric, best=sl, iupac=True)
+            assert len(pos) == int(off[-1]) and (dist <= kk).all(), (k, kk, sl, metric)
 # refinement branches (tests/test_gpu_refine.py): a local-sort overflow in round 2 of the direct path, the direct
 # path's probe (2^20 tied after round 1, large groups), 64-bit round-0 keys of the reduced string
 import ctypes
