@@ -618,12 +618,41 @@ int b200sa_unbwt_dev(b200sa_ctx *ctx, uint64_t n, uint32_t ndocs, const uint8_t 
  * reporter rules above carry over with each piece's offset and length from a per-slot table: the partition lemma
  * needs only threshold + 1 disjoint pieces, not a cover, so each occurrence is still reported once.  Device
  * workspace (computed, not measured): what the call takes without the flag, plus 1 byte per query byte for the
- * canonical copy and 8 bytes per slot for the piece table. */
+ * canonical copy and 8 bytes per slot for the piece table.
+ *
+ * ---- both DNA strands (DESIGN.md 6b f-18) ----
+ * With B200SA_APPROX_BOTH_STRANDS (bit 28) in k, each query is also searched as its reverse complement, and q
+ * gets one list over both strands.  The flag combines with B200SA_APPROX_EDIT, with B200SA_APPROX_BEST |
+ * B200SA_APPROX_SLACK(s), with B200SA_APPROX_IUPAC, or with any mix of them; the threshold is decoded as above.
+ * Without it nothing changes.  comp swaps A <-> T, C <-> G, a <-> t and c <-> g, and every other byte (U
+ * included) is its own complement.  With B200SA_APPROX_IUPAC the class of comp(x) is the set of the complements
+ * of x's class: A <-> T, C <-> G, U -> A, R <-> Y, K <-> M, B <-> V, D <-> H, and S, W, N themselves, in either
+ * case; the byte check runs first, on d_queries, and its detail names the offset there.  rc(q)[x] =
+ * comp(q[m - 1 - x]).  A minus-strand occurrence of q at p is an occurrence of rc(q) at p under the call's metric,
+ * threshold and IUPAC setting, with d(p) the distance computed for rc(q): p is the leftmost text position of the
+ * window or alignment, and the window and document-end rules are as above.  q's list is the union of (p, +) over
+ * q's occurrences and (p, -) over rc(q)'s, ordered by (p, strand) with + first; d_mismatches[i] = d(p) |
+ * (minus ? B200SA_APPROX_MINUS : 0), and with d_mismatches = NULL one p can appear twice.  Offsets and total
+ * count both strands.  With B200SA_APPROX_BEST, best(q) is the least d over both strands, t(q) = min(threshold,
+ * best(q) + s), and q lists both strands' occurrences at t(q).  So the + entries are exactly the call without the
+ * flag on q (at t(q) with B200SA_APPROX_BEST), the - entries exactly that call on rc(q) with bit 31 set, a
+ * palindrome (rc(q) = q) lists each occurrence twice, m = 0 lists nothing and 0 < m <= threshold lists every
+ * window twice.  q_off[nq] above B200SA_MAX_N / 2, or 2 * nq * (threshold + 1) >= 2^32 - 1, returns
+ * B200SA_ERR_TOO_LARGE in phase approx_check, before any kernel reads the queries.
+ * Method: a doubled batch, entry 2q = q and entry 2q + 1 = rc(q) (built from the canonical copy with
+ * B200SA_APPROX_IUPAC), is searched as 2 nq queries; its sorted (entry, p) keys are merged per query by a binary
+ * search in the other strand's sublist.  With B200SA_APPROX_BEST a query and its reverse complement are live as
+ * a pair with one best.  Device workspace (computed, not measured): 2 bytes per query byte and 32 per query for
+ * the doubled batch and its offsets, plus what the search takes for 2 nq queries, and with B200SA_APPROX_BEST 8
+ * bytes per fetched entry for staging.  Phases: strand_queries after approx_check, strand_merge before end; the
+ * other phases keep their names and meaning. */
 #define B200SA_APPROX_MAX_K 31
 #define B200SA_APPROX_EDIT 0x10000u
 #define B200SA_APPROX_BEST 0x100000u                      /* bit 20 */
 #define B200SA_APPROX_SLACK(s) ((uint32_t)(s) << 8)       /* 0 <= s <= 31, only with B200SA_APPROX_BEST */
 #define B200SA_APPROX_IUPAC 0x1000000u                    /* bit 24 */
+#define B200SA_APPROX_BOTH_STRANDS 0x10000000u            /* bit 28, in k */
+#define B200SA_APPROX_MINUS 0x80000000u                   /* bit 31, in d_mismatches entries */
 int b200sa_approx_positions_dev(b200sa_ctx *ctx, const uint8_t *d_text, uint64_t n, const uint32_t *d_sa,
                                 const uint8_t *d_queries, const uint64_t *d_q_off, uint32_t nq, uint32_t k,
                                 uint64_t *d_offsets, uint32_t *d_pos, uint32_t *d_mismatches, uint64_t cap,

@@ -1,5 +1,6 @@
 """Approximate positions (occurrences with at most k mismatches, or within k edits with metric="edit", with
-best=s only each query's best hits, and with iupac=True queries in IUPAC nucleotide codes) over a device-resident
+best=s only each query's best hits, with iupac=True queries in IUPAC nucleotide codes, and with strands="both" the
+reverse complement's hits as well) over a device-resident
 table: the part SuffixTable and DocumentSuffixTable share.  A table supplies `_device` and
 `_bwt_arrays()` -> (d_text, d_table, d_doc_starts or None, ndocs), its text and table on the device; the LCP
 array is not needed."""
@@ -12,6 +13,8 @@ MAX_K = 31                # B200SA_APPROX_MAX_K
 EDIT = 0x10000            # B200SA_APPROX_EDIT
 BEST = 0x100000           # B200SA_APPROX_BEST
 IUPAC = 0x1000000         # B200SA_APPROX_IUPAC
+BOTH_STRANDS = 0x10000000  # B200SA_APPROX_BOTH_STRANDS
+MINUS = 0x80000000        # B200SA_APPROX_MINUS
 METRICS = {"hamming": 0, "edit": EDIT}
 
 
@@ -31,19 +34,27 @@ def _iupac(iupac):
     return IUPAC if iupac else 0
 
 
-def _call(table, queries, k, fetch, metric="hamming", best=None, iupac=False):
+def _strands(strands):
+    """The k bit of strands=: 0 for "forward", B200SA_APPROX_BOTH_STRANDS for "both"."""
+    if not isinstance(strands, str) or strands not in ("forward", "both"):
+        raise ValueError("strands must be 'forward' or 'both', got %r" % (strands,))
+    return BOTH_STRANDS if strands == "both" else 0
+
+
+def _call(table, queries, k, fetch, metric="hamming", best=None, iupac=False, strands="forward"):
     """(offsets u64[nq + 1], positions u32[], distances u32[]); positions and distances are None without
     fetch (the cap = 0 call).  metric "hamming" counts mismatches, "edit" the Levenshtein distance; best=s keeps
     each query's occurrences within s of its least distance (include/b200sa.h, B200SA_APPROX_BEST); iupac=True reads
     the queries as IUPAC nucleotide codes, matched against the uppercase text bytes A C G T only
-    (B200SA_APPROX_IUPAC)."""
+    (B200SA_APPROX_IUPAC); strands="both" adds the reverse complement's occurrences, the distances of those carrying
+    B200SA_APPROX_MINUS (B200SA_APPROX_BOTH_STRANDS)."""
     import torch
     k = int(k)
     if not 0 <= k <= MAX_K:
         raise ValueError("k must be in 0 .. %d, got %d" % (MAX_K, k))
     if metric not in METRICS:
         raise ValueError("metric must be 'hamming' or 'edit', got %r" % (metric,))
-    kf = k | METRICS[metric] | _flags(best) | _iupac(iupac)
+    kf = k | METRICS[metric] | _flags(best) | _iupac(iupac) | _strands(strands)
     qs = [_as_bytes(q) for q in queries]
     nq, n = len(qs), len(table)
     d_t, d_r, d_s, ndocs = table._bwt_arrays()
@@ -79,15 +90,25 @@ def _call(table, queries, k, fetch, metric="hamming", best=None, iupac=False):
     return offsets, pos[:total].cpu().numpy().view(np.uint32), mis[:total].cpu().numpy().view(np.uint32)
 
 
-def positions_batch(table, queries, k, metric="hamming", best=None, iupac=False):
-    return _call(table, queries, k, True, metric, best, iupac)
+def _split(dist):
+    """(distances with B200SA_APPROX_MINUS cleared, minus bool[])"""
+    return dist & np.uint32(MINUS - 1), (dist & np.uint32(MINUS)) != 0
 
 
-def positions(table, query, k, metric="hamming", best=None, iupac=False):
-    _, pos, mis = _call(table, [query], k, True, metric, best, iupac)
-    return pos, mis
+def positions_batch(table, queries, k, metric="hamming", best=None, iupac=False, strands="forward"):
+    off, pos, dist = _call(table, queries, k, True, metric, best, iupac, strands)
+    if strands == "forward":
+        return off, pos, dist
+    return (off, pos) + _split(dist)
 
 
-def counts(table, queries, k, metric="hamming", best=None, iupac=False):
-    off, _, _ = _call(table, queries, k, False, metric, best, iupac)
+def positions(table, query, k, metric="hamming", best=None, iupac=False, strands="forward"):
+    _, pos, dist = _call(table, [query], k, True, metric, best, iupac, strands)
+    if strands == "forward":
+        return pos, dist
+    return (pos,) + _split(dist)
+
+
+def counts(table, queries, k, metric="hamming", best=None, iupac=False, strands="forward"):
+    off, _, _ = _call(table, queries, k, False, metric, best, iupac, strands)
     return np.diff(off.astype(np.int64)).astype(np.uint64)

@@ -39,6 +39,7 @@
 #include "edit.cuh"
 #include "best.cuh"
 #include "iupac.cuh"
+#include "strand.cuh"
 #include "nccl_dyn.h"
 
 using namespace b200sa;
@@ -86,6 +87,7 @@ struct b200sa_ctx {
     DevBuf tree_out;                           // output staging of b200sa_suffix_tree
     DevBuf docs_starts, docs_out;              // doc_starts and output staging of b200sa_docs_build
     DevBuf icode;                              // approx positions with B200SA_APPROX_IUPAC: the canonical queries
+    DevBuf strand, sstage;                     // with B200SA_APPROX_BOTH_STRANDS: the doubled batch, the staged hits
     uint32_t cls_calls = 0;
     // multi-GPU (SURVEY 8e): communicator owned or attached, NCCL resolved at run time
     ncclComm_t comm = nullptr;
@@ -1290,7 +1292,7 @@ void b200sa_ctx_destroy(b200sa_ctx *c) {
     DevBuf *bufs[] = {&c->text, &c->sa, &c->lcp, &c->pred, &c->stype, &c->lmsb, &c->lmsrank, &c->lmspos, &c->lmslist,
                       &c->lmspred, &c->sorted, &c->flag, &c->reduced, &c->sa_r, &c->blkstate, &c->carry, &c->tables,
                       &c->small, &c->scan_partial, &c->radix_cnt, &c->blkcnt, &c->k32b, &c->k64a, &c->k64b, &c->v0,
-                      &c->v1, &c->p0, &c->p1, &c->g0, &c->g1, &c->rank, &c->isa, &c->qbuf, &c->os_hist, &c->os_status, &c->packed, &c->phik, &c->phiv, &c->runscr, &c->plcp_samp, &c->scan_state, &c->cls_state, &c->lmsdesc, &c->steplog, &c->hist_copies, &c->tree_out, &c->docs_starts, &c->docs_out, &c->icode, &c->sh_a, &c->sh_b, &c->sh_c, &c->sh_d, &c->sh_e, &c->sh_f, &c->sh_small};
+                      &c->v1, &c->p0, &c->p1, &c->g0, &c->g1, &c->rank, &c->isa, &c->qbuf, &c->os_hist, &c->os_status, &c->packed, &c->phik, &c->phiv, &c->runscr, &c->plcp_samp, &c->scan_state, &c->cls_state, &c->lmsdesc, &c->steplog, &c->hist_copies, &c->tree_out, &c->docs_starts, &c->docs_out, &c->icode, &c->strand, &c->sstage, &c->sh_a, &c->sh_b, &c->sh_c, &c->sh_d, &c->sh_e, &c->sh_f, &c->sh_small};
     for (DevBuf *b : bufs) if (b->p) cudaFree(b->p);
     for (cudaEvent_t e : c->event_pool) cudaEventDestroy(e);
     if (c->h_pin) cudaFreeHost(c->h_pin);
@@ -2886,7 +2888,7 @@ int b200sa_unbwt_dev(b200sa_ctx *c, uint64_t n, uint32_t ndocs, const uint8_t *d
     return leave(c, unbwt_core(c, (uint32_t)n, ndocs, d_bwt, d_term_rows, d_text_out, d_doc_starts_out));
 }
 
-// ------------------------------------------------------------ approximate positions (DESIGN 6b f-14 .. f-17)
+// ------------------------------------------------------------ approximate positions (DESIGN 6b f-14 .. f-18)
 // The checks of a call (nq >= 1, k its threshold): q_off on the device with q_off[nq] read back as *q_bytes,
 // doc_starts (d_starts non-null for documents), and the sizes.  Phase approx_check.
 static int approx_prep(b200sa_ctx *c, uint32_t n, const uint32_t *d_starts, uint32_t ndocs, const uint8_t *d_queries,
@@ -3023,7 +3025,51 @@ static int approx_search(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const
     return B200SA_OK;
 }
 
-// nq >= 1, k = threshold | flags as approx_args accepts it, without B200SA_APPROX_BEST.
+// B200SA_APPROX_BOTH_STRANDS: the doubled batch of 2 nq queries and 2 q_bytes bytes must fit BestPick's scan word
+// (bytes below 2^32) and the slot count.  Phase approx_check, before any kernel reads the queries.
+static int strand_check(b200sa_ctx *c, uint64_t q_bytes, uint32_t nq, uint32_t k) {
+    if (q_bytes > B200SA_MAX_N / 2)
+        return fail(c, B200SA_ERR_TOO_LARGE,
+                    "approx positions: with B200SA_APPROX_BOTH_STRANDS, queries longer than (2^32-4096) / 2 bytes");
+    if (2ull * nq * (k + 1) >= 0xFFFFFFFFull)
+        return fail(c, B200SA_ERR_TOO_LARGE,
+                    "approx positions: with B200SA_APPROX_BOTH_STRANDS, 2 * nq * (k + 1) of 2^32 - 1 or more slots");
+    return B200SA_OK;
+}
+
+// The doubled batch (strand.cuh) of the nq queries in c->strand: *eq / *eoff its 2 q_bytes bytes and 2 nq + 1
+// offsets, *doff room for the 2 nq + 1 offsets of its search.  canon: d_queries is the IUPAC canonical copy.
+// Phase strand_queries.
+static int strand_queries(b200sa_ctx *c, const uint8_t *d_queries, const uint64_t *d_q_off, uint32_t nq,
+                          uint64_t q_bytes, bool canon, const uint8_t **eq, const uint64_t **eoff, uint64_t **doff) {
+    TRY(mark(c, "strand_queries"));
+    const size_t ne1 = (size_t)2 * nq + 1;
+    TRY(ensure(c, c->strand, ne1 * 16 + (size_t)q_bytes * 2));
+    uint64_t *o2 = ptr<uint64_t>(c->strand);
+    uint8_t *q2 = reinterpret_cast<uint8_t *>(o2 + 2 * ne1);
+    LAUNCH(c, k_strand_queries, cdiv((uint64_t)nq * 32, BLK), d_queries, d_q_off, nq, canon, q2, o2);
+    *eq = q2;
+    *eoff = o2;
+    *doff = o2 + ne1;
+    return B200SA_OK;
+}
+
+// The caller's offsets (offsets[q] = doff[2q]) and, when emitted, the both-strand lists from the total hits of the
+// doubled batch at its offsets doff (src: the sorted keys or the staged positions, val their distances).
+// Phase strand_merge.
+template <class Src>
+static int strand_merge(b200sa_ctx *c, Src src, const uint32_t *val, uint64_t total, bool emitted,
+                        const uint64_t *doff, uint32_t nq, uint64_t *d_offsets, uint32_t *d_pos, uint32_t *d_mis) {
+    typedef unsigned long long u64;
+    TRY(mark(c, "strand_merge"));
+    LAUNCH(c, k_strand_offsets, cdiv((uint64_t)nq + 1, BLK), (const u64 *)doff, nq, reinterpret_cast<u64 *>(d_offsets));
+    if (emitted)
+        LAUNCH(c, k_strand_merge<Src>, cdiv(total, BLK), src, val, total, (const u64 *)doff, 2 * nq, d_pos, d_mis);
+    return B200SA_OK;
+}
+
+// nq >= 1, k = threshold | flags as approx_args accepts it, without B200SA_APPROX_BEST.  With
+// B200SA_APPROX_BOTH_STRANDS the search runs on the doubled batch and k_strand_merge replaces k_approx_gather.
 template <class EndF>
 static int approx_core(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const uint32_t *d_sa,
                        const uint32_t *d_starts, uint32_t ndocs, const uint8_t *d_queries, const uint64_t *d_q_off,
@@ -3033,15 +3079,24 @@ static int approx_core(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const u
     const uint32_t k = kf & 0xFFFFu;
     uint64_t q_bytes;
     TRY(approx_prep(c, n, d_starts, ndocs, d_queries, d_q_off, nq, k, &q_bytes));
-    const bool iupac = (kf & B200SA_APPROX_IUPAC) != 0;
+    const bool iupac = (kf & B200SA_APPROX_IUPAC) != 0, both = (kf & B200SA_APPROX_BOTH_STRANDS) != 0;
+    if (both) TRY(strand_check(c, q_bytes, nq, k));
     if (iupac) TRY(iupac_canon(c, d_queries, q_bytes, &d_queries));
     if (n == 0) return approx_nothing(c, d_offsets, nq);
+    const uint8_t *eq = d_queries;
+    const uint64_t *eoff = d_q_off;
+    uint64_t *soff = d_offsets;
+    if (both) TRY(strand_queries(c, d_queries, d_q_off, nq, q_bytes, iupac, &eq, &eoff, &soff));
     uint64_t *ko = nullptr;
     uint32_t *vo = nullptr;
     int pbits = 0;
-    TRY(approx_search(c, d_text, n, d_sa, d_starts, ndocs, d_queries, d_q_off, nq, k, (kf & B200SA_APPROX_EDIT) != 0,
-                      iupac, d_offsets, cap, total, end, &ko, &vo, &pbits));
-    if (*total > 0 && *total <= cap)
+    TRY(approx_search(c, d_text, n, d_sa, d_starts, ndocs, eq, eoff, both ? 2 * nq : nq, k,
+                      (kf & B200SA_APPROX_EDIT) != 0, iupac, soff, cap, total, end, &ko, &vo, &pbits));
+    const bool emitted = *total > 0 && *total <= cap;
+    if (both)
+        TRY(strand_merge(c, StrandKeys{(const u64 *)ko, pbits}, vo, *total, emitted, soff, nq, d_offsets, d_pos,
+                         d_mis));
+    else if (emitted)
         LAUNCH(c, k_approx_gather, cdiv(*total, BLK), (const u64 *)ko, (const uint32_t *)vo, *total,
                (u64)((1ull << pbits) - 1), d_pos, d_mis);
     TRY(mark(c, "end"));
@@ -3051,8 +3106,10 @@ static int approx_core(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const u
 }
 
 // The batch a BestPick selects: *nb queries, map[i] the query of entry i; their bytes and offsets at *bq / *boff,
-// the call's own arrays when every query is picked, else gathered into c->qbuf and coff.
-static int best_batch(b200sa_ctx *c, const uint8_t *d_queries, const uint64_t *d_q_off, uint32_t nq, BestPick pick,
+// the call's own arrays when every query is picked, else gathered into c->qbuf and coff.  Pick: BestPick, or
+// StrandPick over the entries of the doubled batch.
+template <class Pick>
+static int best_batch(b200sa_ctx *c, const uint8_t *d_queries, const uint64_t *d_q_off, uint32_t nq, Pick pick,
                       uint32_t *map, uint64_t *coff, uint32_t *nb, const uint8_t **bq, const uint64_t **boff) {
     typedef unsigned long long u64;
     uint32_t *words = ptr<uint32_t>(c->small);           // [8, 10) (batch size << 32) | batch bytes
@@ -3069,11 +3126,14 @@ static int best_batch(b200sa_ctx *c, const uint8_t *d_queries, const uint64_t *d
     return B200SA_OK;
 }
 
-// nq >= 1, k = threshold | B200SA_APPROX_SLACK(s) | B200SA_APPROX_BEST, optionally | B200SA_APPROX_EDIT and
-// | B200SA_APPROX_IUPAC (the batches are then gathered from the canonical copy).
+// nq >= 1, k = threshold | B200SA_APPROX_SLACK(s) | B200SA_APPROX_BEST, optionally | B200SA_APPROX_EDIT,
+// | B200SA_APPROX_IUPAC (the batches are then gathered from the canonical copy) and | B200SA_APPROX_BOTH_STRANDS.
 // Rounds t = 0 .. threshold over the live queries (best.cuh), then one emission per distinct final threshold.
-// Phases: approx_check; per round best_compact, the search's phases, best_update; per emitted group
-// best_compact, the search's phases, best_scatter.
+// With B200SA_APPROX_BOTH_STRANDS the entries are those of the doubled batch, a query and its reverse complement
+// are live as a pair with one best (strand.cuh), the groups scatter into c->sstage over the doubled offsets and
+// one k_strand_merge writes the caller's arrays.
+// Phases: approx_check; strand_queries with the flag; per round best_compact, the search's phases, best_update;
+// per emitted group best_compact, the search's phases, best_scatter; strand_merge with the flag.
 template <class EndF>
 static int approx_best_core(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const uint32_t *d_sa,
                             const uint32_t *d_starts, uint32_t ndocs, const uint8_t *d_queries,
@@ -3081,20 +3141,27 @@ static int approx_best_core(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, co
                             uint32_t *d_mis, uint64_t cap, uint64_t *total, EndF end) {
     typedef unsigned long long u64;
     const uint32_t k = kf & 0xFFu, s = (kf >> 8) & 0xFFu;
-    const bool edit = (kf & B200SA_APPROX_EDIT) != 0, iupac = (kf & B200SA_APPROX_IUPAC) != 0;
+    const bool edit = (kf & B200SA_APPROX_EDIT) != 0, iupac = (kf & B200SA_APPROX_IUPAC) != 0,
+               both = (kf & B200SA_APPROX_BOTH_STRANDS) != 0;
     uint64_t q_bytes;
     c->stats.doubling_rounds = 0;
     TRY(approx_prep(c, n, d_starts, ndocs, d_queries, d_q_off, nq, k, &q_bytes));
+    if (both) TRY(strand_check(c, q_bytes, nq, k));
     if (iupac) TRY(iupac_canon(c, d_queries, q_bytes, &d_queries));
     if (n == 0) return approx_nothing(c, d_offsets, nq);
-    TRY(ensure(c, c->k32b, (size_t)nq * 9));             // cnt, map (u32), best (u8) per query
-    TRY(ensure(c, c->rank, ((size_t)nq + 1) * 16));      // the batch's q_off, the search's offsets
-    TRY(ensure(c, c->qbuf, (size_t)q_bytes));
-    uint32_t *cnt = ptr<uint32_t>(c->k32b), *map = cnt + nq;
-    uint8_t *best = reinterpret_cast<uint8_t *>(map + nq);
-    uint64_t *coff = ptr<uint64_t>(c->rank), *soff = coff + nq + 1;
+    const uint8_t *eq = d_queries;                       // the entries: the queries, or the doubled batch
+    const uint64_t *eoff = d_q_off;
+    uint64_t *eo = d_offsets;                            // the entries' output offsets
+    if (both) TRY(strand_queries(c, d_queries, d_q_off, nq, q_bytes, iupac, &eq, &eoff, &eo));
+    const uint32_t ne = both ? 2 * nq : nq;
+    TRY(ensure(c, c->k32b, (size_t)ne * 8 + nq));        // cnt, map (u32) per entry, best (u8) per query
+    TRY(ensure(c, c->rank, ((size_t)ne + 1) * 16));      // the batch's q_off, the search's offsets
+    TRY(ensure(c, c->qbuf, (size_t)q_bytes * (both ? 2 : 1)));
+    uint32_t *cnt = ptr<uint32_t>(c->k32b), *map = cnt + ne;
+    uint8_t *best = reinterpret_cast<uint8_t *>(map + ne);
+    uint64_t *coff = ptr<uint64_t>(c->rank), *soff = coff + ne + 1;
     uint32_t *words = ptr<uint32_t>(c->small);           // [10] rounds where a query ended, [12, 14) total
-    CU_TRY(c, cudaMemsetAsync(cnt, 0, (size_t)nq * 4, c->stream));
+    CU_TRY(c, cudaMemsetAsync(cnt, 0, (size_t)ne * 4, c->stream));
     CU_TRY(c, cudaMemsetAsync(best, BEST_NONE, nq, c->stream));
     CU_TRY(c, cudaMemsetAsync(words + 8, 0, 24, c->stream));
     uint64_t *ko = nullptr, rtotal = 0;
@@ -3102,37 +3169,52 @@ static int approx_best_core(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, co
     int pbits = 0;
     const uint8_t *bq;
     const uint64_t *boff;
+    auto batch = [&](uint32_t t, bool group) {
+        if (both) return best_batch(c, eq, eoff, ne, StrandPick{eoff, best, ne, t, s, k, group}, map, coff, &nb, &bq,
+                                    &boff);
+        return best_batch(c, eq, eoff, ne, BestPick{eoff, best, ne, t, s, k, group}, map, coff, &nb, &bq, &boff);
+    };
     for (uint32_t t = 0; t <= k; t++) {
         TRY(mark(c, "best_compact"));
-        TRY(best_batch(c, d_queries, d_q_off, nq, BestPick{d_q_off, best, nq, t, s, k, false}, map, coff, &nb, &bq,
-                       &boff));
+        TRY(batch(t, false));
         if (nb == 0) break;
         rounds++;
         TRY(approx_search(c, d_text, n, d_sa, d_starts, ndocs, bq, boff, nb, t, edit, iupac, soff, 0, &rtotal, end, &ko, &vo,
                           &pbits));
         TRY(mark(c, "best_update"));
-        LAUNCH(c, k_best_update, cdiv(nb, BLK), (const uint32_t *)map, (const u64 *)soff, nb, t, s, k, best, cnt,
-               words + 10);
+        if (both)
+            LAUNCH(c, k_strand_update, cdiv(nb / 2, BLK), (const uint32_t *)map, (const u64 *)soff, nb, t, s, k, best,
+                   cnt, words + 10);
+        else
+            LAUNCH(c, k_best_update, cdiv(nb, BLK), (const uint32_t *)map, (const u64 *)soff, nb, t, s, k, best, cnt,
+                   words + 10);
     }
     c->stats.doubling_rounds = rounds;
-    TRY((dev_scan<OpSum64>(c, InCount64{cnt, nq}, OutStoreExcl64{reinterpret_cast<u64 *>(d_offsets)}, (uint64_t)nq + 1,
+    TRY((dev_scan<OpSum64>(c, InCount64{cnt, ne}, OutStoreExcl64{reinterpret_cast<u64 *>(eo)}, (uint64_t)ne + 1,
                            reinterpret_cast<u64 *>(words + 12))));
     TRY(read_words(c, words + 10, 4));
     const uint32_t ended = c->h_pin[0];
     *total = pin_u64(c, 2);
-    if (*total > 0 && *total <= cap) {
+    const bool emitted = *total > 0 && *total <= cap;
+    uint32_t *gpos = d_pos, *gmis = d_mis;               // where the groups scatter
+    if (both && emitted) {
+        TRY(ensure(c, c->sstage, (size_t)*total * 8));
+        gpos = ptr<uint32_t>(c->sstage);
+        gmis = gpos + *total;
+    }
+    if (emitted) {
         for (uint32_t t = 0; t <= k; t++) {
             if (!(ended >> t & 1u)) continue;
             TRY(mark(c, "best_compact"));
-            TRY(best_batch(c, d_queries, d_q_off, nq, BestPick{d_q_off, best, nq, t, s, k, true}, map, coff, &nb, &bq,
-                           &boff));
+            TRY(batch(t, true));
             TRY(approx_search(c, d_text, n, d_sa, d_starts, ndocs, bq, boff, nb, t, edit, iupac, soff, ~0ull, &rtotal, end,
                               &ko, &vo, &pbits));
             TRY(mark(c, "best_scatter"));
             LAUNCH(c, k_best_scatter, cdiv(rtotal, BLK), (const u64 *)ko, (const uint32_t *)vo, rtotal, pbits,
-                   (const u64 *)soff, (const uint32_t *)map, (const u64 *)d_offsets, d_pos, d_mis);
+                   (const u64 *)soff, (const uint32_t *)map, (const u64 *)eo, gpos, gmis);
         }
     }
+    if (both) TRY(strand_merge(c, StrandStaged{gpos}, gmis, *total, emitted, eo, nq, d_offsets, d_pos, d_mis));
     TRY(mark(c, "end"));
     CU_TRY(c, cudaGetLastError());
     CU_TRY(c, cudaStreamSynchronize(c->stream));
@@ -3144,18 +3226,19 @@ static int approx_args(b200sa_ctx *c, uint64_t n, const void *text, const void *
     if (!c) return B200SA_ERR_BAD_ARG;
     if (!total || !offsets || (nq > 0 && !q_off) || (cap > 0 && !pos) || (n > 0 && (!text || !sa))) return null_ptr(c);
     if (k & B200SA_APPROX_BEST) {
-        if (k & ~(0xFFFFu | B200SA_APPROX_EDIT | B200SA_APPROX_BEST | B200SA_APPROX_IUPAC) ||
+        if (k & ~(0xFFFFu | B200SA_APPROX_EDIT | B200SA_APPROX_BEST | B200SA_APPROX_IUPAC |
+                  B200SA_APPROX_BOTH_STRANDS) ||
             (k & 0xFFu) > B200SA_APPROX_MAX_K ||
             ((k >> 8) & 0xFFu) > B200SA_APPROX_MAX_K)
             return fail(c, B200SA_ERR_BAD_ARG,
                         "approx positions: with B200SA_APPROX_BEST, k must be a threshold up to B200SA_APPROX_MAX_K | "
-                        "B200SA_APPROX_SLACK(s) with s up to B200SA_APPROX_MAX_K, optionally | B200SA_APPROX_EDIT "
-                        "and | B200SA_APPROX_IUPAC");
+                        "B200SA_APPROX_SLACK(s) with s up to B200SA_APPROX_MAX_K, optionally | B200SA_APPROX_EDIT, "
+                        "| B200SA_APPROX_IUPAC and | B200SA_APPROX_BOTH_STRANDS");
     } else {
-        if (k & ~(0xFFFFu | B200SA_APPROX_EDIT | B200SA_APPROX_IUPAC))
+        if (k & ~(0xFFFFu | B200SA_APPROX_EDIT | B200SA_APPROX_IUPAC | B200SA_APPROX_BOTH_STRANDS))
             return fail(c, B200SA_ERR_BAD_ARG,
-                        "approx positions: k must be a threshold up to B200SA_APPROX_MAX_K, optionally | B200SA_APPROX_EDIT "
-                        "and | B200SA_APPROX_IUPAC");
+                        "approx positions: k must be a threshold up to B200SA_APPROX_MAX_K, optionally | "
+                        "B200SA_APPROX_EDIT, | B200SA_APPROX_IUPAC and | B200SA_APPROX_BOTH_STRANDS");
         if ((k & 0xFFFFu) > B200SA_APPROX_MAX_K)
             return fail(c, B200SA_ERR_BAD_ARG, "approx positions: k above B200SA_APPROX_MAX_K");
     }

@@ -451,8 +451,8 @@ class DocumentSuffixTable:
         is a symbol of its own."""
         return _bwt.bwt_runs(self)
 
-    # ---- approximate positions (DESIGN 6b f-14 .. f-17)
-    def approximate_positions(self, query, k, *, metric="hamming", best=None, iupac=False):
+    # ---- approximate positions (DESIGN 6b f-14 .. f-18)
+    def approximate_positions(self, query, k, *, metric="hamming", best=None, iupac=False, strands="forward"):
         """(positions u32[], mismatches u32[]): every position p of the concatenation whose window of m bytes
         lies inside p's document and differs from the query (m bytes) in at most k bytes, 0 <= k <= 31, by
         ascending p, with that number of mismatches beside it (b200sa_docs_approx_positions_dev).  locate()
@@ -469,21 +469,28 @@ class DocumentSuffixTable:
         either case), which matches the uppercase text bytes A C G T of its class (B200SA_APPROX_IUPAC); any
         other query byte raises B200SA_ERR_BAD_ARG.  Lowercase (soft-masked) text bases, N, U and every other
         text byte match no code and count as a mismatch: uppercase a soft-masked text before building the
-        table.  Combines with metric= and best=; a non-bool value raises ValueError."""
-        return _approx.positions(self, query, k, metric, best, iupac)
+        table.  Combines with metric= and best=; a non-bool value raises ValueError.
+        strands="both" also lists the occurrences of the query's reverse complement (A <-> T, C <-> G in either
+        case; with iupac=True each code's class complemented, R <-> Y, K <-> M, B <-> V, D <-> H, U -> A) as
+        minus-strand hits at the leftmost text position of their window or alignment
+        (B200SA_APPROX_BOTH_STRANDS), and returns (positions, distances, minus): one list by (p, strand) with
+        the plus hit first, minus a bool array; with best= best(q) is taken over both strands.  strands="forward"
+        (the default) searches the query alone; any other value raises ValueError."""
+        return _approx.positions(self, query, k, metric, best, iupac, strands)
 
-    def approximate_positions_batch(self, queries, k, *, metric="hamming", best=None, iupac=False):
+    def approximate_positions_batch(self, queries, k, *, metric="hamming", best=None, iupac=False, strands="forward"):
         """(offsets u64[nq + 1], positions u32[], mismatches u32[]): query q's occurrences with at most k
         mismatches (or within k edits, metric="edit") are positions[offsets[q]:offsets[q + 1]], as
         approximate_positions returns them; best=0 gives each query's best hits, with best(q) in the
-        distance column (best= and iupac= as in approximate_positions)."""
-        return _approx.positions_batch(self, queries, k, metric, best, iupac)
+        distance column (best= and iupac= as in approximate_positions).  strands="both" returns (offsets,
+        positions, distances, minus) with both strands in each query's list, as approximate_positions does."""
+        return _approx.positions_batch(self, queries, k, metric, best, iupac, strands)
 
-    def approximate_counts(self, queries, k, *, metric="hamming", best=None, iupac=False):
+    def approximate_counts(self, queries, k, *, metric="hamming", best=None, iupac=False, strands="forward"):
         """u64[nq]: the number of occurrences with at most k mismatches (or within k edits, metric="edit") of
         every query, without fetching them; best=0 counts each query's best hits, those at distance best(q)
-        (best= and iupac= as in approximate_positions)."""
-        return _approx.counts(self, queries, k, metric, best, iupac)
+        (best= and iupac= as in approximate_positions); strands="both" counts the hits of both strands."""
+        return _approx.counts(self, queries, k, metric, best, iupac, strands)
 
     def top_documents(self, query, k) -> np.ndarray:
         """(document, count) rows of the min(k, df) documents that contain `query` most often, by count

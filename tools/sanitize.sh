@@ -188,6 +188,16 @@ for k, tab in enumerate([single] + [DocumentSuffixTable(docs) for docs in doc_se
         for metric in ("hamming", "edit"):
             off, pos, dist = tab.approximate_positions_batch(iu_qs, kk, metric=metric, best=sl, iupac=True)
             assert len(pos) == int(off[-1]) and (dist <= kk).all(), (k, kk, sl, metric)
+# both strands: the doubled batch (plain and canonical complements), the key merge and, with best hits, the pair
+# rounds, the staging scatter and the staged merge
+for k, tab in enumerate([single] + [DocumentSuffixTable(docs) for docs in doc_sets] +
+                        [SuffixTable(b"A" * 5000), DocumentSuffixTable([b"", b"AC", b"", b"G"])]):
+    for kk, sl in ((0, None), (3, None), (31, None), (3, 0), (3, 1)):
+        for metric in ("hamming", "edit"):
+            for iu, qs in ((False, ap_qs + [b"GAATTC", b"a" * 9]), (True, iu_qs)):
+                off, pos, dist, minus = tab.approximate_positions_batch(qs, kk, metric=metric, best=sl, iupac=iu,
+                                                                        strands="both")
+                assert len(pos) == len(minus) == int(off[-1]) and (dist <= kk).all(), (k, kk, sl, metric, iu)
 # refinement branches (tests/test_gpu_refine.py): a local-sort overflow in round 2 of the direct path, the direct
 # path's probe (2^20 tied after round 1, large groups), 64-bit round-0 keys of the reduced string
 import ctypes
