@@ -645,7 +645,44 @@ int b200sa_unbwt_dev(b200sa_ctx *ctx, uint64_t n, uint32_t ndocs, const uint8_t 
  * a pair with one best.  Device workspace (computed, not measured): 2 bytes per query byte and 32 per query for
  * the doubled batch and its offsets, plus what the search takes for 2 nq queries, and with B200SA_APPROX_BEST 8
  * bytes per fetched entry for staging.  Phases: strand_queries after approx_check, strand_merge before end; the
- * other phases keep their names and meaning. */
+ * other phases keep their names and meaning.
+ *
+ * ---- approximate document listing (DESIGN.md 6b f-19) ----
+ * With B200SA_APPROX_DOCUMENTS (bit 29) in k, b200sa_docs_approx_positions_dev lists the documents that contain
+ * each query within the threshold instead of the hits.  The flag is accepted by the documents entry alone, in any
+ * mix with B200SA_APPROX_EDIT, B200SA_APPROX_BEST | B200SA_APPROX_SLACK(s), B200SA_APPROX_IUPAC and
+ * B200SA_APPROX_BOTH_STRANDS; the threshold is decoded as without it.  On b200sa_approx_positions_dev bit 29 is an
+ * unknown bit (B200SA_ERR_BAD_ARG, detail naming B200SA_APPROX_MAX_K); any other unknown bit on the documents
+ * entry is B200SA_ERR_BAD_ARG with a detail that names B200SA_APPROX_MAX_K and B200SA_APPROX_DOCUMENTS.  Without
+ * the flag nothing changes.  Definition:
+ *  - L(q) is the list the same call with bit 29 cleared returns for q: entries (p, d(p)) by ascending p, or
+ *    (p, d(p), strand) by (p, strand) with + first under B200SA_APPROX_BOTH_STRANDS.
+ *  - doc(p) is the last d with doc_starts[d] <= p, as in b200sa_doc_ids_dev; an empty document holds no position
+ *    and is never listed.
+ *  - q's list has one entry per distinct doc(p) over L(q), by ascending document index: d_pos[i] is the document,
+ *    d_mismatches[i] (may be NULL) the least d(p) over that document's entries of L(q), with B200SA_APPROX_MINUS
+ *    set (under B200SA_APPROX_BOTH_STRANDS) exactly when no + entry of that document reaches that least distance:
+ *    the document's first entry in (d, strand) order, + first.
+ *  - With B200SA_APPROX_BEST, best(q) and t(q) are those of the call without the flag, over the whole collection,
+ *    not per document: a document is listed iff it holds an occurrence at distance <= t(q).
+ *  - Protocol: the listing protocol.  d_offsets (nq + 1, exclusive) and *total count documents and are always
+ *    written; d_pos and d_mismatches are written only when total <= cap, never past total.  With cap = 0,
+ *    offsets[q + 1] - offsets[q] is q's approximate document frequency.
+ *  - Unchanged from the call without the flag: the other argument checks and error codes, the TOO_LARGE slot and
+ *    query-length checks, nq = 0, n = 0, m = 0, the bytes read, synchronisation and the meaning of
+ *    b200sa_last_stats().doubling_rounds.
+ *  - So every document count is at most the call's hit count without the flag; at threshold 0 with the Hamming
+ *    metric, one strand and no IUPAC, q's documents are those b200sa_docs_list_dev lists for q's exact range, each
+ *    at distance 0; a palindromic query (rc(q) = q) never has B200SA_APPROX_MINUS set.
+ * Method: q's final list is built as without the flag, but always emitted, into staging: ordered by p (or by
+ * (p, strand)), so each document's hits are contiguous within a query.  One thread per staged hit marks the hits
+ * that start a query's list or change document, a scan of the marks numbers the (query, document) segments and
+ * gives the offsets, each segment start writes its document, and the least (d << 1) | minus of a segment is taken
+ * with an atomicMin, so the result does not depend on the order of the hits.  Device workspace (computed, not
+ * measured): what the fetch call without the flag takes for the whole hit list (even the cap = 0 call emits every
+ * hit), plus 20 bytes per hit for the staged list, its marks and their scan, and 8 bytes per query.  Phases: those
+ * of the call without the flag (with its emission phases even at cap = 0), then adocs_mark and, when the listing
+ * fits, adocs_emit, before end. */
 #define B200SA_APPROX_MAX_K 31
 #define B200SA_APPROX_EDIT 0x10000u
 #define B200SA_APPROX_BEST 0x100000u                      /* bit 20 */
@@ -653,6 +690,7 @@ int b200sa_unbwt_dev(b200sa_ctx *ctx, uint64_t n, uint32_t ndocs, const uint8_t 
 #define B200SA_APPROX_IUPAC 0x1000000u                    /* bit 24 */
 #define B200SA_APPROX_BOTH_STRANDS 0x10000000u            /* bit 28, in k */
 #define B200SA_APPROX_MINUS 0x80000000u                   /* bit 31, in d_mismatches entries */
+#define B200SA_APPROX_DOCUMENTS 0x20000000u               /* bit 29, in k, documents entry only */
 int b200sa_approx_positions_dev(b200sa_ctx *ctx, const uint8_t *d_text, uint64_t n, const uint32_t *d_sa,
                                 const uint8_t *d_queries, const uint64_t *d_q_off, uint32_t nq, uint32_t k,
                                 uint64_t *d_offsets, uint32_t *d_pos, uint32_t *d_mismatches, uint64_t cap,

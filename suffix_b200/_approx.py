@@ -1,6 +1,6 @@
 """Approximate positions (occurrences with at most k mismatches, or within k edits with metric="edit", with
 best=s only each query's best hits, with iupac=True queries in IUPAC nucleotide codes, and with strands="both" the
-reverse complement's hits as well) over a device-resident
+reverse complement's hits as well), and the documents that hold them, over a device-resident
 table: the part SuffixTable and DocumentSuffixTable share.  A table supplies `_device` and
 `_bwt_arrays()` -> (d_text, d_table, d_doc_starts or None, ndocs), its text and table on the device; the LCP
 array is not needed."""
@@ -15,6 +15,7 @@ BEST = 0x100000           # B200SA_APPROX_BEST
 IUPAC = 0x1000000         # B200SA_APPROX_IUPAC
 BOTH_STRANDS = 0x10000000  # B200SA_APPROX_BOTH_STRANDS
 MINUS = 0x80000000        # B200SA_APPROX_MINUS
+DOCUMENTS = 0x20000000    # B200SA_APPROX_DOCUMENTS
 METRICS = {"hamming": 0, "edit": EDIT}
 
 
@@ -41,20 +42,21 @@ def _strands(strands):
     return BOTH_STRANDS if strands == "both" else 0
 
 
-def _call(table, queries, k, fetch, metric="hamming", best=None, iupac=False, strands="forward"):
+def _call(table, queries, k, fetch, metric="hamming", best=None, iupac=False, strands="forward", documents=False):
     """(offsets u64[nq + 1], positions u32[], distances u32[]); positions and distances are None without
     fetch (the cap = 0 call).  metric "hamming" counts mismatches, "edit" the Levenshtein distance; best=s keeps
     each query's occurrences within s of its least distance (include/b200sa.h, B200SA_APPROX_BEST); iupac=True reads
     the queries as IUPAC nucleotide codes, matched against the uppercase text bytes A C G T only
     (B200SA_APPROX_IUPAC); strands="both" adds the reverse complement's occurrences, the distances of those carrying
-    B200SA_APPROX_MINUS (B200SA_APPROX_BOTH_STRANDS)."""
+    B200SA_APPROX_MINUS (B200SA_APPROX_BOTH_STRANDS); documents=True (a DocumentSuffixTable only) lists the
+    documents that hold q's hits instead, with the least distance in each (B200SA_APPROX_DOCUMENTS)."""
     import torch
     k = int(k)
     if not 0 <= k <= MAX_K:
         raise ValueError("k must be in 0 .. %d, got %d" % (MAX_K, k))
     if metric not in METRICS:
         raise ValueError("metric must be 'hamming' or 'edit', got %r" % (metric,))
-    kf = k | METRICS[metric] | _flags(best) | _iupac(iupac) | _strands(strands)
+    kf = k | METRICS[metric] | _flags(best) | _iupac(iupac) | _strands(strands) | (DOCUMENTS if documents else 0)
     qs = [_as_bytes(q) for q in queries]
     nq, n = len(qs), len(table)
     d_t, d_r, d_s, ndocs = table._bwt_arrays()
@@ -112,3 +114,22 @@ def positions(table, query, k, metric="hamming", best=None, iupac=False, strands
 def counts(table, queries, k, metric="hamming", best=None, iupac=False, strands="forward"):
     off, _, _ = _call(table, queries, k, False, metric, best, iupac, strands)
     return np.diff(off.astype(np.int64)).astype(np.uint64)
+
+
+def documents_batch(table, queries, k, metric="hamming", best=None, iupac=False, strands="forward"):
+    off, docs, dist = _call(table, queries, k, True, metric, best, iupac, strands, documents=True)
+    if strands == "forward":
+        return off, docs, dist
+    return (off, docs) + _split(dist)
+
+
+def documents(table, query, k, metric="hamming", best=None, iupac=False, strands="forward"):
+    _, docs, dist = _call(table, [query], k, True, metric, best, iupac, strands, documents=True)
+    if strands == "forward":
+        return docs, dist
+    return (docs,) + _split(dist)
+
+
+def document_frequencies(table, queries, k, metric="hamming", best=None, iupac=False, strands="forward"):
+    off, _, _ = _call(table, queries, k, False, metric, best, iupac, strands, documents=True)
+    return np.diff(off.astype(np.int64)).astype(np.uint32)

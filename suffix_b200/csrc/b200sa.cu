@@ -40,6 +40,7 @@
 #include "best.cuh"
 #include "iupac.cuh"
 #include "strand.cuh"
+#include "approx_docs.cuh"
 #include "nccl_dyn.h"
 
 using namespace b200sa;
@@ -88,6 +89,7 @@ struct b200sa_ctx {
     DevBuf docs_starts, docs_out;              // doc_starts and output staging of b200sa_docs_build
     DevBuf icode;                              // approx positions with B200SA_APPROX_IUPAC: the canonical queries
     DevBuf strand, sstage;                     // with B200SA_APPROX_BOTH_STRANDS: the doubled batch, the staged hits
+    DevBuf adoff, adocs;                       // with B200SA_APPROX_DOCUMENTS: the hit offsets, the staged hits
     uint32_t cls_calls = 0;
     // multi-GPU (SURVEY 8e): communicator owned or attached, NCCL resolved at run time
     ncclComm_t comm = nullptr;
@@ -1292,7 +1294,7 @@ void b200sa_ctx_destroy(b200sa_ctx *c) {
     DevBuf *bufs[] = {&c->text, &c->sa, &c->lcp, &c->pred, &c->stype, &c->lmsb, &c->lmsrank, &c->lmspos, &c->lmslist,
                       &c->lmspred, &c->sorted, &c->flag, &c->reduced, &c->sa_r, &c->blkstate, &c->carry, &c->tables,
                       &c->small, &c->scan_partial, &c->radix_cnt, &c->blkcnt, &c->k32b, &c->k64a, &c->k64b, &c->v0,
-                      &c->v1, &c->p0, &c->p1, &c->g0, &c->g1, &c->rank, &c->isa, &c->qbuf, &c->os_hist, &c->os_status, &c->packed, &c->phik, &c->phiv, &c->runscr, &c->plcp_samp, &c->scan_state, &c->cls_state, &c->lmsdesc, &c->steplog, &c->hist_copies, &c->tree_out, &c->docs_starts, &c->docs_out, &c->icode, &c->strand, &c->sstage, &c->sh_a, &c->sh_b, &c->sh_c, &c->sh_d, &c->sh_e, &c->sh_f, &c->sh_small};
+                      &c->v1, &c->p0, &c->p1, &c->g0, &c->g1, &c->rank, &c->isa, &c->qbuf, &c->os_hist, &c->os_status, &c->packed, &c->phik, &c->phiv, &c->runscr, &c->plcp_samp, &c->scan_state, &c->cls_state, &c->lmsdesc, &c->steplog, &c->hist_copies, &c->tree_out, &c->docs_starts, &c->docs_out, &c->icode, &c->strand, &c->sstage, &c->adoff, &c->adocs, &c->sh_a, &c->sh_b, &c->sh_c, &c->sh_d, &c->sh_e, &c->sh_f, &c->sh_small};
     for (DevBuf *b : bufs) if (b->p) cudaFree(b->p);
     for (cudaEvent_t e : c->event_pool) cudaEventDestroy(e);
     if (c->h_pin) cudaFreeHost(c->h_pin);
@@ -2888,7 +2890,7 @@ int b200sa_unbwt_dev(b200sa_ctx *c, uint64_t n, uint32_t ndocs, const uint8_t *d
     return leave(c, unbwt_core(c, (uint32_t)n, ndocs, d_bwt, d_term_rows, d_text_out, d_doc_starts_out));
 }
 
-// ------------------------------------------------------------ approximate positions (DESIGN 6b f-14 .. f-18)
+// ------------------------------------------------------------ approximate positions (DESIGN 6b f-14 .. f-19)
 // The checks of a call (nq >= 1, k its threshold): q_off on the device with q_off[nq] read back as *q_bytes,
 // doc_starts (d_starts non-null for documents), and the sizes.  Phase approx_check.
 static int approx_prep(b200sa_ctx *c, uint32_t n, const uint32_t *d_starts, uint32_t ndocs, const uint8_t *d_queries,
@@ -3068,8 +3070,59 @@ static int strand_merge(b200sa_ctx *c, Src src, const uint32_t *val, uint64_t to
     return B200SA_OK;
 }
 
+// B200SA_APPROX_DOCUMENTS: the offsets of the final hit lists, which the search or the scan of the best rounds
+// writes in place of the caller's.
+static int adocs_offsets(b200sa_ctx *c, uint32_t nq, uint64_t **hoff) {
+    TRY(ensure(c, c->adoff, ((size_t)nq + 1) * 8));
+    *hoff = ptr<uint64_t>(c->adoff);
+    return B200SA_OK;
+}
+
+// B200SA_APPROX_DOCUMENTS: the staging of htotal >= 1 final hits in c->adocs, laid out as the segment scan
+// (htotal + 1 u64), then the positions *hpos, the distances *hmis and the marks (htotal u32 each).
+static int adocs_stage(b200sa_ctx *c, uint64_t htotal, uint32_t **hpos, uint32_t **hmis) {
+    TRY(ensure(c, c->adocs, ((size_t)htotal + 1) * 8 + (size_t)htotal * 12));
+    *hpos = reinterpret_cast<uint32_t *>(ptr<uint64_t>(c->adocs) + htotal + 1);
+    *hmis = *hpos + htotal;
+    return B200SA_OK;
+}
+
+// B200SA_APPROX_DOCUMENTS: the staged final lists (*total hits at offsets hoff, from adocs_stage) reduced per
+// (query, document) into the caller's offsets and, when the listing fits cap, d_pos and d_mis; *total becomes the
+// number of listed documents.  Phases adocs_mark (marks, scan, offsets) and adocs_emit.
+static int adocs_reduce(b200sa_ctx *c, const uint32_t *d_starts, uint32_t ndocs, uint32_t nq, const uint64_t *hoff,
+                        uint64_t *d_offsets, uint32_t *d_pos, uint32_t *d_mis, uint64_t cap, uint64_t *total) {
+    typedef unsigned long long u64;
+    const uint64_t htotal = *total;
+    TRY(mark(c, "adocs_mark"));
+    if (htotal == 0) {
+        CU_TRY(c, cudaMemsetAsync(d_offsets, 0, ((size_t)nq + 1) * 8, c->stream));
+        return B200SA_OK;
+    }
+    u64 *seg = ptr<u64>(c->adocs);
+    const uint32_t *hpos = reinterpret_cast<const uint32_t *>(seg + htotal + 1), *hmis = hpos + htotal;
+    uint32_t *marks = reinterpret_cast<uint32_t *>(seg + htotal + 1) + 2 * htotal;
+    uint32_t *words = ptr<uint32_t>(c->small);           // [20, 22) the number of listed documents
+    LAUNCH(c, k_adocs_mark, cdiv(htotal, BLK), hpos, htotal, (const u64 *)hoff, nq, d_starts, ndocs, marks);
+    TRY((dev_scan<OpSum64>(c, InCount64{marks, htotal}, OutStoreExcl64{seg}, htotal + 1,
+                           reinterpret_cast<u64 *>(words + 20))));
+    LAUNCH(c, k_adocs_offsets, cdiv((uint64_t)nq + 1, BLK), (const u64 *)hoff, (const u64 *)seg, nq,
+           reinterpret_cast<u64 *>(d_offsets));
+    TRY(read_words(c, words + 20, 2));
+    *total = pin_u64(c, 0);
+    if (*total > cap) return B200SA_OK;
+    TRY(mark(c, "adocs_emit"));
+    uint32_t *least = d_mis ? marks : nullptr;           // the marks are spent; their room holds the least words
+    if (least) CU_TRY(c, cudaMemsetAsync(least, 0xFF, (size_t)*total * 4, c->stream));
+    LAUNCH(c, k_adocs_emit, cdiv(htotal, BLK), hpos, hmis, htotal, (const u64 *)seg, d_starts, ndocs, d_pos, least);
+    if (least) LAUNCH(c, k_adocs_dist, cdiv(*total, BLK), (const uint32_t *)least, *total, d_mis);
+    return B200SA_OK;
+}
+
 // nq >= 1, k = threshold | flags as approx_args accepts it, without B200SA_APPROX_BEST.  With
 // B200SA_APPROX_BOTH_STRANDS the search runs on the doubled batch and k_strand_merge replaces k_approx_gather.
+// With B200SA_APPROX_DOCUMENTS the search always emits, the final list lands in staging with its offsets in
+// c->adoff, and adocs_reduce writes the caller's arrays.
 template <class EndF>
 static int approx_core(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const uint32_t *d_sa,
                        const uint32_t *d_starts, uint32_t ndocs, const uint8_t *d_queries, const uint64_t *d_q_off,
@@ -3079,26 +3132,32 @@ static int approx_core(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const u
     const uint32_t k = kf & 0xFFFFu;
     uint64_t q_bytes;
     TRY(approx_prep(c, n, d_starts, ndocs, d_queries, d_q_off, nq, k, &q_bytes));
-    const bool iupac = (kf & B200SA_APPROX_IUPAC) != 0, both = (kf & B200SA_APPROX_BOTH_STRANDS) != 0;
+    const bool iupac = (kf & B200SA_APPROX_IUPAC) != 0, both = (kf & B200SA_APPROX_BOTH_STRANDS) != 0,
+               docs = (kf & B200SA_APPROX_DOCUMENTS) != 0;
     if (both) TRY(strand_check(c, q_bytes, nq, k));
     if (iupac) TRY(iupac_canon(c, d_queries, q_bytes, &d_queries));
     if (n == 0) return approx_nothing(c, d_offsets, nq);
+    uint64_t *hoff = d_offsets;                          // the final list's offsets
+    if (docs) TRY(adocs_offsets(c, nq, &hoff));
     const uint8_t *eq = d_queries;
     const uint64_t *eoff = d_q_off;
-    uint64_t *soff = d_offsets;
+    uint64_t *soff = hoff;
     if (both) TRY(strand_queries(c, d_queries, d_q_off, nq, q_bytes, iupac, &eq, &eoff, &soff));
     uint64_t *ko = nullptr;
     uint32_t *vo = nullptr;
     int pbits = 0;
+    const uint64_t scap = docs ? ~0ull : cap;            // with B200SA_APPROX_DOCUMENTS every hit is staged
     TRY(approx_search(c, d_text, n, d_sa, d_starts, ndocs, eq, eoff, both ? 2 * nq : nq, k,
-                      (kf & B200SA_APPROX_EDIT) != 0, iupac, soff, cap, total, end, &ko, &vo, &pbits));
-    const bool emitted = *total > 0 && *total <= cap;
+                      (kf & B200SA_APPROX_EDIT) != 0, iupac, soff, scap, total, end, &ko, &vo, &pbits));
+    const bool emitted = *total > 0 && *total <= scap;
+    uint32_t *fpos = d_pos, *fmis = d_mis;               // where the final list lands
+    if (docs && emitted) TRY(adocs_stage(c, *total, &fpos, &fmis));
     if (both)
-        TRY(strand_merge(c, StrandKeys{(const u64 *)ko, pbits}, vo, *total, emitted, soff, nq, d_offsets, d_pos,
-                         d_mis));
+        TRY(strand_merge(c, StrandKeys{(const u64 *)ko, pbits}, vo, *total, emitted, soff, nq, hoff, fpos, fmis));
     else if (emitted)
         LAUNCH(c, k_approx_gather, cdiv(*total, BLK), (const u64 *)ko, (const uint32_t *)vo, *total,
-               (u64)((1ull << pbits) - 1), d_pos, d_mis);
+               (u64)((1ull << pbits) - 1), fpos, fmis);
+    if (docs) TRY(adocs_reduce(c, d_starts, ndocs, nq, hoff, d_offsets, d_pos, d_mis, cap, total));
     TRY(mark(c, "end"));
     CU_TRY(c, cudaGetLastError());
     CU_TRY(c, cudaStreamSynchronize(c->stream));
@@ -3134,6 +3193,8 @@ static int best_batch(b200sa_ctx *c, const uint8_t *d_queries, const uint64_t *d
 // one k_strand_merge writes the caller's arrays.
 // Phases: approx_check; strand_queries with the flag; per round best_compact, the search's phases, best_update;
 // per emitted group best_compact, the search's phases, best_scatter; strand_merge with the flag.
+// With B200SA_APPROX_DOCUMENTS the groups are always emitted, the final list lands in staging with its offsets in
+// c->adoff, and adocs_reduce (phases adocs_mark, adocs_emit) writes the caller's arrays.
 template <class EndF>
 static int approx_best_core(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const uint32_t *d_sa,
                             const uint32_t *d_starts, uint32_t ndocs, const uint8_t *d_queries,
@@ -3142,16 +3203,18 @@ static int approx_best_core(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, co
     typedef unsigned long long u64;
     const uint32_t k = kf & 0xFFu, s = (kf >> 8) & 0xFFu;
     const bool edit = (kf & B200SA_APPROX_EDIT) != 0, iupac = (kf & B200SA_APPROX_IUPAC) != 0,
-               both = (kf & B200SA_APPROX_BOTH_STRANDS) != 0;
+               both = (kf & B200SA_APPROX_BOTH_STRANDS) != 0, docs = (kf & B200SA_APPROX_DOCUMENTS) != 0;
     uint64_t q_bytes;
     c->stats.doubling_rounds = 0;
     TRY(approx_prep(c, n, d_starts, ndocs, d_queries, d_q_off, nq, k, &q_bytes));
     if (both) TRY(strand_check(c, q_bytes, nq, k));
     if (iupac) TRY(iupac_canon(c, d_queries, q_bytes, &d_queries));
     if (n == 0) return approx_nothing(c, d_offsets, nq);
+    uint64_t *hoff = d_offsets;                          // the final list's offsets
+    if (docs) TRY(adocs_offsets(c, nq, &hoff));
     const uint8_t *eq = d_queries;                       // the entries: the queries, or the doubled batch
     const uint64_t *eoff = d_q_off;
-    uint64_t *eo = d_offsets;                            // the entries' output offsets
+    uint64_t *eo = hoff;                                 // the entries' output offsets
     if (both) TRY(strand_queries(c, d_queries, d_q_off, nq, q_bytes, iupac, &eq, &eoff, &eo));
     const uint32_t ne = both ? 2 * nq : nq;
     TRY(ensure(c, c->k32b, (size_t)ne * 8 + nq));        // cnt, map (u32) per entry, best (u8) per query
@@ -3195,8 +3258,11 @@ static int approx_best_core(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, co
     TRY(read_words(c, words + 10, 4));
     const uint32_t ended = c->h_pin[0];
     *total = pin_u64(c, 2);
-    const bool emitted = *total > 0 && *total <= cap;
-    uint32_t *gpos = d_pos, *gmis = d_mis;               // where the groups scatter
+    const uint64_t scap = docs ? ~0ull : cap;            // with B200SA_APPROX_DOCUMENTS every hit is staged
+    const bool emitted = *total > 0 && *total <= scap;
+    uint32_t *fpos = d_pos, *fmis = d_mis;               // where the final list lands
+    if (docs && emitted) TRY(adocs_stage(c, *total, &fpos, &fmis));
+    uint32_t *gpos = fpos, *gmis = fmis;                 // where the groups scatter
     if (both && emitted) {
         TRY(ensure(c, c->sstage, (size_t)*total * 8));
         gpos = ptr<uint32_t>(c->sstage);
@@ -3214,7 +3280,8 @@ static int approx_best_core(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, co
                    (const u64 *)soff, (const uint32_t *)map, (const u64 *)eo, gpos, gmis);
         }
     }
-    if (both) TRY(strand_merge(c, StrandStaged{gpos}, gmis, *total, emitted, eo, nq, d_offsets, d_pos, d_mis));
+    if (both) TRY(strand_merge(c, StrandStaged{gpos}, gmis, *total, emitted, eo, nq, hoff, fpos, fmis));
+    if (docs) TRY(adocs_reduce(c, d_starts, ndocs, nq, hoff, d_offsets, d_pos, d_mis, cap, total));
     TRY(mark(c, "end"));
     CU_TRY(c, cudaGetLastError());
     CU_TRY(c, cudaStreamSynchronize(c->stream));
@@ -3222,23 +3289,33 @@ static int approx_best_core(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, co
 }
 
 static int approx_args(b200sa_ctx *c, uint64_t n, const void *text, const void *sa, const void *q_off, uint32_t nq,
-                       uint32_t k, const void *offsets, const void *pos, uint64_t cap, const void *total) {
+                       uint32_t k, const void *offsets, const void *pos, uint64_t cap, const void *total,
+                       bool docs = false) {
     if (!c) return B200SA_ERR_BAD_ARG;
     if (!total || !offsets || (nq > 0 && !q_off) || (cap > 0 && !pos) || (n > 0 && (!text || !sa))) return null_ptr(c);
+    const uint32_t listing = docs ? B200SA_APPROX_DOCUMENTS : 0u;    // accepted by the documents entry alone
     if (k & B200SA_APPROX_BEST) {
         if (k & ~(0xFFFFu | B200SA_APPROX_EDIT | B200SA_APPROX_BEST | B200SA_APPROX_IUPAC |
-                  B200SA_APPROX_BOTH_STRANDS) ||
+                  B200SA_APPROX_BOTH_STRANDS | listing) ||
             (k & 0xFFu) > B200SA_APPROX_MAX_K ||
             ((k >> 8) & 0xFFu) > B200SA_APPROX_MAX_K)
             return fail(c, B200SA_ERR_BAD_ARG,
-                        "approx positions: with B200SA_APPROX_BEST, k must be a threshold up to B200SA_APPROX_MAX_K | "
-                        "B200SA_APPROX_SLACK(s) with s up to B200SA_APPROX_MAX_K, optionally | B200SA_APPROX_EDIT, "
-                        "| B200SA_APPROX_IUPAC and | B200SA_APPROX_BOTH_STRANDS");
+                        docs ? "approx positions: with B200SA_APPROX_BEST, k must be a threshold up to "
+                               "B200SA_APPROX_MAX_K | B200SA_APPROX_SLACK(s) with s up to B200SA_APPROX_MAX_K, "
+                               "optionally | B200SA_APPROX_EDIT, | B200SA_APPROX_IUPAC, | B200SA_APPROX_BOTH_STRANDS "
+                               "and | B200SA_APPROX_DOCUMENTS"
+                             : "approx positions: with B200SA_APPROX_BEST, k must be a threshold up to "
+                               "B200SA_APPROX_MAX_K | B200SA_APPROX_SLACK(s) with s up to B200SA_APPROX_MAX_K, "
+                               "optionally | B200SA_APPROX_EDIT, | B200SA_APPROX_IUPAC and | "
+                               "B200SA_APPROX_BOTH_STRANDS");
     } else {
-        if (k & ~(0xFFFFu | B200SA_APPROX_EDIT | B200SA_APPROX_IUPAC | B200SA_APPROX_BOTH_STRANDS))
+        if (k & ~(0xFFFFu | B200SA_APPROX_EDIT | B200SA_APPROX_IUPAC | B200SA_APPROX_BOTH_STRANDS | listing))
             return fail(c, B200SA_ERR_BAD_ARG,
-                        "approx positions: k must be a threshold up to B200SA_APPROX_MAX_K, optionally | "
-                        "B200SA_APPROX_EDIT, | B200SA_APPROX_IUPAC and | B200SA_APPROX_BOTH_STRANDS");
+                        docs ? "approx positions: k must be a threshold up to B200SA_APPROX_MAX_K, optionally | "
+                               "B200SA_APPROX_EDIT, | B200SA_APPROX_IUPAC, | B200SA_APPROX_BOTH_STRANDS and | "
+                               "B200SA_APPROX_DOCUMENTS"
+                             : "approx positions: k must be a threshold up to B200SA_APPROX_MAX_K, optionally | "
+                               "B200SA_APPROX_EDIT, | B200SA_APPROX_IUPAC and | B200SA_APPROX_BOTH_STRANDS");
         if ((k & 0xFFFFu) > B200SA_APPROX_MAX_K)
             return fail(c, B200SA_ERR_BAD_ARG, "approx positions: k above B200SA_APPROX_MAX_K");
     }
@@ -3266,7 +3343,7 @@ int b200sa_docs_approx_positions_dev(b200sa_ctx *c, const uint8_t *d_text, uint6
                                      const uint64_t *d_q_off, uint32_t nq, uint32_t k, uint64_t *d_offsets,
                                      uint32_t *d_pos, uint32_t *d_mismatches, uint64_t cap, uint64_t *total,
                                      void *stream) {
-    TRY(approx_args(c, n, d_text, d_gsa, d_q_off, nq, k, d_offsets, d_pos, cap, total));
+    TRY(approx_args(c, n, d_text, d_gsa, d_q_off, nq, k, d_offsets, d_pos, cap, total, true));
     if ((n > 0 || ndocs > 0) && !d_doc_starts) return null_ptr(c);
     if (ndocs == 0 && n > 0) return no_docs(c);
     TRY(enter(c, stream));

@@ -451,7 +451,7 @@ class DocumentSuffixTable:
         is a symbol of its own."""
         return _bwt.bwt_runs(self)
 
-    # ---- approximate positions (DESIGN 6b f-14 .. f-18)
+    # ---- approximate positions (DESIGN 6b f-14 .. f-19)
     def approximate_positions(self, query, k, *, metric="hamming", best=None, iupac=False, strands="forward"):
         """(positions u32[], mismatches u32[]): every position p of the concatenation whose window of m bytes
         lies inside p's document and differs from the query (m bytes) in at most k bytes, 0 <= k <= 31, by
@@ -491,6 +491,30 @@ class DocumentSuffixTable:
         every query, without fetching them; best=0 counts each query's best hits, those at distance best(q)
         (best= and iupac= as in approximate_positions); strands="both" counts the hits of both strands."""
         return _approx.counts(self, queries, k, metric, best, iupac, strands)
+
+    def approximate_documents(self, query, k, *, metric="hamming", best=None, iupac=False, strands="forward"):
+        """(documents u32[], distances u32[]): the documents that hold an occurrence of the query within k, as
+        approximate_positions finds them, by ascending document, each with the least distance of its
+        occurrences there (b200sa_docs_approx_positions_dev with B200SA_APPROX_DOCUMENTS).  The listing is
+        made on the device from the hits, which never cross PCIe.  Empty documents are never listed.  With
+        best=s, best(q) and its threshold are those of approximate_positions, taken over the whole collection:
+        a document is listed iff it holds a hit at distance <= min(k, best(q) + s).  strands="both" returns
+        (documents, distances, minus), minus set when the least distance in that document is reached on the
+        minus strand only.  metric=, best=, iupac= and strands= are checked as in approximate_positions."""
+        return _approx.documents(self, query, k, metric, best, iupac, strands)
+
+    def approximate_documents_batch(self, queries, k, *, metric="hamming", best=None, iupac=False,
+                                    strands="forward"):
+        """(offsets u64[nq + 1], documents u32[], distances u32[]): query q's documents are
+        documents[offsets[q]:offsets[q + 1]], as approximate_documents returns them; one count call, then one
+        fetch call sized by it.  strands="both" returns (offsets, documents, distances, minus)."""
+        return _approx.documents_batch(self, queries, k, metric, best, iupac, strands)
+
+    def approximate_document_frequencies(self, queries, k, *, metric="hamming", best=None, iupac=False,
+                                         strands="forward"):
+        """u32[nq]: the number of documents that hold an occurrence of each query within k (keywords as in
+        approximate_documents), from the count call alone, without fetching the listing."""
+        return _approx.document_frequencies(self, queries, k, metric, best, iupac, strands)
 
     def top_documents(self, query, k) -> np.ndarray:
         """(document, count) rows of the min(k, df) documents that contain `query` most often, by count

@@ -198,6 +198,20 @@ for k, tab in enumerate([single] + [DocumentSuffixTable(docs) for docs in doc_se
                 off, pos, dist, minus = tab.approximate_positions_batch(qs, kk, metric=metric, best=sl, iupac=iu,
                                                                         strands="both")
                 assert len(pos) == len(minus) == int(off[-1]) and (dist <= kk).all(), (k, kk, sl, metric, iu)
+# approximate document listing: the staged hit lists of every mix (one strand and both, plain and IUPAC, with and
+# without best hits), the marks, their scan, the offsets, the emission and the least-distance pass, and the count
+# call alone
+for k, docs in enumerate(doc_sets + [[b"", b"AC", b"", b"G"], [b"A"] * 50 + [b""]]):
+    tab = DocumentSuffixTable(docs)
+    for kk, sl in ((0, None), (3, None), (31, None), (3, 0), (3, 1)):
+        for metric in ("hamming", "edit"):
+            for iu, qs in ((False, ap_qs + [b"GAATTC", b"a" * 9]), (True, iu_qs)):
+                for strands in ("forward", "both"):
+                    kw = dict(metric=metric, best=sl, iupac=iu, strands=strands)
+                    res = tab.approximate_documents_batch(qs, kk, **kw)
+                    off, ds, dist = res[:3]
+                    assert len(ds) == int(off[-1]) and (dist <= kk).all() and (ds < len(docs)).all(), (k, kk, sl)
+                    assert (tab.approximate_document_frequencies(qs, kk, **kw) == np.diff(off.astype(np.int64))).all()
 # refinement branches (tests/test_gpu_refine.py): a local-sort overflow in round 2 of the direct path, the direct
 # path's probe (2^20 tied after round 1, large groups), 64-bit round-0 keys of the reduced string
 import ctypes
