@@ -682,7 +682,58 @@ int b200sa_unbwt_dev(b200sa_ctx *ctx, uint64_t n, uint32_t ndocs, const uint8_t 
  * measured): what the fetch call without the flag takes for the whole hit list (even the cap = 0 call emits every
  * hit), plus 20 bytes per hit for the staged list, its marks and their scan, and 8 bytes per query.  Phases: those
  * of the call without the flag (with its emission phases even at cap = 0), then adocs_mark and, when the listing
- * fits, adocs_emit, before end. */
+ * fits, adocs_emit, before end.
+ *
+ * ---- alignments of the hits (DESIGN.md 6b f-20) ----
+ * With B200SA_APPROX_ALIGN (bit 27) in k, b200sa_docs_approx_positions_dev lists the alignment operations of the
+ * hits instead of the hits.  The flag is accepted by the documents entry alone, in any mix with
+ * B200SA_APPROX_EDIT, B200SA_APPROX_BEST | B200SA_APPROX_SLACK(s), B200SA_APPROX_IUPAC and
+ * B200SA_APPROX_BOTH_STRANDS; a single text goes through that entry as one document (doc_starts = {0}, ndocs = 1,
+ * G = sa).  B200SA_APPROX_ALIGN | B200SA_APPROX_DOCUMENTS returns B200SA_ERR_BAD_ARG with a detail that names
+ * both; on b200sa_approx_positions_dev bit 27 is an unknown bit as before.  Without the flag nothing changes.
+ * Definition:
+ *  - L(q) is the list the same call with bit 27 cleared returns for q: hits (p, d, strand) by p, or by
+ *    (p, strand) with + first; best(q) and t(q) are that call's.
+ *  - Q is q for a + hit and rc(q) for a - hit (the complement above, IUPAC classes included), m = |Q|, E = the
+ *    end of p's document.  match(x, t) is T[t] == Q[x], or with B200SA_APPROX_IUPAC "T[t] is in the class of
+ *    Q[x]" (only uppercase A C G T in the text match).
+ *  - Hamming: window position x gives = if match(x, p + x), else X; end = p + m.
+ *  - Edit: D(x, t) for 0 <= x <= m, p <= t <= E: D(m, t) = 0; D(x, E) = m - x; otherwise D(x, t) =
+ *    min(D(x+1, t+1) + [not match(x, t)], D(x+1, t) + 1, D(x, t+1) + 1), so D(0, p) = d.  The canonical walk
+ *    starts at (x, t) = (0, p) and, while x < m, takes the first move that holds: (1) t < E and D(x, t) =
+ *    D(x+1, t+1) + [not match]: = or X, x+1, t+1; (2) D(x, t) = D(x+1, t) + 1: I (a query byte with no text
+ *    byte), x+1; (3) otherwise D (a text byte with no query byte), t+1.  end = the final t.
+ *  - Adjacent moves with one code merge into one operation.  Operations are in text order: a - hit's describe
+ *    rc(q) against T[p, end), as SAM does for reverse-strand reads.  So the lengths of X, I and D sum to d, those of
+ *    =, X and I to m, those of =, X and D to end - p; end <= E; the last operation is never D; a hit has at most
+ *    2d + 1 operations (and at least one: m = 0 has no hits).
+ *  - Band lemma: every cell the walk visits lies on a diagonal t - p - x in [-d, d] (each step off the diagonal
+ *    costs 1).  A neighbour on an optimal continuation has an optimal path inside the band and one that is not
+ *    fails the equality banded or not, so a DP over those 2d + 1 <= 63 diagonals, with values saturated at
+ *    d + 1, takes the same walk.  The device recomputes D(0, p) and checks it against the staged d; a difference
+ *    returns B200SA_ERR_INTERNAL, which is never expected.
+ *  - Output, the listing protocol with operations as entries: d_offsets (nq + 1, exclusive) and *total count
+ *    operations and are always written; entries go by hit as in L(q), and within a hit in walk order.  d_pos[i] is
+ *    the hit's p, d_mismatches[i] the operation as a BAM word, len << 4 | code with I = 1, D = 2, = 7, X = 8,
+ *    and B200SA_APPROX_MINUS on every operation of a - hit.  A hit is a maximal run of one query's entries with
+ *    equal (p, minus).  d_pos and d_mismatches are written only when total <= cap, never past total;
+ *    d_mismatches is required when cap > 0 (NULL returns B200SA_ERR_BAD_ARG).  cap = 0 counts only, but stages
+ *    and aligns every hit, as B200SA_APPROX_DOCUMENTS does.
+ *  - Limits, checked in phase approx_check: a query longer than 2^27 - 1 bytes (operation lengths leave bit 31
+ *    for B200SA_APPROX_MINUS), or with B200SA_APPROX_EDIT longer than B200SA_APPROX_ALIGN_MAX_M bytes (the bound
+ *    of the traceback's shared memory), returns B200SA_ERR_TOO_LARGE with a detail naming the limit.
+ *  - Unchanged from the call without the flag: the other argument checks and error codes, nq = 0, n = 0, the
+ *    bytes read, synchronisation and b200sa_last_stats().doubling_rounds.
+ * Method: the final hit list is staged as with B200SA_APPROX_DOCUMENTS.  One count kernel aligns every hit and
+ * keeps its merged words at a stride of 2 threshold + 1 words: Hamming one thread per hit; edit one warp per hit,
+ * lane l holding diagonals l and l + 32, the row's deletion move a warp suffix-minimum scan, and each row's 2-bit
+ * move choices (16 bytes) in shared memory, walked forward by one lane.  A scan of the counts gives each hit's
+ * first entry and the offsets, and an emit kernel copies the words.  Device workspace (computed, not measured):
+ * what the fetch call without the flag takes for the whole hit list, plus 20 bytes per hit for the staged list,
+ * the counts and their scan, 4 (2 threshold + 1) bytes per hit for the words, and 8 bytes per query; with
+ * B200SA_APPROX_EDIT, 16 bytes of shared memory per row of the longest query in the batch per resident warp
+ * (64 KB per warp at B200SA_APPROX_ALIGN_MAX_M).  Phases: those of the call without the flag (with its emission
+ * phases even at cap = 0), then align_count, align_scan and, when the listing fits, align_emit, before end. */
 #define B200SA_APPROX_MAX_K 31
 #define B200SA_APPROX_EDIT 0x10000u
 #define B200SA_APPROX_BEST 0x100000u                      /* bit 20 */
@@ -691,6 +742,8 @@ int b200sa_unbwt_dev(b200sa_ctx *ctx, uint64_t n, uint32_t ndocs, const uint8_t 
 #define B200SA_APPROX_BOTH_STRANDS 0x10000000u            /* bit 28, in k */
 #define B200SA_APPROX_MINUS 0x80000000u                   /* bit 31, in d_mismatches entries */
 #define B200SA_APPROX_DOCUMENTS 0x20000000u               /* bit 29, in k, documents entry only */
+#define B200SA_APPROX_ALIGN 0x8000000u                    /* bit 27, in k, documents entry only */
+#define B200SA_APPROX_ALIGN_MAX_M 4096                    /* the longest query B200SA_APPROX_EDIT aligns */
 int b200sa_approx_positions_dev(b200sa_ctx *ctx, const uint8_t *d_text, uint64_t n, const uint32_t *d_sa,
                                 const uint8_t *d_queries, const uint64_t *d_q_off, uint32_t nq, uint32_t k,
                                 uint64_t *d_offsets, uint32_t *d_pos, uint32_t *d_mismatches, uint64_t cap,

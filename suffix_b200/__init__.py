@@ -9,3 +9,4 @@ from .tree import Node, SuffixTree  # noqa: F401,E402
 from .docs import DocumentSuffixTable  # noqa: F401,E402
 from .docs_tree import DocumentNode, DocumentSuffixTree  # noqa: F401,E402
 from ._bwt import inverse_bwt, inverse_bwt_documents  # noqa: F401,E402
+from ._approx import cigar_string  # noqa: F401,E402

@@ -1,6 +1,6 @@
 """Approximate positions (occurrences with at most k mismatches, or within k edits with metric="edit", with
 best=s only each query's best hits, with iupac=True queries in IUPAC nucleotide codes, and with strands="both" the
-reverse complement's hits as well), and the documents that hold them, over a device-resident
+reverse complement's hits as well), the documents that hold them, and their alignments, over a device-resident
 table: the part SuffixTable and DocumentSuffixTable share.  A table supplies `_device` and
 `_bwt_arrays()` -> (d_text, d_table, d_doc_starts or None, ndocs), its text and table on the device; the LCP
 array is not needed."""
@@ -16,6 +16,8 @@ IUPAC = 0x1000000         # B200SA_APPROX_IUPAC
 BOTH_STRANDS = 0x10000000  # B200SA_APPROX_BOTH_STRANDS
 MINUS = 0x80000000        # B200SA_APPROX_MINUS
 DOCUMENTS = 0x20000000    # B200SA_APPROX_DOCUMENTS
+ALIGN = 0x8000000         # B200SA_APPROX_ALIGN
+OPS = "MIDNSHP=X"         # the BAM operation codes
 METRICS = {"hamming": 0, "edit": EDIT}
 
 
@@ -42,25 +44,31 @@ def _strands(strands):
     return BOTH_STRANDS if strands == "both" else 0
 
 
-def _call(table, queries, k, fetch, metric="hamming", best=None, iupac=False, strands="forward", documents=False):
+def _call(table, queries, k, fetch, metric="hamming", best=None, iupac=False, strands="forward", documents=False,
+          align=False):
     """(offsets u64[nq + 1], positions u32[], distances u32[]); positions and distances are None without
     fetch (the cap = 0 call).  metric "hamming" counts mismatches, "edit" the Levenshtein distance; best=s keeps
     each query's occurrences within s of its least distance (include/b200sa.h, B200SA_APPROX_BEST); iupac=True reads
     the queries as IUPAC nucleotide codes, matched against the uppercase text bytes A C G T only
     (B200SA_APPROX_IUPAC); strands="both" adds the reverse complement's occurrences, the distances of those carrying
     B200SA_APPROX_MINUS (B200SA_APPROX_BOTH_STRANDS); documents=True (a DocumentSuffixTable only) lists the
-    documents that hold q's hits instead, with the least distance in each (B200SA_APPROX_DOCUMENTS)."""
+    documents that hold q's hits instead, with the least distance in each (B200SA_APPROX_DOCUMENTS); align=True
+    lists the alignment operations of q's hits instead, as (offsets, p, BAM word) entries (B200SA_APPROX_ALIGN),
+    a single text going through the documents entry as one document."""
     import torch
     k = int(k)
     if not 0 <= k <= MAX_K:
         raise ValueError("k must be in 0 .. %d, got %d" % (MAX_K, k))
     if metric not in METRICS:
         raise ValueError("metric must be 'hamming' or 'edit', got %r" % (metric,))
-    kf = k | METRICS[metric] | _flags(best) | _iupac(iupac) | _strands(strands) | (DOCUMENTS if documents else 0)
+    kf = (k | METRICS[metric] | _flags(best) | _iupac(iupac) | _strands(strands) | (DOCUMENTS if documents else 0) |
+          (ALIGN if align else 0))
     qs = [_as_bytes(q) for q in queries]
     nq, n = len(qs), len(table)
     d_t, d_r, d_s, ndocs = table._bwt_arrays()
     dev = torch.device("cuda", table._device)
+    if align and d_s is None:
+        d_s, ndocs = _one_document(table, dev), 1
     off = np.zeros(nq + 1, dtype=np.uint64)
     off[1:] = np.cumsum([len(q) for q in qs])
     d_q = torch.from_numpy(np.frombuffer(b"".join(qs) or b"\0", dtype=np.uint8).copy()).to(dev)
@@ -133,3 +141,53 @@ def documents(table, query, k, metric="hamming", best=None, iupac=False, strands
 def document_frequencies(table, queries, k, metric="hamming", best=None, iupac=False, strands="forward"):
     off, _, _ = _call(table, queries, k, False, metric, best, iupac, strands, documents=True)
     return np.diff(off.astype(np.int64)).astype(np.uint32)
+
+
+def _one_document(table, dev):
+    """doc_starts = {0} on the device, kept on the table: a single text as a collection of one document."""
+    import torch
+    if getattr(table, "_dev_one_doc", None) is None:
+        table._dev_one_doc = torch.zeros(1, dtype=torch.int32, device=dev)
+    return table._dev_one_doc
+
+
+def cigar_string(words):
+    """The CIGAR string of BAM words (len << 4 | code), e.g. "12=1X7=1I2="; bit 31 is ignored."""
+    return "".join("%d%s" % ((int(w) & 0x7FFFFFFF) >> 4, OPS[int(w) & 15]) for w in words)
+
+
+def _hits(off, pos, words):
+    """The hits of an operation listing: (hit offsets u64[nq + 1], positions, distances, minus, ends,
+    cigar_offsets u64[h + 1], cigar u32[]).  A hit is a maximal run of one query's entries with equal (p, minus);
+    its distance is the length of its X, I and D operations, its end p plus that of =, X and D."""
+    off = off.astype(np.int64)
+    total = int(off[-1])
+    q = np.repeat(np.arange(len(off) - 1), np.diff(off))
+    minus = (words & np.uint32(MINUS)) != 0
+    first = np.ones(total, dtype=bool)
+    first[1:] = (q[1:] != q[:-1]) | (pos[1:] != pos[:-1]) | (minus[1:] != minus[:-1])
+    starts = np.flatnonzero(first)
+    hoff = np.concatenate([[0], np.cumsum(first)])[off].astype(np.uint64)
+    cigar = words & np.uint32(MINUS - 1)
+    lens, code = (cigar >> 4).astype(np.int64), cigar & np.uint32(15)
+    if len(starts):
+        dist = np.add.reduceat(np.where(code != 7, lens, 0), starts)
+        span = np.add.reduceat(np.where(code != 1, lens, 0), starts)
+    else:
+        dist = span = np.zeros(0, dtype=np.int64)
+    p = pos[starts]
+    cigar_off = np.append(starts, total).astype(np.uint64)
+    return (hoff, p, dist.astype(np.uint32), minus[starts], (p.astype(np.int64) + span).astype(np.uint32), cigar_off,
+            cigar)
+
+
+def alignments_batch(table, queries, k, metric="hamming", best=None, iupac=False, strands="forward"):
+    off, pos, words = _call(table, queries, k, True, metric, best, iupac, strands, align=True)
+    hoff, p, dist, minus, ends, cigar_off, cigar = _hits(off, pos, words)
+    if strands == "forward":
+        return hoff, p, dist, ends, cigar_off, cigar
+    return hoff, p, dist, minus, ends, cigar_off, cigar
+
+
+def alignments(table, query, k, metric="hamming", best=None, iupac=False, strands="forward"):
+    return alignments_batch(table, [query], k, metric, best, iupac, strands)[1:]

@@ -1,0 +1,214 @@
+// align.cuh -- the alignment of every approximate occurrence as CIGAR operations (DESIGN 6b f-20), the
+// B200SA_APPROX_ALIGN flag of b200sa_docs_approx_positions_dev.
+//
+// The call builds q's final list as it would without the flag, but into the staging of approx_docs.cuh.  A count
+// kernel aligns every staged hit and keeps its operations, merged into BAM words (len << 4 | code), at a fixed
+// stride of 2k + 1 words per hit (a hit at distance d has at most 2d + 1 operations); a scan of the counts gives
+// each hit's first entry, k_adocs_offsets reads the caller's offsets off it, and k_align_emit copies the words.
+//
+// Hamming (k_align_hamming, one thread per hit): position x of the window is = or X.
+// Edit (k_align_edit, one warp per hit): D(x, t) is the least cost of aligning Q[x, m) to a prefix of T[t, E),
+// E the end of p's document; rows x = m - 1 .. 0 are computed over the 2d + 1 diagonals t - p - x in [-d, d]
+// with values saturated at d + 1.  Lane l holds diagonals l and l + 32.  The diagonal move and the insertion come
+// from the row below (same diagonal, one diagonal down), the deletion D(x, t + 1) + 1 is a suffix minimum of
+// D + diagonal over the row, taken with shuffles.  Each row's 2-bit move choices (4 ballots, 16 bytes) go to
+// shared memory; lane 0 then walks them forward from (0, p).  Every cell of the canonical walk lies in the band,
+// and a neighbour that is on an optimal continuation has an in-band optimal path, so the banded choices are the
+// full DP's.  D(0, p) must equal the staged d; a difference sets the error word (never expected).
+#pragma once
+#include "iupac.cuh"
+#include "strand.cuh"
+
+namespace b200sa {
+
+enum : uint32_t { ALIGN_I = 1, ALIGN_D = 2, ALIGN_EQ = 7, ALIGN_X = 8 };
+
+// The staged hits and what aligning them reads.  qs: the queries (the canonical copy with iupac), hoff the
+// nq + 1 offsets of the staged lists, hpos / hmis the htotal positions and distances (B200SA_APPROX_MINUS on a
+// minus hit); ops gets stride words per hit, cnt the number used, err is set on a broken invariant.
+struct AlignArgs {
+    const uint8_t *text;
+    const uint32_t *starts;
+    uint32_t ndocs, n;
+    const uint8_t *qs;
+    const uint64_t *qoff;
+    uint32_t nq;
+    const unsigned long long *hoff;
+    const uint32_t *hpos, *hmis;
+    uint64_t htotal;
+    bool iupac;
+    uint32_t stride;
+    uint32_t *ops, *cnt, *err;
+};
+
+// Query symbol x of hit (o, m, minus): q[x], or rc(q)[x] = comp(q[m - 1 - x]) on a minus hit.
+struct AlignQuery {
+    const uint8_t *q;
+    uint32_t m;
+    bool minus, iupac;
+    __device__ __forceinline__ uint32_t at(uint32_t x) const {
+        return minus ? strand_comp(__ldg(q + m - 1 - x), iupac) : __ldg(q + x);
+    }
+    __device__ __forceinline__ bool match(uint32_t t, uint32_t c) const { return iupac ? iupac_in(t, c) : t == c; }
+};
+
+__device__ __forceinline__ AlignQuery align_query(const AlignArgs &A, uint64_t i) {
+    uint32_t a = 0, b = A.nq;                                     // the query of hit i: the last q with hoff[q] <= i
+    while (b - a > 1) {
+        const uint32_t mid = a + (b - a) / 2;
+        if (A.hoff[mid] <= i) a = mid; else b = mid;
+    }
+    const uint64_t o = A.qoff[a];
+    return AlignQuery{A.qs + o, (uint32_t)(A.qoff[a + 1] - o), (A.hmis[i] & B200SA_APPROX_MINUS) != 0, A.iupac};
+}
+
+// Merges adjacent moves with one code into BAM words at out[0, stride).
+struct AlignSink {
+    uint32_t *out, stride, n = 0, code = 0, len = 0;
+    __device__ __forceinline__ void flush() {
+        if (len && n < stride) out[n] = len << 4 | code;
+        if (len) n++;
+    }
+    __device__ __forceinline__ void push(uint32_t c) {
+        if (c == code) { len++; return; }
+        flush();
+        code = c;
+        len = 1;
+    }
+};
+
+// One thread per staged hit.
+__global__ void __launch_bounds__(BLK) k_align_hamming(AlignArgs A) {
+    const uint64_t i = (uint64_t)blockIdx.x * BLK + threadIdx.x;
+    if (i >= A.htotal) return;
+    const AlignQuery Q = align_query(A, i);
+    const uint8_t *__restrict__ t = A.text + A.hpos[i];
+    AlignSink s{A.ops + i * A.stride, A.stride};
+    uint32_t x_count = 0;
+    for (uint32_t x = 0; x < Q.m; x++) {
+        const bool eq = Q.match(__ldg(t + x), Q.at(x));
+        x_count += !eq;
+        s.push(eq ? ALIGN_EQ : ALIGN_X);
+    }
+    s.flush();
+    A.cnt[i] = s.n;
+    if (x_count != (A.hmis[i] & ~B200SA_APPROX_MINUS) || s.n > A.stride) atomicOr(A.err, 1u);
+}
+
+// One warp per staged hit; rows words of dynamic shared memory (4 per query row) per warp, rows >= the longest
+// query of the batch.  The block has blockDim.x / 32 warps.
+__global__ void __launch_bounds__(BLK) k_align_edit(AlignArgs A, uint32_t rows) {
+    extern __shared__ uint4 s_moves[];
+    const uint32_t l = lane_id(), w = threadIdx.x >> 5;
+    const uint64_t i = (uint64_t)blockIdx.x * (blockDim.x >> 5) + w;
+    if (i >= A.htotal) return;
+    uint4 *mv = s_moves + (size_t)w * rows;
+    const AlignQuery Q = align_query(A, i);
+    const uint32_t p = A.hpos[i], d = A.hmis[i] & ~B200SA_APPROX_MINUS;
+    const uint32_t E = docs_end(A.starts, A.ndocs, A.n, docs_find(A.starts, A.ndocs, p));
+    const int32_t INF = (int32_t)d + 1, W = 2 * (int32_t)d + 1, j0 = (int32_t)l, j1 = (int32_t)l + 32;
+    const bool wide = W > 32;                                     // uniform: the upper half holds cells
+    // cell j of row x is t = p + x + j - d; a cell with t < p or t > E is outside the DP and holds INF
+    auto tt = [&](uint32_t x, int32_t j) { return (int64_t)p + x + j - (int32_t)d; };
+    auto in = [&](uint32_t x, int32_t j) { const int64_t t = tt(x, j); return j < W && t >= p && t <= E; };
+    int32_t r0 = in(Q.m, j0) ? 0 : INF, r1 = in(Q.m, j1) ? 0 : INF;   // row m: D(m, t) = 0
+    for (uint32_t x = Q.m; x-- > 0;) {
+        const uint32_t qc = Q.at(x);
+        // the row below at diagonal j - 1 (the insertion's source)
+        int32_t u0 = __shfl_up_sync(0xffffffffu, r0, 1), u1 = __shfl_up_sync(0xffffffffu, r1, 1);
+        const int32_t top = __shfl_sync(0xffffffffu, r0, 31);
+        if (l == 0) { u0 = INF; u1 = top; }
+        int32_t a0 = INF, a1 = INF, m0 = 1, m1 = 1;
+        const bool v0 = in(x, j0), v1 = in(x, j1);
+        const int64_t t0 = tt(x, j0), t1 = tt(x, j1);
+        if (v0) {
+            if (t0 < E) { m0 = !Q.match(__ldg(A.text + t0), qc); a0 = r0 + m0; }
+            a0 = min(a0, u0 + 1);
+        }
+        if (v1) {
+            if (t1 < E) { m1 = !Q.match(__ldg(A.text + t1), qc); a1 = r1 + m1; }
+            a1 = min(a1, u1 + 1);
+        }
+        // the deletion: D(j) = min over j' >= j of a(j') + j' - j, a suffix minimum of a + j
+        int32_t s0 = min(a0, INF) + j0, s1 = min(a1, INF) + j1;
+        if (wide) {
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) {
+                const int32_t y = __shfl_down_sync(0xffffffffu, s1, o);
+                if (l + o < 32) s1 = min(s1, y);
+            }
+        }
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const int32_t y = __shfl_down_sync(0xffffffffu, s0, o);
+            if (l + o < 32) s0 = min(s0, y);
+        }
+        if (wide) s0 = min(s0, __shfl_sync(0xffffffffu, s1, 0));
+        const int32_t n0 = v0 ? min(s0 - j0, INF) : INF, n1 = v1 ? min(s1 - j1, INF) : INF;
+        // the first move that holds: 1 diagonal, 2 insertion, 3 deletion
+        const uint32_t c0 = (t0 < E && n0 == r0 + m0) ? 1u : n0 == u0 + 1 ? 2u : 3u;
+        const uint32_t c1 = (t1 < E && n1 == r1 + m1) ? 1u : n1 == u1 + 1 ? 2u : 3u;
+        const uint32_t b0 = __ballot_sync(0xffffffffu, c0 & 1u), b1 = __ballot_sync(0xffffffffu, c0 & 2u);
+        const uint32_t b2 = __ballot_sync(0xffffffffu, c1 & 1u), b3 = __ballot_sync(0xffffffffu, c1 & 2u);
+        if (l == 0) mv[x] = make_uint4(b0, b1, b2, b3);
+        r0 = n0;
+        r1 = n1;
+    }
+    const int32_t dist = __shfl_sync(0xffffffffu, (int32_t)d < 32 ? r0 : r1, (int32_t)d & 31);
+    __syncwarp();
+    if (l != 0) return;
+    AlignSink s{A.ops + i * A.stride, A.stride};
+    bool bad = dist != (int32_t)d;
+    uint32_t x = 0, t = p, cost = 0;
+    while (x < Q.m && !bad) {
+        const int32_t j = (int32_t)(t - p) - (int32_t)x + (int32_t)d;
+        if (j < 0 || j >= W) { bad = true; break; }
+        const uint4 r = mv[x];
+        const uint32_t lo = j < 32 ? r.x : r.z, hi = j < 32 ? r.y : r.w, b = (uint32_t)j & 31u;
+        const uint32_t c = (lo >> b & 1u) | (hi >> b & 1u) << 1;
+        if (c == 1u) {
+            const bool eq = Q.match(__ldg(A.text + t), Q.at(x));
+            cost += !eq;
+            s.push(eq ? ALIGN_EQ : ALIGN_X);
+            x++;
+            t++;
+        } else if (c == 2u) {
+            cost++;
+            s.push(ALIGN_I);
+            x++;
+        } else {
+            cost++;
+            s.push(ALIGN_D);
+            t++;
+        }
+    }
+    s.flush();
+    A.cnt[i] = s.n;
+    if (bad || cost != d || t > E || s.n > A.stride) atomicOr(A.err, 1u);
+}
+
+// Hit i's cnt[i] words at its first entry seg[i]: d_pos gets p, d_mis the word with B200SA_APPROX_MINUS from the
+// hit's distance.
+__global__ void __launch_bounds__(BLK) k_align_emit(const uint32_t *__restrict__ hpos,
+                                                    const uint32_t *__restrict__ hmis, uint64_t htotal,
+                                                    const unsigned long long *__restrict__ seg,
+                                                    const uint32_t *__restrict__ cnt,
+                                                    const uint32_t *__restrict__ ops, uint32_t stride,
+                                                    uint32_t *pos, uint32_t *mis) {
+    const uint64_t i = (uint64_t)blockIdx.x * BLK + threadIdx.x;
+    if (i >= htotal) return;
+    const uint64_t o = seg[i];
+    const uint32_t p = hpos[i], minus = hmis[i] & B200SA_APPROX_MINUS, c = cnt[i];
+    for (uint32_t j = 0; j < c; j++) {
+        pos[o + j] = p;
+        mis[o + j] = ops[i * stride + j] | minus;
+    }
+}
+
+// *mmax = the longest of the nq queries (atomicMax).
+__global__ void __launch_bounds__(BLK) k_align_mmax(const uint64_t *__restrict__ qoff, uint32_t nq, uint32_t *mmax) {
+    const uint64_t q = (uint64_t)blockIdx.x * BLK + threadIdx.x;
+    if (q < nq) atomicMax(mmax, (uint32_t)(qoff[q + 1] - qoff[q]));
+}
+
+}  // namespace b200sa

@@ -41,6 +41,7 @@
 #include "iupac.cuh"
 #include "strand.cuh"
 #include "approx_docs.cuh"
+#include "align.cuh"
 #include "nccl_dyn.h"
 
 using namespace b200sa;
@@ -90,6 +91,7 @@ struct b200sa_ctx {
     DevBuf icode;                              // approx positions with B200SA_APPROX_IUPAC: the canonical queries
     DevBuf strand, sstage;                     // with B200SA_APPROX_BOTH_STRANDS: the doubled batch, the staged hits
     DevBuf adoff, adocs;                       // with B200SA_APPROX_DOCUMENTS: the hit offsets, the staged hits
+    DevBuf aops;                               // with B200SA_APPROX_ALIGN: each hit's operations
     uint32_t cls_calls = 0;
     // multi-GPU (SURVEY 8e): communicator owned or attached, NCCL resolved at run time
     ncclComm_t comm = nullptr;
@@ -1294,7 +1296,7 @@ void b200sa_ctx_destroy(b200sa_ctx *c) {
     DevBuf *bufs[] = {&c->text, &c->sa, &c->lcp, &c->pred, &c->stype, &c->lmsb, &c->lmsrank, &c->lmspos, &c->lmslist,
                       &c->lmspred, &c->sorted, &c->flag, &c->reduced, &c->sa_r, &c->blkstate, &c->carry, &c->tables,
                       &c->small, &c->scan_partial, &c->radix_cnt, &c->blkcnt, &c->k32b, &c->k64a, &c->k64b, &c->v0,
-                      &c->v1, &c->p0, &c->p1, &c->g0, &c->g1, &c->rank, &c->isa, &c->qbuf, &c->os_hist, &c->os_status, &c->packed, &c->phik, &c->phiv, &c->runscr, &c->plcp_samp, &c->scan_state, &c->cls_state, &c->lmsdesc, &c->steplog, &c->hist_copies, &c->tree_out, &c->docs_starts, &c->docs_out, &c->icode, &c->strand, &c->sstage, &c->adoff, &c->adocs, &c->sh_a, &c->sh_b, &c->sh_c, &c->sh_d, &c->sh_e, &c->sh_f, &c->sh_small};
+                      &c->v1, &c->p0, &c->p1, &c->g0, &c->g1, &c->rank, &c->isa, &c->qbuf, &c->os_hist, &c->os_status, &c->packed, &c->phik, &c->phiv, &c->runscr, &c->plcp_samp, &c->scan_state, &c->cls_state, &c->lmsdesc, &c->steplog, &c->hist_copies, &c->tree_out, &c->docs_starts, &c->docs_out, &c->icode, &c->strand, &c->sstage, &c->adoff, &c->adocs, &c->aops, &c->sh_a, &c->sh_b, &c->sh_c, &c->sh_d, &c->sh_e, &c->sh_f, &c->sh_small};
     for (DevBuf *b : bufs) if (b->p) cudaFree(b->p);
     for (cudaEvent_t e : c->event_pool) cudaEventDestroy(e);
     if (c->h_pin) cudaFreeHost(c->h_pin);
@@ -2890,7 +2892,7 @@ int b200sa_unbwt_dev(b200sa_ctx *c, uint64_t n, uint32_t ndocs, const uint8_t *d
     return leave(c, unbwt_core(c, (uint32_t)n, ndocs, d_bwt, d_term_rows, d_text_out, d_doc_starts_out));
 }
 
-// ------------------------------------------------------------ approximate positions (DESIGN 6b f-14 .. f-19)
+// ------------------------------------------------------------ approximate positions (DESIGN 6b f-14 .. f-20)
 // The checks of a call (nq >= 1, k its threshold): q_off on the device with q_off[nq] read back as *q_bytes,
 // doc_starts (d_starts non-null for documents), and the sizes.  Phase approx_check.
 static int approx_prep(b200sa_ctx *c, uint32_t n, const uint32_t *d_starts, uint32_t ndocs, const uint8_t *d_queries,
@@ -3119,10 +3121,80 @@ static int adocs_reduce(b200sa_ctx *c, const uint32_t *d_starts, uint32_t ndocs,
     return B200SA_OK;
 }
 
+// B200SA_APPROX_ALIGN: the longest of the nq queries into *mmax, and the query-length limits.  Phase approx_check.
+static int align_check(b200sa_ctx *c, const uint64_t *d_q_off, uint32_t nq, bool edit, uint32_t *mmax) {
+    uint32_t *words = ptr<uint32_t>(c->small);           // [24] the longest query
+    CU_TRY(c, cudaMemsetAsync(words + 24, 0, 4, c->stream));
+    LAUNCH(c, k_align_mmax, cdiv((uint64_t)nq, BLK), d_q_off, nq, words + 24);
+    TRY(read_words(c, words + 24, 1));
+    *mmax = c->h_pin[0];
+    if (*mmax > (1u << 27) - 1)
+        return fail(c, B200SA_ERR_TOO_LARGE,
+                    "approx positions: with B200SA_APPROX_ALIGN, a query longer than 2^27 - 1 bytes");
+    if (edit && *mmax > B200SA_APPROX_ALIGN_MAX_M)
+        return fail(c, B200SA_ERR_TOO_LARGE,
+                    "approx positions: with B200SA_APPROX_ALIGN and B200SA_APPROX_EDIT, a query longer than "
+                    "B200SA_APPROX_ALIGN_MAX_M bytes");
+    return B200SA_OK;
+}
+
+// B200SA_APPROX_ALIGN: the staged final lists (*total hits at offsets hoff, from adocs_stage) aligned into the
+// caller's offsets and, when the listing fits cap, d_pos and d_mis; *total becomes the number of operations.  qs:
+// the queries (the canonical copy with iupac), k the threshold, mmax the longest query.  Phases align_count,
+// align_scan and align_emit.
+static int align_list(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const uint32_t *d_starts, uint32_t ndocs,
+                      const uint8_t *qs, const uint64_t *d_q_off, uint32_t nq, uint32_t k, bool edit, bool iupac,
+                      uint32_t mmax, const uint64_t *hoff, uint64_t *d_offsets, uint32_t *d_pos, uint32_t *d_mis,
+                      uint64_t cap, uint64_t *total) {
+    typedef unsigned long long u64;
+    const uint64_t htotal = *total;
+    TRY(mark(c, "align_count"));
+    if (htotal == 0) {
+        CU_TRY(c, cudaMemsetAsync(d_offsets, 0, ((size_t)nq + 1) * 8, c->stream));
+        return B200SA_OK;
+    }
+    u64 *seg = ptr<u64>(c->adocs);
+    uint32_t *hpos = reinterpret_cast<uint32_t *>(seg + htotal + 1), *hmis = hpos + htotal, *cnt = hmis + htotal;
+    uint32_t *words = ptr<uint32_t>(c->small);           // [20, 22) the number of operations, [22] the error word
+    const uint32_t stride = 2 * k + 1;
+    TRY(ensure(c, c->aops, (size_t)htotal * stride * 4));
+    CU_TRY(c, cudaMemsetAsync(words + 22, 0, 4, c->stream));
+    const AlignArgs A{d_text, d_starts, ndocs, n, qs, d_q_off, nq, (const u64 *)hoff, hpos, hmis, htotal, iupac,
+                      stride, ptr<uint32_t>(c->aops), cnt, words + 22};
+    if (edit) {
+        // 16 bytes of choices per query row and warp: as many warps per block (up to 8) as fit 48 KB, at least one
+        const size_t per_warp = (size_t)max(mmax, 1u) * 16;
+        const uint32_t aw = (uint32_t)std::max<size_t>(1, std::min<size_t>(NWARP, 49152 / per_warp));
+        const size_t smem = per_warp * aw;
+        if (smem > 49152)
+            CU_TRY(c, cudaFuncSetAttribute(k_align_edit, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        k_align_edit<<<(uint32_t)cdiv(htotal, aw), aw * 32, smem, c->stream>>>(A, max(mmax, 1u));
+        c->launches++;
+    } else {
+        LAUNCH(c, k_align_hamming, cdiv(htotal, BLK), A);
+    }
+    TRY(mark(c, "align_scan"));
+    TRY((dev_scan<OpSum64>(c, InCount64{cnt, htotal}, OutStoreExcl64{seg}, htotal + 1,
+                           reinterpret_cast<u64 *>(words + 20))));
+    LAUNCH(c, k_adocs_offsets, cdiv((uint64_t)nq + 1, BLK), (const u64 *)hoff, (const u64 *)seg, nq,
+           reinterpret_cast<u64 *>(d_offsets));
+    TRY(read_words(c, words + 20, 3));
+    if (c->h_pin[2])
+        return fail(c, B200SA_ERR_INTERNAL, "approx positions: with B200SA_APPROX_ALIGN, an alignment's cost differs "
+                                            "from its hit's distance");
+    *total = pin_u64(c, 0);
+    if (*total > cap) return B200SA_OK;
+    TRY(mark(c, "align_emit"));
+    LAUNCH(c, k_align_emit, cdiv(htotal, BLK), (const uint32_t *)hpos, (const uint32_t *)hmis, htotal,
+           (const u64 *)seg, (const uint32_t *)cnt, (const uint32_t *)ptr<uint32_t>(c->aops), stride, d_pos, d_mis);
+    return B200SA_OK;
+}
+
 // nq >= 1, k = threshold | flags as approx_args accepts it, without B200SA_APPROX_BEST.  With
 // B200SA_APPROX_BOTH_STRANDS the search runs on the doubled batch and k_strand_merge replaces k_approx_gather.
 // With B200SA_APPROX_DOCUMENTS the search always emits, the final list lands in staging with its offsets in
-// c->adoff, and adocs_reduce writes the caller's arrays.
+// c->adoff, and adocs_reduce writes the caller's arrays; with B200SA_APPROX_ALIGN the same staging feeds
+// align_list instead.
 template <class EndF>
 static int approx_core(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const uint32_t *d_sa,
                        const uint32_t *d_starts, uint32_t ndocs, const uint8_t *d_queries, const uint64_t *d_q_off,
@@ -3133,12 +3205,15 @@ static int approx_core(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const u
     uint64_t q_bytes;
     TRY(approx_prep(c, n, d_starts, ndocs, d_queries, d_q_off, nq, k, &q_bytes));
     const bool iupac = (kf & B200SA_APPROX_IUPAC) != 0, both = (kf & B200SA_APPROX_BOTH_STRANDS) != 0,
-               docs = (kf & B200SA_APPROX_DOCUMENTS) != 0;
+               docs = (kf & B200SA_APPROX_DOCUMENTS) != 0, align = (kf & B200SA_APPROX_ALIGN) != 0,
+               edit = (kf & B200SA_APPROX_EDIT) != 0, stage = docs || align;
     if (both) TRY(strand_check(c, q_bytes, nq, k));
+    uint32_t mmax = 0;
+    if (align) TRY(align_check(c, d_q_off, nq, edit, &mmax));
     if (iupac) TRY(iupac_canon(c, d_queries, q_bytes, &d_queries));
     if (n == 0) return approx_nothing(c, d_offsets, nq);
     uint64_t *hoff = d_offsets;                          // the final list's offsets
-    if (docs) TRY(adocs_offsets(c, nq, &hoff));
+    if (stage) TRY(adocs_offsets(c, nq, &hoff));
     const uint8_t *eq = d_queries;
     const uint64_t *eoff = d_q_off;
     uint64_t *soff = hoff;
@@ -3146,18 +3221,21 @@ static int approx_core(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const u
     uint64_t *ko = nullptr;
     uint32_t *vo = nullptr;
     int pbits = 0;
-    const uint64_t scap = docs ? ~0ull : cap;            // with B200SA_APPROX_DOCUMENTS every hit is staged
-    TRY(approx_search(c, d_text, n, d_sa, d_starts, ndocs, eq, eoff, both ? 2 * nq : nq, k,
-                      (kf & B200SA_APPROX_EDIT) != 0, iupac, soff, scap, total, end, &ko, &vo, &pbits));
+    const uint64_t scap = stage ? ~0ull : cap;           // with B200SA_APPROX_DOCUMENTS or _ALIGN every hit is staged
+    TRY(approx_search(c, d_text, n, d_sa, d_starts, ndocs, eq, eoff, both ? 2 * nq : nq, k, edit, iupac, soff, scap,
+                      total, end, &ko, &vo, &pbits));
     const bool emitted = *total > 0 && *total <= scap;
     uint32_t *fpos = d_pos, *fmis = d_mis;               // where the final list lands
-    if (docs && emitted) TRY(adocs_stage(c, *total, &fpos, &fmis));
+    if (stage && emitted) TRY(adocs_stage(c, *total, &fpos, &fmis));
     if (both)
         TRY(strand_merge(c, StrandKeys{(const u64 *)ko, pbits}, vo, *total, emitted, soff, nq, hoff, fpos, fmis));
     else if (emitted)
         LAUNCH(c, k_approx_gather, cdiv(*total, BLK), (const u64 *)ko, (const uint32_t *)vo, *total,
                (u64)((1ull << pbits) - 1), fpos, fmis);
     if (docs) TRY(adocs_reduce(c, d_starts, ndocs, nq, hoff, d_offsets, d_pos, d_mis, cap, total));
+    if (align)
+        TRY(align_list(c, d_text, n, d_starts, ndocs, d_queries, d_q_off, nq, k, edit, iupac, mmax, hoff, d_offsets,
+                       d_pos, d_mis, cap, total));
     TRY(mark(c, "end"));
     CU_TRY(c, cudaGetLastError());
     CU_TRY(c, cudaStreamSynchronize(c->stream));
@@ -3194,7 +3272,8 @@ static int best_batch(b200sa_ctx *c, const uint8_t *d_queries, const uint64_t *d
 // Phases: approx_check; strand_queries with the flag; per round best_compact, the search's phases, best_update;
 // per emitted group best_compact, the search's phases, best_scatter; strand_merge with the flag.
 // With B200SA_APPROX_DOCUMENTS the groups are always emitted, the final list lands in staging with its offsets in
-// c->adoff, and adocs_reduce (phases adocs_mark, adocs_emit) writes the caller's arrays.
+// c->adoff, and adocs_reduce (phases adocs_mark, adocs_emit) writes the caller's arrays; with B200SA_APPROX_ALIGN
+// align_list (phases align_count, align_scan, align_emit) does.
 template <class EndF>
 static int approx_best_core(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const uint32_t *d_sa,
                             const uint32_t *d_starts, uint32_t ndocs, const uint8_t *d_queries,
@@ -3203,15 +3282,18 @@ static int approx_best_core(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, co
     typedef unsigned long long u64;
     const uint32_t k = kf & 0xFFu, s = (kf >> 8) & 0xFFu;
     const bool edit = (kf & B200SA_APPROX_EDIT) != 0, iupac = (kf & B200SA_APPROX_IUPAC) != 0,
-               both = (kf & B200SA_APPROX_BOTH_STRANDS) != 0, docs = (kf & B200SA_APPROX_DOCUMENTS) != 0;
+               both = (kf & B200SA_APPROX_BOTH_STRANDS) != 0, docs = (kf & B200SA_APPROX_DOCUMENTS) != 0,
+               align = (kf & B200SA_APPROX_ALIGN) != 0, stage = docs || align;
     uint64_t q_bytes;
     c->stats.doubling_rounds = 0;
     TRY(approx_prep(c, n, d_starts, ndocs, d_queries, d_q_off, nq, k, &q_bytes));
     if (both) TRY(strand_check(c, q_bytes, nq, k));
+    uint32_t mmax = 0;
+    if (align) TRY(align_check(c, d_q_off, nq, edit, &mmax));
     if (iupac) TRY(iupac_canon(c, d_queries, q_bytes, &d_queries));
     if (n == 0) return approx_nothing(c, d_offsets, nq);
     uint64_t *hoff = d_offsets;                          // the final list's offsets
-    if (docs) TRY(adocs_offsets(c, nq, &hoff));
+    if (stage) TRY(adocs_offsets(c, nq, &hoff));
     const uint8_t *eq = d_queries;                       // the entries: the queries, or the doubled batch
     const uint64_t *eoff = d_q_off;
     uint64_t *eo = hoff;                                 // the entries' output offsets
@@ -3258,10 +3340,10 @@ static int approx_best_core(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, co
     TRY(read_words(c, words + 10, 4));
     const uint32_t ended = c->h_pin[0];
     *total = pin_u64(c, 2);
-    const uint64_t scap = docs ? ~0ull : cap;            // with B200SA_APPROX_DOCUMENTS every hit is staged
+    const uint64_t scap = stage ? ~0ull : cap;           // with B200SA_APPROX_DOCUMENTS or _ALIGN every hit is staged
     const bool emitted = *total > 0 && *total <= scap;
     uint32_t *fpos = d_pos, *fmis = d_mis;               // where the final list lands
-    if (docs && emitted) TRY(adocs_stage(c, *total, &fpos, &fmis));
+    if (stage && emitted) TRY(adocs_stage(c, *total, &fpos, &fmis));
     uint32_t *gpos = fpos, *gmis = fmis;                 // where the groups scatter
     if (both && emitted) {
         TRY(ensure(c, c->sstage, (size_t)*total * 8));
@@ -3282,6 +3364,9 @@ static int approx_best_core(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, co
     }
     if (both) TRY(strand_merge(c, StrandStaged{gpos}, gmis, *total, emitted, eo, nq, hoff, fpos, fmis));
     if (docs) TRY(adocs_reduce(c, d_starts, ndocs, nq, hoff, d_offsets, d_pos, d_mis, cap, total));
+    if (align)
+        TRY(align_list(c, d_text, n, d_starts, ndocs, d_queries, d_q_off, nq, k, edit, iupac, mmax, hoff, d_offsets,
+                       d_pos, d_mis, cap, total));
     TRY(mark(c, "end"));
     CU_TRY(c, cudaGetLastError());
     CU_TRY(c, cudaStreamSynchronize(c->stream));
@@ -3293,7 +3378,7 @@ static int approx_args(b200sa_ctx *c, uint64_t n, const void *text, const void *
                        bool docs = false) {
     if (!c) return B200SA_ERR_BAD_ARG;
     if (!total || !offsets || (nq > 0 && !q_off) || (cap > 0 && !pos) || (n > 0 && (!text || !sa))) return null_ptr(c);
-    const uint32_t listing = docs ? B200SA_APPROX_DOCUMENTS : 0u;    // accepted by the documents entry alone
+    const uint32_t listing = docs ? B200SA_APPROX_DOCUMENTS | B200SA_APPROX_ALIGN : 0u;  // documents entry alone
     if (k & B200SA_APPROX_BEST) {
         if (k & ~(0xFFFFu | B200SA_APPROX_EDIT | B200SA_APPROX_BEST | B200SA_APPROX_IUPAC |
                   B200SA_APPROX_BOTH_STRANDS | listing) ||
@@ -3303,7 +3388,7 @@ static int approx_args(b200sa_ctx *c, uint64_t n, const void *text, const void *
                         docs ? "approx positions: with B200SA_APPROX_BEST, k must be a threshold up to "
                                "B200SA_APPROX_MAX_K | B200SA_APPROX_SLACK(s) with s up to B200SA_APPROX_MAX_K, "
                                "optionally | B200SA_APPROX_EDIT, | B200SA_APPROX_IUPAC, | B200SA_APPROX_BOTH_STRANDS "
-                               "and | B200SA_APPROX_DOCUMENTS"
+                               "and | B200SA_APPROX_DOCUMENTS, or | B200SA_APPROX_ALIGN"
                              : "approx positions: with B200SA_APPROX_BEST, k must be a threshold up to "
                                "B200SA_APPROX_MAX_K | B200SA_APPROX_SLACK(s) with s up to B200SA_APPROX_MAX_K, "
                                "optionally | B200SA_APPROX_EDIT, | B200SA_APPROX_IUPAC and | "
@@ -3313,7 +3398,7 @@ static int approx_args(b200sa_ctx *c, uint64_t n, const void *text, const void *
             return fail(c, B200SA_ERR_BAD_ARG,
                         docs ? "approx positions: k must be a threshold up to B200SA_APPROX_MAX_K, optionally | "
                                "B200SA_APPROX_EDIT, | B200SA_APPROX_IUPAC, | B200SA_APPROX_BOTH_STRANDS and | "
-                               "B200SA_APPROX_DOCUMENTS"
+                               "B200SA_APPROX_DOCUMENTS, or | B200SA_APPROX_ALIGN"
                              : "approx positions: k must be a threshold up to B200SA_APPROX_MAX_K, optionally | "
                                "B200SA_APPROX_EDIT, | B200SA_APPROX_IUPAC and | B200SA_APPROX_BOTH_STRANDS");
         if ((k & 0xFFFFu) > B200SA_APPROX_MAX_K)
@@ -3344,6 +3429,12 @@ int b200sa_docs_approx_positions_dev(b200sa_ctx *c, const uint8_t *d_text, uint6
                                      uint32_t *d_pos, uint32_t *d_mismatches, uint64_t cap, uint64_t *total,
                                      void *stream) {
     TRY(approx_args(c, n, d_text, d_gsa, d_q_off, nq, k, d_offsets, d_pos, cap, total, true));
+    if ((k & B200SA_APPROX_ALIGN) && (k & B200SA_APPROX_DOCUMENTS))
+        return fail(c, B200SA_ERR_BAD_ARG,
+                    "approx positions: B200SA_APPROX_ALIGN and B200SA_APPROX_DOCUMENTS do not combine");
+    if ((k & B200SA_APPROX_ALIGN) && cap > 0 && !d_mismatches)
+        return fail(c, B200SA_ERR_BAD_ARG,
+                    "approx positions: with B200SA_APPROX_ALIGN, d_mismatches is required when cap > 0");
     if ((n > 0 || ndocs > 0) && !d_doc_starts) return null_ptr(c);
     if (ndocs == 0 && n > 0) return no_docs(c);
     TRY(enter(c, stream));

@@ -279,7 +279,7 @@ class SuffixTable:
         from . import _bwt
         return _bwt.bwt_runs(self)
 
-    # ---- approximate positions (DESIGN 6b f-14 .. f-18)
+    # ---- approximate positions (DESIGN 6b f-14 .. f-18, f-20)
     def approximate_positions(self, query, k, *, metric="hamming", best=None, iupac=False, strands="forward"):
         """(positions u32[], mismatches u32[]): every p with p + m <= n where text[p:p + m] differs from
         the query (m bytes) in at most k bytes, 0 <= k <= 31, by ascending p, with that number of
@@ -323,6 +323,28 @@ class SuffixTable:
         (best= and iupac= as in approximate_positions); strands="both" counts the hits of both strands."""
         from . import _approx
         return _approx.counts(self, queries, k, metric, best, iupac, strands)
+
+    def approximate_alignments(self, query, k, *, metric="hamming", best=None, iupac=False, strands="forward"):
+        """(positions u32[], distances u32[], ends u32[], cigar_offsets u64[h + 1], cigar u32[]): the hits of
+        approximate_positions, in its order, each with its alignment (B200SA_APPROX_ALIGN on
+        b200sa_docs_approx_positions_dev, the text as one document, computed on the device).  Hit i aligns the query to text[positions[i]:ends[i]]; its operations are
+        cigar[cigar_offsets[i]:cigar_offsets[i + 1]], BAM words len << 4 | code (I 1, D 2, = 7, X 8), in text
+        order; suffix_b200.cigar_string turns them into "12=1X7=".  With metric="edit" the alignment is the
+        canonical walk of include/b200sa.h, which prefers a substitution or match, then an insertion, then a
+        deletion; the query must then be at most 4096 bytes (B200SA_APPROX_ALIGN_MAX_M).  distances and ends are
+        read off the operations.  strands="both" returns (positions, distances, minus, ends, cigar_offsets,
+        cigar), and a minus hit's operations align the reverse complement, as SAM does.  Keywords are checked as
+        in approximate_positions."""
+        from . import _approx
+        return _approx.alignments(self, query, k, metric, best, iupac, strands)
+
+    def approximate_alignments_batch(self, queries, k, *, metric="hamming", best=None, iupac=False,
+                                     strands="forward"):
+        """(offsets u64[nq + 1], positions, distances, ends, cigar_offsets, cigar): query q's hits are
+        [offsets[q], offsets[q + 1]) of positions, distances and ends, as approximate_alignments returns them;
+        one count call, then one fetch call sized by it.  strands="both" puts minus after distances."""
+        from . import _approx
+        return _approx.alignments_batch(self, queries, k, metric, best, iupac, strands)
 
     # ---- persistence (SURVEY 8f-2): the only "wire format" the reference API implies is
     # from_parts/into_parts (src/table.rs:111-127): text bytes + little-endian u32 table.

@@ -212,6 +212,19 @@ for k, docs in enumerate(doc_sets + [[b"", b"AC", b"", b"G"], [b"A"] * 50 + [b""
                     off, ds, dist = res[:3]
                     assert len(ds) == int(off[-1]) and (dist <= kk).all() and (ds < len(docs)).all(), (k, kk, sl)
                     assert (tab.approximate_document_frequencies(qs, kk, **kw) == np.diff(off.astype(np.int64))).all()
+# alignments of the hits: the staged hit lists of every mix, the Hamming and edit count kernels (one warp per hit,
+# its move choices in shared memory), the scan, the offsets and the emission, and the count call alone; a single
+# text goes through the documents entry
+for k, docs in enumerate(doc_sets + [[b"", b"AC", b"", b"G"], [b"A"] * 50 + [b""]]):
+    for tab in (DocumentSuffixTable(docs),) + ((SuffixTable(docs[0]),) if len(docs) == 1 else ()):
+        for kk, sl in ((0, None), (3, None), (31, None), (3, 0), (3, 1)):
+            for metric in ("hamming", "edit"):
+                for iu, qs in ((False, ap_qs + [b"GAATTC", b"a" * 9]), (True, iu_qs)):
+                    for strands in ("forward", "both"):
+                        res = tab.approximate_alignments_batch(qs, kk, metric=metric, best=sl, iupac=iu,
+                                                               strands=strands)
+                        off, pos, dist = res[:3]
+                        assert len(pos) == int(off[-1]) and (dist <= kk).all() and res[-2][-1] == len(res[-1]), k
 # refinement branches (tests/test_gpu_refine.py): a local-sort overflow in round 2 of the direct path, the direct
 # path's probe (2^20 tied after round 1, large groups), 64-bit round-0 keys of the reduced string
 import ctypes
