@@ -2893,6 +2893,24 @@ int b200sa_unbwt_dev(b200sa_ctx *c, uint64_t n, uint32_t ndocs, const uint8_t *d
 }
 
 // ------------------------------------------------------------ approximate positions (DESIGN 6b f-14 .. f-20)
+// The k of a call as approx_args decodes it: the threshold, B200SA_APPROX_BEST's slack, and the flags.
+struct ApproxFlags {
+    uint32_t k, s;
+    bool edit, best, iupac, both, docs, align;
+    bool stage;                                          // docs || align: the final lists go to staging
+};
+
+// The words of c->small through which the approximate search hands results from its kernels to the host; a u64
+// takes two words, low word first.  [0] the range flag of DListChunks, [2, 4) the search's items, [4, 6) its total
+// (the search clears [0, 6)); [8, 10) (batch size << 32) | batch bytes of best_batch, [10] the rounds where a query
+// ended, [12, 14) the best rounds' total (the rounds clear [8, 14)); [16, 18) the least (offset << 8) | byte that
+// iupac_canon rejects; [20, 22) the number of listed documents or alignment operations, [22] align_list's error
+// word; [24] the longest query.
+enum ApproxWord : uint32_t {
+    AW_FLAG = 0, AW_ITEMS = 2, AW_TOTAL = 4, AW_BATCH = 8, AW_ENDED = 10, AW_BEST_TOTAL = 12, AW_IUPAC_BAD = 16,
+    AW_LISTED = 20, AW_ALIGN_ERR = 22, AW_MMAX = 24
+};
+
 // The checks of a call (nq >= 1, k its threshold): q_off on the device with q_off[nq] read back as *q_bytes,
 // doc_starts (d_starts non-null for documents), and the sizes.  Phase approx_check.
 static int approx_prep(b200sa_ctx *c, uint32_t n, const uint32_t *d_starts, uint32_t ndocs, const uint8_t *d_queries,
@@ -2923,14 +2941,14 @@ static int approx_nothing(b200sa_ctx *c, uint64_t *d_offsets, uint32_t nq) {
 // first byte that is not an IUPAC letter.  Phase approx_check.
 static int iupac_canon(b200sa_ctx *c, const uint8_t *d_queries, uint64_t q_bytes, const uint8_t **out) {
     typedef unsigned long long u64;
-    uint32_t *words = ptr<uint32_t>(c->small);           // [16, 18) the least (offset << 8) | byte rejected
+    uint32_t *words = ptr<uint32_t>(c->small);
     TRY(ensure(c, c->icode, (size_t)q_bytes));
-    CU_TRY(c, cudaMemsetAsync(words + 16, 0xFF, 8, c->stream));
+    CU_TRY(c, cudaMemsetAsync(words + AW_IUPAC_BAD, 0xFF, 8, c->stream));
     if (q_bytes > 0)
         LAUNCH(c, k_iupac_code, cdiv(q_bytes, BLK), d_queries, q_bytes, ptr<uint8_t>(c->icode),
-               reinterpret_cast<u64 *>(words + 16));
+               reinterpret_cast<u64 *>(words + AW_IUPAC_BAD));
     CU_TRY(c, cudaGetLastError());
-    TRY(read_words(c, words + 16, 2));
+    TRY(read_words(c, words + AW_IUPAC_BAD, 2));
     const uint64_t bad = pin_u64(c, 0);
     if (bad != ~0ull) {
         char m[200];
@@ -2944,6 +2962,14 @@ static int iupac_canon(b200sa_ctx *c, const uint8_t *d_queries, uint64_t q_bytes
     return B200SA_OK;
 }
 
+// The count (EMIT false) or emit pass of the search for the metric and the query alphabet.
+typedef void (*ApproxKernel)(ApproxArgs, uint32_t *, const unsigned long long *, int, unsigned long long *, uint32_t *);
+template <bool EMIT>
+static ApproxKernel approx_kernel(bool edit, bool iupac) {
+    if (iupac) return edit ? k_approx_edit_iupac<EMIT> : k_approx_iupac<EMIT>;
+    return edit ? k_approx_edit<EMIT> : k_approx<EMIT>;
+}
+
 // One search of nq >= 1 queries at threshold k on n >= 1 bytes: d_offsets (nq + 1) and *total, read back.  When
 // 0 < total <= cap it also emits and sorts: *ko / *vo then hold the keys (q << *pbits) | p in (q, p) order and
 // their distances.  Phases: approx_pieces, approx_scan, approx_count, and approx_emit, approx_sort when it
@@ -2955,7 +2981,7 @@ static int approx_search(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const
                          uint32_t nq, uint32_t k, bool edit, bool iupac, uint64_t *d_offsets, uint64_t cap,
                          uint64_t *total, EndF end, uint64_t **ko, uint32_t **vo, int *pbits_out) {
     typedef unsigned long long u64;
-    uint32_t *words = ptr<uint32_t>(c->small);           // [0] check bits, [2, 4) items, [4, 6) total
+    uint32_t *words = ptr<uint32_t>(c->small);
     const uint32_t P = k + 1;
     const uint64_t nslots = (uint64_t)nq * P;
     TRY(mark(c, "approx_pieces"));
@@ -2968,13 +2994,13 @@ static int approx_search(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const
         LAUNCH(c, (k_approx_pieces<EndF>), cdiv(nslots, BLK), d_text, n, d_sa, d_queries, d_q_off, nq, P, ps, pe, end);
     }
     TRY(mark(c, "approx_scan"));
-    CU_TRY(c, cudaMemsetAsync(words, 0, 24, c->stream));
+    CU_TRY(c, cudaMemsetAsync(words + AW_FLAG, 0, (AW_TOTAL + 2 - AW_FLAG) * 4, c->stream));
     TRY(ensure(c, c->k64a, ((size_t)nslots + 1) * 8));
-    u64 *item_start = ptr<u64>(c->k64a), *d_items = reinterpret_cast<u64 *>(words + 2),
-        *d_total = reinterpret_cast<u64 *>(words + 4);
-    TRY((dev_scan<OpSum64>(c, DListChunks{ps, pe, (uint32_t)nslots, n, words}, OutStoreExcl64{item_start},
+    u64 *item_start = ptr<u64>(c->k64a), *d_items = reinterpret_cast<u64 *>(words + AW_ITEMS),
+        *d_total = reinterpret_cast<u64 *>(words + AW_TOTAL);
+    TRY((dev_scan<OpSum64>(c, DListChunks{ps, pe, (uint32_t)nslots, n, words + AW_FLAG}, OutStoreExcl64{item_start},
                            nslots + 1, d_items)));
-    TRY(read_words(c, words + 2, 2));
+    TRY(read_words(c, words + AW_ITEMS, 2));
     const uint64_t items = pin_u64(c, 0);
     if (items > (uint64_t)0x7fffffff * NWARP)
         return fail(c, B200SA_ERR_TOO_LARGE, "approx positions: more than 2^31 * 8 chunks of 1024 candidates in one batch");
@@ -2986,22 +3012,13 @@ static int approx_search(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const
     const ApproxArgs A{d_text, d_sa, d_starts, ndocs, n, d_queries, d_q_off, (uint32_t)nslots, P, k, ps, pe,
                        item_start, items};
     const int pbits = bit_length(n - 1);
-    if (items && iupac && edit)
-        LAUNCH(c, k_approx_edit_iupac<false>, cdiv(items, NWARP), A, cnt, (const u64 *)nullptr, pbits, (u64 *)nullptr,
-               (uint32_t *)nullptr);
-    else if (items && iupac)
-        LAUNCH(c, k_approx_iupac<false>, cdiv(items, NWARP), A, cnt, (const u64 *)nullptr, pbits, (u64 *)nullptr,
-               (uint32_t *)nullptr);
-    else if (items && edit)
-        LAUNCH(c, k_approx_edit<false>, cdiv(items, NWARP), A, cnt, (const u64 *)nullptr, pbits, (u64 *)nullptr,
-               (uint32_t *)nullptr);
-    else if (items)
-        LAUNCH(c, k_approx<false>, cdiv(items, NWARP), A, cnt, (const u64 *)nullptr, pbits, (u64 *)nullptr,
-               (uint32_t *)nullptr);
+    if (items)
+        LAUNCH(c, approx_kernel<false>(edit, iupac), cdiv(items, NWARP), A, cnt, (const u64 *)nullptr, pbits,
+               (u64 *)nullptr, (uint32_t *)nullptr);
     TRY((dev_scan<OpSum64>(c, InCount64{cnt, items}, OutStoreExcl64{item_off}, items + 1, d_total)));
     LAUNCH(c, k_approx_qoff, cdiv((uint64_t)nq + 1, BLK), item_start, item_off, nq, P,
            reinterpret_cast<u64 *>(d_offsets));
-    TRY(read_words(c, words + 4, 2));
+    TRY(read_words(c, words + AW_TOTAL, 2));
     *total = pin_u64(c, 0);
     *pbits_out = pbits;
     if (*total > 0 && *total <= cap) {
@@ -3010,18 +3027,8 @@ static int approx_search(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const
         TRY(ensure(c, c->g1, (size_t)*total * 8));
         TRY(ensure(c, c->v0, (size_t)*total * 4));
         TRY(ensure(c, c->v1, (size_t)*total * 4));
-        if (iupac && edit)
-            LAUNCH(c, k_approx_edit_iupac<true>, cdiv(items, NWARP), A, cnt, (const u64 *)item_off, pbits,
-                   ptr<u64>(c->g0), ptr<uint32_t>(c->v0));
-        else if (iupac)
-            LAUNCH(c, k_approx_iupac<true>, cdiv(items, NWARP), A, cnt, (const u64 *)item_off, pbits, ptr<u64>(c->g0),
-                   ptr<uint32_t>(c->v0));
-        else if (edit)
-            LAUNCH(c, k_approx_edit<true>, cdiv(items, NWARP), A, cnt, (const u64 *)item_off, pbits, ptr<u64>(c->g0),
-                   ptr<uint32_t>(c->v0));
-        else
-            LAUNCH(c, k_approx<true>, cdiv(items, NWARP), A, cnt, (const u64 *)item_off, pbits, ptr<u64>(c->g0),
-                   ptr<uint32_t>(c->v0));
+        LAUNCH(c, approx_kernel<true>(edit, iupac), cdiv(items, NWARP), A, cnt, (const u64 *)item_off, pbits,
+               ptr<u64>(c->g0), ptr<uint32_t>(c->v0));
         TRY(mark(c, "approx_sort"));                     // by (q, p)
         TRY(sort_pairs<uint64_t>(c, ptr<uint64_t>(c->g0), ptr<uint32_t>(c->v0), ptr<uint64_t>(c->g1),
                                  ptr<uint32_t>(c->v1), *total, bit_length(nq - 1) + pbits, ko, vo));
@@ -3104,13 +3111,13 @@ static int adocs_reduce(b200sa_ctx *c, const uint32_t *d_starts, uint32_t ndocs,
     u64 *seg = ptr<u64>(c->adocs);
     const uint32_t *hpos = reinterpret_cast<const uint32_t *>(seg + htotal + 1), *hmis = hpos + htotal;
     uint32_t *marks = reinterpret_cast<uint32_t *>(seg + htotal + 1) + 2 * htotal;
-    uint32_t *words = ptr<uint32_t>(c->small);           // [20, 22) the number of listed documents
+    uint32_t *words = ptr<uint32_t>(c->small);
     LAUNCH(c, k_adocs_mark, cdiv(htotal, BLK), hpos, htotal, (const u64 *)hoff, nq, d_starts, ndocs, marks);
     TRY((dev_scan<OpSum64>(c, InCount64{marks, htotal}, OutStoreExcl64{seg}, htotal + 1,
-                           reinterpret_cast<u64 *>(words + 20))));
+                           reinterpret_cast<u64 *>(words + AW_LISTED))));
     LAUNCH(c, k_adocs_offsets, cdiv((uint64_t)nq + 1, BLK), (const u64 *)hoff, (const u64 *)seg, nq,
            reinterpret_cast<u64 *>(d_offsets));
-    TRY(read_words(c, words + 20, 2));
+    TRY(read_words(c, words + AW_LISTED, 2));
     *total = pin_u64(c, 0);
     if (*total > cap) return B200SA_OK;
     TRY(mark(c, "adocs_emit"));
@@ -3123,10 +3130,10 @@ static int adocs_reduce(b200sa_ctx *c, const uint32_t *d_starts, uint32_t ndocs,
 
 // B200SA_APPROX_ALIGN: the longest of the nq queries into *mmax, and the query-length limits.  Phase approx_check.
 static int align_check(b200sa_ctx *c, const uint64_t *d_q_off, uint32_t nq, bool edit, uint32_t *mmax) {
-    uint32_t *words = ptr<uint32_t>(c->small);           // [24] the longest query
-    CU_TRY(c, cudaMemsetAsync(words + 24, 0, 4, c->stream));
-    LAUNCH(c, k_align_mmax, cdiv((uint64_t)nq, BLK), d_q_off, nq, words + 24);
-    TRY(read_words(c, words + 24, 1));
+    uint32_t *words = ptr<uint32_t>(c->small);
+    CU_TRY(c, cudaMemsetAsync(words + AW_MMAX, 0, 4, c->stream));
+    LAUNCH(c, k_align_mmax, cdiv((uint64_t)nq, BLK), d_q_off, nq, words + AW_MMAX);
+    TRY(read_words(c, words + AW_MMAX, 1));
     *mmax = c->h_pin[0];
     if (*mmax > (1u << 27) - 1)
         return fail(c, B200SA_ERR_TOO_LARGE,
@@ -3155,12 +3162,12 @@ static int align_list(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const ui
     }
     u64 *seg = ptr<u64>(c->adocs);
     uint32_t *hpos = reinterpret_cast<uint32_t *>(seg + htotal + 1), *hmis = hpos + htotal, *cnt = hmis + htotal;
-    uint32_t *words = ptr<uint32_t>(c->small);           // [20, 22) the number of operations, [22] the error word
+    uint32_t *words = ptr<uint32_t>(c->small);
     const uint32_t stride = 2 * k + 1;
     TRY(ensure(c, c->aops, (size_t)htotal * stride * 4));
-    CU_TRY(c, cudaMemsetAsync(words + 22, 0, 4, c->stream));
+    CU_TRY(c, cudaMemsetAsync(words + AW_ALIGN_ERR, 0, 4, c->stream));
     const AlignArgs A{d_text, d_starts, ndocs, n, qs, d_q_off, nq, (const u64 *)hoff, hpos, hmis, htotal, iupac,
-                      stride, ptr<uint32_t>(c->aops), cnt, words + 22};
+                      stride, ptr<uint32_t>(c->aops), cnt, words + AW_ALIGN_ERR};
     if (edit) {
         // 16 bytes of choices per query row and warp: as many warps per block (up to 8) as fit 48 KB, at least one
         const size_t per_warp = (size_t)max(mmax, 1u) * 16;
@@ -3175,11 +3182,11 @@ static int align_list(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const ui
     }
     TRY(mark(c, "align_scan"));
     TRY((dev_scan<OpSum64>(c, InCount64{cnt, htotal}, OutStoreExcl64{seg}, htotal + 1,
-                           reinterpret_cast<u64 *>(words + 20))));
+                           reinterpret_cast<u64 *>(words + AW_LISTED))));
     LAUNCH(c, k_adocs_offsets, cdiv((uint64_t)nq + 1, BLK), (const u64 *)hoff, (const u64 *)seg, nq,
            reinterpret_cast<u64 *>(d_offsets));
-    TRY(read_words(c, words + 20, 3));
-    if (c->h_pin[2])
+    TRY(read_words(c, words + AW_LISTED, AW_ALIGN_ERR + 1 - AW_LISTED));
+    if (c->h_pin[AW_ALIGN_ERR - AW_LISTED])
         return fail(c, B200SA_ERR_INTERNAL, "approx positions: with B200SA_APPROX_ALIGN, an alignment's cost differs "
                                             "from its hit's distance");
     *total = pin_u64(c, 0);
@@ -3190,58 +3197,6 @@ static int align_list(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const ui
     return B200SA_OK;
 }
 
-// nq >= 1, k = threshold | flags as approx_args accepts it, without B200SA_APPROX_BEST.  With
-// B200SA_APPROX_BOTH_STRANDS the search runs on the doubled batch and k_strand_merge replaces k_approx_gather.
-// With B200SA_APPROX_DOCUMENTS the search always emits, the final list lands in staging with its offsets in
-// c->adoff, and adocs_reduce writes the caller's arrays; with B200SA_APPROX_ALIGN the same staging feeds
-// align_list instead.
-template <class EndF>
-static int approx_core(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const uint32_t *d_sa,
-                       const uint32_t *d_starts, uint32_t ndocs, const uint8_t *d_queries, const uint64_t *d_q_off,
-                       uint32_t nq, uint32_t kf, uint64_t *d_offsets, uint32_t *d_pos, uint32_t *d_mis, uint64_t cap,
-                       uint64_t *total, EndF end) {
-    typedef unsigned long long u64;
-    const uint32_t k = kf & 0xFFFFu;
-    uint64_t q_bytes;
-    TRY(approx_prep(c, n, d_starts, ndocs, d_queries, d_q_off, nq, k, &q_bytes));
-    const bool iupac = (kf & B200SA_APPROX_IUPAC) != 0, both = (kf & B200SA_APPROX_BOTH_STRANDS) != 0,
-               docs = (kf & B200SA_APPROX_DOCUMENTS) != 0, align = (kf & B200SA_APPROX_ALIGN) != 0,
-               edit = (kf & B200SA_APPROX_EDIT) != 0, stage = docs || align;
-    if (both) TRY(strand_check(c, q_bytes, nq, k));
-    uint32_t mmax = 0;
-    if (align) TRY(align_check(c, d_q_off, nq, edit, &mmax));
-    if (iupac) TRY(iupac_canon(c, d_queries, q_bytes, &d_queries));
-    if (n == 0) return approx_nothing(c, d_offsets, nq);
-    uint64_t *hoff = d_offsets;                          // the final list's offsets
-    if (stage) TRY(adocs_offsets(c, nq, &hoff));
-    const uint8_t *eq = d_queries;
-    const uint64_t *eoff = d_q_off;
-    uint64_t *soff = hoff;
-    if (both) TRY(strand_queries(c, d_queries, d_q_off, nq, q_bytes, iupac, &eq, &eoff, &soff));
-    uint64_t *ko = nullptr;
-    uint32_t *vo = nullptr;
-    int pbits = 0;
-    const uint64_t scap = stage ? ~0ull : cap;           // with B200SA_APPROX_DOCUMENTS or _ALIGN every hit is staged
-    TRY(approx_search(c, d_text, n, d_sa, d_starts, ndocs, eq, eoff, both ? 2 * nq : nq, k, edit, iupac, soff, scap,
-                      total, end, &ko, &vo, &pbits));
-    const bool emitted = *total > 0 && *total <= scap;
-    uint32_t *fpos = d_pos, *fmis = d_mis;               // where the final list lands
-    if (stage && emitted) TRY(adocs_stage(c, *total, &fpos, &fmis));
-    if (both)
-        TRY(strand_merge(c, StrandKeys{(const u64 *)ko, pbits}, vo, *total, emitted, soff, nq, hoff, fpos, fmis));
-    else if (emitted)
-        LAUNCH(c, k_approx_gather, cdiv(*total, BLK), (const u64 *)ko, (const uint32_t *)vo, *total,
-               (u64)((1ull << pbits) - 1), fpos, fmis);
-    if (docs) TRY(adocs_reduce(c, d_starts, ndocs, nq, hoff, d_offsets, d_pos, d_mis, cap, total));
-    if (align)
-        TRY(align_list(c, d_text, n, d_starts, ndocs, d_queries, d_q_off, nq, k, edit, iupac, mmax, hoff, d_offsets,
-                       d_pos, d_mis, cap, total));
-    TRY(mark(c, "end"));
-    CU_TRY(c, cudaGetLastError());
-    CU_TRY(c, cudaStreamSynchronize(c->stream));
-    return B200SA_OK;
-}
-
 // The batch a BestPick selects: *nb queries, map[i] the query of entry i; their bytes and offsets at *bq / *boff,
 // the call's own arrays when every query is picked, else gathered into c->qbuf and coff.  Pick: BestPick, or
 // StrandPick over the entries of the doubled batch.
@@ -3249,9 +3204,10 @@ template <class Pick>
 static int best_batch(b200sa_ctx *c, const uint8_t *d_queries, const uint64_t *d_q_off, uint32_t nq, Pick pick,
                       uint32_t *map, uint64_t *coff, uint32_t *nb, const uint8_t **bq, const uint64_t **boff) {
     typedef unsigned long long u64;
-    uint32_t *words = ptr<uint32_t>(c->small);           // [8, 10) (batch size << 32) | batch bytes
-    TRY((dev_scan<OpSum64>(c, pick, BestPickOut{nq, map, coff}, (uint64_t)nq + 1, reinterpret_cast<u64 *>(words + 8))));
-    TRY(read_words(c, words + 8, 2));
+    uint32_t *words = ptr<uint32_t>(c->small);
+    TRY((dev_scan<OpSum64>(c, pick, BestPickOut{nq, map, coff}, (uint64_t)nq + 1,
+                           reinterpret_cast<u64 *>(words + AW_BATCH))));
+    TRY(read_words(c, words + AW_BATCH, 2));
     *nb = (uint32_t)(pin_u64(c, 0) >> 32);
     *bq = d_queries;
     *boff = d_q_off;
@@ -3263,89 +3219,97 @@ static int best_batch(b200sa_ctx *c, const uint8_t *d_queries, const uint64_t *d
     return B200SA_OK;
 }
 
-// nq >= 1, k = threshold | B200SA_APPROX_SLACK(s) | B200SA_APPROX_BEST, optionally | B200SA_APPROX_EDIT,
-// | B200SA_APPROX_IUPAC (the batches are then gathered from the canonical copy) and | B200SA_APPROX_BOTH_STRANDS.
-// Rounds t = 0 .. threshold over the live queries (best.cuh), then one emission per distinct final threshold.
-// With B200SA_APPROX_BOTH_STRANDS the entries are those of the doubled batch, a query and its reverse complement
-// are live as a pair with one best (strand.cuh), the groups scatter into c->sstage over the doubled offsets and
-// one k_strand_merge writes the caller's arrays.
-// Phases: approx_check; strand_queries with the flag; per round best_compact, the search's phases, best_update;
-// per emitted group best_compact, the search's phases, best_scatter; strand_merge with the flag.
-// With B200SA_APPROX_DOCUMENTS the groups are always emitted, the final list lands in staging with its offsets in
-// c->adoff, and adocs_reduce (phases adocs_mark, adocs_emit) writes the caller's arrays; with B200SA_APPROX_ALIGN
-// align_list (phases align_count, align_scan, align_emit) does.
+// The ne entries the search runs on: the queries, or with B200SA_APPROX_BOTH_STRANDS the doubled batch of
+// strand_queries; q their bytes, off their offsets, out the offsets of their lists.
+struct ApproxEntries { const uint8_t *q; const uint64_t *off; uint64_t *out; uint32_t ne; };
+
+// Where the final lists land: their offsets off, positions pos and distances mis, written when 0 < total <= cap.
+// The caller's arrays and cap, or with B200SA_APPROX_DOCUMENTS or _ALIGN the offsets in c->adoff and every hit, even
+// at cap = 0, in the staging of adocs_stage.
+struct ApproxFinal { uint64_t *off; uint32_t *pos, *mis; uint64_t cap; };
+
+// Without B200SA_APPROX_BEST: one search of the entries at the threshold, whose sorted keys k_approx_gather, or with
+// B200SA_APPROX_BOTH_STRANDS k_strand_merge, writes as the final lists.  Phases: the search's; strand_merge with
+// both strands.
 template <class EndF>
-static int approx_best_core(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const uint32_t *d_sa,
-                            const uint32_t *d_starts, uint32_t ndocs, const uint8_t *d_queries,
-                            const uint64_t *d_q_off, uint32_t nq, uint32_t kf, uint64_t *d_offsets, uint32_t *d_pos,
-                            uint32_t *d_mis, uint64_t cap, uint64_t *total, EndF end) {
+static int approx_plain(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const uint32_t *d_sa,
+                        const uint32_t *d_starts, uint32_t ndocs, EndF end, const ApproxFlags &f,
+                        const ApproxEntries &e, uint32_t nq, ApproxFinal fin, uint64_t *total) {
     typedef unsigned long long u64;
-    const uint32_t k = kf & 0xFFu, s = (kf >> 8) & 0xFFu;
-    const bool edit = (kf & B200SA_APPROX_EDIT) != 0, iupac = (kf & B200SA_APPROX_IUPAC) != 0,
-               both = (kf & B200SA_APPROX_BOTH_STRANDS) != 0, docs = (kf & B200SA_APPROX_DOCUMENTS) != 0,
-               align = (kf & B200SA_APPROX_ALIGN) != 0, stage = docs || align;
-    uint64_t q_bytes;
-    c->stats.doubling_rounds = 0;
-    TRY(approx_prep(c, n, d_starts, ndocs, d_queries, d_q_off, nq, k, &q_bytes));
-    if (both) TRY(strand_check(c, q_bytes, nq, k));
-    uint32_t mmax = 0;
-    if (align) TRY(align_check(c, d_q_off, nq, edit, &mmax));
-    if (iupac) TRY(iupac_canon(c, d_queries, q_bytes, &d_queries));
-    if (n == 0) return approx_nothing(c, d_offsets, nq);
-    uint64_t *hoff = d_offsets;                          // the final list's offsets
-    if (stage) TRY(adocs_offsets(c, nq, &hoff));
-    const uint8_t *eq = d_queries;                       // the entries: the queries, or the doubled batch
-    const uint64_t *eoff = d_q_off;
-    uint64_t *eo = hoff;                                 // the entries' output offsets
-    if (both) TRY(strand_queries(c, d_queries, d_q_off, nq, q_bytes, iupac, &eq, &eoff, &eo));
-    const uint32_t ne = both ? 2 * nq : nq;
+    uint64_t *ko = nullptr;
+    uint32_t *vo = nullptr;
+    int pbits = 0;
+    TRY(approx_search(c, d_text, n, d_sa, d_starts, ndocs, e.q, e.off, e.ne, f.k, f.edit, f.iupac, e.out, fin.cap,
+                      total, end, &ko, &vo, &pbits));
+    const bool emitted = *total > 0 && *total <= fin.cap;
+    if (f.stage && emitted) TRY(adocs_stage(c, *total, &fin.pos, &fin.mis));
+    if (f.both)
+        TRY(strand_merge(c, StrandKeys{(const u64 *)ko, pbits}, vo, *total, emitted, e.out, nq, fin.off, fin.pos,
+                         fin.mis));
+    else if (emitted)
+        LAUNCH(c, k_approx_gather, cdiv(*total, BLK), (const u64 *)ko, (const uint32_t *)vo, *total,
+               (u64)((1ull << pbits) - 1), fin.pos, fin.mis);
+    return B200SA_OK;
+}
+
+// B200SA_APPROX_BEST: rounds t = 0 .. threshold over the live queries (best.cuh), then one emission per distinct
+// final threshold, whose groups k_best_scatter moves to their entries' lists.  With B200SA_APPROX_BOTH_STRANDS a
+// query and its reverse complement are live as a pair with one best (strand.cuh), the groups scatter into
+// c->sstage and one k_strand_merge writes the final lists.  The batches are gathered from e.q, the IUPAC canonical
+// copy with that flag.  Phases: per round best_compact, the search's, best_update; per emitted group best_compact,
+// the search's, best_scatter; strand_merge with both strands.
+template <class EndF>
+static int approx_best(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const uint32_t *d_sa,
+                       const uint32_t *d_starts, uint32_t ndocs, EndF end, const ApproxFlags &f,
+                       const ApproxEntries &e, uint32_t nq, uint64_t q_bytes, ApproxFinal fin, uint64_t *total) {
+    typedef unsigned long long u64;
+    const uint32_t ne = e.ne, k = f.k, s = f.s;
     TRY(ensure(c, c->k32b, (size_t)ne * 8 + nq));        // cnt, map (u32) per entry, best (u8) per query
     TRY(ensure(c, c->rank, ((size_t)ne + 1) * 16));      // the batch's q_off, the search's offsets
-    TRY(ensure(c, c->qbuf, (size_t)q_bytes * (both ? 2 : 1)));
+    TRY(ensure(c, c->qbuf, (size_t)q_bytes * (f.both ? 2 : 1)));
     uint32_t *cnt = ptr<uint32_t>(c->k32b), *map = cnt + ne;
     uint8_t *best = reinterpret_cast<uint8_t *>(map + ne);
     uint64_t *coff = ptr<uint64_t>(c->rank), *soff = coff + ne + 1;
-    uint32_t *words = ptr<uint32_t>(c->small);           // [10] rounds where a query ended, [12, 14) total
+    uint32_t *words = ptr<uint32_t>(c->small);
     CU_TRY(c, cudaMemsetAsync(cnt, 0, (size_t)ne * 4, c->stream));
     CU_TRY(c, cudaMemsetAsync(best, BEST_NONE, nq, c->stream));
-    CU_TRY(c, cudaMemsetAsync(words + 8, 0, 24, c->stream));
+    CU_TRY(c, cudaMemsetAsync(words + AW_BATCH, 0, (AW_BEST_TOTAL + 2 - AW_BATCH) * 4, c->stream));
     uint64_t *ko = nullptr, rtotal = 0;
     uint32_t *vo = nullptr, nb = 0, rounds = 0;
     int pbits = 0;
     const uint8_t *bq;
     const uint64_t *boff;
     auto batch = [&](uint32_t t, bool group) {
-        if (both) return best_batch(c, eq, eoff, ne, StrandPick{eoff, best, ne, t, s, k, group}, map, coff, &nb, &bq,
-                                    &boff);
-        return best_batch(c, eq, eoff, ne, BestPick{eoff, best, ne, t, s, k, group}, map, coff, &nb, &bq, &boff);
+        if (f.both)
+            return best_batch(c, e.q, e.off, ne, StrandPick{e.off, best, ne, t, s, k, group}, map, coff, &nb, &bq,
+                              &boff);
+        return best_batch(c, e.q, e.off, ne, BestPick{e.off, best, ne, t, s, k, group}, map, coff, &nb, &bq, &boff);
     };
     for (uint32_t t = 0; t <= k; t++) {
         TRY(mark(c, "best_compact"));
         TRY(batch(t, false));
         if (nb == 0) break;
         rounds++;
-        TRY(approx_search(c, d_text, n, d_sa, d_starts, ndocs, bq, boff, nb, t, edit, iupac, soff, 0, &rtotal, end, &ko, &vo,
-                          &pbits));
+        TRY(approx_search(c, d_text, n, d_sa, d_starts, ndocs, bq, boff, nb, t, f.edit, f.iupac, soff, 0, &rtotal, end,
+                          &ko, &vo, &pbits));
         TRY(mark(c, "best_update"));
-        if (both)
+        if (f.both)
             LAUNCH(c, k_strand_update, cdiv(nb / 2, BLK), (const uint32_t *)map, (const u64 *)soff, nb, t, s, k, best,
-                   cnt, words + 10);
+                   cnt, words + AW_ENDED);
         else
             LAUNCH(c, k_best_update, cdiv(nb, BLK), (const uint32_t *)map, (const u64 *)soff, nb, t, s, k, best, cnt,
-                   words + 10);
+                   words + AW_ENDED);
     }
     c->stats.doubling_rounds = rounds;
-    TRY((dev_scan<OpSum64>(c, InCount64{cnt, ne}, OutStoreExcl64{reinterpret_cast<u64 *>(eo)}, (uint64_t)ne + 1,
-                           reinterpret_cast<u64 *>(words + 12))));
-    TRY(read_words(c, words + 10, 4));
+    TRY((dev_scan<OpSum64>(c, InCount64{cnt, ne}, OutStoreExcl64{reinterpret_cast<u64 *>(e.out)}, (uint64_t)ne + 1,
+                           reinterpret_cast<u64 *>(words + AW_BEST_TOTAL))));
+    TRY(read_words(c, words + AW_ENDED, AW_BEST_TOTAL + 2 - AW_ENDED));
     const uint32_t ended = c->h_pin[0];
-    *total = pin_u64(c, 2);
-    const uint64_t scap = stage ? ~0ull : cap;           // with B200SA_APPROX_DOCUMENTS or _ALIGN every hit is staged
-    const bool emitted = *total > 0 && *total <= scap;
-    uint32_t *fpos = d_pos, *fmis = d_mis;               // where the final list lands
-    if (stage && emitted) TRY(adocs_stage(c, *total, &fpos, &fmis));
-    uint32_t *gpos = fpos, *gmis = fmis;                 // where the groups scatter
-    if (both && emitted) {
+    *total = pin_u64(c, AW_BEST_TOTAL - AW_ENDED);
+    const bool emitted = *total > 0 && *total <= fin.cap;
+    if (f.stage && emitted) TRY(adocs_stage(c, *total, &fin.pos, &fin.mis));
+    uint32_t *gpos = fin.pos, *gmis = fin.mis;           // where the groups scatter
+    if (f.both && emitted) {
         TRY(ensure(c, c->sstage, (size_t)*total * 8));
         gpos = ptr<uint32_t>(c->sstage);
         gmis = gpos + *total;
@@ -3355,56 +3319,86 @@ static int approx_best_core(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, co
             if (!(ended >> t & 1u)) continue;
             TRY(mark(c, "best_compact"));
             TRY(batch(t, true));
-            TRY(approx_search(c, d_text, n, d_sa, d_starts, ndocs, bq, boff, nb, t, edit, iupac, soff, ~0ull, &rtotal, end,
-                              &ko, &vo, &pbits));
+            TRY(approx_search(c, d_text, n, d_sa, d_starts, ndocs, bq, boff, nb, t, f.edit, f.iupac, soff, ~0ull,
+                              &rtotal, end, &ko, &vo, &pbits));
             TRY(mark(c, "best_scatter"));
             LAUNCH(c, k_best_scatter, cdiv(rtotal, BLK), (const u64 *)ko, (const uint32_t *)vo, rtotal, pbits,
-                   (const u64 *)soff, (const uint32_t *)map, (const u64 *)eo, gpos, gmis);
+                   (const u64 *)soff, (const uint32_t *)map, (const u64 *)e.out, gpos, gmis);
         }
     }
-    if (both) TRY(strand_merge(c, StrandStaged{gpos}, gmis, *total, emitted, eo, nq, hoff, fpos, fmis));
-    if (docs) TRY(adocs_reduce(c, d_starts, ndocs, nq, hoff, d_offsets, d_pos, d_mis, cap, total));
-    if (align)
-        TRY(align_list(c, d_text, n, d_starts, ndocs, d_queries, d_q_off, nq, k, edit, iupac, mmax, hoff, d_offsets,
-                       d_pos, d_mis, cap, total));
+    if (f.both) TRY(strand_merge(c, StrandStaged{gpos}, gmis, *total, emitted, e.out, nq, fin.off, fin.pos, fin.mis));
+    return B200SA_OK;
+}
+
+// nq >= 1 queries as f asks.  The checks; the IUPAC canonical copy, which every later kernel reads; with
+// B200SA_APPROX_BOTH_STRANDS the doubled batch; then approx_plain or approx_best writes each query's final list.
+// With B200SA_APPROX_DOCUMENTS that list is staged and adocs_reduce writes the caller's arrays; with
+// B200SA_APPROX_ALIGN align_list does.  `doubling_rounds` is set only with B200SA_APPROX_BEST.
+// Phases: approx_check; strand_queries with both strands; the middle's; adocs_mark, adocs_emit with
+// B200SA_APPROX_DOCUMENTS or align_count, align_scan, align_emit with B200SA_APPROX_ALIGN.
+template <class EndF>
+static int approx_run(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const uint32_t *d_sa,
+                      const uint32_t *d_starts, uint32_t ndocs, const uint8_t *d_queries, const uint64_t *d_q_off,
+                      uint32_t nq, const ApproxFlags &f, uint64_t *d_offsets, uint32_t *d_pos, uint32_t *d_mis,
+                      uint64_t cap, uint64_t *total, EndF end) {
+    if (f.best) c->stats.doubling_rounds = 0;
+    uint64_t q_bytes;
+    TRY(approx_prep(c, n, d_starts, ndocs, d_queries, d_q_off, nq, f.k, &q_bytes));
+    if (f.both) TRY(strand_check(c, q_bytes, nq, f.k));
+    uint32_t mmax = 0;
+    if (f.align) TRY(align_check(c, d_q_off, nq, f.edit, &mmax));
+    if (f.iupac) TRY(iupac_canon(c, d_queries, q_bytes, &d_queries));
+    if (n == 0) return approx_nothing(c, d_offsets, nq);
+    ApproxFinal fin{d_offsets, d_pos, d_mis, f.stage ? ~0ull : cap};
+    if (f.stage) TRY(adocs_offsets(c, nq, &fin.off));
+    ApproxEntries e{d_queries, d_q_off, fin.off, nq};
+    if (f.both) {
+        TRY(strand_queries(c, d_queries, d_q_off, nq, q_bytes, f.iupac, &e.q, &e.off, &e.out));
+        e.ne = 2 * nq;
+    }
+    if (f.best)
+        TRY(approx_best(c, d_text, n, d_sa, d_starts, ndocs, end, f, e, nq, q_bytes, fin, total));
+    else
+        TRY(approx_plain(c, d_text, n, d_sa, d_starts, ndocs, end, f, e, nq, fin, total));
+    if (f.docs) TRY(adocs_reduce(c, d_starts, ndocs, nq, fin.off, d_offsets, d_pos, d_mis, cap, total));
+    if (f.align)
+        TRY(align_list(c, d_text, n, d_starts, ndocs, d_queries, d_q_off, nq, f.k, f.edit, f.iupac, mmax, fin.off,
+                       d_offsets, d_pos, d_mis, cap, total));
     TRY(mark(c, "end"));
     CU_TRY(c, cudaGetLastError());
     CU_TRY(c, cudaStreamSynchronize(c->stream));
     return B200SA_OK;
 }
 
+// The argument checks shared by both entry points, and k decoded into *f.  docs: the documents entry, the only one
+// that takes B200SA_APPROX_DOCUMENTS and B200SA_APPROX_ALIGN.
 static int approx_args(b200sa_ctx *c, uint64_t n, const void *text, const void *sa, const void *q_off, uint32_t nq,
-                       uint32_t k, const void *offsets, const void *pos, uint64_t cap, const void *total,
-                       bool docs = false) {
+                       uint32_t k, const void *offsets, const void *pos, uint64_t cap, const void *total, bool docs,
+                       ApproxFlags *f) {
     if (!c) return B200SA_ERR_BAD_ARG;
     if (!total || !offsets || (nq > 0 && !q_off) || (cap > 0 && !pos) || (n > 0 && (!text || !sa))) return null_ptr(c);
-    const uint32_t listing = docs ? B200SA_APPROX_DOCUMENTS | B200SA_APPROX_ALIGN : 0u;  // documents entry alone
-    if (k & B200SA_APPROX_BEST) {
-        if (k & ~(0xFFFFu | B200SA_APPROX_EDIT | B200SA_APPROX_BEST | B200SA_APPROX_IUPAC |
-                  B200SA_APPROX_BOTH_STRANDS | listing) ||
-            (k & 0xFFu) > B200SA_APPROX_MAX_K ||
-            ((k >> 8) & 0xFFu) > B200SA_APPROX_MAX_K)
-            return fail(c, B200SA_ERR_BAD_ARG,
-                        docs ? "approx positions: with B200SA_APPROX_BEST, k must be a threshold up to "
-                               "B200SA_APPROX_MAX_K | B200SA_APPROX_SLACK(s) with s up to B200SA_APPROX_MAX_K, "
-                               "optionally | B200SA_APPROX_EDIT, | B200SA_APPROX_IUPAC, | B200SA_APPROX_BOTH_STRANDS "
-                               "and | B200SA_APPROX_DOCUMENTS, or | B200SA_APPROX_ALIGN"
-                             : "approx positions: with B200SA_APPROX_BEST, k must be a threshold up to "
-                               "B200SA_APPROX_MAX_K | B200SA_APPROX_SLACK(s) with s up to B200SA_APPROX_MAX_K, "
-                               "optionally | B200SA_APPROX_EDIT, | B200SA_APPROX_IUPAC and | "
-                               "B200SA_APPROX_BOTH_STRANDS");
-    } else {
-        if (k & ~(0xFFFFu | B200SA_APPROX_EDIT | B200SA_APPROX_IUPAC | B200SA_APPROX_BOTH_STRANDS | listing))
-            return fail(c, B200SA_ERR_BAD_ARG,
-                        docs ? "approx positions: k must be a threshold up to B200SA_APPROX_MAX_K, optionally | "
-                               "B200SA_APPROX_EDIT, | B200SA_APPROX_IUPAC, | B200SA_APPROX_BOTH_STRANDS and | "
-                               "B200SA_APPROX_DOCUMENTS, or | B200SA_APPROX_ALIGN"
-                             : "approx positions: k must be a threshold up to B200SA_APPROX_MAX_K, optionally | "
-                               "B200SA_APPROX_EDIT, | B200SA_APPROX_IUPAC and | B200SA_APPROX_BOTH_STRANDS");
-        if ((k & 0xFFFFu) > B200SA_APPROX_MAX_K)
-            return fail(c, B200SA_ERR_BAD_ARG, "approx positions: k above B200SA_APPROX_MAX_K");
+    const bool best = (k & B200SA_APPROX_BEST) != 0;
+    const uint32_t accepted = 0xFFFFu | B200SA_APPROX_EDIT | B200SA_APPROX_IUPAC | B200SA_APPROX_BOTH_STRANDS |
+                              (best ? B200SA_APPROX_BEST : 0u) |
+                              (docs ? B200SA_APPROX_DOCUMENTS | B200SA_APPROX_ALIGN : 0u);
+    // with B200SA_APPROX_BEST the threshold and the slack are a byte each, and either above the limit is a bad k
+    if ((k & ~accepted) || (best && ((k & 0xFFu) > B200SA_APPROX_MAX_K || ((k >> 8) & 0xFFu) > B200SA_APPROX_MAX_K))) {
+        const std::string m =
+            std::string("approx positions: ") + (best ? "with B200SA_APPROX_BEST, " : "") +
+            "k must be a threshold up to B200SA_APPROX_MAX_K" +
+            (best ? " | B200SA_APPROX_SLACK(s) with s up to B200SA_APPROX_MAX_K" : "") +
+            ", optionally | B200SA_APPROX_EDIT, | B200SA_APPROX_IUPAC" +
+            (docs ? ", | B200SA_APPROX_BOTH_STRANDS and | B200SA_APPROX_DOCUMENTS, or | B200SA_APPROX_ALIGN"
+                  : " and | B200SA_APPROX_BOTH_STRANDS");
+        return fail(c, B200SA_ERR_BAD_ARG, m.c_str());
     }
+    if (!best && (k & 0xFFFFu) > B200SA_APPROX_MAX_K)
+        return fail(c, B200SA_ERR_BAD_ARG, "approx positions: k above B200SA_APPROX_MAX_K");
     if (n > B200SA_MAX_N) return too_long(c);
+    const bool listing = (k & B200SA_APPROX_DOCUMENTS) != 0, align = (k & B200SA_APPROX_ALIGN) != 0;
+    *f = ApproxFlags{best ? k & 0xFFu : k & 0xFFFFu, best ? (k >> 8) & 0xFFu : 0u, (k & B200SA_APPROX_EDIT) != 0,
+                     best, (k & B200SA_APPROX_IUPAC) != 0, (k & B200SA_APPROX_BOTH_STRANDS) != 0, listing, align,
+                     listing || align};
     return B200SA_OK;
 }
 
@@ -3412,15 +3406,13 @@ int b200sa_approx_positions_dev(b200sa_ctx *c, const uint8_t *d_text, uint64_t n
                                 const uint8_t *d_queries, const uint64_t *d_q_off, uint32_t nq, uint32_t k,
                                 uint64_t *d_offsets, uint32_t *d_pos, uint32_t *d_mismatches, uint64_t cap,
                                 uint64_t *total, void *stream) {
-    TRY(approx_args(c, n, d_text, d_sa, d_q_off, nq, k, d_offsets, d_pos, cap, total));
+    ApproxFlags f;
+    TRY(approx_args(c, n, d_text, d_sa, d_q_off, nq, k, d_offsets, d_pos, cap, total, false, &f));
     TRY(enter(c, stream));
     *total = 0;
     if (nq == 0) return leave(c, empty_batch(c, d_offsets));
-    if (k & B200SA_APPROX_BEST)
-        return leave(c, approx_best_core(c, d_text, (uint32_t)n, d_sa, nullptr, 0, d_queries, d_q_off, nq, k, d_offsets,
-                                         d_pos, d_mismatches, cap, total, TextEnd{(uint32_t)n}));
-    return leave(c, approx_core(c, d_text, (uint32_t)n, d_sa, nullptr, 0, d_queries, d_q_off, nq, k, d_offsets, d_pos,
-                                d_mismatches, cap, total, TextEnd{(uint32_t)n}));
+    return leave(c, approx_run(c, d_text, (uint32_t)n, d_sa, nullptr, 0, d_queries, d_q_off, nq, f, d_offsets, d_pos,
+                               d_mismatches, cap, total, TextEnd{(uint32_t)n}));
 }
 
 int b200sa_docs_approx_positions_dev(b200sa_ctx *c, const uint8_t *d_text, uint64_t n, const uint32_t *d_gsa,
@@ -3428,11 +3420,12 @@ int b200sa_docs_approx_positions_dev(b200sa_ctx *c, const uint8_t *d_text, uint6
                                      const uint64_t *d_q_off, uint32_t nq, uint32_t k, uint64_t *d_offsets,
                                      uint32_t *d_pos, uint32_t *d_mismatches, uint64_t cap, uint64_t *total,
                                      void *stream) {
-    TRY(approx_args(c, n, d_text, d_gsa, d_q_off, nq, k, d_offsets, d_pos, cap, total, true));
-    if ((k & B200SA_APPROX_ALIGN) && (k & B200SA_APPROX_DOCUMENTS))
+    ApproxFlags f;
+    TRY(approx_args(c, n, d_text, d_gsa, d_q_off, nq, k, d_offsets, d_pos, cap, total, true, &f));
+    if (f.align && f.docs)
         return fail(c, B200SA_ERR_BAD_ARG,
                     "approx positions: B200SA_APPROX_ALIGN and B200SA_APPROX_DOCUMENTS do not combine");
-    if ((k & B200SA_APPROX_ALIGN) && cap > 0 && !d_mismatches)
+    if (f.align && cap > 0 && !d_mismatches)
         return fail(c, B200SA_ERR_BAD_ARG,
                     "approx positions: with B200SA_APPROX_ALIGN, d_mismatches is required when cap > 0");
     if ((n > 0 || ndocs > 0) && !d_doc_starts) return null_ptr(c);
@@ -3440,12 +3433,8 @@ int b200sa_docs_approx_positions_dev(b200sa_ctx *c, const uint8_t *d_text, uint6
     TRY(enter(c, stream));
     *total = 0;
     if (nq == 0) return leave(c, empty_batch(c, d_offsets));
-    if (k & B200SA_APPROX_BEST)
-        return leave(c, approx_best_core(c, d_text, (uint32_t)n, d_gsa, d_doc_starts, ndocs, d_queries, d_q_off, nq, k,
-                                         d_offsets, d_pos, d_mismatches, cap, total,
-                                         DocsEnd{d_doc_starts, ndocs, (uint32_t)n}));
-    return leave(c, approx_core(c, d_text, (uint32_t)n, d_gsa, d_doc_starts, ndocs, d_queries, d_q_off, nq, k, d_offsets,
-                                d_pos, d_mismatches, cap, total, DocsEnd{d_doc_starts, ndocs, (uint32_t)n}));
+    return leave(c, approx_run(c, d_text, (uint32_t)n, d_gsa, d_doc_starts, ndocs, d_queries, d_q_off, nq, f,
+                               d_offsets, d_pos, d_mismatches, cap, total, DocsEnd{d_doc_starts, ndocs, (uint32_t)n}));
 }
 
 // ------------------------------------------------------------ multi-GPU: communicator + sharded LMS sort
