@@ -10,9 +10,10 @@
 // that slot when the window [p, p + m) lies in s's document (the text), no piece i < j matches exactly
 // there and the pieces other than j add at most k mismatches.  The first exactly matching piece is thus the
 // one reporter of an occurrence: nothing is emitted twice and no de-duplication is needed.
-// Slot ranges are cut into chunks of 1024 ranks numbered by a u64 scan (DListChunks); one warp walks one
-// (slot, chunk) item, one rank per lane per step.  A count pass, a scan, then an emit pass of the same walk
-// that writes (q, p) keys in item order, sorted afterwards.
+// Slot ranges are cut into chunks of 1024 ranks numbered by a u64 scan (DListChunks), as the listing of
+// docs_list.cuh cuts its ranges; one warp walks one (slot, chunk) item (approx_item), one rank per lane per
+// step.  A count pass, a scan, k_dlist_qoff with a stride of P slots, then an emit pass of the same walk that
+// writes (q, p) keys in item order, sorted afterwards.
 #pragma once
 #include "docs_list.cuh"
 
@@ -58,94 +59,121 @@ struct ApproxArgs {
     uint64_t items;
 };
 
-// Whether the suffix at s, a candidate of piece j at offset oj of the query qq of m bytes, starts an
-// occurrence this slot reports; then *p_out = its position and *mis_out = its mismatches.  whole: m <= k.
-__device__ __forceinline__ bool approx_verify(const ApproxArgs &A, uint32_t s, const uint8_t *__restrict__ qq,
-                                              uint32_t m, uint32_t j, uint32_t oj, bool whole, uint32_t *p_out,
-                                              uint32_t *mis_out) {
-    if (s < oj) return false;
-    const uint32_t p = s - oj;
-    uint32_t ds = 0, de = A.n;
+// The (slot, chunk) item a warp walks: query q of m bytes at qq, its piece j at offset oj (0 in the whole-table
+// slot, whole) and the ranks [lo, hi) of the slot's range in the chunk.
+struct ApproxItem {
+    uint32_t q, j, m, oj;
+    bool whole;
+    const uint8_t *qq;
+    uint64_t lo, hi;
+};
+template <class Pieces>
+__device__ __forceinline__ ApproxItem approx_item(const ApproxArgs &A, uint64_t item) {
+    const DListItem it = dlist_item(A.item_start, A.nslots, A.ps, A.pe, item);
+    const uint32_t q = it.r / A.P, j = it.r % A.P;
+    const uint64_t qo = A.qoff[q];
+    const uint32_t m = (uint32_t)(A.qoff[q + 1] - qo);
+    const bool whole = Pieces::whole(A, it.r, m);
+    return {q, j, m, whole ? 0u : Pieces::off(A, it.r, m, j), whole, A.qs + qo, it.lo, it.hi};
+}
+
+// The document [*ds, *de) that holds position s, or the text [0, n)
+__device__ __forceinline__ void approx_doc(const ApproxArgs &A, uint32_t s, uint32_t *ds, uint32_t *de) {
+    *ds = 0;
+    *de = A.n;
     if (A.starts) {
         const uint32_t d = docs_find(A.starts, A.ndocs, s);
-        ds = __ldg(A.starts + d);
-        de = docs_end(A.starts, A.ndocs, A.n, d);
+        *ds = __ldg(A.starts + d);
+        *de = docs_end(A.starts, A.ndocs, A.n, d);
     }
-    if (p < ds || (uint64_t)p + m > de) return false;
-    const uint8_t *__restrict__ t = A.text + p;
-    uint32_t mis = 0;
-    if (whole) {
-        for (uint32_t x = 0; x < m; x++) mis += __ldg(t + x) != __ldg(qq + x);
-    } else {
-        // piece i = [a, b) with a = i*m/P, stepped by m/P and the remainder m%P
-        const uint32_t step = m / A.P, rem = m % A.P;
-        uint32_t a = 0, r = 0;
-        for (uint32_t i = 0; i < A.P; i++) {
-            uint32_t b = a + step;
-            r += rem;
-            if (r >= A.P) { b++; r -= A.P; }
-            if (i != j) {
-                uint32_t mi = 0;
-                for (uint32_t x = a; x < b && mis + mi <= A.k; x++) mi += __ldg(t + x) != __ldg(qq + x);
-                if (i < j && mi == 0) return false;          // slot i reports it
-                mis += mi;
-                if (mis > A.k) return false;
-            }
-            a = b;
-        }
-    }
-    *p_out = p;
-    *mis_out = mis;
+}
+
+// Whether the piece bytes pq[0, len) are the text's at t
+__device__ __forceinline__ bool approx_piece_at(const uint8_t *__restrict__ t, const uint8_t *__restrict__ pq,
+                                                uint32_t len) {
+    for (uint32_t y = 0; y < len; y++)
+        if (__ldg(t + y) != __ldg(pq + y)) return false;
     return true;
 }
 
-// f-14's pieces: piece j = [j*m/P, (j+1)*m/P), a whole-table slot for m <= k, and approx_verify.  The walks
-// of k_approx and k_approx_edit take the pieces as a policy, so that B200SA_APPROX_IUPAC (iupac.cuh) reuses them.
+// The pieces [a, b) of a query of m bytes in order, piece i = [i*m/P, (i+1)*m/P): next() steps to the following
+// piece by m/P and the remainder m%P, with no division per piece.
+struct CutStep {
+    uint32_t P, step, rem, a = 0, b = 0, r = 0;
+    __device__ __forceinline__ CutStep(uint32_t m, uint32_t P) : P(P), step(m / P), rem(m % P) {}
+    __device__ __forceinline__ void next() {
+        a = b;
+        b += step;
+        r += rem;
+        if (r >= P) { b++; r -= P; }
+    }
+};
+
+// The pieces of a query, as a policy of the walks of k_approx (verify) and k_approx_edit (CLASSES, whole_hits,
+// reports): f-14's pieces and byte equality here, the piece table and the class test (miss) of IupacPieces
+// (iupac.cuh).  whole(slot, m): whether the slot is the whole table; off: the offset of piece j.
 struct CutPieces {
-    __device__ __forceinline__ bool whole(const ApproxArgs &A, uint32_t, uint32_t m) const { return m <= A.k; }
-    __device__ __forceinline__ uint32_t off(const ApproxArgs &A, uint32_t, uint32_t m, uint32_t j) const {
+    static __device__ __forceinline__ bool whole(const ApproxArgs &A, uint32_t, uint32_t m) { return m <= A.k; }
+    static __device__ __forceinline__ uint32_t off(const ApproxArgs &A, uint32_t, uint32_t m, uint32_t j) {
         return approx_cut(m, A.P, j);
     }
-    __device__ __forceinline__ bool verify(const ApproxArgs &A, uint32_t s, const uint8_t *__restrict__ qq, uint32_t m,
-                                           uint32_t, uint32_t j, uint32_t oj, bool whole, uint32_t *p_out,
-                                           uint32_t *mis_out) const {
-        return approx_verify(A, s, qq, m, j, oj, whole, p_out, mis_out);
+    // Whether the suffix at s, a candidate of the item's slot, starts an occurrence this slot reports; then
+    // *p_out = its position and *mis_out = its mismatches.
+    static __device__ __forceinline__ bool verify(const ApproxArgs &A, const ApproxItem &w, uint32_t s,
+                                                  uint32_t *p_out, uint32_t *mis_out) {
+        if (s < w.oj) return false;
+        const uint32_t p = s - w.oj;
+        uint32_t ds, de;
+        approx_doc(A, s, &ds, &de);
+        if (p < ds || (uint64_t)p + w.m > de) return false;
+        const uint8_t *__restrict__ t = A.text + p;
+        const uint8_t *__restrict__ qq = w.qq;
+        uint32_t mis = 0;
+        if (w.whole) {
+            for (uint32_t x = 0; x < w.m; x++) mis += __ldg(t + x) != __ldg(qq + x);
+        } else {
+            CutStep pc(w.m, A.P);
+            for (uint32_t i = 0; i < A.P; i++) {
+                pc.next();
+                if (i == w.j) continue;
+                uint32_t mi = 0;
+                for (uint32_t x = pc.a; x < pc.b && mis + mi <= A.k; x++) mi += __ldg(t + x) != __ldg(qq + x);
+                if (i < w.j && mi == 0) return false;        // slot i reports it
+                mis += mi;
+                if (mis > A.k) return false;
+            }
+        }
+        *p_out = p;
+        *mis_out = mis;
+        return true;
     }
+    static constexpr bool CLASSES = false;      // byte equality, which edit_verify tests inline
+    // dist(s) <= m <= k in the whole-table slot
+    static __device__ __forceinline__ uint64_t whole_hits(const uint8_t *, int32_t k) { return 1ull << k; }
+    static __device__ __noinline__ bool reports(const ApproxArgs &A, int64_t p, uint32_t s,
+                                                const uint8_t *__restrict__ qq, uint32_t m, uint32_t q, uint32_t j,
+                                                uint32_t oj, uint32_t ds, uint32_t de);     // edit.cuh
 };
 
 // EMIT = false: cnt[item] = the occurrences the item reports.  EMIT = true: the same walk writes them from
 // item_off[item] on, in rank order: key = (q << pbits) | p, val = mis(p).
 template <bool EMIT, class Pieces>
-__device__ __forceinline__ void approx_walk(ApproxArgs A, Pieces pc, uint32_t *cnt,
-                                            const unsigned long long *item_off, int pbits, unsigned long long *key,
-                                            uint32_t *val) {
+__device__ __forceinline__ void approx_walk(ApproxArgs A, uint32_t *cnt, const unsigned long long *item_off, int pbits,
+                                            unsigned long long *key, uint32_t *val) {
     const uint64_t item = ((uint64_t)blockIdx.x * BLK + threadIdx.x) >> 5;
     if (item >= A.items) return;                                  // whole warps
     const uint32_t l = lane_id();
-    uint32_t a = 0, b = A.nslots;                                 // the last slot whose first item <= item
-    while (b - a > 1) {
-        const uint32_t mid = a + (b - a) / 2;
-        if (A.item_start[mid] <= item) a = mid; else b = mid;
-    }
-    const uint32_t q = a / A.P, j = a % A.P;
-    const uint32_t s0 = A.ps[a], e0 = A.pe[a];
-    const uint64_t blk = s0 / DLIST_CHUNK + (item - A.item_start[a]);
-    const uint64_t lo = blk * DLIST_CHUNK > s0 ? blk * DLIST_CHUNK : s0;
-    const uint64_t hi = blk * DLIST_CHUNK + DLIST_CHUNK < e0 ? blk * DLIST_CHUNK + DLIST_CHUNK : e0;
-    const uint64_t qo = A.qoff[q];
-    const uint32_t m = (uint32_t)(A.qoff[q + 1] - qo);
-    const bool whole = pc.whole(A, a, m);
-    const uint32_t oj = whole ? 0u : pc.off(A, a, m, j);
+    const ApproxItem w = approx_item<Pieces>(A, item);
     const uint64_t base = EMIT ? item_off[item] : 0;
     uint32_t count = 0;
-    for (uint64_t i0 = lo; i0 < hi; i0 += 32) {                   // the same trip count on every lane
+    for (uint64_t i0 = w.lo; i0 < w.hi; i0 += 32) {               // the same trip count on every lane
         const uint64_t i = i0 + l;
         uint32_t p = 0, mis = 0;
-        const bool hit = i < hi && pc.verify(A, A.sa[i], A.qs + qo, m, q, j, oj, whole, &p, &mis);
+        const bool hit = i < w.hi && Pieces::verify(A, w, A.sa[i], &p, &mis);
         const uint32_t m0 = __ballot_sync(FULL, hit);
         if (EMIT && hit) {
             const uint64_t slot = base + count + __popc(m0 & lanemask_lt());
-            key[slot] = ((unsigned long long)q << pbits) | p;
+            key[slot] = ((unsigned long long)w.q << pbits) | p;
             val[slot] = mis;
         }
         count += __popc(m0);
@@ -156,16 +184,7 @@ __device__ __forceinline__ void approx_walk(ApproxArgs A, Pieces pc, uint32_t *c
 template <bool EMIT>
 __global__ void __launch_bounds__(BLK) k_approx(ApproxArgs A, uint32_t *cnt, const unsigned long long *item_off,
                                                 int pbits, unsigned long long *key, uint32_t *val) {
-    approx_walk<EMIT>(A, CutPieces{}, cnt, item_off, pbits, key, val);
-}
-
-// offsets[q] = the output offset of query q's first item (its slots are q*P .. q*P + P - 1)
-__global__ void __launch_bounds__(BLK) k_approx_qoff(const unsigned long long *__restrict__ item_start,
-                                                     const unsigned long long *__restrict__ item_off, uint32_t nq,
-                                                     uint32_t P, unsigned long long *offsets) {
-    const uint64_t q = (uint64_t)blockIdx.x * BLK + threadIdx.x;
-    if (q > nq) return;
-    offsets[q] = item_off[item_start[q * P]];
+    approx_walk<EMIT, CutPieces>(A, cnt, item_off, pbits, key, val);
 }
 
 // The sorted keys and values into the caller's arrays (mis may be NULL).

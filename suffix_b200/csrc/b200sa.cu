@@ -2211,7 +2211,8 @@ static int docs_list_front(b200sa_ctx *c, uint32_t n, const uint32_t *d_g, const
                       (uint32_t *)nullptr, (uint32_t *)nullptr);
     TRY(mark(c, "dlist_scan"));
     TRY((dev_scan<OpSum64>(c, InCount64{cnt, items}, OutStoreExcl64{item_off}, items + 1, d_total)));
-    LAUNCH(c, k_dlist_qoff, cdiv((uint64_t)nq + 1, BLK), item_start, item_off, nq, reinterpret_cast<u64 *>(d_offsets));
+    LAUNCH(c, k_dlist_qoff, cdiv((uint64_t)nq + 1, BLK), item_start, item_off, nq, 1u,
+           reinterpret_cast<u64 *>(d_offsets));
     TRY(read_words(c, words + 4, 2));
     *total = pin_u64(c, 0);
     *Aout = A;
@@ -3016,7 +3017,7 @@ static int approx_search(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const
         LAUNCH(c, approx_kernel<false>(edit, iupac), cdiv(items, NWARP), A, cnt, (const u64 *)nullptr, pbits,
                (u64 *)nullptr, (uint32_t *)nullptr);
     TRY((dev_scan<OpSum64>(c, InCount64{cnt, items}, OutStoreExcl64{item_off}, items + 1, d_total)));
-    LAUNCH(c, k_approx_qoff, cdiv((uint64_t)nq + 1, BLK), item_start, item_off, nq, P,
+    LAUNCH(c, k_dlist_qoff, cdiv((uint64_t)nq + 1, BLK), item_start, item_off, nq, P,
            reinterpret_cast<u64 *>(d_offsets));
     TRY(read_words(c, words + AW_TOTAL, 2));
     *total = pin_u64(c, 0);

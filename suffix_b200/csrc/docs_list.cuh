@@ -56,6 +56,27 @@ struct OutStoreExcl64 {
     __device__ void operator()(uint64_t i, unsigned long long exc, unsigned long long) const { out[i] = exc; }
 };
 
+// Item `item` of the ranges [rs[r], re[r]) cut into chunks, item_start[r] being range r's first item: its range
+// r (the last one whose first item <= item), its chunk blk of DLIST_CHUNK ranks and the ranks [lo, hi) of the
+// range inside that chunk.
+struct DListItem {
+    uint32_t r;
+    uint64_t blk, lo, hi;
+};
+__device__ __forceinline__ DListItem dlist_item(const unsigned long long *item_start, uint32_t nr, const uint32_t *rs,
+                                                const uint32_t *re, uint64_t item) {
+    uint32_t a = 0, b = nr;
+    while (b - a > 1) {
+        const uint32_t mid = a + (b - a) / 2;
+        if (item_start[mid] <= item) a = mid; else b = mid;
+    }
+    const uint32_t s = rs[a], e = re[a];
+    const uint64_t blk = s / DLIST_CHUNK + (item - item_start[a]);
+    const uint64_t lo = blk * DLIST_CHUNK > s ? blk * DLIST_CHUNK : s;
+    const uint64_t hi = blk * DLIST_CHUNK + DLIST_CHUNK < e ? blk * DLIST_CHUNK + DLIST_CHUNK : e;
+    return {a, blk, lo, hi};
+}
+
 struct DListArgs {
     AnsvLevels L;                            // lv[0] = prev; lv[1] / lv[2] exist when n > 32 / n > 1024
     const uint32_t *qs, *qe;
@@ -74,15 +95,9 @@ __global__ void __launch_bounds__(BLK) k_dlist(DListArgs A, uint32_t *cnt, const
     const uint64_t item = ((uint64_t)blockIdx.x * BLK + threadIdx.x) >> 5;
     if (item >= A.items) return;                                  // whole warps
     const uint32_t l = lane_id();
-    uint32_t a = 0, b = A.nq;                                     // the last query whose first item <= item
-    while (b - a > 1) {
-        uint32_t m = a + (b - a) / 2;
-        if (A.item_start[m] <= item) a = m; else b = m;
-    }
-    const uint32_t s = A.qs[a], e = A.qe[a];
-    const uint64_t blk2 = s / DLIST_CHUNK + (item - A.item_start[a]);
-    const uint64_t lo = blk2 * DLIST_CHUNK > s ? blk2 * DLIST_CHUNK : s;
-    const uint64_t hi = blk2 * DLIST_CHUNK + DLIST_CHUNK < e ? blk2 * DLIST_CHUNK + DLIST_CHUNK : e;
+    const DListItem it = dlist_item(A.item_start, A.nq, A.qs, A.qe, item);
+    const uint32_t s = A.qs[it.r], e = A.qe[it.r];
+    const uint64_t blk2 = it.blk, lo = it.lo, hi = it.hi;
     uint32_t count = 0;
     const uint64_t base = EMIT ? item_off[item] : 0;
     if (A.L.nlev < 3 || A.L.lv[2][blk2] <= s) {
@@ -121,13 +136,15 @@ __global__ void __launch_bounds__(BLK) k_dlist(DListArgs A, uint32_t *cnt, const
     if (!EMIT && l == 0) cnt[item] = count;
 }
 
-// offsets[q] = the listing offset of query q's first item (item_start[nq] = items, item_off[items] = total)
+// offsets[q] = the output offset of query q's first item, its ranges being q*stride .. q*stride + stride - 1: one
+// per query for the listing, the P slots of its pieces for approx.cuh (item_start[nq * stride] = items,
+// item_off[items] = total)
 __global__ void __launch_bounds__(BLK) k_dlist_qoff(const unsigned long long *__restrict__ item_start,
                                                     const unsigned long long *__restrict__ item_off, uint32_t nq,
-                                                    unsigned long long *offsets) {
+                                                    uint32_t stride, unsigned long long *offsets) {
     uint64_t q = (uint64_t)blockIdx.x * BLK + threadIdx.x;
     if (q > nq) return;
-    offsets[q] = item_off[item_start[q]];
+    offsets[q] = item_off[item_start[q * stride]];
 }
 
 }  // namespace b200sa

@@ -3,16 +3,17 @@
 //
 // The partition lemma holds for Levenshtein distance too (Baeza-Yates & Navarro): an alignment of a query of
 // m > k bytes with at most k edits leaves one of its P = k + 1 pieces matched exactly, shifted by at most k from
-// its place in the query.  So the slots, chunks and count -> scan -> emit -> sort flow of approx.cuh carry over;
-// only the candidate's work differs.
+// its place in the query.  So the slots, chunks and count -> scan -> emit -> sort flow of approx.cuh carry over,
+// and with them the item (approx_item), the document window (approx_doc) and the pieces (CutPieces); only the
+// candidate's work differs.
 // A candidate is a rank i of slot (q, j), s = R[i], c = s - o_j.  It considers the starts p of s's document
 // [ds, de) with |p - c| <= k (at most 2k + 1 <= 63: one 64-bit mask per lane).  An alignment of cost <= k that
 // starts at such a p stays within diagonals t - x in [c - 2k, c + 2k] (t a text, x a query position), so one
 // reversed Sellers DP (query read backwards, text leftwards, a free end) over that band of 4k + 1 diagonals gives
 // dist(p) exactly wherever it is <= k, for all of the window's starts at once.
 // Reporter: R(p) is the least (i, s'') with piece i exactly at s'' inside p's document and |s'' - o_i - p| <= k;
-// the candidate emits p iff dist(p) <= k and R(p) = (j, s).  The lemma makes R(p) exist for every occurrence, so
-// each is emitted once, and the count pass is exact without de-duplication.
+// the candidate emits p iff dist(p) <= k and R(p) = (j, s) (the policy's reports).  The lemma makes R(p) exist
+// for every occurrence, so each is emitted once, and the count pass is exact without de-duplication.
 // A query of 0 < m <= k keeps the whole-table slot; there each rank reports its own position s with dist(s).
 #pragma once
 #include "approx.cuh"
@@ -24,27 +25,21 @@ constexpr int EDIT_BAND = 4 * B200SA_APPROX_MAX_K + 1;    // diagonals of the wi
 // Whether piece bytes pq[0, len) occur at x, with [x, x + len) inside [ds, de)
 __device__ __forceinline__ bool edit_piece_at(const uint8_t *__restrict__ text, int64_t x,
                                               const uint8_t *__restrict__ pq, uint32_t len, uint32_t ds, uint32_t de) {
-    if (x < (int64_t)ds || x + len > (int64_t)de) return false;
-    for (uint32_t y = 0; y < len; y++)
-        if (__ldg(text + x + y) != __ldg(pq + y)) return false;
-    return true;
+    return x >= (int64_t)ds && x + len <= (int64_t)de && approx_piece_at(text + x, pq, len);
 }
 
 // Whether candidate (j, s) is R(p) for the start p of [ds, de): no piece i < j within k of its place, and no
 // occurrence of piece j at s'' < s within k of its place.  Called only for starts within k; kept out of line,
 // which keeps k_approx_edit<true> free of spills.
-__device__ __noinline__ bool edit_reports(const ApproxArgs &A, int64_t p, uint32_t s, const uint8_t *__restrict__ qq,
-                                             uint32_t m, uint32_t j, uint32_t oj, uint32_t ds, uint32_t de) {
+__device__ __noinline__ bool CutPieces::reports(const ApproxArgs &A, int64_t p, uint32_t s,
+                                                const uint8_t *__restrict__ qq, uint32_t m, uint32_t, uint32_t j,
+                                                uint32_t oj, uint32_t ds, uint32_t de) {
     const int32_t k = (int32_t)A.k;
-    const uint32_t step = m / A.P, rem = m % A.P;          // piece i = [a, b), a = i*m/P
-    uint32_t a = 0, r = 0;
+    CutStep pc(m, A.P);
     for (uint32_t i = 0; i < j; i++) {
-        uint32_t b = a + step;
-        r += rem;
-        if (r >= A.P) { b++; r -= A.P; }
+        pc.next();
         for (int32_t d = -k; d <= k; d++)
-            if (edit_piece_at(A.text, p + a + d, qq + a, b - a, ds, de)) return false;
-        a = b;
+            if (edit_piece_at(A.text, p + pc.a + d, qq + pc.a, pc.b - pc.a, ds, de)) return false;
     }
     const uint32_t len = approx_cut(m, A.P, j + 1) - oj;
     for (int64_t x = p + oj - k; x < (int64_t)s; x++)
@@ -52,33 +47,19 @@ __device__ __noinline__ bool edit_reports(const ApproxArgs &A, int64_t p, uint32
     return true;
 }
 
-// f-14's pieces and byte equality for the edit walk; whole: dist(s) <= m <= k.
-struct EditCut : CutPieces {
-    static constexpr bool CLASSES = false;          // byte equality
-    __device__ __forceinline__ uint64_t whole_hits(const uint8_t *, int32_t k) const { return 1ull << k; }
-    __device__ __forceinline__ bool reports(const ApproxArgs &A, int64_t p, uint32_t s, const uint8_t *__restrict__ qq,
-                                            uint32_t m, uint32_t, uint32_t j, uint32_t oj, uint32_t ds,
-                                            uint32_t de) const {
-        return edit_reports(A, p, s, qq, m, j, oj, ds, de);
-    }
-};
-
 // The starts this candidate reports, bit b for p = c - k + b, with *c_out = c and v[k + b] = dist(p).  v holds
 // one band row: v[d] = D(x, t) at t = c - 2k + x + d, D(x, t) = min over e of ED(q[x, m), T[t, e)), e <= de,
-// saturated at k + 1.  whole: the whole-table slot, only p = s (o_j = 0).  Pieces: EditCut or IupacPieces.
+// saturated at k + 1.  whole: the whole-table slot, only p = s (o_j = 0).  Pieces: CutPieces or IupacPieces.
 template <class Pieces>
-__device__ __forceinline__ uint64_t edit_verify(const ApproxArgs &A, const Pieces &pc, uint32_t s,
-                                                const uint8_t *__restrict__ qq, uint32_t m, uint32_t q, uint32_t j,
-                                                uint32_t oj, bool whole, uint8_t *v, int64_t *c_out) {
+__device__ __forceinline__ uint64_t edit_verify(const ApproxArgs &A, const ApproxItem &w, uint32_t s, uint8_t *v,
+                                                int64_t *c_out) {
     const int32_t k = (int32_t)A.k, W = 4 * k + 1;
     const uint32_t INF = (uint32_t)k + 1;
-    uint32_t ds = 0, de = A.n;
-    if (A.starts) {
-        const uint32_t dd = docs_find(A.starts, A.ndocs, s);
-        ds = __ldg(A.starts + dd);
-        de = docs_end(A.starts, A.ndocs, A.n, dd);
-    }
-    const int64_t c = (int64_t)s - oj, base = c - 2 * k;
+    const uint8_t *__restrict__ qq = w.qq;
+    const uint32_t m = w.m;
+    uint32_t ds, de;
+    approx_doc(A, s, &ds, &de);
+    const int64_t c = (int64_t)s - w.oj, base = c - 2 * k;
     *c_out = c;
     for (int32_t d = 0; d < W; d++) {                      // row m: the empty rest of the query ends anywhere
         const int64_t t = base + m + d;
@@ -92,8 +73,10 @@ __device__ __forceinline__ uint64_t edit_verify(const ApproxArgs &A, const Piece
             const int64_t t = base + x + d;
             uint32_t y = INF;
             if (t >= (int64_t)ds && t < (int64_t)de) {
-                if constexpr (Pieces::CLASSES)                 // the byte test written inline, as before
-                    y = min(min(right, up) + 1, old + pc.miss(__ldg(A.text + t), qc));
+                // the byte test written inline: through a miss() member, ptxas spends three predicate instructions
+                // per unrolled cell where this spends one (8 more in k_approx_edit)
+                if constexpr (Pieces::CLASSES)
+                    y = min(min(right, up) + 1, old + Pieces::miss(__ldg(A.text + t), qc));
                 else
                     y = min(min(right, up) + 1, old + (__ldg(A.text + t) != qc));
             } else if (t == (int64_t)de) {
@@ -107,12 +90,12 @@ __device__ __forceinline__ uint64_t edit_verify(const ApproxArgs &A, const Piece
         }
         if (low > (uint32_t)k) return 0;                   // every path to row 0 passes this row
     }
-    if (whole) return pc.whole_hits(v, k);
+    if (w.whole) return Pieces::whole_hits(v, k);
     const int64_t lo = max((int64_t)ds, c - k), hi = min((int64_t)de - 1, c + k);
     uint64_t hits = 0;
     for (int64_t p = lo; p <= hi; p++) {
         const uint32_t b = (uint32_t)(p - (c - k));
-        if (v[k + b] <= (uint32_t)k && pc.reports(A, p, s, qq, m, q, j, oj, ds, de)) hits |= 1ull << b;
+        if (v[k + b] <= (uint32_t)k && Pieces::reports(A, p, s, qq, m, w.q, w.j, w.oj, ds, de)) hits |= 1ull << b;
     }
     return hits;
 }
@@ -120,32 +103,18 @@ __device__ __forceinline__ uint64_t edit_verify(const ApproxArgs &A, const Piece
 // EMIT = false: cnt[item] = the occurrences the item reports.  EMIT = true: the same walk writes them from
 // item_off[item] on: key = (q << pbits) | p, val = dist(p).  v: the kernel's band row of EDIT_BAND bytes.
 template <bool EMIT, class Pieces>
-__device__ __forceinline__ void edit_walk(ApproxArgs A, Pieces pc, uint8_t *v, uint32_t *cnt,
-                                          const unsigned long long *item_off, int pbits, unsigned long long *key,
-                                          uint32_t *val) {
+__device__ __forceinline__ void edit_walk(ApproxArgs A, uint8_t *v, uint32_t *cnt, const unsigned long long *item_off,
+                                          int pbits, unsigned long long *key, uint32_t *val) {
     const uint64_t item = ((uint64_t)blockIdx.x * BLK + threadIdx.x) >> 5;
     if (item >= A.items) return;                                  // whole warps
     const uint32_t l = lane_id();
-    uint32_t a = 0, b = A.nslots;                                 // the last slot whose first item <= item
-    while (b - a > 1) {
-        const uint32_t mid = a + (b - a) / 2;
-        if (A.item_start[mid] <= item) a = mid; else b = mid;
-    }
-    const uint32_t q = a / A.P, j = a % A.P;
-    const uint32_t s0 = A.ps[a], e0 = A.pe[a];
-    const uint64_t blk = s0 / DLIST_CHUNK + (item - A.item_start[a]);
-    const uint64_t lo = blk * DLIST_CHUNK > s0 ? blk * DLIST_CHUNK : s0;
-    const uint64_t hi = blk * DLIST_CHUNK + DLIST_CHUNK < e0 ? blk * DLIST_CHUNK + DLIST_CHUNK : e0;
-    const uint64_t qo = A.qoff[q];
-    const uint32_t m = (uint32_t)(A.qoff[q + 1] - qo);
-    const bool whole = pc.whole(A, a, m);
-    const uint32_t oj = whole ? 0u : pc.off(A, a, m, j);
+    const ApproxItem w = approx_item<Pieces>(A, item);
     const uint64_t base = EMIT ? item_off[item] : 0;
     uint32_t count = 0;
-    for (uint64_t i0 = lo; i0 < hi; i0 += 32) {                   // the same trip count on every lane
+    for (uint64_t i0 = w.lo; i0 < w.hi; i0 += 32) {               // the same trip count on every lane
         const uint64_t i = i0 + l;
         int64_t c = 0;
-        const uint64_t hits = i < hi ? edit_verify(A, pc, A.sa[i], A.qs + qo, m, q, j, oj, whole, v, &c) : 0;
+        const uint64_t hits = i < w.hi ? edit_verify<Pieces>(A, w, A.sa[i], v, &c) : 0;
         const uint32_t h = __popcll(hits);
         uint32_t incl = h;                                        // inclusive warp scan of the lanes' hits
         for (int o = 1; o < 32; o <<= 1) {
@@ -153,7 +122,7 @@ __device__ __forceinline__ void edit_walk(ApproxArgs A, Pieces pc, uint8_t *v, u
             if (l >= (uint32_t)o) incl += y;
         }
         if (EMIT && hits) {
-            const unsigned long long kq = (unsigned long long)q << pbits;
+            const unsigned long long kq = (unsigned long long)w.q << pbits;
             unsigned long long *ks = key + base + count + incl - h;
             uint32_t *vs = val + base + count + incl - h;
             #pragma unroll 1
@@ -172,7 +141,7 @@ template <bool EMIT>
 __global__ void __launch_bounds__(BLK) k_approx_edit(ApproxArgs A, uint32_t *cnt, const unsigned long long *item_off,
                                                      int pbits, unsigned long long *key, uint32_t *val) {
     uint8_t v[EDIT_BAND];
-    edit_walk<EMIT>(A, EditCut{}, v, cnt, item_off, pbits, key, val);
+    edit_walk<EMIT, CutPieces>(A, v, cnt, item_off, pbits, key, val);
 }
 
 }  // namespace b200sa

@@ -13,6 +13,7 @@
 // sum L_i < P keeps the whole-table slot: every rank is a candidate and is verified in full.  The piece of slot
 // q*P + j is (offset, length) in entry q*P + j of the piece table; length 0 marks the whole-table slot.  The table
 // follows pe in the same buffer (iupac_table), so the walks find it from ApproxArgs and keep no pointer live.
+// IupacPieces gives the walks these pieces and the class test in place of CutPieces.
 #pragma once
 #include "edit.cuh"
 
@@ -124,83 +125,61 @@ __global__ void __launch_bounds__(BLK) k_iupac_pieces(const uint8_t *__restrict_
     }
 }
 
-// Whether the concrete piece bytes pq[0, len) are the text's at t
-__device__ __forceinline__ bool iupac_piece_at(const uint8_t *__restrict__ t, const uint8_t *__restrict__ pq,
-                                               uint32_t len) {
-    for (uint32_t y = 0; y < len; y++)
-        if (__ldg(t + y) != __ldg(pq + y)) return false;
-    return true;
-}
-
-// As approx_verify, with the class test over all m symbols and the pieces pc[0, j) of the query's table.
-__device__ __forceinline__ bool iupac_verify(const ApproxArgs &A, const uint2 *__restrict__ pc, uint32_t s,
-                                             const uint8_t *__restrict__ qq, uint32_t m, uint32_t j, uint32_t oj,
-                                             bool whole, uint32_t *p_out, uint32_t *mis_out) {
-    if (s < oj) return false;
-    const uint32_t p = s - oj;
-    uint32_t ds = 0, de = A.n;
-    if (A.starts) {
-        const uint32_t d = docs_find(A.starts, A.ndocs, s);
-        ds = __ldg(A.starts + d);
-        de = docs_end(A.starts, A.ndocs, A.n, d);
-    }
-    if (p < ds || (uint64_t)p + m > de) return false;
-    const uint8_t *__restrict__ t = A.text + p;
-    uint32_t mis = 0;
-    for (uint32_t x = 0; x < m; x++) {
-        mis += !iupac_in(__ldg(t + x), __ldg(qq + x));
-        if (mis > A.k) return false;
-    }
-    if (!whole)
-        for (uint32_t i = 0; i < j; i++) {
-            const uint2 pi = pc[i];
-            if (iupac_piece_at(t + pi.x, qq + pi.x, pi.y)) return false;     // slot i reports it
-        }
-    *p_out = p;
-    *mis_out = mis;
-    return true;
-}
-
-// edit_reports with the pieces [0, j] of query q's table.  Out of line, as edit_reports is.
-__device__ __noinline__ bool iupac_edit_reports(const ApproxArgs &A, int64_t p, uint32_t s,
-                                                const uint8_t *__restrict__ qq, uint32_t q, uint32_t j, uint32_t ds,
-                                                uint32_t de) {
-    const int32_t k = (int32_t)A.k;
-    const uint2 *__restrict__ pc = iupac_table(A) + (uint64_t)q * A.P;
-    for (uint32_t i = 0; i < j; i++) {
-        const uint2 pi = pc[i];
-        for (int32_t d = -k; d <= k; d++)
-            if (edit_piece_at(A.text, p + pi.x + d, qq + pi.x, pi.y, ds, de)) return false;
-    }
-    const uint2 pj = pc[j];
-    for (int64_t x = p + pj.x - k; x < (int64_t)s; x++)
-        if (edit_piece_at(A.text, x, qq + pj.x, pj.y, ds, de)) return false;
-    return true;
-}
-
-// The pieces of the piece table and the class test, for approx_walk and edit_walk.
+// The pieces of the piece table and the class test: CutPieces' members for the canonical queries.
 struct IupacPieces {
-    __device__ __forceinline__ bool whole(const ApproxArgs &A, uint32_t slot, uint32_t) const {
+    static __device__ __forceinline__ bool whole(const ApproxArgs &A, uint32_t slot, uint32_t) {
         return iupac_table(A)[slot].y == 0;
     }
-    __device__ __forceinline__ uint32_t off(const ApproxArgs &A, uint32_t slot, uint32_t, uint32_t) const {
+    static __device__ __forceinline__ uint32_t off(const ApproxArgs &A, uint32_t slot, uint32_t, uint32_t) {
         return iupac_table(A)[slot].x;
     }
-    __device__ __forceinline__ bool verify(const ApproxArgs &A, uint32_t s, const uint8_t *__restrict__ qq, uint32_t m,
-                                           uint32_t q, uint32_t j, uint32_t oj, bool whole, uint32_t *p_out,
-                                           uint32_t *mis_out) const {
-        return iupac_verify(A, iupac_table(A) + (uint64_t)q * A.P, s, qq, m, j, oj, whole, p_out, mis_out);
+    // The class test over all m symbols, then the pieces [0, j) of the query's table.
+    static __device__ __forceinline__ bool verify(const ApproxArgs &A, const ApproxItem &w, uint32_t s,
+                                                  uint32_t *p_out, uint32_t *mis_out) {
+        if (s < w.oj) return false;
+        const uint32_t p = s - w.oj;
+        uint32_t ds, de;
+        approx_doc(A, s, &ds, &de);
+        if (p < ds || (uint64_t)p + w.m > de) return false;
+        const uint8_t *__restrict__ t = A.text + p;
+        const uint8_t *__restrict__ qq = w.qq;
+        uint32_t mis = 0;
+        for (uint32_t x = 0; x < w.m; x++) {
+            mis += !iupac_in(__ldg(t + x), __ldg(qq + x));
+            if (mis > A.k) return false;
+        }
+        if (!w.whole) {
+            const uint2 *__restrict__ pc = iupac_table(A) + (uint64_t)w.q * A.P;
+            for (uint32_t i = 0; i < w.j; i++) {
+                const uint2 pi = pc[i];
+                if (approx_piece_at(t + pi.x, qq + pi.x, pi.y)) return false;     // slot i reports it
+            }
+        }
+        *p_out = p;
+        *mis_out = mis;
+        return true;
     }
     static constexpr bool CLASSES = true;
-    __device__ __forceinline__ bool miss(uint32_t t, uint32_t qc) const { return !iupac_in(t, qc); }
-    // whole: m may exceed k here, so dist(s) = v[2k] is tested
-    __device__ __forceinline__ uint64_t whole_hits(const uint8_t *v, int32_t k) const {
+    static __device__ __forceinline__ bool miss(uint32_t t, uint32_t qc) { return !iupac_in(t, qc); }
+    // m may exceed k here, so dist(s) = v[2k] is tested
+    static __device__ __forceinline__ uint64_t whole_hits(const uint8_t *v, int32_t k) {
         return v[2 * k] <= (uint32_t)k ? 1ull << k : 0ull;
     }
-    __device__ __forceinline__ bool reports(const ApproxArgs &A, int64_t p, uint32_t s, const uint8_t *__restrict__ qq,
-                                            uint32_t, uint32_t q, uint32_t j, uint32_t, uint32_t ds,
-                                            uint32_t de) const {
-        return iupac_edit_reports(A, p, s, qq, q, j, ds, de);
+    // CutPieces::reports with the pieces [0, j] of query q's table; out of line for the same reason.
+    static __device__ __noinline__ bool reports(const ApproxArgs &A, int64_t p, uint32_t s,
+                                                const uint8_t *__restrict__ qq, uint32_t, uint32_t q, uint32_t j,
+                                                uint32_t, uint32_t ds, uint32_t de) {
+        const int32_t k = (int32_t)A.k;
+        const uint2 *__restrict__ pc = iupac_table(A) + (uint64_t)q * A.P;
+        for (uint32_t i = 0; i < j; i++) {
+            const uint2 pi = pc[i];
+            for (int32_t d = -k; d <= k; d++)
+                if (edit_piece_at(A.text, p + pi.x + d, qq + pi.x, pi.y, ds, de)) return false;
+        }
+        const uint2 pj = pc[j];
+        for (int64_t x = p + pj.x - k; x < (int64_t)s; x++)
+            if (edit_piece_at(A.text, x, qq + pj.x, pj.y, ds, de)) return false;
+        return true;
     }
 };
 
@@ -209,7 +188,7 @@ struct IupacPieces {
 template <bool EMIT>
 __global__ void __launch_bounds__(BLK, 4) k_approx_iupac(ApproxArgs A, uint32_t *cnt, const unsigned long long *item_off,
                                                          int pbits, unsigned long long *key, uint32_t *val) {
-    approx_walk<EMIT>(A, IupacPieces{}, cnt, item_off, pbits, key, val);
+    approx_walk<EMIT, IupacPieces>(A, cnt, item_off, pbits, key, val);
 }
 
 template <bool EMIT>
@@ -217,7 +196,7 @@ __global__ void __launch_bounds__(BLK) k_approx_edit_iupac(ApproxArgs A, uint32_
                                                            const unsigned long long *item_off, int pbits,
                                                            unsigned long long *key, uint32_t *val) {
     uint8_t v[EDIT_BAND];
-    edit_walk<EMIT>(A, IupacPieces{}, v, cnt, item_off, pbits, key, val);
+    edit_walk<EMIT, IupacPieces>(A, v, cnt, item_off, pbits, key, val);
 }
 
 }  // namespace b200sa
