@@ -275,65 +275,29 @@ static int radix_pass(b200sa_ctx *c, DigF dig, MoveF mv, uint64_t n) {
     return B200SA_OK;
 }
 
-// Sorts (ka,va) by the low `bits` of the key with the one-sweep passes of
-// common.cuh; *kout/*vout point at the buffer pair holding the result.
-template <class K, int OSI>
-static int sort_pairs_t(b200sa_ctx *c, K *ka, uint32_t *va, K *kb, uint32_t *vb, uint64_t n, int bits,
-                      K **kout, uint32_t **vout) {
-    *kout = ka;
-    *vout = va;
-    if (n == 0 || bits <= 0) return B200SA_OK;
-    int npass = (bits + 7) / 8;
-    if (npass > OS_MAX_PASSES) npass = OS_MAX_PASSES;
-    uint32_t tiles = cdiv(n, OSI * BLK);
-    size_t status_bytes = (size_t)tiles * 256 * 8;
-    TRY(ensure(c, c->os_hist, OS_MAX_PASSES * 256 * 4 + 64));
-    TRY(ensure(c, c->os_status, status_bytes));
-    uint32_t *ghist = ptr<uint32_t>(c->os_hist);
-    uint32_t *ticket = ghist + OS_MAX_PASSES * 256;
-    CU_TRY(c, cudaMemsetAsync(ghist, 0, OS_MAX_PASSES * 256 * 4 + 64, c->stream));
-    uint32_t hb = cdiv(n, TILE) < grid_cap(c) ? cdiv(n, TILE) : grid_cap(c);
-    {
-        size_t shm = (size_t)NWARP * npass * 256 * 4;
-        auto kfn = k_os_hist<K, LoadArr<K>>;
-        CU_TRY(c, cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(NWARP * OS_MAX_PASSES * 256 * 4)));
-        kfn<<<hb, BLK, shm, c->stream>>>(LoadArr<K>{ka}, n, npass, 0u, ghist, (K *)nullptr);
-        c->launches++;
-    }
-    LAUNCH(c, k_os_scan, (uint32_t)npass, ghist);
-    for (int p = 0; p < npass; p++) {
-        CU_TRY(c, cudaMemsetAsync(c->os_status.p, 0, status_bytes, c->stream));
-        LAUNCH(c, (k_os_pass<K, LoadArr<K>, LoadArr<uint32_t>, OSI>), tiles, LoadArr<K>{ka}, LoadArr<uint32_t>{va}, kb, vb, n,
-               (uint32_t)(8 * p), ghist + p * 256,
-               reinterpret_cast<volatile unsigned long long *>(c->os_status.p), ticket + p);
-        K *tk = ka; ka = kb; kb = tk;
-        uint32_t *tv = va; va = vb; vb = tv;
-    }
-    CU_TRY(c, cudaGetLastError());
-    *kout = ka;
-    *vout = va;
-    return B200SA_OK;
+// Keys per thread of the one-sweep passes.  From 2^20 items the tiles are wide (16 keys per thread for 32-bit
+// keys, 12 for 64-bit keys: what fits 48 KB of static shared memory): half the tiles, look-backs and per-tile
+// scans per key.  B200SA_SORT_ITEMS=8|16 forces the width, and B200SA_SORT_NARROW the narrow tiles.
+static bool os_wide(uint64_t n) {
+    if (const char *e = getenv("B200SA_SORT_ITEMS")) return atoi(e) == 16;
+    return n >= (1u << 20) && !getenv("B200SA_SORT_NARROW");
 }
 
-// Large inputs take wider tiles (16 keys per thread for 32-bit keys, 12 for 64-bit keys: what fits 48 KB of
-// static shared memory): half the tiles, look-backs and per-tile scans per key.
-template <class K>
-static int sort_pairs(b200sa_ctx *c, K *ka, uint32_t *va, K *kb, uint32_t *vb, uint64_t n, int bits,
-                      K **kout, uint32_t **vout) {
-    if (n >= (1u << 20) && !getenv("B200SA_SORT_NARROW"))
-        return sort_pairs_t<K, (sizeof(K) == 4 ? 16 : 12)>(c, ka, va, kb, vb, n, bits, kout, vout);
-    return sort_pairs_t<K, ITEMS>(c, ka, va, kb, vb, n, bits, kout, vout);
-}
+// Where the first pass of a one-sweep sort reads its keys.  IN_PLACE: from ka; a sort of no bits leaves (ka, va)
+// as they are.  FROM_FUNCTORS: the histogram kernel gathers them from the key functor into kb (free until the
+// second pass writes it) and the first pass writes (ka, va); at least one pass runs, so the result always lands
+// in a buffer pair.
+enum OsFirst { IN_PLACE, FROM_FUNCTORS };
 
-// Same sort, but the first pass reads its (key, value) items from functors (no materialised
-// input arrays); at least one pass runs, so the result always lands in a buffer pair.  The passes
-// sort by key bits [shift0, shift0 + bits).
-template <class K, class KeyF, class ValF, int OSI = ITEMS>
-static int sort_pairs_from(b200sa_ctx *c, KeyF keyf, ValF valf, K *ka, uint32_t *va, K *kb, uint32_t *vb, uint64_t n,
-                           int bits, K **kout, uint32_t **vout, uint32_t shift0 = 0) {
+// Sorts n items by key bits [shift0, shift0 + bits) with the one-sweep passes of common.cuh, OSI keys per
+// thread.  The histogram reads the keys through keyf and the first pass the values through valf; *kout/*vout
+// point at the buffer pair holding the result.
+template <OsFirst FIRST, int OSI, class K, class KeyF, class ValF>
+static int os_sort_items(b200sa_ctx *c, KeyF keyf, ValF valf, K *ka, uint32_t *va, K *kb, uint32_t *vb, uint64_t n,
+                         int bits, uint32_t shift0, K **kout, uint32_t **vout) {
     *kout = ka;
     *vout = va;
-    if (n == 0) return B200SA_OK;
+    if (n == 0 || (FIRST == IN_PLACE && bits <= 0)) return B200SA_OK;
     int npass = (bits + 7) / 8;
     if (npass < 1) npass = 1;
     if (npass > OS_MAX_PASSES) npass = OS_MAX_PASSES;
@@ -349,24 +313,54 @@ static int sort_pairs_from(b200sa_ctx *c, KeyF keyf, ValF valf, K *ka, uint32_t 
         size_t shm = (size_t)NWARP * npass * 256 * 4;
         auto kfn = k_os_hist<K, KeyF>;
         CU_TRY(c, cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(NWARP * OS_MAX_PASSES * 256 * 4)));
-        kfn<<<hb, BLK, shm, c->stream>>>(keyf, n, npass, shift0, ghist, kb);   // kb <- the keys (free until pass 2 writes it)
+        kfn<<<hb, BLK, shm, c->stream>>>(keyf, n, npass, shift0, ghist, FIRST == FROM_FUNCTORS ? kb : (K *)nullptr);
         c->launches++;
     }
     LAUNCH(c, k_os_scan, (uint32_t)npass, ghist);
     volatile unsigned long long *status = reinterpret_cast<volatile unsigned long long *>(c->os_status.p);
-    CU_TRY(c, cudaMemsetAsync(c->os_status.p, 0, status_bytes, c->stream));
-    LAUNCH(c, (k_os_pass<K, LoadArr<K>, ValF, OSI>), tiles, LoadArr<K>{kb}, valf, ka, va, n, shift0, ghist, status, ticket);
-    for (int p = 1; p < npass; p++) {
+    if (FIRST == FROM_FUNCTORS) {       // the first pass reads the gathered keys in kb and writes (ka, va)
+        std::swap(ka, kb);
+        std::swap(va, vb);
+    }
+    for (int p = 0; p < npass; p++) {
         CU_TRY(c, cudaMemsetAsync(c->os_status.p, 0, status_bytes, c->stream));
-        LAUNCH(c, (k_os_pass<K, LoadArr<K>, LoadArr<uint32_t>, OSI>), tiles, LoadArr<K>{ka}, LoadArr<uint32_t>{va}, kb, vb, n,
-               shift0 + (uint32_t)(8 * p), ghist + p * 256, status, ticket + p);
-        K *tk = ka; ka = kb; kb = tk;
-        uint32_t *tv = va; va = vb; vb = tv;
+        const uint32_t shift = shift0 + (uint32_t)(8 * p);
+        if (p == 0)
+            LAUNCH(c, (k_os_pass<K, LoadArr<K>, ValF, OSI>), tiles, LoadArr<K>{ka}, valf, kb, vb, n, shift, ghist, status,
+                   ticket);
+        else
+            LAUNCH(c, (k_os_pass<K, LoadArr<K>, LoadArr<uint32_t>, OSI>), tiles, LoadArr<K>{ka}, LoadArr<uint32_t>{va}, kb,
+                   vb, n, shift, ghist + p * 256, status, ticket + p);
+        std::swap(ka, kb);
+        std::swap(va, vb);
     }
     CU_TRY(c, cudaGetLastError());
     *kout = ka;
     *vout = va;
     return B200SA_OK;
+}
+
+template <OsFirst FIRST, class K, class KeyF, class ValF>
+static int os_sort(b200sa_ctx *c, KeyF keyf, ValF valf, K *ka, uint32_t *va, K *kb, uint32_t *vb, uint64_t n, int bits,
+                   uint32_t shift0, K **kout, uint32_t **vout) {
+    if (os_wide(n))
+        return os_sort_items<FIRST, sizeof(K) == 4 ? 16 : 12>(c, keyf, valf, ka, va, kb, vb, n, bits, shift0, kout, vout);
+    return os_sort_items<FIRST, ITEMS>(c, keyf, valf, ka, va, kb, vb, n, bits, shift0, kout, vout);
+}
+
+// Sorts (ka, va) by the low `bits` of the key.
+template <class K>
+static int sort_pairs(b200sa_ctx *c, K *ka, uint32_t *va, K *kb, uint32_t *vb, uint64_t n, int bits,
+                      K **kout, uint32_t **vout) {
+    return os_sort<IN_PLACE>(c, LoadArr<K>{ka}, LoadArr<uint32_t>{va}, ka, va, kb, vb, n, bits, 0u, kout, vout);
+}
+
+// Sorts the items (keyf(i), valf(i)) by key bits [shift0, shift0 + bits), with (ka, va) and (kb, vb) as the
+// buffer pairs.
+template <class K, class KeyF, class ValF>
+static int sort_pairs_from(b200sa_ctx *c, KeyF keyf, ValF valf, K *ka, uint32_t *va, K *kb, uint32_t *vb, uint64_t n,
+                           int bits, K **kout, uint32_t **vout, uint32_t shift0 = 0) {
+    return os_sort<FROM_FUNCTORS>(c, keyf, valf, ka, va, kb, vb, n, bits, shift0, kout, vout);
 }
 
 static int bit_length(uint64_t x) {
@@ -579,8 +573,6 @@ static int lms_direct_sort_t(b200sa_ctx *c, uint32_t n, uint32_t m, uint32_t **l
     uint32_t *grpA = ptr<uint32_t>(c->g0), *grpB = ptr<uint32_t>(c->g1);
     uint32_t *posA = ptr<uint32_t>(c->sa_r), *posB = ptr<uint32_t>(c->rank);
     unsigned long long *d_tot = reinterpret_cast<unsigned long long *>(sm + 16);
-    const char *items_env = getenv("B200SA_SORT_ITEMS");            // keys per thread of the one-sweep passes: 8 | 16
-    const bool wide = items_env ? atoi(items_env) == 16 : (m >= (1u << 20) && !getenv("B200SA_SORT_NARROW"));
     LmsKeyDesc<BITS> kf{W, ptr<uint32_t>(c->lmsdesc)};
     LmsValDesc vf{ptr<uint32_t>(c->lmsdesc)};
     // 2-bit text: two passes on the top 16 key bits (the first 8 characters), then k_lms_bucket_sort sorts every
@@ -589,14 +581,8 @@ static int lms_direct_sort_t(b200sa_ctx *c, uint32_t n, uint32_t m, uint32_t **l
     bool bucketed = false;
     if (BITS == 2 && !getenv("B200SA_LMS_SORT4")) {
         TRY(mark(c, "lms_sort"));
-        if (wide)
-            TRY((sort_pairs_from<uint32_t, LmsKeyDesc<BITS>, LmsValDesc, 16>(c, kf, vf, ptr<uint32_t>(c->k32b), ptr<uint32_t>(c->v0),
-                                                                             ptr<uint32_t>(c->reduced), ptr<uint32_t>(c->v1), m,
-                                                                             16, &Ks, &Ps, 16u)));
-        else
-            TRY((sort_pairs_from<uint32_t, LmsKeyDesc<BITS>, LmsValDesc, ITEMS>(c, kf, vf, ptr<uint32_t>(c->k32b), ptr<uint32_t>(c->v0),
-                                                                                ptr<uint32_t>(c->reduced), ptr<uint32_t>(c->v1), m,
-                                                                                16, &Ks, &Ps, 16u)));
+        TRY(sort_pairs_from(c, kf, vf, ptr<uint32_t>(c->k32b), ptr<uint32_t>(c->v0), ptr<uint32_t>(c->reduced),
+                            ptr<uint32_t>(c->v1), m, 16, &Ks, &Ps, 16u));
         TRY(mark(c, "lms_groups"));
         uint32_t *Pout = ptr<uint32_t>(c->k32b);                    // keys of the first pass: dead after the second
         CU_TRY(c, cudaMemsetAsync(sm + 16, 0, 12, c->stream));      // [16] tied count, [18] bucket overflow
@@ -622,14 +608,8 @@ static int lms_direct_sort_t(b200sa_ctx *c, uint32_t n, uint32_t m, uint32_t **l
     }
     if (!bucketed) {
         TRY(mark(c, "lms_sort"));
-        if (wide)
-            TRY((sort_pairs_from<uint32_t, LmsKeyDesc<BITS>, LmsValDesc, 16>(c, kf, vf, ptr<uint32_t>(c->k32b), ptr<uint32_t>(c->v0),
-                                                                             ptr<uint32_t>(c->reduced), ptr<uint32_t>(c->v1), m,
-                                                                             bit_length(range - 1), &Ks, &Ps)));
-        else
-            TRY((sort_pairs_from<uint32_t, LmsKeyDesc<BITS>, LmsValDesc, ITEMS>(c, kf, vf, ptr<uint32_t>(c->k32b), ptr<uint32_t>(c->v0),
-                                                                                ptr<uint32_t>(c->reduced), ptr<uint32_t>(c->v1), m,
-                                                                                bit_length(range - 1), &Ks, &Ps)));
+        TRY(sort_pairs_from(c, kf, vf, ptr<uint32_t>(c->k32b), ptr<uint32_t>(c->v0), ptr<uint32_t>(c->reduced),
+                            ptr<uint32_t>(c->v1), m, bit_length(range - 1), &Ks, &Ps));
         // groups of equal windows; members of non-singleton groups -> active list
         TRY(mark(c, "lms_groups"));
         size_t fw = ((size_t)m + 31) / 32 + 1;
@@ -1207,17 +1187,6 @@ static int build_lcp_dev(b200sa_ctx *c, const uint8_t *d_text, uint64_t n, uint3
         c->stats = st;
     }
     return rc;
-}
-
-// Sorts the cnt ranks of `vals` (the A ranks of b200sa_docs_build) by the key of kf (wider tiles for large inputs, as sort_pairs).
-template <class K, class KeyF>
-static int docs_sort(b200sa_ctx *c, KeyF kf, const uint32_t *vals, K *ka, uint32_t *va, K *kb, uint32_t *vb,
-                     uint32_t cnt, int bits, K **kout, uint32_t **vout) {
-    LoadArr<uint32_t> vf{vals};
-    if (cnt >= (1u << 20))
-        return sort_pairs_from<K, KeyF, LoadArr<uint32_t>, (sizeof(K) == 4 ? 16 : 12)>(c, kf, vf, ka, va, kb, vb, cnt, bits,
-                                                                                       kout, vout);
-    return sort_pairs_from<K, KeyF, LoadArr<uint32_t>, ITEMS>(c, kf, vf, ka, va, kb, vb, cnt, bits, kout, vout);
 }
 
 // ================================================================= C ABI
@@ -1857,19 +1826,19 @@ static int docs_core(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const uin
         int shift;
         if (lb + rb + db <= 64 && !(e2 && atoi(e2) == 1)) {
             DocsKey kf{L, sa, rem, d_starts, alist, ndocs, rb, db, true};
-            TRY(docs_sort<uint64_t>(c, kf, alist, ptr<uint64_t>(c->k64a), v0, ptr<uint64_t>(c->k64b), v1, na,
-                                    lb + rb + db, &K, &V));
+            TRY(sort_pairs_from(c, kf, LoadArr<uint32_t>{alist}, ptr<uint64_t>(c->k64a), v0, ptr<uint64_t>(c->k64b), v1,
+                                na, lb + rb + db, &K, &V));
             shift = rb + db;
         } else {
             // (lo, r, d) does not fit 64 bits: a stable sort by d, then one by (lo, r)
             uint32_t *K1, *V1;
             DocsDocKey kd{sa, d_starts, alist, ndocs};
-            TRY(docs_sort<uint32_t>(c, kd, alist, ptr<uint32_t>(c->k64a), v0, ptr<uint32_t>(c->k64b), v1, na, db,
-                                    &K1, &V1));
+            TRY(sort_pairs_from(c, kd, LoadArr<uint32_t>{alist}, ptr<uint32_t>(c->k64a), v0, ptr<uint32_t>(c->k64b), v1,
+                                na, db, &K1, &V1));
             uint32_t *other = V1 == v0 ? v1 : v0;          // V1 is read only by the first pass of the second sort
             DocsKey kf{L, sa, rem, d_starts, V1, ndocs, rb, 0, false};
-            TRY(docs_sort<uint64_t>(c, kf, V1, ptr<uint64_t>(c->k64a), other, ptr<uint64_t>(c->k64b), V1, na,
-                                    lb + rb, &K, &V));
+            TRY(sort_pairs_from(c, kf, LoadArr<uint32_t>{V1}, ptr<uint64_t>(c->k64a), other, ptr<uint64_t>(c->k64b), V1,
+                                na, lb + rb, &K, &V));
             shift = rb;
         }
         TRY(mark(c, "docs_place"));
@@ -1977,12 +1946,10 @@ static int docs_tree_args(b200sa_ctx *c, uint64_t n, const void *gsa, const void
     return B200SA_OK;
 }
 
-// The tree's document-sort key: the document of a rank.
-template <int OSI>
+// The ranks stably by their document (the tree's document-sort key), in the buffers p0, p1, v0 and v1.
 static int dtree_sort(b200sa_ctx *c, const uint32_t *doc, uint32_t n, int bits, uint32_t **kout, uint32_t **vout) {
-    return sort_pairs_from<uint32_t, LoadArr<uint32_t>, LoadIndex, OSI>(
-        c, LoadArr<uint32_t>{doc}, LoadIndex{}, ptr<uint32_t>(c->p0), ptr<uint32_t>(c->p1), ptr<uint32_t>(c->v0),
-        ptr<uint32_t>(c->v1), n, bits, kout, vout);
+    return sort_pairs_from(c, LoadArr<uint32_t>{doc}, LoadIndex{}, ptr<uint32_t>(c->p0), ptr<uint32_t>(c->p1),
+                           ptr<uint32_t>(c->v0), ptr<uint32_t>(c->v1), n, bits, kout, vout);
 }
 
 // n >= 1, ndocs >= 1, device inputs and outputs (capacity >= 2n each).  Phases: docs_check (when
@@ -2024,8 +1991,7 @@ static int docs_tree_core(b200sa_ctx *c, uint32_t n, const uint32_t *d_g, const 
     TRY(ensure(c, c->p1, (size_t)n * 4));
     uint32_t *dk, *rk;
     const int db = bit_length(ndocs - 1);
-    if (n >= (1u << 20)) TRY(dtree_sort<16>(c, doc, n, db, &dk, &rk));
-    else TRY(dtree_sort<ITEMS>(c, doc, n, db, &dk, &rk));
+    TRY(dtree_sort(c, doc, n, db, &dk, &rk));
     TRY(mark(c, "dtree_pairs"));
     TRY(ensure(c, c->g1, ((size_t)N + 1) * 4));
     uint32_t *pairs = ptr<uint32_t>(c->g1);
@@ -2155,8 +2121,7 @@ static int docs_list_index_core(b200sa_ctx *c, uint32_t n, const uint32_t *d_g, 
     TRY(ensure(c, c->v1, (size_t)n * 4));
     uint32_t *dk, *rk;
     const int db = bit_length(ndocs - 1);
-    if (n >= (1u << 20)) TRY(dtree_sort<16>(c, doc, n, db, &dk, &rk));
-    else TRY(dtree_sort<ITEMS>(c, doc, n, db, &dk, &rk));
+    TRY(dtree_sort(c, doc, n, db, &dk, &rk));
     TRY(mark(c, "dlist_prev"));
     LAUNCH(c, k_dlist_prev, cdiv(n, BLK), dk, rk, n, d_byd, d_prev);
     TRY(mark(c, "end"));
@@ -2798,9 +2763,7 @@ static int unbwt_sort(b200sa_ctx *c, KeyF kf, DevBuf &ka, DevBuf &va, DevBuf &kb
     TRY(ensure(c, kb, (size_t)cnt * 4));
     if (bits > 8) TRY(ensure(c, vb, (size_t)cnt * 4));    // one pass never writes vb
     uint32_t *a = ptr<uint32_t>(ka), *v = ptr<uint32_t>(va), *b = ptr<uint32_t>(kb), *w = ptr<uint32_t>(vb);
-    if (cnt >= (1u << 20) && !getenv("B200SA_SORT_NARROW"))
-        return sort_pairs_from<uint32_t, KeyF, LoadIndex, 16>(c, kf, LoadIndex{}, a, v, b, w, cnt, bits, kout, vout);
-    return sort_pairs_from<uint32_t, KeyF, LoadIndex, ITEMS>(c, kf, LoadIndex{}, a, v, b, w, cnt, bits, kout, vout);
+    return sort_pairs_from(c, kf, LoadIndex{}, a, v, b, w, cnt, bits, kout, vout);
 }
 
 constexpr uint32_t BWT_RULER_DEFAULT = 64;

@@ -83,9 +83,10 @@ def test_random_short(ctx, monkeypatch):
             check(ctx, monkeypatch, t, old_too=(n % 8 == 0))
 
 
-def _text_with_m(target):
-    """A prefix of G_dna whose LMS count is exactly `target`."""
-    base = gen.dna(int(target * 3.6) + 1000, seed=gen.SEED_DNA + target)
+def _text_with_m(target, base=None):
+    """A prefix of `base` (by default G_dna) whose LMS count is exactly `target`."""
+    if base is None:
+        base = gen.dna(int(target * 3.6) + 1000, seed=gen.SEED_DNA + target)
     p = lms_positions(base)
     # a prefix that ends two characters after the target-th LMS position keeps exactly `target` of them
     # (the last character of a prefix is L-type, the character before it cannot become LMS)
