@@ -21,6 +21,7 @@
 #include "common.cuh"
 #include "classify.cuh"
 #include "classify2.cuh"
+#include "classify_packed.cuh"
 #include "induce.cuh"
 #include "induce6.cuh"
 #include "pipeline_kernels.cuh"
@@ -99,6 +100,7 @@ struct b200sa_ctx {
     int nranks = 1, comm_rank = 0;
     DevBuf sh_a, sh_b, sh_c, sh_d, sh_e, sh_f, sh_small;
     bool lms_asc_ready = false;       // c->lmspos / c->lmsrank (text order) valid for the current text
+    bool lms_keys_ready = false;      // k_classify_packed ran: window keys in c->reduced, their digit counts in c->os_hist
     uint32_t scan_epoch = 0, scan_tiles_cap = 0;
     uint32_t sigma = 256;            // distinct bytes of the current text
     int bits = 8;                    // bits per char of the packed text of the current call (2, 4 or 8 = raw)
@@ -286,8 +288,10 @@ static bool os_wide(uint64_t n) {
 // Where the first pass of a one-sweep sort reads its keys.  IN_PLACE: from ka; a sort of no bits leaves (ka, va)
 // as they are.  FROM_FUNCTORS: the histogram kernel gathers them from the key functor into kb (free until the
 // second pass writes it) and the first pass writes (ka, va); at least one pass runs, so the result always lands
-// in a buffer pair.
-enum OsFirst { IN_PLACE, FROM_FUNCTORS };
+// in a buffer pair.  FROM_KEYS: as FROM_FUNCTORS, but a kernel before the sort has already written the keys to kb
+// and the digit counts of every pass to c->os_hist (zeroed, tickets included, before that kernel): no histogram
+// kernel, and keyf is not called.
+enum OsFirst { IN_PLACE, FROM_FUNCTORS, FROM_KEYS };
 
 // Sorts n items by key bits [shift0, shift0 + bits) with the one-sweep passes of common.cuh, OSI keys per
 // thread.  The histogram reads the keys through keyf and the first pass the values through valf; *kout/*vout
@@ -307,9 +311,9 @@ static int os_sort_items(b200sa_ctx *c, KeyF keyf, ValF valf, K *ka, uint32_t *v
     TRY(ensure(c, c->os_status, status_bytes));
     uint32_t *ghist = ptr<uint32_t>(c->os_hist);
     uint32_t *ticket = ghist + OS_MAX_PASSES * 256;
-    CU_TRY(c, cudaMemsetAsync(ghist, 0, OS_MAX_PASSES * 256 * 4 + 64, c->stream));
     uint32_t hb = cdiv(n, TILE) < grid_cap(c) ? cdiv(n, TILE) : grid_cap(c);
-    {
+    if (FIRST != FROM_KEYS) {
+        CU_TRY(c, cudaMemsetAsync(ghist, 0, OS_MAX_PASSES * 256 * 4 + 64, c->stream));
         size_t shm = (size_t)NWARP * npass * 256 * 4;
         auto kfn = k_os_hist<K, KeyF>;
         CU_TRY(c, cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(NWARP * OS_MAX_PASSES * 256 * 4)));
@@ -318,7 +322,7 @@ static int os_sort_items(b200sa_ctx *c, KeyF keyf, ValF valf, K *ka, uint32_t *v
     }
     LAUNCH(c, k_os_scan, (uint32_t)npass, ghist);
     volatile unsigned long long *status = reinterpret_cast<volatile unsigned long long *>(c->os_status.p);
-    if (FIRST == FROM_FUNCTORS) {       // the first pass reads the gathered keys in kb and writes (ka, va)
+    if (FIRST != IN_PLACE) {            // the first pass reads the gathered keys in kb and writes (ka, va)
         std::swap(ka, kb);
         std::swap(va, vb);
     }
@@ -508,8 +512,8 @@ static int reduced_sa(b200sa_ctx *c, uint32_t *R, uint32_t m, uint32_t names, ui
 
 // ------------------------------------------------------- packed text
 // Chooses 2 / 4 bits per char when the alphabet allows it and packs the text;
-// code_of/alpha live in the tables buffer.
-static int pack_text(b200sa_ctx *c, const uint8_t *text, uint64_t n, uint32_t sigma) {
+// code_of/alpha live in the tables buffer.  packed2: the classification already packed a 2-bit text.
+static int pack_text(b200sa_ctx *c, const uint8_t *text, uint64_t n, uint32_t sigma, bool packed2 = false) {
     uint32_t *tab = ptr<uint32_t>(c->tables);
     c->bits = 8;
     c->ptext = text;
@@ -519,8 +523,12 @@ static int pack_text(b200sa_ctx *c, const uint8_t *text, uint64_t n, uint32_t si
     uint32_t cpw = 32 / c->bits;
     uint64_t words = (n + cpw - 1) / cpw;
     TRY(ensure(c, c->packed, words * 4 + 32));  // + padding for text_bits() / text_bits_wide()
-    if (c->bits == 2) LAUNCH(c, (k_pack<2>), cdiv(words, BLK), text, n, tab + T_CODE, ptr<uint32_t>(c->packed));
-    else LAUNCH(c, (k_pack<4>), cdiv(words, BLK), text, n, tab + T_CODE, ptr<uint32_t>(c->packed));
+    if (c->bits == 2 && !packed2)
+        LAUNCH(c, (k_pack<2>), cdiv(words, BLK), text, n, tab + T_CODE, ptr<uint32_t>(c->packed), (const uint32_t *)nullptr,
+               (const uint32_t *)nullptr, (const uint32_t *)nullptr, (uint32_t *)nullptr);
+    else if (c->bits == 4)
+        LAUNCH(c, (k_pack<4>), cdiv(words, BLK), text, n, tab + T_CODE, ptr<uint32_t>(c->packed), (const uint32_t *)nullptr,
+               (const uint32_t *)nullptr, (const uint32_t *)nullptr, (uint32_t *)nullptr);
     CU_TRY(c, cudaGetLastError());
     c->ptext = c->packed.p;
     return B200SA_OK;
@@ -581,8 +589,12 @@ static int lms_direct_sort_t(b200sa_ctx *c, uint32_t n, uint32_t m, uint32_t **l
     bool bucketed = false;
     if (BITS == 2 && !getenv("B200SA_LMS_SORT4")) {
         TRY(mark(c, "lms_sort"));
-        TRY(sort_pairs_from(c, kf, vf, ptr<uint32_t>(c->k32b), ptr<uint32_t>(c->v0), ptr<uint32_t>(c->reduced),
-                            ptr<uint32_t>(c->v1), m, 16, &Ks, &Ps, 16u));
+        if (c->lms_keys_ready)      // k_classify_packed wrote the keys to c->reduced and their digit counts
+            TRY((os_sort<FROM_KEYS>(c, kf, vf, ptr<uint32_t>(c->k32b), ptr<uint32_t>(c->v0), ptr<uint32_t>(c->reduced),
+                                    ptr<uint32_t>(c->v1), (uint64_t)m, 16, 16u, &Ks, &Ps)));
+        else
+            TRY(sort_pairs_from(c, kf, vf, ptr<uint32_t>(c->k32b), ptr<uint32_t>(c->v0), ptr<uint32_t>(c->reduced),
+                                ptr<uint32_t>(c->v1), m, 16, &Ks, &Ps, 16u));
         TRY(mark(c, "lms_groups"));
         uint32_t *Pout = ptr<uint32_t>(c->k32b);                    // keys of the first pass: dead after the second
         CU_TRY(c, cudaMemsetAsync(sm + 16, 0, 12, c->stream));      // [16] tied count, [18] bucket overflow
@@ -775,8 +787,8 @@ static int launch_induce(b200sa_ctx *c, bool spass, const uint8_t *text, uint32_
 
 // ------------------------------------------------------- the level driver
 // After the histogram is known: packed text and the grid of the persistent induce kernels.
-static int post_classify(b200sa_ctx *c, const uint8_t *text, uint64_t n, uint32_t sigma) {
-    TRY(pack_text(c, text, n, sigma));
+static int post_classify(b200sa_ctx *c, const uint8_t *text, uint64_t n, uint32_t sigma, bool packed2 = false) {
+    TRY(pack_text(c, text, n, sigma, packed2));
     // few buckets -> long lists, latency bound -> more blocks per SM; many buckets -> grid-sync bound -> one per SM
     int bps = sigma <= 16 ? 3 : (sigma <= 64 ? 2 : 1);
     if (c->induce_bps_env) bps = c->induce_bps_env;
@@ -789,8 +801,16 @@ static int post_classify(b200sa_ctx *c, const uint8_t *text, uint64_t n, uint32_
 
 // K1 fused (classify2.cuh): one pass -> type / LMS bitmaps, (byte, type) histogram, bucket
 // tables, LMS positions in descending text order (c->lmsdesc), packed text.
+// packed_first: the alphabet is found first (k_byte_hist -> k_alpha_from_hist, sigma on the device; see the
+// sampled packing below) and a
+// text of at most 4 distinct bytes is packed at 2 bits and classified from its packed words by
+// k_classify_packed, which also writes the LMS sort's window keys (c->lms_keys_ready); for a larger
+// alphabet those kernels return at once and k_classify_fused classifies the bytes.  The one host read after
+// the classification stays the only one.  B200SA_CLASSIFY_BYTES=1 (or B200SA_NOPACK) keeps the byte
+// classifier on every text (cross-check).
 static int classify_fused_dev(b200sa_ctx *c, const uint8_t *text, uint64_t n, uint32_t *m_out,
-                              ShardEdge edge = ShardEdge{-1, -1, ST_L}, bool pack = true) {
+                              ShardEdge edge = ShardEdge{-1, -1, ST_L}, bool pack = true, bool packed_first = false) {
+    const bool try2 = packed_first && pack && !getenv("B200SA_CLASSIFY_BYTES") && !getenv("B200SA_NOPACK");
     uint64_t nw = (n + 31) / 32;
     uint32_t nbc = cdiv(nw, CLS_WORDS);
     TRY(ensure(c, c->stype, nw * 4));
@@ -809,15 +829,47 @@ static int classify_fused_dev(b200sa_ctx *c, const uint8_t *text, uint64_t n, ui
     ScanState S;
     TRY(scan_state_for(c, nbc, &S));
     Cls2State CS{ptr<uint32_t>(c->cls_state), (++c->cls_calls) * 8u};
+    const uint32_t *d_sigma2 = nullptr;
+    if (try2) {
+        // The alphabet of the first 1 MiB codes the packing; a byte outside it sets sm[4] (d_miss), and only
+        // then do the alphabet of the whole text and a second packing run, so that a text whose sample holds
+        // its whole alphabet (the usual case) is read once before the classification instead of twice.
+        CU_TRY(c, cudaMemsetAsync(hist, 0, 256 * 4, c->stream));
+        const uint64_t ns = n < (1u << 20) ? n : (1u << 20);
+        uint32_t *d_miss = sm + 4;
+        d_sigma2 = sm + 3;
+        auto byte_grid = [&](uint64_t len) { uint32_t g = cdiv(len, BLK * 64); return g > grid_cap(c) ? grid_cap(c) : g; };
+        uint64_t pw = (n + 15) / 16;
+        TRY(ensure(c, c->packed, pw * 4 + 32));
+        LAUNCH(c, k_byte_hist, byte_grid(ns), text, ns, hist, (const uint32_t *)nullptr);
+        LAUNCH(c, k_alpha_from_hist, 1, hist, tab + T_CODE, tab + T_ALPHA, sm + 3, (const uint32_t *)nullptr);
+        LAUNCH(c, (k_pack<2>), cdiv(pw, BLK), text, n, tab + T_CODE, ptr<uint32_t>(c->packed), d_sigma2,
+               (const uint32_t *)nullptr, (const uint32_t *)hist, d_miss);
+        if (n > ns) {
+            LAUNCH(c, k_byte_hist, byte_grid(n), text, n, hist, (const uint32_t *)d_miss);
+            LAUNCH(c, k_alpha_from_hist, 1, hist, tab + T_CODE, tab + T_ALPHA, sm + 3, (const uint32_t *)d_miss);
+            LAUNCH(c, (k_pack<2>), cdiv(pw, BLK), text, n, tab + T_CODE, ptr<uint32_t>(c->packed), d_sigma2,
+                   (const uint32_t *)d_miss, (const uint32_t *)nullptr, (uint32_t *)nullptr);
+        }
+        // the window keys go where the LMS sort's key gathering would put them; the digit counts of its two
+        // passes (and their tickets) are zeroed here instead of there
+        TRY(ensure(c, c->reduced, (size_t)(n / 2 + 2) * 4));
+        TRY(ensure(c, c->os_hist, OS_MAX_PASSES * 256 * 4 + 64));
+        CU_TRY(c, cudaMemsetAsync(c->os_hist.p, 0, OS_MAX_PASSES * 256 * 4 + 64, c->stream));
+        uint32_t nt2 = (uint32_t)cdiv(n, (uint64_t)CP_TILE_CHARS);
+        LAUNCH(c, k_classify_packed, nt2, ptr<uint32_t>(c->packed), n, nt2, d_sigma2, tab + T_ALPHA, S, CS,
+               ptr<uint32_t>(c->stype), ptr<uint32_t>(c->lmsb), ptr<uint32_t>(c->hist_copies), ptr<uint32_t>(c->lmsdesc),
+               ptr<uint32_t>(c->reduced), ptr<uint32_t>(c->os_hist), sm);
+    }
     // B200SA_CLASSIFY_TMA=1: the tile arrives by one cp.async.bulk (UBLKCP) + mbarrier instead of 512 vector
     // loads.  With several resident one-tile CTAs per SM the load latency is already covered, so the bulk
     // copy buys nothing here and stays opt-in.
     if (getenv("B200SA_CLASSIFY_TMA") == nullptr)
         LAUNCH(c, k_classify_fused<false>, nbc, text, n, nbc, S, CS, ptr<uint32_t>(c->stype), ptr<uint32_t>(c->lmsb),
-               ptr<uint32_t>(c->hist_copies), ptr<uint32_t>(c->lmsdesc), sm, edge);
+               ptr<uint32_t>(c->hist_copies), ptr<uint32_t>(c->lmsdesc), sm, edge, d_sigma2);
     else
         LAUNCH(c, k_classify_fused<true>, nbc, text, n, nbc, S, CS, ptr<uint32_t>(c->stype), ptr<uint32_t>(c->lmsb),
-               ptr<uint32_t>(c->hist_copies), ptr<uint32_t>(c->lmsdesc), sm, edge);
+               ptr<uint32_t>(c->hist_copies), ptr<uint32_t>(c->lmsdesc), sm, edge, d_sigma2);
     LAUNCH(c, k_hist_fold, 1u, ptr<uint32_t>(c->hist_copies), hist);
     LAUNCH(c, k_bucket_tables, 1, hist, tab + T_BSTART, tab + T_LCNT, tab + T_SCNT, tab + T_LMSOFF, tab + T_CODE,
            tab + T_ALPHA, sm + 3);
@@ -826,7 +878,10 @@ static int classify_fused_dev(b200sa_ctx *c, const uint8_t *text, uint64_t n, ui
         CU_TRY(c, cudaMemcpyAsync(c->h_tab, tab + T_BSTART, 513 * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream));
     TRY(read_words(c, sm, 4));
     uint32_t m = c->h_pin[0], sigma = c->h_pin[3];
-    if (pack) TRY(post_classify(c, text, n, sigma));
+    c->lms_keys_ready = try2 && sigma <= 4;
+    if (getenv("B200SA_TRACE"))
+        fprintf(stderr, "[b200sa] classify: sigma=%u, %s\n", sigma, c->lms_keys_ready ? "packed 2-bit words" : "bytes");
+    if (pack) TRY(post_classify(c, text, n, sigma, c->lms_keys_ready));
     c->lms_asc_ready = false;
     *m_out = m;
     return B200SA_OK;
@@ -922,10 +977,11 @@ static int build_dev(b200sa_ctx *c, const uint8_t *d_text, uint64_t n, uint32_t 
     uint32_t m = 0;
     if (getenv("B200SA_CLASSIFY_V1")) {          // three-kernel classifier (classify.cuh) + reversed position list
         TRY(classify_dev(c, text, n, &m));
+        c->lms_keys_ready = false;
         TRY(ensure(c, c->lmsdesc, (size_t)m * 4 + 16));
         if (m > 0) LAUNCH(c, k_reverse_u32, cdiv(m, BLK), ptr<uint32_t>(c->lmspos), m, ptr<uint32_t>(c->lmsdesc));
     } else {
-        TRY(classify_fused_dev(c, text, n, &m));
+        TRY(classify_fused_dev(c, text, n, &m, ShardEdge{-1, -1, ST_L}, true, true));
     }
     c->stats.m = m; c->last_m = m;
     c->stats.induce_blocks = c->cur_induce_blocks;
@@ -1078,8 +1134,8 @@ static int lcp_dev(b200sa_ctx *c, const uint8_t *d_text, uint64_t n, const uint3
         CU_TRY(c, cudaMemsetAsync(tab + T_HIST, 0, 256 * 4, c->stream));
         uint32_t hb = cdiv(n, BLK * 64);
         if (hb > grid_cap(c)) hb = grid_cap(c);
-        LAUNCH(c, k_byte_hist, hb, text, n, tab + T_HIST);
-        LAUNCH(c, k_alpha_from_hist, 1, tab + T_HIST, tab + T_CODE, tab + T_ALPHA, sm + 3);
+        LAUNCH(c, k_byte_hist, hb, text, n, tab + T_HIST, (const uint32_t *)nullptr);
+        LAUNCH(c, k_alpha_from_hist, 1, tab + T_HIST, tab + T_CODE, tab + T_ALPHA, sm + 3, (const uint32_t *)nullptr);
         TRY(read_words(c, sm + 3, 1));
         TRY(pack_text(c, text, n, c->h_pin[0]));
     }
@@ -3741,8 +3797,8 @@ static int lcp_sharded_core(b200sa_ctx *c, uint8_t *d_text, uint64_t n, uint32_t
         CU_TRY(c, cudaMemsetAsync(tab + T_HIST, 0, 256 * 4, c->stream));
         uint32_t hb = cdiv(n, BLK * 64);
         if (hb > grid_cap(c)) hb = grid_cap(c);
-        LAUNCH(c, k_byte_hist, hb, d_text, n, tab + T_HIST);
-        LAUNCH(c, k_alpha_from_hist, 1, tab + T_HIST, tab + T_CODE, tab + T_ALPHA, sm + 3);
+        LAUNCH(c, k_byte_hist, hb, d_text, n, tab + T_HIST, (const uint32_t *)nullptr);
+        LAUNCH(c, k_alpha_from_hist, 1, tab + T_HIST, tab + T_CODE, tab + T_ALPHA, sm + 3, (const uint32_t *)nullptr);
         TRY(read_words(c, sm, 16));
         if (c->h_pin[12] != 0)        // identical on every rank: all fail together
             return fail(c, B200SA_ERR_BAD_ARG, "table is not a permutation of 0..n-1 (index out of range or repeated)");
@@ -3834,6 +3890,42 @@ int b200sa_test_classify(b200sa_ctx *c, const uint8_t *text, uint64_t n, uint32_
 int b200sa_test_classify_fused(b200sa_ctx *c, const uint8_t *text, uint64_t n, uint32_t *stype_words, uint32_t *lms_words,
                                uint32_t *hist768, uint32_t *lmspos_desc, uint64_t cap_lms, uint64_t *m_out) {
     return test_classify(c, true, text, n, stype_words, lms_words, hist768, lmspos_desc, cap_lms, m_out);
+}
+
+// The classification of a host text of at most 4 distinct bytes from its 2-bit packed words
+// (k_classify_packed), copied back: the bitmaps, hist768, the LMS positions in descending order, their
+// window keys and the digit counts of key bits 16-23 / 24-31 (dig512).  A text with a larger alphabet is an
+// argument error.  Only the tests call it, through ctypes; it is not part of the C headers.
+static int test_classify_packed_core(b200sa_ctx *c, const uint8_t *text, uint64_t n, uint32_t *stype_words,
+                                     uint32_t *lms_words, uint32_t *hist768, uint32_t *lmsdesc, uint32_t *keys,
+                                     uint32_t *dig512, uint64_t cap_lms, uint64_t *m_out) {
+    TRY(ensure(c, c->text, n));
+    CU_TRY(c, cudaMemcpyAsync(c->text.p, text, n, cudaMemcpyHostToDevice, c->stream));
+    uint32_t m = 0;
+    TRY(classify_fused_dev(c, ptr<uint8_t>(c->text), n, &m, ShardEdge{-1, -1, ST_L}, true, true));
+    if (!c->lms_keys_ready)
+        return fail(c, B200SA_ERR_BAD_ARG, "test classify packed: the text needs at most 4 distinct bytes");
+    uint64_t nw = (n + 31) / 32, k = m < cap_lms ? m : cap_lms;
+    if (stype_words) CU_TRY(c, cudaMemcpyAsync(stype_words, c->stype.p, nw * 4, cudaMemcpyDeviceToHost, c->stream));
+    if (lms_words) CU_TRY(c, cudaMemcpyAsync(lms_words, c->lmsb.p, nw * 4, cudaMemcpyDeviceToHost, c->stream));
+    if (hist768) CU_TRY(c, cudaMemcpyAsync(hist768, ptr<uint32_t>(c->tables) + T_HIST, 768 * 4, cudaMemcpyDeviceToHost, c->stream));
+    if (lmsdesc && k) CU_TRY(c, cudaMemcpyAsync(lmsdesc, c->lmsdesc.p, k * 4, cudaMemcpyDeviceToHost, c->stream));
+    if (keys && k) CU_TRY(c, cudaMemcpyAsync(keys, c->reduced.p, k * 4, cudaMemcpyDeviceToHost, c->stream));
+    if (dig512) CU_TRY(c, cudaMemcpyAsync(dig512, c->os_hist.p, 512 * 4, cudaMemcpyDeviceToHost, c->stream));
+    CU_TRY(c, cudaStreamSynchronize(c->stream));
+    if (m_out) *m_out = m;
+    return B200SA_OK;
+}
+
+extern "C" int b200sa_test_classify_packed(b200sa_ctx *c, const uint8_t *text, uint64_t n, uint32_t *stype_words,
+                                           uint32_t *lms_words, uint32_t *hist768, uint32_t *lmsdesc, uint32_t *keys,
+                                           uint32_t *dig512, uint64_t cap_lms, uint64_t *m_out) {
+    if (!c) return B200SA_ERR_BAD_ARG;
+    if (!text) return null_ptr(c);
+    if (n < 2 || n > B200SA_MAX_N) return fail(c, B200SA_ERR_BAD_ARG, "test classify packed: n must be in [2, 2^32-4096]");
+    TRY(enter(c, nullptr));
+    return leave(c, test_classify_packed_core(c, text, n, stype_words, lms_words, hist768, lmsdesc, keys, dig512,
+                                              cap_lms, m_out));
 }
 
 static int test_scan_core(b200sa_ctx *c, const uint32_t *in, uint64_t n, int op, uint32_t *out_excl, uint32_t *total) {

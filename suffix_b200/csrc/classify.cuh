@@ -226,16 +226,16 @@ __global__ void __launch_bounds__(BLK) k_bucket_tables(const uint32_t *hist768, 
 }
 
 // Which byte values occur (for b200sa_lcp_dev, which has no classification): hist256[b] = 1 for present
-// bytes -- k_alpha_from_hist only asks "> 0".  16 bytes per load, a 256-bit set per thread in registers.
-__global__ void __launch_bounds__(BLK) k_byte_hist(const uint8_t *__restrict__ text, uint64_t n, uint32_t *hist256) {
-    __shared__ uint32_t s_set[8];
-    if (threadIdx.x < 8) s_set[threadIdx.x] = 0;
+// bytes -- k_alpha_from_hist only asks "> 0".  16 bytes per load; every byte stores a flag to shared memory
+// (one byte extract + one store: a bit set in registers costs eight selects per byte and made the kernel
+// instruction-bound at a third of the HBM bandwidth; equal flags in one word are not bank conflicts).
+// gate (may be null): run only when *gate != 0.
+__global__ void __launch_bounds__(BLK) k_byte_hist(const uint8_t *__restrict__ text, uint64_t n, uint32_t *hist256,
+                                                   const uint32_t *gate) {
+    if (gate && *gate == 0u) return;
+    __shared__ uint8_t s_seen[256];
+    s_seen[threadIdx.x] = 0;
     __syncthreads();
-    uint32_t m[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-    auto put = [&](uint32_t b) {
-#pragma unroll
-        for (int k = 0; k < 8; k++) m[k] |= ((b >> 5) == (uint32_t)k) ? (1u << (b & 31u)) : 0u;
-    };
     const uint64_t nv = n / 16;
     for (uint64_t i = (uint64_t)blockIdx.x * BLK + threadIdx.x; i < nv; i += (uint64_t)gridDim.x * BLK) {
         uint4 v = __ldg(reinterpret_cast<const uint4 *>(text) + i);
@@ -243,21 +243,16 @@ __global__ void __launch_bounds__(BLK) k_byte_hist(const uint8_t *__restrict__ t
 #pragma unroll
         for (int q = 0; q < 4; q++) {
             uint32_t x = wds[q];
-            if (q > 0 && x == wds[q - 1]) continue;
-            put(x & 0xffu); put((x >> 8) & 0xffu); put((x >> 16) & 0xffu); put(x >> 24);
+            s_seen[x & 0xffu] = 1; s_seen[(x >> 8) & 0xffu] = 1; s_seen[(x >> 16) & 0xffu] = 1; s_seen[x >> 24] = 1;
         }
     }
-    if (blockIdx.x == 0) for (uint64_t i = nv * 16 + threadIdx.x; i < n; i += BLK) put(__ldg(text + i));
-#pragma unroll
-    for (int k = 0; k < 8; k++) {
-        uint32_t v = __reduce_or_sync(FULL, m[k]);
-        if (lane_id() == 0 && v) atomicOr(&s_set[k], v);
-    }
+    if (blockIdx.x == 0) for (uint64_t i = nv * 16 + threadIdx.x; i < n; i += BLK) s_seen[__ldg(text + i)] = 1;
     __syncthreads();
-    if ((s_set[threadIdx.x >> 5] >> (threadIdx.x & 31)) & 1u) hist256[threadIdx.x] = 1u;
+    if (s_seen[threadIdx.x]) hist256[threadIdx.x] = 1u;
 }
 __global__ void __launch_bounds__(BLK) k_alpha_from_hist(const uint32_t *hist256, uint32_t *code_of, uint32_t *alpha,
-                                                         uint32_t *sigma) {
+                                                         uint32_t *sigma, const uint32_t *gate) {
+    if (gate && *gate == 0u) return;                 // gate (may be null): as in k_byte_hist
     __shared__ uint32_t s_w[NWARP + 1];
     uint32_t c = threadIdx.x, total;
     uint32_t present = hist256[c] > 0 ? 1u : 0u;
@@ -274,33 +269,56 @@ __global__ void __launch_bounds__(BLK) k_alpha_from_hist(const uint32_t *hist256
 // 32/BITS chars per u32 word, char i at bit (i % CPW) * BITS.  BITS == 8 is the
 // raw byte text.  Small alphabets make the text L2-resident (100 MB DNA ->
 // 25 MB), which turns the random T[s-1] gathers of the induce into L2 hits.
+// Device-side conditions (each may be null), for packing before the host has read the alphabet:
+//   d_sigma  pack only when *d_sigma fits BITS;
+//   gate     pack only when *gate != 0;
+//   present  the codes come from the bytes flagged here (k_byte_hist of a sample of the text); a byte
+//            without a flag sets *d_miss, and the words that hold it are not valid.
 template <int BITS>
 __global__ void __launch_bounds__(BLK) k_pack(const uint8_t *__restrict__ text, uint64_t n,
-                                              const uint32_t *__restrict__ code_of, uint32_t *packed) {
+                                              const uint32_t *__restrict__ code_of, uint32_t *packed,
+                                              const uint32_t *d_sigma, const uint32_t *gate,
+                                              const uint32_t *present, uint32_t *d_miss) {
     constexpr int CPW = 32 / BITS;
+    if (gate && *gate == 0u) return;
+    if (d_sigma && *d_sigma > (1u << BITS)) return;
     __shared__ uint8_t s_lut[256];
-    s_lut[threadIdx.x] = (uint8_t)code_of[threadIdx.x];
+    s_lut[threadIdx.x] = (uint8_t)(code_of[threadIdx.x] | (present && present[threadIdx.x] == 0u ? 0x80u : 0u));
     __syncthreads();
     uint64_t w = (uint64_t)blockIdx.x * BLK + threadIdx.x;
     uint64_t p0 = w * CPW;
     if (p0 >= n) return;
-    uint32_t out = 0;
+    uint32_t out = 0, any = 0;                       // any: OR of the table entries (bit 7: a byte without a code)
+    constexpr uint32_t MASK = (1u << BITS) - 1u;
     if (p0 + CPW <= n) {
         if (CPW == 16) {
             uint4 v = __ldg(reinterpret_cast<const uint4 *>(text + p0));
             uint32_t q[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
-            for (int j = 0; j < 16; j++) out |= (uint32_t)s_lut[(q[j >> 2] >> ((j & 3) * 8)) & 0xffu] << (j * BITS);
+            for (int j = 0; j < 16; j++) {
+                uint32_t e = s_lut[(q[j >> 2] >> ((j & 3) * 8)) & 0xffu];
+                any |= e;
+                out |= (e & MASK) << (j * BITS);
+            }
         } else {
             uint2 v = __ldg(reinterpret_cast<const uint2 *>(text + p0));
             uint32_t q[2] = {v.x, v.y};
 #pragma unroll
-            for (int j = 0; j < 8; j++) out |= (uint32_t)s_lut[(q[j >> 2] >> ((j & 3) * 8)) & 0xffu] << (j * BITS);
+            for (int j = 0; j < 8; j++) {
+                uint32_t e = s_lut[(q[j >> 2] >> ((j & 3) * 8)) & 0xffu];
+                any |= e;
+                out |= (e & MASK) << (j * BITS);
+            }
         }
     } else {
-        for (int j = 0; j < CPW && p0 + j < n; j++) out |= (uint32_t)s_lut[__ldg(text + p0 + j)] << (j * BITS);
+        for (int j = 0; j < CPW && p0 + j < n; j++) {
+            uint32_t e = s_lut[__ldg(text + p0 + j)];
+            any |= e;
+            out |= (e & MASK) << (j * BITS);
+        }
     }
     packed[w] = out;
+    if (d_miss && (any & 0x80u)) *d_miss = 1u;
 }
 
 template <int BITS>

@@ -105,7 +105,10 @@ template <bool TMA>
 __global__ void __launch_bounds__(BLK) k_classify_fused(const uint8_t *__restrict__ text, uint64_t n, uint32_t ntiles,
                                                         ScanState S, Cls2State CS, uint32_t *stype, uint32_t *lmsb,
                                                         uint32_t *hist768, uint32_t *lmspos_desc, uint32_t *d_m,
-                                                        ShardEdge edge) {
+                                                        ShardEdge edge, const uint32_t *d_sigma_packed) {
+    // d_sigma_packed (may be null): the device-side alphabet size when k_classify_packed was launched too;
+    // 2-bit text is its job, so every block returns before it takes a ticket
+    if (d_sigma_packed && *d_sigma_packed <= 4u) return;
     __shared__ uint32_t s_warp[NWARP];
     __shared__ uint32_t s_sw[BLK];
     __shared__ uint32_t s_hist[NWARP][768];

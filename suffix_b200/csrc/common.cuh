@@ -284,7 +284,9 @@ __device__ __forceinline__ typename Op::T tile_walk(const ScanState &S, uint32_t
 __device__ __forceinline__ void tile_publish_u32(const ScanState &S, uint32_t tile, uint32_t block_total) {
     if (tile > 0) st_relaxed_u64(S.pk + tile, ((unsigned long long)(S.epoch + 1u) << 32) | block_total);
 }
-constexpr int LB_K = 1;      // descriptors per lane and round trip: the walk looks at 32 * LB_K predecessors at once
+constexpr int LB_K = 1;      // descriptors per lane and round trip: the walk looks at 32 * K predecessors at once (K = LB_K
+                             // unless the kernel asks for more)
+template <int K = LB_K>
 __device__ __forceinline__ uint32_t tile_walk_u32(const ScanState &S, uint32_t tile, uint32_t block_total, bool last,
                                                   uint32_t *d_total) {
     const uint32_t l = lane_id();
@@ -298,14 +300,14 @@ __device__ __forceinline__ uint32_t tile_walk_u32(const ScanState &S, uint32_t t
         int64_t t0 = (int64_t)tile - 1;
         bool done = false;
         while (!done) {
-            unsigned long long v[LB_K];
+            unsigned long long v[K];
 #pragma unroll
-            for (int j = 0; j < LB_K; j++) {           // nearest predecessors in v[0] (lane 0 nearest)
+            for (int j = 0; j < K; j++) {           // nearest predecessors in v[0] (lane 0 nearest)
                 int64_t tt = t0 - (int64_t)(l + 32u * j);
                 v[j] = tt >= 0 ? ld_relaxed_u64(S.pk + tt) : before;
             }
 #pragma unroll
-            for (int j = 0; j < LB_K; j++) {
+            for (int j = 0; j < K; j++) {
                 if (done) break;
                 int64_t tt = t0 - (int64_t)(l + 32u * j);
                 uint32_t st = (uint32_t)(v[j] >> 32) - S.epoch;
@@ -315,7 +317,7 @@ __device__ __forceinline__ uint32_t tile_walk_u32(const ScanState &S, uint32_t t
                 prefix += __reduce_add_sync(FULL, (l <= first) ? (uint32_t)v[j] : 0u);
                 done = im != 0u;
             }
-            t0 -= 32 * LB_K;
+            t0 -= 32 * K;
         }
     }
     if (l == 0) {
