@@ -733,7 +733,42 @@ int b200sa_unbwt_dev(b200sa_ctx *ctx, uint64_t n, uint32_t ndocs, const uint8_t 
  * the counts and their scan, 4 (2 threshold + 1) bytes per hit for the words, and 8 bytes per query; with
  * B200SA_APPROX_EDIT, 16 bytes of shared memory per row of the longest query in the batch per resident warp
  * (64 KB per warp at B200SA_APPROX_ALIGN_MAX_M).  Phases: those of the call without the flag (with its emission
- * phases even at cap = 0), then align_count, align_scan and, when the listing fits, align_emit, before end. */
+ * phases even at cap = 0), then align_count, align_scan and, when the listing fits, align_emit, before end.
+ *
+ * ---- fixed symbols in IUPAC queries (DESIGN.md 6b f-21) ----
+ * With B200SA_APPROX_FIXED (bit 25) in k, b200sa_docs_approx_positions_dev keeps the lowercase symbols of each
+ * query fixed: they must match their class, and the threshold is spent on the other symbols only.  This is the
+ * usual definition of a CRISPR off-target (a PAM such as "ngg" must match; mismatches and bulges fall in the
+ * spacer).  The flag is accepted by the documents entry alone, and only with B200SA_APPROX_IUPAC; alongside it
+ * it mixes freely with B200SA_APPROX_EDIT, B200SA_APPROX_BEST | B200SA_APPROX_SLACK(s),
+ * B200SA_APPROX_BOTH_STRANDS, B200SA_APPROX_DOCUMENTS and B200SA_APPROX_ALIGN.  A single text goes through that
+ * entry as one document.  On b200sa_approx_positions_dev bit 25 is an unknown bit as before; without
+ * B200SA_APPROX_IUPAC it returns B200SA_ERR_BAD_ARG with a detail that names both flags.  Without the flag nothing
+ * changes.  Definition:
+ *  - A query symbol is fixed when its byte is a lowercase IUPAC letter (a c g t u r y s w k m b d h v n), free
+ *    when it is uppercase.  Classes do not change: lowercase means its uppercase class.  So a batch of uppercase
+ *    queries means exactly what it means without the flag.
+ *  - Hamming: p is an occurrence iff the window fits in its document, every fixed x has T[p + x] in the class of
+ *    q[x], and mis(p), counted over the free x only, is at most the threshold.
+ *  - Edit: dist(p) is the least cost of an alignment as above under three rules: a fixed symbol is aligned as =,
+ *    never X or I; a text byte with no query byte (D) never sits directly before or after a fixed symbol (no D
+ *    move at (x, t) when q[x] is fixed, or x >= 1 and q[x - 1] is fixed); when no alignment keeps the rules,
+ *    dist(p) is infinite.
+ *  - Everything else keeps its meaning on these distances: best(q) and t(q); the strands, rc(q) carrying its
+ *    marks reversed (fixed(rc(q))[x] = fixed(q)[m - 1 - x]); the document listing; and the canonical walk of
+ *    B200SA_APPROX_ALIGN, which takes its first allowed move.  So with B200SA_APPROX_ALIGN no X or I falls on a
+ *    fixed position and no D touches one.
+ *  - So a query with no lowercase symbol gives the call without the flag, bit for bit; the Hamming list is the
+ *    list without the flag filtered to the windows whose fixed symbols match, at unchanged distances; and a query
+ *    whose symbols are all fixed gives, under either metric at any threshold, the Hamming hits at threshold 0.
+ * Method: a mark per query byte (1 = fixed), made from the original bytes beside the canonical copy, follows the
+ * queries through the doubled batch of both strands (reversed for rc(q)), the compacted batches of the best
+ * rounds and the alignment.  The pieces and reporters are those of B200SA_APPROX_IUPAC: the constrained
+ * occurrences are a subset of the unconstrained ones, so one of the threshold + 1 pieces is still intact.
+ * Verification rejects a window on a fixed miss and counts the free misses; the edit band DP and the alignment's
+ * traceback forbid the three moves.  Device workspace (computed, not measured): what the call takes without the
+ * flag, plus 1 byte per query byte for the marks (2 with B200SA_APPROX_BOTH_STRANDS, and as much again for a
+ * compacted batch with B200SA_APPROX_BEST).  Phases: those of the call without the flag. */
 #define B200SA_APPROX_MAX_K 31
 #define B200SA_APPROX_EDIT 0x10000u
 #define B200SA_APPROX_BEST 0x100000u                      /* bit 20 */
@@ -744,6 +779,7 @@ int b200sa_unbwt_dev(b200sa_ctx *ctx, uint64_t n, uint32_t ndocs, const uint8_t 
 #define B200SA_APPROX_DOCUMENTS 0x20000000u               /* bit 29, in k, documents entry only */
 #define B200SA_APPROX_ALIGN 0x8000000u                    /* bit 27, in k, documents entry only */
 #define B200SA_APPROX_ALIGN_MAX_M 4096                    /* the longest query B200SA_APPROX_EDIT aligns */
+#define B200SA_APPROX_FIXED 0x2000000u                    /* bit 25, in k, documents entry only, with B200SA_APPROX_IUPAC */
 int b200sa_approx_positions_dev(b200sa_ctx *ctx, const uint8_t *d_text, uint64_t n, const uint32_t *d_sa,
                                 const uint8_t *d_queries, const uint64_t *d_q_off, uint32_t nq, uint32_t k,
                                 uint64_t *d_offsets, uint32_t *d_pos, uint32_t *d_mismatches, uint64_t cap,

@@ -1,9 +1,9 @@
 """Approximate positions (occurrences with at most k mismatches, or within k edits with metric="edit", with
-best=s only each query's best hits, with iupac=True queries in IUPAC nucleotide codes, and with strands="both" the
-reverse complement's hits as well), the documents that hold them, and their alignments, over a device-resident
-table: the part SuffixTable and DocumentSuffixTable share.  A table supplies `_device` and
-`_bwt_arrays()` -> (d_text, d_table, d_doc_starts or None, ndocs), its text and table on the device; the LCP
-array is not needed."""
+best=s only each query's best hits, with iupac=True queries in IUPAC nucleotide codes, with fixed=True their
+lowercase symbols fixed, and with strands="both" the reverse complement's hits as well), the documents that hold
+them, and their alignments, over a device-resident table: the part SuffixTable and DocumentSuffixTable share.  A
+table supplies `_device` and `_bwt_arrays()` -> (d_text, d_table, d_doc_starts or None, ndocs), its text and table
+on the device; the LCP array is not needed."""
 import numpy as np
 
 from . import _lib
@@ -17,6 +17,7 @@ BOTH_STRANDS = 0x10000000  # B200SA_APPROX_BOTH_STRANDS
 MINUS = 0x80000000        # B200SA_APPROX_MINUS
 DOCUMENTS = 0x20000000    # B200SA_APPROX_DOCUMENTS
 ALIGN = 0x8000000         # B200SA_APPROX_ALIGN
+FIXED = 0x2000000         # B200SA_APPROX_FIXED
 OPS = "MIDNSHP=X"         # the BAM operation codes
 METRICS = {"hamming": 0, "edit": EDIT}
 
@@ -37,6 +38,15 @@ def _iupac(iupac):
     return IUPAC if iupac else 0
 
 
+def _fixed(fixed, iupac):
+    """The k bit of fixed=: B200SA_APPROX_FIXED for True (which needs iupac=True), 0 for False."""
+    if not isinstance(fixed, (bool, np.bool_)):
+        raise ValueError("fixed must be True or False, got %r" % (fixed,))
+    if fixed and not iupac:
+        raise ValueError("fixed=True requires iupac=True")
+    return FIXED if fixed else 0
+
+
 def _strands(strands):
     """The k bit of strands=: 0 for "forward", B200SA_APPROX_BOTH_STRANDS for "both"."""
     if not isinstance(strands, str) or strands not in ("forward", "both"):
@@ -45,7 +55,7 @@ def _strands(strands):
 
 
 def _call(table, queries, k, fetch, metric="hamming", best=None, iupac=False, strands="forward", documents=False,
-          align=False):
+          align=False, fixed=False):
     """(offsets u64[nq + 1], positions u32[], distances u32[]); positions and distances are None without
     fetch (the cap = 0 call).  metric "hamming" counts mismatches, "edit" the Levenshtein distance; best=s keeps
     each query's occurrences within s of its least distance (include/b200sa.h, B200SA_APPROX_BEST); iupac=True reads
@@ -53,21 +63,23 @@ def _call(table, queries, k, fetch, metric="hamming", best=None, iupac=False, st
     (B200SA_APPROX_IUPAC); strands="both" adds the reverse complement's occurrences, the distances of those carrying
     B200SA_APPROX_MINUS (B200SA_APPROX_BOTH_STRANDS); documents=True (a DocumentSuffixTable only) lists the
     documents that hold q's hits instead, with the least distance in each (B200SA_APPROX_DOCUMENTS); align=True
-    lists the alignment operations of q's hits instead, as (offsets, p, BAM word) entries (B200SA_APPROX_ALIGN),
-    a single text going through the documents entry as one document."""
+    lists the alignment operations of q's hits instead, as (offsets, p, BAM word) entries (B200SA_APPROX_ALIGN);
+    fixed=True (with iupac=True) keeps the lowercase query symbols fixed: they must match their class and take no
+    edit, and the threshold is spent on the uppercase ones (B200SA_APPROX_FIXED).  With align or fixed a single
+    text goes through the documents entry as one document."""
     import torch
     k = int(k)
     if not 0 <= k <= MAX_K:
         raise ValueError("k must be in 0 .. %d, got %d" % (MAX_K, k))
     if metric not in METRICS:
         raise ValueError("metric must be 'hamming' or 'edit', got %r" % (metric,))
-    kf = (k | METRICS[metric] | _flags(best) | _iupac(iupac) | _strands(strands) | (DOCUMENTS if documents else 0) |
-          (ALIGN if align else 0))
+    kf = (k | METRICS[metric] | _flags(best) | _iupac(iupac) | _fixed(fixed, iupac) | _strands(strands) |
+          (DOCUMENTS if documents else 0) | (ALIGN if align else 0))
     qs = [_as_bytes(q) for q in queries]
     nq, n = len(qs), len(table)
     d_t, d_r, d_s, ndocs = table._bwt_arrays()
     dev = torch.device("cuda", table._device)
-    if align and d_s is None:
+    if (align or fixed) and d_s is None:
         d_s, ndocs = _one_document(table, dev), 1
     off = np.zeros(nq + 1, dtype=np.uint64)
     off[1:] = np.cumsum([len(q) for q in qs])
@@ -105,41 +117,41 @@ def _split(dist):
     return dist & np.uint32(MINUS - 1), (dist & np.uint32(MINUS)) != 0
 
 
-def positions_batch(table, queries, k, metric="hamming", best=None, iupac=False, strands="forward"):
-    off, pos, dist = _call(table, queries, k, True, metric, best, iupac, strands)
+def positions_batch(table, queries, k, metric="hamming", best=None, iupac=False, strands="forward", fixed=False):
+    off, pos, dist = _call(table, queries, k, True, metric, best, iupac, strands, fixed=fixed)
     if strands == "forward":
         return off, pos, dist
     return (off, pos) + _split(dist)
 
 
-def positions(table, query, k, metric="hamming", best=None, iupac=False, strands="forward"):
-    _, pos, dist = _call(table, [query], k, True, metric, best, iupac, strands)
+def positions(table, query, k, metric="hamming", best=None, iupac=False, strands="forward", fixed=False):
+    _, pos, dist = _call(table, [query], k, True, metric, best, iupac, strands, fixed=fixed)
     if strands == "forward":
         return pos, dist
     return (pos,) + _split(dist)
 
 
-def counts(table, queries, k, metric="hamming", best=None, iupac=False, strands="forward"):
-    off, _, _ = _call(table, queries, k, False, metric, best, iupac, strands)
+def counts(table, queries, k, metric="hamming", best=None, iupac=False, strands="forward", fixed=False):
+    off, _, _ = _call(table, queries, k, False, metric, best, iupac, strands, fixed=fixed)
     return np.diff(off.astype(np.int64)).astype(np.uint64)
 
 
-def documents_batch(table, queries, k, metric="hamming", best=None, iupac=False, strands="forward"):
-    off, docs, dist = _call(table, queries, k, True, metric, best, iupac, strands, documents=True)
+def documents_batch(table, queries, k, metric="hamming", best=None, iupac=False, strands="forward", fixed=False):
+    off, docs, dist = _call(table, queries, k, True, metric, best, iupac, strands, documents=True, fixed=fixed)
     if strands == "forward":
         return off, docs, dist
     return (off, docs) + _split(dist)
 
 
-def documents(table, query, k, metric="hamming", best=None, iupac=False, strands="forward"):
-    _, docs, dist = _call(table, [query], k, True, metric, best, iupac, strands, documents=True)
+def documents(table, query, k, metric="hamming", best=None, iupac=False, strands="forward", fixed=False):
+    _, docs, dist = _call(table, [query], k, True, metric, best, iupac, strands, documents=True, fixed=fixed)
     if strands == "forward":
         return docs, dist
     return (docs,) + _split(dist)
 
 
-def document_frequencies(table, queries, k, metric="hamming", best=None, iupac=False, strands="forward"):
-    off, _, _ = _call(table, queries, k, False, metric, best, iupac, strands, documents=True)
+def document_frequencies(table, queries, k, metric="hamming", best=None, iupac=False, strands="forward", fixed=False):
+    off, _, _ = _call(table, queries, k, False, metric, best, iupac, strands, documents=True, fixed=fixed)
     return np.diff(off.astype(np.int64)).astype(np.uint32)
 
 
@@ -181,13 +193,13 @@ def _hits(off, pos, words):
             cigar)
 
 
-def alignments_batch(table, queries, k, metric="hamming", best=None, iupac=False, strands="forward"):
-    off, pos, words = _call(table, queries, k, True, metric, best, iupac, strands, align=True)
+def alignments_batch(table, queries, k, metric="hamming", best=None, iupac=False, strands="forward", fixed=False):
+    off, pos, words = _call(table, queries, k, True, metric, best, iupac, strands, align=True, fixed=fixed)
     hoff, p, dist, minus, ends, cigar_off, cigar = _hits(off, pos, words)
     if strands == "forward":
         return hoff, p, dist, ends, cigar_off, cigar
     return hoff, p, dist, minus, ends, cigar_off, cigar
 
 
-def alignments(table, query, k, metric="hamming", best=None, iupac=False, strands="forward"):
-    return alignments_batch(table, [query], k, metric, best, iupac, strands)[1:]
+def alignments(table, query, k, metric="hamming", best=None, iupac=False, strands="forward", fixed=False):
+    return alignments_batch(table, [query], k, metric, best, iupac, strands, fixed)[1:]

@@ -15,6 +15,9 @@
 // shared memory; lane 0 then walks them forward from (0, p).  Every cell of the canonical walk lies in the band,
 // and a neighbour that is on an optimal continuation has an in-band optimal path, so the banded choices are the
 // full DP's.  D(0, p) must equal the staged d; a difference sets the error word (never expected).
+// B200SA_APPROX_FIXED (DESIGN 6b f-21): the Hamming words need nothing new (a fixed position of a hit always
+// matches); k_align_edit<true> keeps X and I off fixed symbols and has no D in a row x where Q[x] or Q[x - 1] is
+// fixed, in its DP and in its move choices, so the walk takes the first allowed move.
 #pragma once
 #include "iupac.cuh"
 #include "strand.cuh"
@@ -33,6 +36,7 @@ struct AlignArgs {
     const uint8_t *qs;
     const uint64_t *qoff;
     uint32_t nq;
+    uint32_t fixed;                          // B200SA_APPROX_FIXED: the marks of the query bytes start at qs + fixed
     const unsigned long long *hoff;
     const uint32_t *hpos, *hmis;
     uint64_t htotal;
@@ -96,7 +100,8 @@ __global__ void __launch_bounds__(BLK) k_align_hamming(AlignArgs A) {
 }
 
 // One warp per staged hit; rows words of dynamic shared memory (4 per query row) per warp, rows >= the longest
-// query of the batch.  The block has blockDim.x / 32 warps.
+// query of the batch.  The block has blockDim.x / 32 warps.  FIXED: A.fixed marks the fixed symbols of q.
+template <bool FIXED>
 __global__ void __launch_bounds__(BLK) k_align_edit(AlignArgs A, uint32_t rows) {
     extern __shared__ uint4 s_moves[];
     const uint32_t l = lane_id(), w = threadIdx.x >> 5;
@@ -112,8 +117,15 @@ __global__ void __launch_bounds__(BLK) k_align_edit(AlignArgs A, uint32_t rows) 
     auto tt = [&](uint32_t x, int32_t j) { return (int64_t)p + x + j - (int32_t)d; };
     auto in = [&](uint32_t x, int32_t j) { const int64_t t = tt(x, j); return j < W && t >= p && t <= E; };
     int32_t r0 = in(Q.m, j0) ? 0 : INF, r1 = in(Q.m, j1) ? 0 : INF;   // row m: D(m, t) = 0
+    const uint8_t *__restrict__ mk = Q.q + A.fixed;
+    auto fixed = [&](uint32_t x) { return __ldg(mk + (Q.minus ? Q.m - 1 - x : x)) != 0; };   // Q[x] is fixed
     for (uint32_t x = Q.m; x-- > 0;) {
         const uint32_t qc = Q.at(x);
+        bool fx = false, nodel = false;                           // Q[x] is fixed; the row has no D move
+        if constexpr (FIXED) {
+            fx = fixed(x);
+            nodel = fx || (x > 0 && fixed(x - 1));
+        }
         // the row below at diagonal j - 1 (the insertion's source)
         int32_t u0 = __shfl_up_sync(0xffffffffu, r0, 1), u1 = __shfl_up_sync(0xffffffffu, r1, 1);
         const int32_t top = __shfl_sync(0xffffffffu, r0, 31);
@@ -121,33 +133,36 @@ __global__ void __launch_bounds__(BLK) k_align_edit(AlignArgs A, uint32_t rows) 
         int32_t a0 = INF, a1 = INF, m0 = 1, m1 = 1;
         const bool v0 = in(x, j0), v1 = in(x, j1);
         const int64_t t0 = tt(x, j0), t1 = tt(x, j1);
+        // a fixed Q[x] takes only the diagonal, and only on a match
         if (v0) {
-            if (t0 < E) { m0 = !Q.match(__ldg(A.text + t0), qc); a0 = r0 + m0; }
-            a0 = min(a0, u0 + 1);
+            if (t0 < E) { m0 = !Q.match(__ldg(A.text + t0), qc); a0 = fx && m0 ? INF : r0 + m0; }
+            if (!fx) a0 = min(a0, u0 + 1);
         }
         if (v1) {
-            if (t1 < E) { m1 = !Q.match(__ldg(A.text + t1), qc); a1 = r1 + m1; }
-            a1 = min(a1, u1 + 1);
+            if (t1 < E) { m1 = !Q.match(__ldg(A.text + t1), qc); a1 = fx && m1 ? INF : r1 + m1; }
+            if (!fx) a1 = min(a1, u1 + 1);
         }
-        // the deletion: D(j) = min over j' >= j of a(j') + j' - j, a suffix minimum of a + j
+        // the deletion: D(j) = min over j' >= j of a(j') + j' - j, a suffix minimum of a + j (uniform: nodel)
         int32_t s0 = min(a0, INF) + j0, s1 = min(a1, INF) + j1;
-        if (wide) {
+        if (!nodel) {
+            if (wide) {
+#pragma unroll
+                for (int o = 1; o < 32; o <<= 1) {
+                    const int32_t y = __shfl_down_sync(0xffffffffu, s1, o);
+                    if (l + o < 32) s1 = min(s1, y);
+                }
+            }
 #pragma unroll
             for (int o = 1; o < 32; o <<= 1) {
-                const int32_t y = __shfl_down_sync(0xffffffffu, s1, o);
-                if (l + o < 32) s1 = min(s1, y);
+                const int32_t y = __shfl_down_sync(0xffffffffu, s0, o);
+                if (l + o < 32) s0 = min(s0, y);
             }
+            if (wide) s0 = min(s0, __shfl_sync(0xffffffffu, s1, 0));
         }
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const int32_t y = __shfl_down_sync(0xffffffffu, s0, o);
-            if (l + o < 32) s0 = min(s0, y);
-        }
-        if (wide) s0 = min(s0, __shfl_sync(0xffffffffu, s1, 0));
         const int32_t n0 = v0 ? min(s0 - j0, INF) : INF, n1 = v1 ? min(s1 - j1, INF) : INF;
-        // the first move that holds: 1 diagonal, 2 insertion, 3 deletion
-        const uint32_t c0 = (t0 < E && n0 == r0 + m0) ? 1u : n0 == u0 + 1 ? 2u : 3u;
-        const uint32_t c1 = (t1 < E && n1 == r1 + m1) ? 1u : n1 == u1 + 1 ? 2u : 3u;
+        // the first move that holds and is allowed: 1 diagonal, 2 insertion, 3 deletion
+        const uint32_t c0 = (t0 < E && !(fx && m0) && n0 == r0 + m0) ? 1u : !fx && n0 == u0 + 1 ? 2u : 3u;
+        const uint32_t c1 = (t1 < E && !(fx && m1) && n1 == r1 + m1) ? 1u : !fx && n1 == u1 + 1 ? 2u : 3u;
         const uint32_t b0 = __ballot_sync(0xffffffffu, c0 & 1u), b1 = __ballot_sync(0xffffffffu, c0 & 2u);
         const uint32_t b2 = __ballot_sync(0xffffffffu, c1 & 1u), b3 = __ballot_sync(0xffffffffu, c1 & 2u);
         if (l == 0) mv[x] = make_uint4(b0, b1, b2, b3);

@@ -110,8 +110,8 @@ struct CutStep {
 };
 
 // The pieces of a query, as a policy of the walks of k_approx (verify) and k_approx_edit (CLASSES, whole_hits,
-// reports): f-14's pieces and byte equality here, the piece table and the class test (miss) of IupacPieces
-// (iupac.cuh).  whole(slot, m): whether the slot is the whole table; off: the offset of piece j.
+// reports, FIXED): f-14's pieces and byte equality here, the piece table and the class test (miss) of IupacPieces
+// and FixedIupacPieces (iupac.cuh).  whole(slot, m): whether the slot is the whole table; off: the offset of piece j.
 struct CutPieces {
     static __device__ __forceinline__ bool whole(const ApproxArgs &A, uint32_t, uint32_t m) { return m <= A.k; }
     static __device__ __forceinline__ uint32_t off(const ApproxArgs &A, uint32_t, uint32_t m, uint32_t j) {
@@ -148,6 +148,7 @@ struct CutPieces {
         return true;
     }
     static constexpr bool CLASSES = false;      // byte equality, which edit_verify tests inline
+    static constexpr bool FIXED = false;        // every query symbol may take an edit
     // dist(s) <= m <= k in the whole-table slot
     static __device__ __forceinline__ uint64_t whole_hits(const uint8_t *, int32_t k) { return 1ull << k; }
     static __device__ __noinline__ bool reports(const ApproxArgs &A, int64_t p, uint32_t s,

@@ -89,7 +89,8 @@ struct b200sa_ctx {
     DevBuf packed, scan_state, cls_state, lmsdesc, steplog, hist_copies;
     DevBuf tree_out;                           // output staging of b200sa_suffix_tree
     DevBuf docs_starts, docs_out;              // doc_starts and output staging of b200sa_docs_build
-    DevBuf icode;                              // approx positions with B200SA_APPROX_IUPAC: the canonical queries
+    DevBuf icode;                              // approx positions with B200SA_APPROX_IUPAC: the canonical queries,
+                                               // then with B200SA_APPROX_FIXED their marks
     DevBuf strand, sstage;                     // with B200SA_APPROX_BOTH_STRANDS: the doubled batch, the staged hits
     DevBuf adoff, adocs;                       // with B200SA_APPROX_DOCUMENTS: the hit offsets, the staged hits
     DevBuf aops;                               // with B200SA_APPROX_ALIGN: each hit's operations
@@ -2912,11 +2913,11 @@ int b200sa_unbwt_dev(b200sa_ctx *c, uint64_t n, uint32_t ndocs, const uint8_t *d
     return leave(c, unbwt_core(c, (uint32_t)n, ndocs, d_bwt, d_term_rows, d_text_out, d_doc_starts_out));
 }
 
-// ------------------------------------------------------------ approximate positions (DESIGN 6b f-14 .. f-20)
+// ------------------------------------------------------------ approximate positions (DESIGN 6b f-14 .. f-21)
 // The k of a call as approx_args decodes it: the threshold, B200SA_APPROX_BEST's slack, and the flags.
 struct ApproxFlags {
     uint32_t k, s;
-    bool edit, best, iupac, both, docs, align;
+    bool edit, best, iupac, fixed, both, docs, align;
     bool stage;                                          // docs || align: the final lists go to staging
 };
 
@@ -2958,11 +2959,13 @@ static int approx_nothing(b200sa_ctx *c, uint64_t *d_offsets, uint32_t nq) {
 }
 
 // B200SA_APPROX_IUPAC: the canonical copy of the q_bytes query bytes into c->icode (*out), or BAD_ARG naming the
-// first byte that is not an IUPAC letter.  Phase approx_check.
-static int iupac_canon(b200sa_ctx *c, const uint8_t *d_queries, uint64_t q_bytes, const uint8_t **out) {
+// first byte that is not an IUPAC letter; with fixed (B200SA_APPROX_FIXED) the marks of the fixed bytes after it
+// (*marks, k_iupac_marks).  Phase approx_check.
+static int iupac_canon(b200sa_ctx *c, const uint8_t *d_queries, uint64_t q_bytes, bool fixed, const uint8_t **out,
+                       const uint8_t **marks) {
     typedef unsigned long long u64;
     uint32_t *words = ptr<uint32_t>(c->small);
-    TRY(ensure(c, c->icode, (size_t)q_bytes));
+    TRY(ensure(c, c->icode, (size_t)q_bytes * (fixed ? 2 : 1)));
     CU_TRY(c, cudaMemsetAsync(words + AW_IUPAC_BAD, 0xFF, 8, c->stream));
     if (q_bytes > 0)
         LAUNCH(c, k_iupac_code, cdiv(q_bytes, BLK), d_queries, q_bytes, ptr<uint8_t>(c->icode),
@@ -2979,13 +2982,20 @@ static int iupac_canon(b200sa_ctx *c, const uint8_t *d_queries, uint64_t q_bytes
         return fail(c, B200SA_ERR_BAD_ARG, m);
     }
     *out = ptr<uint8_t>(c->icode);
+    if (fixed) {
+        *marks = ptr<uint8_t>(c->icode) + q_bytes;
+        if (q_bytes > 0)
+            LAUNCH(c, k_iupac_marks, cdiv(q_bytes, BLK), d_queries, q_bytes, ptr<uint8_t>(c->icode) + q_bytes);
+    }
     return B200SA_OK;
 }
 
-// The count (EMIT false) or emit pass of the search for the metric and the query alphabet.
+// The count (EMIT false) or emit pass of the search for the metric and the query alphabet (fixed: IUPAC queries
+// with fixed symbols).
 typedef void (*ApproxKernel)(ApproxArgs, uint32_t *, const unsigned long long *, int, unsigned long long *, uint32_t *);
 template <bool EMIT>
-static ApproxKernel approx_kernel(bool edit, bool iupac) {
+static ApproxKernel approx_kernel(bool edit, bool iupac, bool fixed) {
+    if (fixed) return edit ? k_approx_edit_iupac_fixed<EMIT> : k_approx_iupac_fixed<EMIT>;
     if (iupac) return edit ? k_approx_edit_iupac<EMIT> : k_approx_iupac<EMIT>;
     return edit ? k_approx_edit<EMIT> : k_approx<EMIT>;
 }
@@ -2994,22 +3004,28 @@ static ApproxKernel approx_kernel(bool edit, bool iupac) {
 // 0 < total <= cap it also emits and sorts: *ko / *vo then hold the keys (q << *pbits) | p in (q, p) order and
 // their distances.  Phases: approx_pieces, approx_scan, approx_count, and approx_emit, approx_sort when it
 // emits.  B200SA_APPROX_EDIT picks k_approx_edit over k_approx; iupac (d_queries then the canonical copy) picks
-// the pieces of k_iupac_pieces and the kernels' IUPAC instantiations; everything else is shared.
+// the pieces of k_iupac_pieces and the kernels' IUPAC instantiations; d_fixed, the marks of the queries' fixed
+// symbols (B200SA_APPROX_FIXED, with iupac) or NULL, their fixed instantiations, with the pointer after the piece
+// table (iupac_marks); everything else is shared.
 template <class EndF>
 static int approx_search(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const uint32_t *d_sa,
                          const uint32_t *d_starts, uint32_t ndocs, const uint8_t *d_queries, const uint64_t *d_q_off,
-                         uint32_t nq, uint32_t k, bool edit, bool iupac, uint64_t *d_offsets, uint64_t cap,
+                         const uint8_t *d_fixed, uint32_t nq, uint32_t k, bool edit, bool iupac, uint64_t *d_offsets,
+                         uint64_t cap,
                          uint64_t *total, EndF end, uint64_t **ko, uint32_t **vo, int *pbits_out) {
     typedef unsigned long long u64;
     uint32_t *words = ptr<uint32_t>(c->small);
     const uint32_t P = k + 1;
     const uint64_t nslots = (uint64_t)nq * P;
     TRY(mark(c, "approx_pieces"));
-    TRY(ensure(c, c->p1, (size_t)nslots * (iupac ? 16 : 8)));   // with iupac, the piece table follows pe
+    // with iupac the piece table follows pe, and with d_fixed the pointer to the marks follows the table
+    TRY(ensure(c, c->p1, (size_t)nslots * (iupac ? 16 : 8) + (d_fixed ? 8 : 0)));
     uint32_t *ps = ptr<uint32_t>(c->p1), *pe = ps + nslots;
     if (iupac) {
         LAUNCH(c, (k_iupac_pieces<EndF>), cdiv(nq, BLK), d_text, n, d_sa, d_queries, d_q_off, nq, P, ps, pe,
                reinterpret_cast<uint2 *>(pe + nslots), end);
+        if (d_fixed)
+            CU_TRY(c, cudaMemcpyAsync(pe + 3 * nslots, &d_fixed, sizeof d_fixed, cudaMemcpyHostToDevice, c->stream));
     } else {
         LAUNCH(c, (k_approx_pieces<EndF>), cdiv(nslots, BLK), d_text, n, d_sa, d_queries, d_q_off, nq, P, ps, pe, end);
     }
@@ -3029,11 +3045,12 @@ static int approx_search(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const
     TRY(ensure(c, c->k64b, ((size_t)items + 1) * 8));
     uint32_t *cnt = ptr<uint32_t>(c->p0);
     u64 *item_off = ptr<u64>(c->k64b);
+    const bool fixed = d_fixed != nullptr;
     const ApproxArgs A{d_text, d_sa, d_starts, ndocs, n, d_queries, d_q_off, (uint32_t)nslots, P, k, ps, pe,
                        item_start, items};
     const int pbits = bit_length(n - 1);
     if (items)
-        LAUNCH(c, approx_kernel<false>(edit, iupac), cdiv(items, NWARP), A, cnt, (const u64 *)nullptr, pbits,
+        LAUNCH(c, approx_kernel<false>(edit, iupac, fixed), cdiv(items, NWARP), A, cnt, (const u64 *)nullptr, pbits,
                (u64 *)nullptr, (uint32_t *)nullptr);
     TRY((dev_scan<OpSum64>(c, InCount64{cnt, items}, OutStoreExcl64{item_off}, items + 1, d_total)));
     LAUNCH(c, k_dlist_qoff, cdiv((uint64_t)nq + 1, BLK), item_start, item_off, nq, P,
@@ -3047,7 +3064,7 @@ static int approx_search(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const
         TRY(ensure(c, c->g1, (size_t)*total * 8));
         TRY(ensure(c, c->v0, (size_t)*total * 4));
         TRY(ensure(c, c->v1, (size_t)*total * 4));
-        LAUNCH(c, approx_kernel<true>(edit, iupac), cdiv(items, NWARP), A, cnt, (const u64 *)item_off, pbits,
+        LAUNCH(c, approx_kernel<true>(edit, iupac, fixed), cdiv(items, NWARP), A, cnt, (const u64 *)item_off, pbits,
                ptr<u64>(c->g0), ptr<uint32_t>(c->v0));
         TRY(mark(c, "approx_sort"));                     // by (q, p)
         TRY(sort_pairs<uint64_t>(c, ptr<uint64_t>(c->g0), ptr<uint32_t>(c->v0), ptr<uint64_t>(c->g1),
@@ -3070,15 +3087,21 @@ static int strand_check(b200sa_ctx *c, uint64_t q_bytes, uint32_t nq, uint32_t k
 
 // The doubled batch (strand.cuh) of the nq queries in c->strand: *eq / *eoff its 2 q_bytes bytes and 2 nq + 1
 // offsets, *doff room for the 2 nq + 1 offsets of its search.  canon: d_queries is the IUPAC canonical copy.
-// Phase strand_queries.
+// fixed (B200SA_APPROX_FIXED): the marks of d_queries, doubled after the bytes into *efx by the same kernel, whose
+// complement leaves the bytes 0 and 1 as they are, so rc(q)'s marks are q's reversed.  Phase strand_queries.
 static int strand_queries(b200sa_ctx *c, const uint8_t *d_queries, const uint64_t *d_q_off, uint32_t nq,
-                          uint64_t q_bytes, bool canon, const uint8_t **eq, const uint64_t **eoff, uint64_t **doff) {
+                          uint64_t q_bytes, bool canon, const uint8_t *fixed, const uint8_t **eq,
+                          const uint64_t **eoff, uint64_t **doff, const uint8_t **efx) {
     TRY(mark(c, "strand_queries"));
     const size_t ne1 = (size_t)2 * nq + 1;
-    TRY(ensure(c, c->strand, ne1 * 16 + (size_t)q_bytes * 2));
+    TRY(ensure(c, c->strand, ne1 * 16 + (size_t)q_bytes * (fixed ? 4 : 2)));
     uint64_t *o2 = ptr<uint64_t>(c->strand);
     uint8_t *q2 = reinterpret_cast<uint8_t *>(o2 + 2 * ne1);
     LAUNCH(c, k_strand_queries, cdiv((uint64_t)nq * 32, BLK), d_queries, d_q_off, nq, canon, q2, o2);
+    if (fixed) {                                         // writes the same offsets again
+        LAUNCH(c, k_strand_queries, cdiv((uint64_t)nq * 32, BLK), fixed, d_q_off, nq, false, q2 + 2 * q_bytes, o2);
+        *efx = q2 + 2 * q_bytes;
+    }
     *eq = q2;
     *eoff = o2;
     *doff = o2 + ne1;
@@ -3168,11 +3191,12 @@ static int align_check(b200sa_ctx *c, const uint64_t *d_q_off, uint32_t nq, bool
 // B200SA_APPROX_ALIGN: the staged final lists (*total hits at offsets hoff, from adocs_stage) aligned into the
 // caller's offsets and, when the listing fits cap, d_pos and d_mis; *total becomes the number of operations.  qs:
 // the queries (the canonical copy with iupac), k the threshold, mmax the longest query.  Phases align_count,
-// align_scan and align_emit.
+// align_scan and align_emit.  fixed: the marks of qs with B200SA_APPROX_FIXED (k_align_edit<true>), after qs in
+// its buffer; else NULL.
 static int align_list(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const uint32_t *d_starts, uint32_t ndocs,
-                      const uint8_t *qs, const uint64_t *d_q_off, uint32_t nq, uint32_t k, bool edit, bool iupac,
-                      uint32_t mmax, const uint64_t *hoff, uint64_t *d_offsets, uint32_t *d_pos, uint32_t *d_mis,
-                      uint64_t cap, uint64_t *total) {
+                      const uint8_t *qs, const uint64_t *d_q_off, const uint8_t *fixed, uint32_t nq, uint32_t k,
+                      bool edit, bool iupac, uint32_t mmax, const uint64_t *hoff, uint64_t *d_offsets,
+                      uint32_t *d_pos, uint32_t *d_mis, uint64_t cap, uint64_t *total) {
     typedef unsigned long long u64;
     const uint64_t htotal = *total;
     TRY(mark(c, "align_count"));
@@ -3186,16 +3210,18 @@ static int align_list(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const ui
     const uint32_t stride = 2 * k + 1;
     TRY(ensure(c, c->aops, (size_t)htotal * stride * 4));
     CU_TRY(c, cudaMemsetAsync(words + AW_ALIGN_ERR, 0, 4, c->stream));
-    const AlignArgs A{d_text, d_starts, ndocs, n, qs, d_q_off, nq, (const u64 *)hoff, hpos, hmis, htotal, iupac,
-                      stride, ptr<uint32_t>(c->aops), cnt, words + AW_ALIGN_ERR};
+    const AlignArgs A{d_text, d_starts, ndocs, n, qs, d_q_off, nq, fixed ? (uint32_t)(fixed - qs) : 0u,
+                      (const u64 *)hoff, hpos, hmis, htotal, iupac, stride, ptr<uint32_t>(c->aops), cnt,
+                      words + AW_ALIGN_ERR};
     if (edit) {
         // 16 bytes of choices per query row and warp: as many warps per block (up to 8) as fit 48 KB, at least one
         const size_t per_warp = (size_t)max(mmax, 1u) * 16;
         const uint32_t aw = (uint32_t)std::max<size_t>(1, std::min<size_t>(NWARP, 49152 / per_warp));
         const size_t smem = per_warp * aw;
+        void (*kernel)(AlignArgs, uint32_t) = fixed ? k_align_edit<true> : k_align_edit<false>;
         if (smem > 49152)
-            CU_TRY(c, cudaFuncSetAttribute(k_align_edit, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        k_align_edit<<<(uint32_t)cdiv(htotal, aw), aw * 32, smem, c->stream>>>(A, max(mmax, 1u));
+            CU_TRY(c, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        kernel<<<(uint32_t)cdiv(htotal, aw), aw * 32, smem, c->stream>>>(A, max(mmax, 1u));
         c->launches++;
     } else {
         LAUNCH(c, k_align_hamming, cdiv(htotal, BLK), A);
@@ -3219,10 +3245,12 @@ static int align_list(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const ui
 
 // The batch a BestPick selects: *nb queries, map[i] the query of entry i; their bytes and offsets at *bq / *boff,
 // the call's own arrays when every query is picked, else gathered into c->qbuf and coff.  Pick: BestPick, or
-// StrandPick over the entries of the doubled batch.
+// StrandPick over the entries of the doubled batch.  fx (B200SA_APPROX_FIXED, else NULL): the queries' marks,
+// which *bfx gets in the same way, gathered into fx_out.
 template <class Pick>
-static int best_batch(b200sa_ctx *c, const uint8_t *d_queries, const uint64_t *d_q_off, uint32_t nq, Pick pick,
-                      uint32_t *map, uint64_t *coff, uint32_t *nb, const uint8_t **bq, const uint64_t **boff) {
+static int best_batch(b200sa_ctx *c, const uint8_t *d_queries, const uint64_t *d_q_off, const uint8_t *fx,
+                      uint32_t nq, Pick pick, uint32_t *map, uint64_t *coff, uint8_t *fx_out, uint32_t *nb,
+                      const uint8_t **bq, const uint64_t **boff, const uint8_t **bfx) {
     typedef unsigned long long u64;
     uint32_t *words = ptr<uint32_t>(c->small);
     TRY((dev_scan<OpSum64>(c, pick, BestPickOut{nq, map, coff}, (uint64_t)nq + 1,
@@ -3231,17 +3259,24 @@ static int best_batch(b200sa_ctx *c, const uint8_t *d_queries, const uint64_t *d
     *nb = (uint32_t)(pin_u64(c, 0) >> 32);
     *bq = d_queries;
     *boff = d_q_off;
+    *bfx = fx;
     if (*nb == nq || *nb == 0) return B200SA_OK;
     LAUNCH(c, k_best_gather, cdiv((uint64_t)*nb * 32, BLK), d_queries, d_q_off, (const uint32_t *)map,
            (const uint64_t *)coff, *nb, ptr<uint8_t>(c->qbuf));
+    if (fx) {
+        LAUNCH(c, k_best_gather, cdiv((uint64_t)*nb * 32, BLK), fx, d_q_off, (const uint32_t *)map,
+               (const uint64_t *)coff, *nb, fx_out);
+        *bfx = fx_out;
+    }
     *bq = ptr<uint8_t>(c->qbuf);
     *boff = coff;
     return B200SA_OK;
 }
 
 // The ne entries the search runs on: the queries, or with B200SA_APPROX_BOTH_STRANDS the doubled batch of
-// strand_queries; q their bytes, off their offsets, out the offsets of their lists.
-struct ApproxEntries { const uint8_t *q; const uint64_t *off; uint64_t *out; uint32_t ne; };
+// strand_queries; q their bytes, off their offsets, out the offsets of their lists, fx the marks of their fixed
+// symbols with B200SA_APPROX_FIXED (else NULL).
+struct ApproxEntries { const uint8_t *q; const uint64_t *off; uint64_t *out; uint32_t ne; const uint8_t *fx; };
 
 // Where the final lists land: their offsets off, positions pos and distances mis, written when 0 < total <= cap.
 // The caller's arrays and cap, or with B200SA_APPROX_DOCUMENTS or _ALIGN the offsets in c->adoff and every hit, even
@@ -3259,8 +3294,8 @@ static int approx_plain(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const 
     uint64_t *ko = nullptr;
     uint32_t *vo = nullptr;
     int pbits = 0;
-    TRY(approx_search(c, d_text, n, d_sa, d_starts, ndocs, e.q, e.off, e.ne, f.k, f.edit, f.iupac, e.out, fin.cap,
-                      total, end, &ko, &vo, &pbits));
+    TRY(approx_search(c, d_text, n, d_sa, d_starts, ndocs, e.q, e.off, e.fx, e.ne, f.k, f.edit, f.iupac, e.out,
+                      fin.cap, total, end, &ko, &vo, &pbits));
     const bool emitted = *total > 0 && *total <= fin.cap;
     if (f.stage && emitted) TRY(adocs_stage(c, *total, &fin.pos, &fin.mis));
     if (f.both)
@@ -3276,8 +3311,9 @@ static int approx_plain(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const 
 // final threshold, whose groups k_best_scatter moves to their entries' lists.  With B200SA_APPROX_BOTH_STRANDS a
 // query and its reverse complement are live as a pair with one best (strand.cuh), the groups scatter into
 // c->sstage and one k_strand_merge writes the final lists.  The batches are gathered from e.q, the IUPAC canonical
-// copy with that flag.  Phases: per round best_compact, the search's, best_update; per emitted group best_compact,
-// the search's, best_scatter; strand_merge with both strands.
+// copy with that flag, and their marks from e.fx with B200SA_APPROX_FIXED.  Phases: per round best_compact, the
+// search's, best_update; per emitted group best_compact, the search's, best_scatter; strand_merge with both
+// strands.
 template <class EndF>
 static int approx_best(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const uint32_t *d_sa,
                        const uint32_t *d_starts, uint32_t ndocs, EndF end, const ApproxFlags &f,
@@ -3286,7 +3322,9 @@ static int approx_best(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const u
     const uint32_t ne = e.ne, k = f.k, s = f.s;
     TRY(ensure(c, c->k32b, (size_t)ne * 8 + nq));        // cnt, map (u32) per entry, best (u8) per query
     TRY(ensure(c, c->rank, ((size_t)ne + 1) * 16));      // the batch's q_off, the search's offsets
-    TRY(ensure(c, c->qbuf, (size_t)q_bytes * (f.both ? 2 : 1)));
+    const size_t eb = (size_t)q_bytes * (f.both ? 2 : 1);          // the bytes of the entries
+    TRY(ensure(c, c->qbuf, eb * (e.fx ? 2 : 1)));                  // a gathered batch, then its marks
+    uint8_t *bmk = ptr<uint8_t>(c->qbuf) + eb;
     uint32_t *cnt = ptr<uint32_t>(c->k32b), *map = cnt + ne;
     uint8_t *best = reinterpret_cast<uint8_t *>(map + ne);
     uint64_t *coff = ptr<uint64_t>(c->rank), *soff = coff + ne + 1;
@@ -3297,21 +3335,22 @@ static int approx_best(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const u
     uint64_t *ko = nullptr, rtotal = 0;
     uint32_t *vo = nullptr, nb = 0, rounds = 0;
     int pbits = 0;
-    const uint8_t *bq;
+    const uint8_t *bq, *bfx;
     const uint64_t *boff;
     auto batch = [&](uint32_t t, bool group) {
         if (f.both)
-            return best_batch(c, e.q, e.off, ne, StrandPick{e.off, best, ne, t, s, k, group}, map, coff, &nb, &bq,
-                              &boff);
-        return best_batch(c, e.q, e.off, ne, BestPick{e.off, best, ne, t, s, k, group}, map, coff, &nb, &bq, &boff);
+            return best_batch(c, e.q, e.off, e.fx, ne, StrandPick{e.off, best, ne, t, s, k, group}, map, coff, bmk,
+                              &nb, &bq, &boff, &bfx);
+        return best_batch(c, e.q, e.off, e.fx, ne, BestPick{e.off, best, ne, t, s, k, group}, map, coff, bmk, &nb,
+                          &bq, &boff, &bfx);
     };
     for (uint32_t t = 0; t <= k; t++) {
         TRY(mark(c, "best_compact"));
         TRY(batch(t, false));
         if (nb == 0) break;
         rounds++;
-        TRY(approx_search(c, d_text, n, d_sa, d_starts, ndocs, bq, boff, nb, t, f.edit, f.iupac, soff, 0, &rtotal, end,
-                          &ko, &vo, &pbits));
+        TRY(approx_search(c, d_text, n, d_sa, d_starts, ndocs, bq, boff, bfx, nb, t, f.edit, f.iupac, soff, 0, &rtotal,
+                          end, &ko, &vo, &pbits));
         TRY(mark(c, "best_update"));
         if (f.both)
             LAUNCH(c, k_strand_update, cdiv(nb / 2, BLK), (const uint32_t *)map, (const u64 *)soff, nb, t, s, k, best,
@@ -3339,7 +3378,7 @@ static int approx_best(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const u
             if (!(ended >> t & 1u)) continue;
             TRY(mark(c, "best_compact"));
             TRY(batch(t, true));
-            TRY(approx_search(c, d_text, n, d_sa, d_starts, ndocs, bq, boff, nb, t, f.edit, f.iupac, soff, ~0ull,
+            TRY(approx_search(c, d_text, n, d_sa, d_starts, ndocs, bq, boff, bfx, nb, t, f.edit, f.iupac, soff, ~0ull,
                               &rtotal, end, &ko, &vo, &pbits));
             TRY(mark(c, "best_scatter"));
             LAUNCH(c, k_best_scatter, cdiv(rtotal, BLK), (const u64 *)ko, (const uint32_t *)vo, rtotal, pbits,
@@ -3350,8 +3389,9 @@ static int approx_best(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const u
     return B200SA_OK;
 }
 
-// nq >= 1 queries as f asks.  The checks; the IUPAC canonical copy, which every later kernel reads; with
-// B200SA_APPROX_BOTH_STRANDS the doubled batch; then approx_plain or approx_best writes each query's final list.
+// nq >= 1 queries as f asks.  The checks; the IUPAC canonical copy, which every later kernel reads, and with
+// B200SA_APPROX_FIXED the marks that follow the queries through every batch; with B200SA_APPROX_BOTH_STRANDS the
+// doubled batch; then approx_plain or approx_best writes each query's final list.
 // With B200SA_APPROX_DOCUMENTS that list is staged and adocs_reduce writes the caller's arrays; with
 // B200SA_APPROX_ALIGN align_list does.  `doubling_rounds` is set only with B200SA_APPROX_BEST.
 // Phases: approx_check; strand_queries with both strands; the middle's; adocs_mark, adocs_emit with
@@ -3367,13 +3407,14 @@ static int approx_run(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const ui
     if (f.both) TRY(strand_check(c, q_bytes, nq, f.k));
     uint32_t mmax = 0;
     if (f.align) TRY(align_check(c, d_q_off, nq, f.edit, &mmax));
-    if (f.iupac) TRY(iupac_canon(c, d_queries, q_bytes, &d_queries));
+    const uint8_t *d_fixed = nullptr;
+    if (f.iupac) TRY(iupac_canon(c, d_queries, q_bytes, f.fixed, &d_queries, &d_fixed));
     if (n == 0) return approx_nothing(c, d_offsets, nq);
     ApproxFinal fin{d_offsets, d_pos, d_mis, f.stage ? ~0ull : cap};
     if (f.stage) TRY(adocs_offsets(c, nq, &fin.off));
-    ApproxEntries e{d_queries, d_q_off, fin.off, nq};
+    ApproxEntries e{d_queries, d_q_off, fin.off, nq, d_fixed};
     if (f.both) {
-        TRY(strand_queries(c, d_queries, d_q_off, nq, q_bytes, f.iupac, &e.q, &e.off, &e.out));
+        TRY(strand_queries(c, d_queries, d_q_off, nq, q_bytes, f.iupac, d_fixed, &e.q, &e.off, &e.out, &e.fx));
         e.ne = 2 * nq;
     }
     if (f.best)
@@ -3382,8 +3423,8 @@ static int approx_run(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const ui
         TRY(approx_plain(c, d_text, n, d_sa, d_starts, ndocs, end, f, e, nq, fin, total));
     if (f.docs) TRY(adocs_reduce(c, d_starts, ndocs, nq, fin.off, d_offsets, d_pos, d_mis, cap, total));
     if (f.align)
-        TRY(align_list(c, d_text, n, d_starts, ndocs, d_queries, d_q_off, nq, f.k, f.edit, f.iupac, mmax, fin.off,
-                       d_offsets, d_pos, d_mis, cap, total));
+        TRY(align_list(c, d_text, n, d_starts, ndocs, d_queries, d_q_off, d_fixed, nq, f.k, f.edit, f.iupac, mmax,
+                       fin.off, d_offsets, d_pos, d_mis, cap, total));
     TRY(mark(c, "end"));
     CU_TRY(c, cudaGetLastError());
     CU_TRY(c, cudaStreamSynchronize(c->stream));
@@ -3391,7 +3432,7 @@ static int approx_run(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const ui
 }
 
 // The argument checks shared by both entry points, and k decoded into *f.  docs: the documents entry, the only one
-// that takes B200SA_APPROX_DOCUMENTS and B200SA_APPROX_ALIGN.
+// that takes B200SA_APPROX_DOCUMENTS, B200SA_APPROX_ALIGN and B200SA_APPROX_FIXED.
 static int approx_args(b200sa_ctx *c, uint64_t n, const void *text, const void *sa, const void *q_off, uint32_t nq,
                        uint32_t k, const void *offsets, const void *pos, uint64_t cap, const void *total, bool docs,
                        ApproxFlags *f) {
@@ -3400,7 +3441,7 @@ static int approx_args(b200sa_ctx *c, uint64_t n, const void *text, const void *
     const bool best = (k & B200SA_APPROX_BEST) != 0;
     const uint32_t accepted = 0xFFFFu | B200SA_APPROX_EDIT | B200SA_APPROX_IUPAC | B200SA_APPROX_BOTH_STRANDS |
                               (best ? B200SA_APPROX_BEST : 0u) |
-                              (docs ? B200SA_APPROX_DOCUMENTS | B200SA_APPROX_ALIGN : 0u);
+                              (docs ? B200SA_APPROX_DOCUMENTS | B200SA_APPROX_ALIGN | B200SA_APPROX_FIXED : 0u);
     // with B200SA_APPROX_BEST the threshold and the slack are a byte each, and either above the limit is a bad k
     if ((k & ~accepted) || (best && ((k & 0xFFu) > B200SA_APPROX_MAX_K || ((k >> 8) & 0xFFu) > B200SA_APPROX_MAX_K))) {
         const std::string m =
@@ -3408,17 +3449,20 @@ static int approx_args(b200sa_ctx *c, uint64_t n, const void *text, const void *
             "k must be a threshold up to B200SA_APPROX_MAX_K" +
             (best ? " | B200SA_APPROX_SLACK(s) with s up to B200SA_APPROX_MAX_K" : "") +
             ", optionally | B200SA_APPROX_EDIT, | B200SA_APPROX_IUPAC" +
-            (docs ? ", | B200SA_APPROX_BOTH_STRANDS and | B200SA_APPROX_DOCUMENTS, or | B200SA_APPROX_ALIGN"
+            (docs ? ", | B200SA_APPROX_BOTH_STRANDS, | B200SA_APPROX_FIXED with B200SA_APPROX_IUPAC and "
+                    "| B200SA_APPROX_DOCUMENTS, or | B200SA_APPROX_ALIGN"
                   : " and | B200SA_APPROX_BOTH_STRANDS");
         return fail(c, B200SA_ERR_BAD_ARG, m.c_str());
     }
+    if ((k & B200SA_APPROX_FIXED) && !(k & B200SA_APPROX_IUPAC))
+        return fail(c, B200SA_ERR_BAD_ARG, "approx positions: B200SA_APPROX_FIXED requires B200SA_APPROX_IUPAC");
     if (!best && (k & 0xFFFFu) > B200SA_APPROX_MAX_K)
         return fail(c, B200SA_ERR_BAD_ARG, "approx positions: k above B200SA_APPROX_MAX_K");
     if (n > B200SA_MAX_N) return too_long(c);
     const bool listing = (k & B200SA_APPROX_DOCUMENTS) != 0, align = (k & B200SA_APPROX_ALIGN) != 0;
     *f = ApproxFlags{best ? k & 0xFFu : k & 0xFFFFu, best ? (k >> 8) & 0xFFu : 0u, (k & B200SA_APPROX_EDIT) != 0,
-                     best, (k & B200SA_APPROX_IUPAC) != 0, (k & B200SA_APPROX_BOTH_STRANDS) != 0, listing, align,
-                     listing || align};
+                     best, (k & B200SA_APPROX_IUPAC) != 0, (k & B200SA_APPROX_FIXED) != 0,
+                     (k & B200SA_APPROX_BOTH_STRANDS) != 0, listing, align, listing || align};
     return B200SA_OK;
 }
 

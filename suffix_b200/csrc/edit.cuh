@@ -49,7 +49,9 @@ __device__ __noinline__ bool CutPieces::reports(const ApproxArgs &A, int64_t p, 
 
 // The starts this candidate reports, bit b for p = c - k + b, with *c_out = c and v[k + b] = dist(p).  v holds
 // one band row: v[d] = D(x, t) at t = c - 2k + x + d, D(x, t) = min over e of ED(q[x, m), T[t, e)), e <= de,
-// saturated at k + 1.  whole: the whole-table slot, only p = s (o_j = 0).  Pieces: CutPieces or IupacPieces.
+// saturated at k + 1.  whole: the whole-table slot, only p = s (o_j = 0).  Pieces: CutPieces, IupacPieces or
+// FixedIupacPieces; with Pieces::FIXED a fixed q[x] is never substituted (X) or inserted (I), and no deleted text
+// byte (D) sits next to one: no D at (x, t) when q[x] or q[x - 1] is fixed (DESIGN 6b f-21).
 template <class Pieces>
 __device__ __forceinline__ uint64_t edit_verify(const ApproxArgs &A, const ApproxItem &w, uint32_t s, uint8_t *v,
                                                 int64_t *c_out) {
@@ -68,6 +70,12 @@ __device__ __forceinline__ uint64_t edit_verify(const ApproxArgs &A, const Appro
     for (int64_t x = (int64_t)m - 1; x >= 0; x--) {        // in place, d downwards: v[d - 1] is still row x + 1
         const uint32_t qc = __ldg(qq + x);
         uint32_t right = INF, low = INF, old = v[W - 1];   // D(x, t + 1); the row's minimum; D(x + 1, t + 1)
+        bool fx = false, nodel = false;                    // q[x] is fixed; the row has no D move
+        if constexpr (Pieces::FIXED) {                     // q's marks, found again each row: one register less
+            const uint8_t *__restrict__ mk = Pieces::marks(A, qq);
+            fx = __ldg(mk + x) != 0;
+            nodel = fx || (x > 0 && __ldg(mk + x - 1) != 0);
+        }
         for (int32_t d = W - 1; d >= 0; d--) {
             const uint32_t up = d > 0 ? v[d - 1] : INF;    // D(x + 1, t)
             const int64_t t = base + x + d;
@@ -75,12 +83,16 @@ __device__ __forceinline__ uint64_t edit_verify(const ApproxArgs &A, const Appro
             if (t >= (int64_t)ds && t < (int64_t)de) {
                 // the byte test written inline: through a miss() member, ptxas spends three predicate instructions
                 // per unrolled cell where this spends one (8 more in k_approx_edit)
-                if constexpr (Pieces::CLASSES)
+                if constexpr (Pieces::FIXED) {
+                    const uint32_t mi = Pieces::miss(__ldg(A.text + t), qc);
+                    y = min(nodel ? INF : right + 1, fx ? (mi ? INF : old) : min(up + 1, old + mi));
+                } else if constexpr (Pieces::CLASSES) {
                     y = min(min(right, up) + 1, old + Pieces::miss(__ldg(A.text + t), qc));
-                else
+                } else {
                     y = min(min(right, up) + 1, old + (__ldg(A.text + t) != qc));
+                }
             } else if (t == (int64_t)de) {
-                y = up + 1;                                // no text left: delete q[x]
+                y = fx ? INF : up + 1;                     // no text left: delete q[x] (never a fixed one)
             }
             y = min(y, INF);
             v[d] = (uint8_t)y;

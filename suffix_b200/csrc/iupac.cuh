@@ -12,8 +12,13 @@
 // exact: a window within k has one of them intact.  For a concrete query they are f-14's pieces.  A query with
 // sum L_i < P keeps the whole-table slot: every rank is a candidate and is verified in full.  The piece of slot
 // q*P + j is (offset, length) in entry q*P + j of the piece table; length 0 marks the whole-table slot.  The table
-// follows pe in the same buffer (iupac_table), so the walks find it from ApproxArgs and keep no pointer live.
-// IupacPieces gives the walks these pieces and the class test in place of CutPieces.
+// follows pe in the same buffer (iupac_table), so the walks find it from ApproxArgs and keep no pointer live; with
+// B200SA_APPROX_FIXED the pointer to the batch's marks follows the table (iupac_marks) for the same reason.
+// IupacPieces gives the walks these pieces and the class test in place of CutPieces.  FixedIupacPieces adds the
+// fixed symbols of B200SA_APPROX_FIXED (DESIGN 6b f-21): the lowercase letters of the query, marked 1 in a copy of
+// one byte per query byte beside the canonical one (k_iupac_marks).  A window with a fixed miss is no occurrence and
+// the free misses are counted; edit_verify keeps X, I and D off them.  The pieces and reporters are IupacPieces':
+// every constrained occurrence is an unconstrained one, so one of the k + 1 pieces is still intact.
 #pragma once
 #include "edit.cuh"
 
@@ -59,6 +64,13 @@ __global__ void __launch_bounds__(BLK) k_iupac_code(const uint8_t *__restrict__ 
     if (!c) atomicMin(bad, ((unsigned long long)i << 8) | b);
 }
 
+// B200SA_APPROX_FIXED: 1 for a fixed (lowercase) query byte, else 0.  Runs after k_iupac_code accepted every byte
+// as a letter, so bit 0x20 tells the case.  One thread per byte.
+__global__ void __launch_bounds__(BLK) k_iupac_marks(const uint8_t *__restrict__ qs, uint64_t bytes, uint8_t *out) {
+    const uint64_t i = (uint64_t)blockIdx.x * BLK + threadIdx.x;
+    if (i < bytes) out[i] = (qs[i] & 0x20u) ? 1 : 0;
+}
+
 // sum over the stretches of qq[0, m) of floor(L_i / t), stopping once it reaches P
 __device__ __forceinline__ uint32_t iupac_fit(const uint8_t *__restrict__ qq, uint32_t m, uint32_t t, uint32_t P) {
     uint32_t sum = 0, run = 0;
@@ -75,6 +87,12 @@ __device__ __forceinline__ uint32_t iupac_fit(const uint8_t *__restrict__ qq, ui
 // The piece table: nslots (offset, length) entries right after pe[0, nslots), 8-byte aligned as ps starts so.
 __device__ __forceinline__ const uint2 *iupac_table(const ApproxArgs &A) {
     return reinterpret_cast<const uint2 *>(A.pe + A.nslots);
+}
+
+// B200SA_APPROX_FIXED: the marks of the batch's query bytes, marks[i] for qs[i], whose pointer the host writes after
+// the piece table.
+__device__ __forceinline__ const uint8_t *iupac_marks(const ApproxArgs &A) {
+    return *reinterpret_cast<const uint8_t *const *>(iupac_table(A) + A.nslots);
 }
 
 // The piece table and the slot ranges of the canonical queries: pieces / ps / pe[q*P + j] (one thread per query;
@@ -136,6 +154,14 @@ struct IupacPieces {
     // The class test over all m symbols, then the pieces [0, j) of the query's table.
     static __device__ __forceinline__ bool verify(const ApproxArgs &A, const ApproxItem &w, uint32_t s,
                                                   uint32_t *p_out, uint32_t *mis_out) {
+        return verify_marked<false>(A, w, s, p_out, mis_out);
+    }
+    // FIXED: a miss on a fixed symbol rejects the window, and only the free misses count.  The count over all m
+    // symbols bounds the free count from above, and a window with a fixed miss is rejected anyway, so the hot loop
+    // stays IupacPieces' and only a window within k reads its marks (then it has no fixed miss and mis is free).
+    template <bool FIXED>
+    static __device__ __forceinline__ bool verify_marked(const ApproxArgs &A, const ApproxItem &w, uint32_t s,
+                                                         uint32_t *p_out, uint32_t *mis_out) {
         if (s < w.oj) return false;
         const uint32_t p = s - w.oj;
         uint32_t ds, de;
@@ -147,6 +173,12 @@ struct IupacPieces {
         for (uint32_t x = 0; x < w.m; x++) {
             mis += !iupac_in(__ldg(t + x), __ldg(qq + x));
             if (mis > A.k) return false;
+        }
+        if constexpr (FIXED) {
+            const uint8_t *__restrict__ mk = iupac_marks(A) + (qq - A.qs);
+            if (mis)
+                for (uint32_t x = 0; x < w.m; x++)
+                    if (__ldg(mk + x) && !iupac_in(__ldg(t + x), __ldg(qq + x))) return false;
         }
         if (!w.whole) {
             const uint2 *__restrict__ pc = iupac_table(A) + (uint64_t)w.q * A.P;
@@ -160,6 +192,7 @@ struct IupacPieces {
         return true;
     }
     static constexpr bool CLASSES = true;
+    static constexpr bool FIXED = false;
     static __device__ __forceinline__ bool miss(uint32_t t, uint32_t qc) { return !iupac_in(t, qc); }
     // m may exceed k here, so dist(s) = v[2k] is tested
     static __device__ __forceinline__ uint64_t whole_hits(const uint8_t *v, int32_t k) {
@@ -183,6 +216,19 @@ struct IupacPieces {
     }
 };
 
+// IupacPieces with the marks of iupac_marks: verify rejects a fixed miss, edit_verify constrains its moves.
+struct FixedIupacPieces : IupacPieces {
+    static __device__ __forceinline__ bool verify(const ApproxArgs &A, const ApproxItem &w, uint32_t s,
+                                                  uint32_t *p_out, uint32_t *mis_out) {
+        return verify_marked<true>(A, w, s, p_out, mis_out);
+    }
+    static constexpr bool FIXED = true;
+    // the marks of the query at qq
+    static __device__ __forceinline__ const uint8_t *marks(const ApproxArgs &A, const uint8_t *qq) {
+        return iupac_marks(A) + (qq - A.qs);
+    }
+};
+
 // The minimum of 4 blocks per SM lets ptxas use up to 64 registers: left to itself it holds the count pass at 32
 // and spills.
 template <bool EMIT>
@@ -197,6 +243,22 @@ __global__ void __launch_bounds__(BLK) k_approx_edit_iupac(ApproxArgs A, uint32_
                                                            unsigned long long *key, uint32_t *val) {
     uint8_t v[EDIT_BAND];
     edit_walk<EMIT, IupacPieces>(A, v, cnt, item_off, pbits, key, val);
+}
+
+// B200SA_APPROX_FIXED: the IUPAC kernels with FixedIupacPieces, under the same launch bounds.
+template <bool EMIT>
+__global__ void __launch_bounds__(BLK, 4) k_approx_iupac_fixed(ApproxArgs A, uint32_t *cnt,
+                                                               const unsigned long long *item_off, int pbits,
+                                                               unsigned long long *key, uint32_t *val) {
+    approx_walk<EMIT, FixedIupacPieces>(A, cnt, item_off, pbits, key, val);
+}
+
+template <bool EMIT>
+__global__ void __launch_bounds__(BLK) k_approx_edit_iupac_fixed(ApproxArgs A, uint32_t *cnt,
+                                                                 const unsigned long long *item_off, int pbits,
+                                                                 unsigned long long *key, uint32_t *val) {
+    uint8_t v[EDIT_BAND];
+    edit_walk<EMIT, FixedIupacPieces>(A, v, cnt, item_off, pbits, key, val);
 }
 
 }  // namespace b200sa

@@ -279,8 +279,9 @@ class SuffixTable:
         from . import _bwt
         return _bwt.bwt_runs(self)
 
-    # ---- approximate positions (DESIGN 6b f-14 .. f-18, f-20)
-    def approximate_positions(self, query, k, *, metric="hamming", best=None, iupac=False, strands="forward"):
+    # ---- approximate positions (DESIGN 6b f-14 .. f-18, f-20, f-21)
+    def approximate_positions(self, query, k, *, metric="hamming", best=None, iupac=False, strands="forward",
+                              fixed=False):
         """(positions u32[], mismatches u32[]): every p with p + m <= n where text[p:p + m] differs from
         the query (m bytes) in at most k bytes, 0 <= k <= 31, by ascending p, with that number of
         mismatches beside it (b200sa_approx_positions_dev).  b"" matches nothing; for k = 0 the positions
@@ -299,6 +300,13 @@ class SuffixTable:
         other query byte raises B200SA_ERR_BAD_ARG.  Lowercase (soft-masked) text bases, N, U and every other
         text byte match no code and count as a mismatch: uppercase a soft-masked text before building the
         table.  Combines with metric= and best=; a non-bool value raises ValueError.
+        fixed=True (with iupac=True; a non-bool value, or fixed=True without iupac=True, raises ValueError) keeps
+        the lowercase symbols of each query fixed (B200SA_APPROX_FIXED, the text going through
+        b200sa_docs_approx_positions_dev as one document on a SuffixTable): a lowercase code still means its
+        uppercase class, but must match it, and takes no substitution, insertion or adjacent deletion, so the
+        threshold is spent on the uppercase symbols alone.  A CRISPR guide written "GACGCTGACGCTGACGCTGAngg"
+        finds off-targets whose PAM is intact, with mismatches and bulges in the spacer only.  A query with no
+        lowercase symbol gives exactly the call without the flag.
         strands="both" also lists the occurrences of the query's reverse complement (A <-> T, C <-> G in either
         case; with iupac=True each code's class complemented, R <-> Y, K <-> M, B <-> V, D <-> H, U -> A) as
         minus-strand hits at the leftmost text position of their window or alignment
@@ -306,23 +314,25 @@ class SuffixTable:
         the plus hit first, minus a bool array; with best= best(q) is taken over both strands.  strands="forward"
         (the default) searches the query alone; any other value raises ValueError."""
         from . import _approx
-        return _approx.positions(self, query, k, metric, best, iupac, strands)
+        return _approx.positions(self, query, k, metric, best, iupac, strands, fixed)
 
-    def approximate_positions_batch(self, queries, k, *, metric="hamming", best=None, iupac=False, strands="forward"):
+    def approximate_positions_batch(self, queries, k, *, metric="hamming", best=None, iupac=False, strands="forward",
+                                    fixed=False):
         """(offsets u64[nq + 1], positions u32[], mismatches u32[]): query q's occurrences with at most k
         mismatches (or within k edits, metric="edit") are positions[offsets[q]:offsets[q + 1]], as
         approximate_positions returns them; best=0 gives each query's best hits, with best(q) in the
-        distance column (best= and iupac= as in approximate_positions).  strands="both" returns (offsets,
+        distance column (best=, iupac= and fixed= as in approximate_positions).  strands="both" returns (offsets,
         positions, distances, minus) with both strands in each query's list, as approximate_positions does."""
         from . import _approx
-        return _approx.positions_batch(self, queries, k, metric, best, iupac, strands)
+        return _approx.positions_batch(self, queries, k, metric, best, iupac, strands, fixed)
 
-    def approximate_counts(self, queries, k, *, metric="hamming", best=None, iupac=False, strands="forward"):
+    def approximate_counts(self, queries, k, *, metric="hamming", best=None, iupac=False, strands="forward",
+                           fixed=False):
         """u64[nq]: the number of occurrences with at most k mismatches (or within k edits, metric="edit") of
         every query, without fetching them; best=0 counts each query's best hits, those at distance best(q)
-        (best= and iupac= as in approximate_positions); strands="both" counts the hits of both strands."""
+        (best=, iupac= and fixed= as in approximate_positions); strands="both" counts the hits of both strands."""
         from . import _approx
-        return _approx.counts(self, queries, k, metric, best, iupac, strands)
+        return _approx.counts(self, queries, k, metric, best, iupac, strands, fixed)
 
     def approximate_alignments(self, query, k, *, metric="hamming", best=None, iupac=False, strands="forward"):
         """(positions u32[], distances u32[], ends u32[], cigar_offsets u64[h + 1], cigar u32[]): the hits of
