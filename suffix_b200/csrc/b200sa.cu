@@ -278,11 +278,11 @@ static int radix_pass(b200sa_ctx *c, DigF dig, MoveF mv, uint64_t n) {
     return B200SA_OK;
 }
 
-// Keys per thread of the one-sweep passes.  From 2^20 items the tiles are wide (16 keys per thread for 32-bit
-// keys, 12 for 64-bit keys: what fits 48 KB of static shared memory): half the tiles, look-backs and per-tile
-// scans per key.  B200SA_SORT_ITEMS=8|16 forces the width, and B200SA_SORT_NARROW the narrow tiles.
+// Keys per thread of the one-sweep passes.  From 2^20 items the tiles are wide (32 keys per thread for 32-bit
+// keys, 16 for 64-bit keys, at two CTAs per SM): a fourth or half of the tiles, look-backs and per-tile scans per key.
+// B200SA_SORT_ITEMS=8 forces the narrow tiles and any other value the wide ones; B200SA_SORT_NARROW the narrow.
 static bool os_wide(uint64_t n) {
-    if (const char *e = getenv("B200SA_SORT_ITEMS")) return atoi(e) == 16;
+    if (const char *e = getenv("B200SA_SORT_ITEMS")) return atoi(e) != ITEMS;
     return n >= (1u << 20) && !getenv("B200SA_SORT_NARROW");
 }
 
@@ -293,6 +293,18 @@ static bool os_wide(uint64_t n) {
 // and the digit counts of every pass to c->os_hist (zeroed, tickets included, before that kernel): no histogram
 // kernel, and keyf is not called.
 enum OsFirst { IN_PLACE, FROM_FUNCTORS, FROM_KEYS };
+
+// One one-sweep pass over `tiles` tiles of OSI * BLK items; the tile is staged in dynamic shared memory.
+template <int OSI, class K, class KeyF, class ValF>
+static int os_pass(b200sa_ctx *c, uint32_t tiles, KeyF keyf, ValF valf, K *kout, uint32_t *vout, uint64_t n,
+                   uint32_t shift, const uint32_t *gbase, volatile unsigned long long *status, uint32_t *ticket) {
+    auto kern = k_os_pass<K, KeyF, ValF, OSI>;
+    constexpr size_t shm = os_stage_bytes<K, OSI>();
+    CU_TRY(c, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)shm));
+    kern<<<tiles, BLK, shm, c->stream>>>(keyf, valf, kout, vout, n, shift, gbase, status, ticket);
+    c->launches++;
+    return B200SA_OK;
+}
 
 // Sorts n items by key bits [shift0, shift0 + bits) with the one-sweep passes of common.cuh, OSI keys per
 // thread.  The histogram reads the keys through keyf and the first pass the values through valf; *kout/*vout
@@ -331,11 +343,10 @@ static int os_sort_items(b200sa_ctx *c, KeyF keyf, ValF valf, K *ka, uint32_t *v
         CU_TRY(c, cudaMemsetAsync(c->os_status.p, 0, status_bytes, c->stream));
         const uint32_t shift = shift0 + (uint32_t)(8 * p);
         if (p == 0)
-            LAUNCH(c, (k_os_pass<K, LoadArr<K>, ValF, OSI>), tiles, LoadArr<K>{ka}, valf, kb, vb, n, shift, ghist, status,
-                   ticket);
+            TRY(os_pass<OSI>(c, tiles, LoadArr<K>{ka}, valf, kb, vb, n, shift, ghist, status, ticket));
         else
-            LAUNCH(c, (k_os_pass<K, LoadArr<K>, LoadArr<uint32_t>, OSI>), tiles, LoadArr<K>{ka}, LoadArr<uint32_t>{va}, kb,
-                   vb, n, shift, ghist + p * 256, status, ticket + p);
+            TRY(os_pass<OSI>(c, tiles, LoadArr<K>{ka}, LoadArr<uint32_t>{va}, kb, vb, n, shift, ghist + p * 256, status,
+                             ticket + p));
         std::swap(ka, kb);
         std::swap(va, vb);
     }
@@ -349,7 +360,7 @@ template <OsFirst FIRST, class K, class KeyF, class ValF>
 static int os_sort(b200sa_ctx *c, KeyF keyf, ValF valf, K *ka, uint32_t *va, K *kb, uint32_t *vb, uint64_t n, int bits,
                    uint32_t shift0, K **kout, uint32_t **vout) {
     if (os_wide(n))
-        return os_sort_items<FIRST, sizeof(K) == 4 ? 16 : 12>(c, keyf, valf, ka, va, kb, vb, n, bits, shift0, kout, vout);
+        return os_sort_items<FIRST, sizeof(K) == 4 ? 32 : 16>(c, keyf, valf, ka, va, kb, vb, n, bits, shift0, kout, vout);
     return os_sort_items<FIRST, ITEMS>(c, keyf, valf, ka, va, kb, vb, n, bits, shift0, kout, vout);
 }
 
@@ -1180,9 +1191,9 @@ static int lcp_dev(b200sa_ctx *c, const uint8_t *d_text, uint64_t n, const uint3
         CU_TRY(c, cudaMemsetAsync(c->os_status.p, 0, status_bytes, c->stream));
         // sa is a permutation: the digit bases are known without a histogram pass
         LAUNCH(c, k_os_perm_base, 1u, ghist, shift, n32);
-        LAUNCH(c, (k_os_pass<uint32_t, LoadArr<uint32_t>, LoadPhiPrev>), tiles, LoadArr<uint32_t>{d_sa}, LoadPhiPrev{d_sa},
-               ptr<uint32_t>(c->phik), ptr<uint32_t>(c->phiv), n, shift, ghist,
-               reinterpret_cast<volatile unsigned long long *>(c->os_status.p), ticket);
+        TRY(os_pass<ITEMS>(c, tiles, LoadArr<uint32_t>{d_sa}, LoadPhiPrev{d_sa}, ptr<uint32_t>(c->phik),
+                           ptr<uint32_t>(c->phiv), n, shift, ghist,
+                           reinterpret_cast<volatile unsigned long long *>(c->os_status.p), ticket));
         LAUNCH(c, k_phi_apply, cdiv(n, BLK), ptr<uint32_t>(c->phik), ptr<uint32_t>(c->phiv), n32, ptr<uint32_t>(c->isa));
     } else {
         LAUNCH(c, k_phi, cdiv(n, BLK), d_sa, n32, ptr<uint32_t>(c->isa));

@@ -28,12 +28,9 @@ __device__ __forceinline__ uint32_t lanemask_lt() {
 #ifndef PEERS_MATCH
 #define PEERS_MATCH 1
 #endif
+// Peers among the lanes in `peers` (all lanes valid: pass FULL and skip the validity ballot).
 template <int NBITS>
-__device__ __forceinline__ uint32_t peer_mask(uint32_t key, bool valid) {
-#if PEERS_MATCH
-    return __match_any_sync(FULL, valid ? key : 0xffffffffu) & __ballot_sync(FULL, valid);
-#else
-    uint32_t peers = __ballot_sync(FULL, valid);
+__device__ __forceinline__ uint32_t peer_mask_ballot_in(uint32_t key, uint32_t peers) {
 #pragma unroll
     for (int b = 0; b < NBITS; b++) {
         bool bit = (key >> b) & 1u;
@@ -41,6 +38,17 @@ __device__ __forceinline__ uint32_t peer_mask(uint32_t key, bool valid) {
         peers &= bit ? bal : ~bal;
     }
     return peers;
+}
+template <int NBITS>
+__device__ __forceinline__ uint32_t peer_mask_ballot(uint32_t key, bool valid) {
+    return peer_mask_ballot_in<NBITS>(key, __ballot_sync(FULL, valid));
+}
+template <int NBITS>
+__device__ __forceinline__ uint32_t peer_mask(uint32_t key, bool valid) {
+#if PEERS_MATCH
+    return __match_any_sync(FULL, valid ? key : 0xffffffffu) & __ballot_sync(FULL, valid);
+#else
+    return peer_mask_ballot<NBITS>(key, valid);
 #endif
 }
 
@@ -442,13 +450,7 @@ __device__ __forceinline__ void hist_add_private(uint32_t *s_warp_hist, uint32_t
 // histograms): fixed 9 ballots instead of a MATCH that iterates over up to 32
 // distinct values.
 __device__ __forceinline__ void hist_add_private_ballot(uint32_t *s_warp_hist, uint32_t key, bool valid) {
-    uint32_t peers = __ballot_sync(FULL, valid);
-#pragma unroll
-    for (int b = 0; b < 8; b++) {
-        bool bit = (key >> b) & 1u;
-        uint32_t bal = __ballot_sync(FULL, bit);
-        peers &= bit ? bal : ~bal;
-    }
+    uint32_t peers = peer_mask_ballot<8>(key, valid);
     if (valid && (peers & lanemask_lt()) == 0) s_warp_hist[key] += (uint32_t)__popc(peers);
     __syncwarp();
 }
@@ -538,9 +540,6 @@ __device__ __forceinline__ void os_store(unsigned long long *p, unsigned long lo
     asm volatile("st.relaxed.gpu.global.u64 [%0], %1;" :: "l"(p), "l"(v) : "memory");
 }
 constexpr int OS_MAX_PASSES = 8;
-#ifndef OS_LOOK
-#define OS_LOOK 3          // predecessor status words in flight per look-back step
-#endif
 
 // dynamic shared memory: [NWARP][npass][256] u32 (64 KB for 8 passes)
 template <class K, class KeyF>
@@ -601,33 +600,46 @@ struct LoadArr {
     __device__ __forceinline__ K operator()(uint64_t i) const { return a[i]; }
     __device__ __forceinline__ K at(uint64_t i, uint32_t) const { return a[i]; }     // key of item i given its value
 };
-// OSI items per thread: 8 (tile of 2048) or 16 (tile of 4096: half the tiles, look-backs and histogram scans per key)
+// OSI items per thread: 8 (tile of 2048) for small sorts; the wide tiles (32 keys per thread for 32-bit keys, 16 for
+// 64-bit keys) take two CTAs per SM and keep every key, value and the look-back word in registers without spills.
 #ifndef OS_MINB_WIDE
-#define OS_MINB_WIDE 3
+#define OS_MINB_WIDE 2
 #endif
+// dynamic shared memory of k_os_pass: the tile's keys and values in digit order
+template <class K, int OSI>
+constexpr size_t os_stage_bytes() { return (size_t)OSI * BLK * (sizeof(K) + sizeof(uint32_t)); }
+// One stable pass.  The tile's digit counts are known before any item is ranked: each warp counts its digits
+// with shared-memory atomics, the counts are published at once (tile 0 publishes them as inclusive), and the
+// load of the nearest predecessor's status word is in flight while the warps rank their items.  Ranking
+// builds each item's peers from 9 ballots (MATCH.ANY iterates over the ~30 distinct digits a warp holds on
+// random keys) and seeds a running (warp, digit) counter with the warp's offset inside the tile; the leader
+// of each peer group advances it with one atomic and hands the old value to its peers by shuffle.  Items go
+// straight to their slot in the staging arrays; the look-back then ends on the first inclusive prefix.
 template <class K, class KeyF, class ValF, int OSI = ITEMS>
 __global__ void __launch_bounds__(BLK, (OSI > 8 ? OS_MINB_WIDE : OS_MINB)) k_os_pass(KeyF keyf, ValF valf, K *kout,
                                                  uint32_t *vout, uint64_t n, uint32_t shift,
                                                  const uint32_t *__restrict__ gbase, volatile unsigned long long *status,
                                                  uint32_t *ticket) {
     __shared__ uint32_t s_wcnt[NWARP][256];
-    __shared__ uint32_t s_tcnt[256], s_texcl[256], s_gb[256];
+    __shared__ uint32_t s_gb[256];
     __shared__ uint32_t s_w[NWARP + 1];
-    __shared__ K s_k[OSI * BLK];
-    __shared__ uint32_t s_v[OSI * BLK];
     __shared__ uint32_t s_tile;
+    extern __shared__ __align__(16) unsigned char s_os_stage[];
+    K *s_k = reinterpret_cast<K *>(s_os_stage);
+    uint32_t *s_v = reinterpret_cast<uint32_t *>(s_k + OSI * BLK);
     if (threadIdx.x == 0) s_tile = atomicAdd(ticket, 1u);
 #pragma unroll
     for (int ww = 0; ww < NWARP; ww++) s_wcnt[ww][threadIdx.x] = 0;
     __syncthreads();
     const uint32_t tile = s_tile, w = warp_id(), l = lane_id();
     const uint64_t tb = (uint64_t)tile * (OSI * BLK);
+    const bool full = tb + OSI * BLK <= n;      // every tile but the last: no bounds, no validity ballot
     K key[OSI];
-    uint32_t val[OSI], d[OSI], rank[OSI], vm = 0;
+    uint32_t val[OSI], vm = 0;
 #pragma unroll
     for (int r = 0; r < OSI; r++) {             // all values first: a key functor that gathers through the value
         uint64_t i = tb + (uint64_t)w * (OSI * 32) + r * 32 + l;   // (position -> text window) then has its eight
-        bool valid = i < n;                                           // dependent loads in flight together
+        bool valid = full || i < n;                                   // dependent loads in flight together
         val[r] = valid ? valf(i) : 0u;
         vm |= (valid ? 1u : 0u) << r;
     }
@@ -635,56 +647,73 @@ __global__ void __launch_bounds__(BLK, (OSI > 8 ? OS_MINB_WIDE : OS_MINB)) k_os_
     for (int r = 0; r < OSI; r++) {
         uint64_t i = tb + (uint64_t)w * (OSI * 32) + r * 32 + l;
         key[r] = ((vm >> r) & 1u) ? keyf.at(i, val[r]) : (K)0;
-        d[r] = (uint32_t)(key[r] >> shift) & 0xffu;
     }
-    tile_rank(d, vm, rank, s_wcnt, s_tcnt);
+    auto digit = [&](int r) { return (uint32_t)(key[r] >> shift) & 0xffu; };
+#pragma unroll
+    for (int r = 0; r < OSI; r++)
+        if ((vm >> r) & 1u) atomicAdd(&s_wcnt[w][digit(r)], 1u);
+    __syncthreads();
+    const uint32_t dg = threadIdx.x;
+    const uint32_t gb = gbase[dg];
+    uint32_t c[NWARP], cnt = 0;
+#pragma unroll
+    for (int ww = 0; ww < NWARP; ww++) {
+        c[ww] = s_wcnt[ww][dg];
+        cnt += c[ww];
+    }
+    unsigned long long *st = const_cast<unsigned long long *>(status);
+    os_store(st + (uint64_t)tile * 256 + dg, (tile == 0 ? OS_INCL : OS_AGG) | cnt);
+    int64_t t = (int64_t)tile - 1;
+    unsigned long long x = t >= 0 ? os_load(st + (uint64_t)t * 256 + dg) : OS_INCL;
+    uint32_t total;
+    const uint32_t texcl = block_incl_scan<OpSum>(cnt, s_w, &total) - cnt;
     {
-        const uint32_t dg = threadIdx.x;
-        uint32_t cnt = s_tcnt[dg], total;
-        uint32_t inc = block_incl_scan<OpSum>(cnt, s_w, &total);
-        uint32_t texcl = inc - cnt;
-        s_texcl[dg] = texcl;
-        unsigned long long *mine = const_cast<unsigned long long *>(status) + (uint64_t)tile * 256 + dg;
-        os_store(mine, OS_AGG | cnt);
-        uint32_t excl = 0;
-        // look back over predecessor tiles, four status words in flight at a time
-        int64_t t = (int64_t)tile - 1;
-        bool done = false;
-        while (t >= 0 && !done) {
-            unsigned long long v[OS_LOOK];
+        uint32_t run = texcl;             // column dg is read and written by thread dg only
 #pragma unroll
-            for (int k = 0; k < OS_LOOK; k++)
-                v[k] = (t - k >= 0) ? os_load(const_cast<unsigned long long *>(status) + (uint64_t)(t - k) * 256 + dg) : OS_INCL;
-#pragma unroll
-            for (int k = 0; k < OS_LOOK; k++) {
-                if (done || t - k < 0) break;
-                unsigned long long x = v[k];
-                while ((x >> 62) == 0) x = os_load(const_cast<unsigned long long *>(status) + (uint64_t)(t - k) * 256 + dg);
-                excl += (uint32_t)(x & OS_VAL);
-                if ((x >> 62) == 2) done = true;
-            }
-            t -= OS_LOOK;
+        for (int ww = 0; ww < NWARP; ww++) {
+            s_wcnt[ww][dg] = run;
+            run += c[ww];
         }
-        os_store(mine, OS_INCL | (unsigned long long)(excl + cnt));
-        s_gb[dg] = gbase[dg] + excl - texcl;
     }
     __syncthreads();
+    const uint32_t lt = lanemask_lt();
 #pragma unroll
     for (int r = 0; r < OSI; r++) {
-        if ((vm >> r) & 1u) {
-            uint32_t p = s_texcl[d[r]] + s_wcnt[w][d[r]] + rank[r];
+        bool valid = (vm >> r) & 1u;
+        uint32_t peers = peer_mask_ballot_in<8>(digit(r), full ? FULL : __ballot_sync(FULL, valid));
+        uint32_t below = __popc(peers & lt), old = 0;
+        if (valid && below == 0) old = atomicAdd(&s_wcnt[w][digit(r)], (uint32_t)__popc(peers));
+        uint32_t p = __shfl_sync(FULL, old, __ffs(peers) - 1) + below;
+        if (valid) {
             s_k[p] = key[r];
             s_v[p] = val[r];
         }
     }
+    // tile 0 is inclusive from the start, so the walk never passes it
+    uint32_t excl = 0;
+    while (true) {
+        while ((x >> 62) == 0) x = os_load(st + (uint64_t)t * 256 + dg);
+        excl += (uint32_t)(x & OS_VAL);
+        if ((x >> 62) == 2) break;
+        t--;
+        x = os_load(st + (uint64_t)t * 256 + dg);
+    }
+    if (tile > 0) os_store(st + (uint64_t)tile * 256 + dg, OS_INCL | (unsigned long long)(excl + cnt));
+    s_gb[dg] = gb + excl - texcl;
     __syncthreads();
     uint64_t left = n - tb;
     uint32_t cnt_tile = left < (uint64_t)(OSI * BLK) ? (uint32_t)left : (uint32_t)(OSI * BLK);
-    for (uint32_t j = threadIdx.x; j < cnt_tile; j += BLK) {
+    auto put = [&](uint32_t j) {
         K k = s_k[j];
         uint32_t dst = s_gb[(uint32_t)(k >> shift) & 0xffu] + j;
         kout[dst] = k;
         vout[dst] = s_v[j];
+    };
+    if (full) {
+#pragma unroll
+        for (int r = 0; r < OSI; r++) put(r * BLK + threadIdx.x);
+    } else {
+        for (uint32_t j = threadIdx.x; j < cnt_tile; j += BLK) put(j);
     }
 }
 
