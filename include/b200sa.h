@@ -768,7 +768,42 @@ int b200sa_unbwt_dev(b200sa_ctx *ctx, uint64_t n, uint32_t ndocs, const uint8_t 
  * Verification rejects a window on a fixed miss and counts the free misses; the edit band DP and the alignment's
  * traceback forbid the three moves.  Device workspace (computed, not measured): what the call takes without the
  * flag, plus 1 byte per query byte for the marks (2 with B200SA_APPROX_BOTH_STRANDS, and as much again for a
- * compacted batch with B200SA_APPROX_BEST).  Phases: those of the call without the flag. */
+ * compacted batch with B200SA_APPROX_BEST).  Phases: those of the call without the flag.
+ *
+ * ---- separate budgets for mismatches, DNA bulges and RNA bulges (DESIGN.md 6b f-22) ----
+ * With B200SA_APPROX_BULGES (bit 21) | B200SA_APPROX_DNA_BULGES(d) | B200SA_APPROX_RNA_BULGES(r) in k, 0 <= d, r <= 3,
+ * b200sa_docs_approx_positions_dev searches with three budgets, as CRISPR off-target tools do: the threshold t = k &
+ * 0xFFFF counts substitutions alone, beside at most d DNA bulges and r RNA bulges.  The flag requires
+ * B200SA_APPROX_EDIT and mixes freely with B200SA_APPROX_IUPAC, B200SA_APPROX_FIXED, B200SA_APPROX_BOTH_STRANDS,
+ * B200SA_APPROX_DOCUMENTS and B200SA_APPROX_ALIGN; a single text goes through that entry as one document.  Each of
+ * these returns B200SA_ERR_BAD_ARG with a detail that names B200SA_APPROX_BULGES: the flag without
+ * B200SA_APPROX_EDIT; the flag with B200SA_APPROX_BEST (the detail names both); t + d + r > B200SA_APPROX_MAX_K; the
+ * flag on b200sa_approx_positions_dev (an unknown bit there, whose detail also names B200SA_APPROX_MAX_K as before).
+ * Bits 17-18 and 22-23 mean something only beside bit 21: without it they are unknown bits as before, with the same
+ * detail.  Without the flag nothing changes.  Definition:
+ *  - An alignment of the whole query Q (q, or rc(q) on a minus hit) to T[p, e), p <= e <= end(p), is made of =, X
+ *    (a substitution), I (a query byte with no text byte: an RNA bulge) and D (a text byte with no query byte: a
+ *    DNA bulge), with match as in B200SA_APPROX_ALIGN (IUPAC classes with B200SA_APPROX_IUPAC).
+ *  - p is an occurrence when some alignment has #X <= t, #D <= d and #I <= r, and with B200SA_APPROX_FIXED also
+ *    keeps the f-21 rules.  dist(p) is the least #X + #I + #D over those alignments; q's list holds (p, dist(p)) by
+ *    ascending p, and both strands, the document listing and the listing protocol are as above on these
+ *    distances.  m = 0 has no occurrences.
+ *  - With B200SA_APPROX_ALIGN each hit gets the canonical alignment of cost dist(p) within the budgets: the walk
+ *    from (0, p) takes, of the moves =/X, I, D in that order (f-20's), the first after which some alignment of the
+ *    rest still keeps the remaining budgets at the remaining cost (with B200SA_APPROX_FIXED, the first allowed one).
+ *    So every CIGAR has at most t X, d D and r I operations, and its X, I and D lengths sum to dist(p).
+ *  - So: with d = r = 0 the call is exactly the Hamming call on the same entry with the same other flags,
+ *    positions and distances bit for bit; the hits are a subset of the B200SA_APPROX_EDIT call at threshold
+ *    t + d + r, each with dist(p) at least the edit distance there; the result only grows with t, d and r.
+ *  - TOO_LARGE: the slot check counts nq * (t + d + r + 1) (2 nq with both strands).
+ * Method: the pieces, slots and flow of B200SA_APPROX_EDIT with P = t + d + r + 1 pieces (the f-14 cut, or f-17's
+ * with B200SA_APPROX_IUPAC; the whole-table slot when they do not fit).  A piece j found at s gives the starts p in
+ * [c - d, c + r], c = s - o_j; the reporter rule is f-15's with the shift window s'' - o_i - p in [-r, d].  A banded
+ * reversed Sellers DP over the 2(d + r) + 1 diagonals keeps, per cell and per (#I, #D) in [0..r] x [0..d], the least
+ * #X, saturated at t + 1, in shared memory; the alignment recomputes the d + r + 1 diagonals of its hit, one thread
+ * per hit, with every row kept in a device buffer of at most 64 MB per batch of hits.  Device workspace (computed,
+ * not measured): what B200SA_APPROX_EDIT takes at threshold t + d + r, and with B200SA_APPROX_ALIGN up to 64 MB for
+ * the rows.  Phases: those of the call without the flag. */
 #define B200SA_APPROX_MAX_K 31
 #define B200SA_APPROX_EDIT 0x10000u
 #define B200SA_APPROX_BEST 0x100000u                      /* bit 20 */
@@ -780,6 +815,9 @@ int b200sa_unbwt_dev(b200sa_ctx *ctx, uint64_t n, uint32_t ndocs, const uint8_t 
 #define B200SA_APPROX_ALIGN 0x8000000u                    /* bit 27, in k, documents entry only */
 #define B200SA_APPROX_ALIGN_MAX_M 4096                    /* the longest query B200SA_APPROX_EDIT aligns */
 #define B200SA_APPROX_FIXED 0x2000000u                    /* bit 25, in k, documents entry only, with B200SA_APPROX_IUPAC */
+#define B200SA_APPROX_BULGES 0x200000u                    /* bit 21, in k, documents entry only, with B200SA_APPROX_EDIT */
+#define B200SA_APPROX_DNA_BULGES(d) ((uint32_t)(d) << 17)  /* bits 17-18, 0 <= d <= 3, only with B200SA_APPROX_BULGES */
+#define B200SA_APPROX_RNA_BULGES(r) ((uint32_t)(r) << 22)  /* bits 22-23, 0 <= r <= 3, only with B200SA_APPROX_BULGES */
 int b200sa_approx_positions_dev(b200sa_ctx *ctx, const uint8_t *d_text, uint64_t n, const uint32_t *d_sa,
                                 const uint8_t *d_queries, const uint64_t *d_q_off, uint32_t nq, uint32_t k,
                                 uint64_t *d_offsets, uint32_t *d_pos, uint32_t *d_mismatches, uint64_t cap,

@@ -18,6 +18,8 @@ MINUS = 0x80000000        # B200SA_APPROX_MINUS
 DOCUMENTS = 0x20000000    # B200SA_APPROX_DOCUMENTS
 ALIGN = 0x8000000         # B200SA_APPROX_ALIGN
 FIXED = 0x2000000         # B200SA_APPROX_FIXED
+BULGES = 0x200000         # B200SA_APPROX_BULGES
+MAX_BULGE = 3             # the most DNA or RNA bulges
 OPS = "MIDNSHP=X"         # the BAM operation codes
 METRICS = {"hamming": 0, "edit": EDIT}
 
@@ -47,6 +49,26 @@ def _fixed(fixed, iupac):
     return FIXED if fixed else 0
 
 
+def _bulges(bulges, k, metric, best):
+    """The k bits of bulges=: 0 for None; for (dna, rna), two ints in 0 .. 3, B200SA_APPROX_BULGES with
+    B200SA_APPROX_DNA_BULGES(dna) | B200SA_APPROX_RNA_BULGES(rna), which need metric="edit", best=None and
+    k + dna + rna <= 31."""
+    if bulges is None:
+        return 0
+    if (not isinstance(bulges, tuple) or len(bulges) != 2 or
+            any(isinstance(b, (bool, np.bool_)) or not isinstance(b, (int, np.integer)) or not 0 <= b <= MAX_BULGE
+                for b in bulges)):
+        raise ValueError("bulges must be None or a tuple (dna, rna) of ints in 0 .. %d, got %r" % (MAX_BULGE, bulges))
+    if metric != "edit":
+        raise ValueError("bulges requires metric='edit'")
+    if best is not None:
+        raise ValueError("bulges does not combine with best")
+    dna, rna = int(bulges[0]), int(bulges[1])
+    if k + dna + rna > MAX_K:
+        raise ValueError("k + dna + rna bulges must be at most %d, got %d" % (MAX_K, k + dna + rna))
+    return BULGES | (dna << 17) | (rna << 22)
+
+
 def _strands(strands):
     """The k bit of strands=: 0 for "forward", B200SA_APPROX_BOTH_STRANDS for "both"."""
     if not isinstance(strands, str) or strands not in ("forward", "both"):
@@ -55,7 +77,7 @@ def _strands(strands):
 
 
 def _call(table, queries, k, fetch, metric="hamming", best=None, iupac=False, strands="forward", documents=False,
-          align=False, fixed=False):
+          align=False, fixed=False, bulges=None):
     """(offsets u64[nq + 1], positions u32[], distances u32[]); positions and distances are None without
     fetch (the cap = 0 call).  metric "hamming" counts mismatches, "edit" the Levenshtein distance; best=s keeps
     each query's occurrences within s of its least distance (include/b200sa.h, B200SA_APPROX_BEST); iupac=True reads
@@ -65,8 +87,10 @@ def _call(table, queries, k, fetch, metric="hamming", best=None, iupac=False, st
     documents that hold q's hits instead, with the least distance in each (B200SA_APPROX_DOCUMENTS); align=True
     lists the alignment operations of q's hits instead, as (offsets, p, BAM word) entries (B200SA_APPROX_ALIGN);
     fixed=True (with iupac=True) keeps the lowercase query symbols fixed: they must match their class and take no
-    edit, and the threshold is spent on the uppercase ones (B200SA_APPROX_FIXED).  With align or fixed a single
-    text goes through the documents entry as one document."""
+    edit, and the threshold is spent on the uppercase ones (B200SA_APPROX_FIXED); bulges=(dna, rna) (with
+    metric="edit" and best=None) makes k the substitution budget beside at most dna DNA bulges (text bytes with no
+    query byte) and rna RNA bulges (query bytes with no text byte) (B200SA_APPROX_BULGES).  With align, fixed or
+    bulges a single text goes through the documents entry as one document."""
     import torch
     k = int(k)
     if not 0 <= k <= MAX_K:
@@ -74,12 +98,12 @@ def _call(table, queries, k, fetch, metric="hamming", best=None, iupac=False, st
     if metric not in METRICS:
         raise ValueError("metric must be 'hamming' or 'edit', got %r" % (metric,))
     kf = (k | METRICS[metric] | _flags(best) | _iupac(iupac) | _fixed(fixed, iupac) | _strands(strands) |
-          (DOCUMENTS if documents else 0) | (ALIGN if align else 0))
+          _bulges(bulges, k, metric, best) | (DOCUMENTS if documents else 0) | (ALIGN if align else 0))
     qs = [_as_bytes(q) for q in queries]
     nq, n = len(qs), len(table)
     d_t, d_r, d_s, ndocs = table._bwt_arrays()
     dev = torch.device("cuda", table._device)
-    if (align or fixed) and d_s is None:
+    if (align or fixed or bulges is not None) and d_s is None:
         d_s, ndocs = _one_document(table, dev), 1
     off = np.zeros(nq + 1, dtype=np.uint64)
     off[1:] = np.cumsum([len(q) for q in qs])
@@ -117,22 +141,23 @@ def _split(dist):
     return dist & np.uint32(MINUS - 1), (dist & np.uint32(MINUS)) != 0
 
 
-def positions_batch(table, queries, k, metric="hamming", best=None, iupac=False, strands="forward", fixed=False):
-    off, pos, dist = _call(table, queries, k, True, metric, best, iupac, strands, fixed=fixed)
+def positions_batch(table, queries, k, metric="hamming", best=None, iupac=False, strands="forward", fixed=False,
+                    bulges=None):
+    off, pos, dist = _call(table, queries, k, True, metric, best, iupac, strands, fixed=fixed, bulges=bulges)
     if strands == "forward":
         return off, pos, dist
     return (off, pos) + _split(dist)
 
 
-def positions(table, query, k, metric="hamming", best=None, iupac=False, strands="forward", fixed=False):
-    _, pos, dist = _call(table, [query], k, True, metric, best, iupac, strands, fixed=fixed)
+def positions(table, query, k, metric="hamming", best=None, iupac=False, strands="forward", fixed=False, bulges=None):
+    _, pos, dist = _call(table, [query], k, True, metric, best, iupac, strands, fixed=fixed, bulges=bulges)
     if strands == "forward":
         return pos, dist
     return (pos,) + _split(dist)
 
 
-def counts(table, queries, k, metric="hamming", best=None, iupac=False, strands="forward", fixed=False):
-    off, _, _ = _call(table, queries, k, False, metric, best, iupac, strands, fixed=fixed)
+def counts(table, queries, k, metric="hamming", best=None, iupac=False, strands="forward", fixed=False, bulges=None):
+    off, _, _ = _call(table, queries, k, False, metric, best, iupac, strands, fixed=fixed, bulges=bulges)
     return np.diff(off.astype(np.int64)).astype(np.uint64)
 
 

@@ -19,7 +19,7 @@
 // matches); k_align_edit<true> keeps X and I off fixed symbols and has no D in a row x where Q[x] or Q[x - 1] is
 // fixed, in its DP and in its move choices, so the walk takes the first allowed move.
 #pragma once
-#include "iupac.cuh"
+#include "bulge.cuh"
 #include "strand.cuh"
 
 namespace b200sa {
@@ -200,6 +200,106 @@ __global__ void __launch_bounds__(BLK) k_align_edit(AlignArgs A, uint32_t rows) 
     s.flush();
     A.cnt[i] = s.n;
     if (bad || cost != d || t > E || s.n > A.stride) atomicOr(A.err, 1u);
+}
+
+// B200SA_APPROX_BULGES (DESIGN 6b f-22): one thread per staged hit i in [h0, h1), budgets tb substitutions, d DNA
+// and r RNA bulges.  F(x, t, i, e) of bulge.cuh (the least #X of Q[x, m) against a prefix of T[t, E) with at most i
+// I and e D moves, saturated at tb + 1) over the d + r + 1 diagonals t - p - x in [-r, d] of the hit's start, every
+// row kept: row x of hit i at scratch + ((i - h0) * rows + x) * (d + r + 1) * NL, cell b = t - p - x + r holding
+// its NL = (r + 1)(d + 1) layers.  The walk from (0, p) with budgets (r, d, tb) and cost dist takes the first move,
+// diagonal, I, D, after which some layer still meets the budgets within the remaining cost (feasible): the f-20
+// order among the moves that keep the hit's cost and budgets.  FIXED: A.fixed marks Q's fixed symbols, whose moves
+// are constrained as in k_align_edit<true>.  The minimum of one block per SM lets ptxas keep the walk out of local
+// memory (it spills at its default of 48 registers).
+template <bool FIXED>
+__global__ void __launch_bounds__(BLK, 1) k_align_bulge(AlignArgs A, uint32_t tb, uint32_t d, uint32_t r, uint64_t h0,
+                                                     uint64_t h1, uint32_t rows, uint8_t *scratch) {
+    const uint64_t i = h0 + (uint64_t)blockIdx.x * BLK + threadIdx.x;
+    if (i >= h1) return;
+    const AlignQuery Q = align_query(A, i);
+    const uint32_t p = A.hpos[i], dist = A.hmis[i] & ~B200SA_APPROX_MINUS;
+    const uint32_t E = docs_end(A.starts, A.ndocs, A.n, docs_find(A.starts, A.ndocs, p));
+    const uint32_t NL = (r + 1) * (d + 1), D1 = d + 1, W = d + r + 1, RB = W * NL, INF = tb + 1;
+    uint8_t *F = scratch + (i - h0) * rows * RB;
+    const uint8_t *__restrict__ mk = Q.q + A.fixed;
+    auto fixed = [&](uint32_t x) { return FIXED && __ldg(mk + (Q.minus ? Q.m - 1 - x : x)) != 0; };
+    auto tt = [&](uint32_t x, uint32_t b) { return (int64_t)p + x + b - r; };
+    for (uint32_t b = 0; b < W; b++) {                             // row m: D(m, t) = 0
+        const int64_t t = tt(Q.m, b);
+        const uint8_t y = (t >= p && t <= E) ? 0 : (uint8_t)INF;
+        for (uint32_t L = 0; L < NL; L++) F[Q.m * RB + b * NL + L] = y;
+    }
+    for (uint32_t x = Q.m; x-- > 0;) {
+        const uint32_t qc = Q.at(x);
+        const bool fx = fixed(x), nodel = fx || (x > 0 && fixed(x - 1));
+        uint8_t *cur = F + x * RB;
+        const uint8_t *below = cur + RB;
+        for (uint32_t b = W; b-- > 0;) {
+            const int64_t t = tt(x, b);
+            const bool txt = t >= p && t < E;
+            const uint32_t mi = txt ? !Q.match(__ldg(A.text + t), qc) : 1u;
+            const bool diag = txt && !(fx && mi), ins = (txt || t == E) && !fx && b > 0, del = txt && !nodel && b + 1 < W;
+            for (uint32_t L = 0; L < NL; L++) {
+                const uint32_t li = L / D1, le = L - li * D1;
+                uint32_t y = diag ? below[b * NL + L] + mi : INF;
+                if (ins && li > 0) y = min(y, (uint32_t)below[(b - 1) * NL + L - D1]);
+                if (del && le > 0) y = min(y, (uint32_t)cur[(b + 1) * NL + L - 1]);
+                cur[b * NL + L] = (uint8_t)min(y, INF);
+            }
+        }
+    }
+    // some alignment of Q[x, m) to T[t, ..) with <= iu I, <= du D and <= xu X moves costs at most C
+    auto feasible = [&](uint32_t x, int64_t t, uint32_t iu, uint32_t du, uint32_t xu, int32_t C) {
+        const int64_t b = t - p - x + r;
+        if (b < 0 || b >= W || C < 0) return false;
+        const uint8_t *cell = F + x * RB + b * NL;
+#pragma unroll 1
+        for (uint32_t li = 0; li <= iu; li++)
+#pragma unroll 1
+            for (uint32_t le = 0; le <= du; le++) {
+                const uint32_t f = cell[li * D1 + le];
+                if (f <= xu && (int32_t)(f + li + le) <= C) return true;
+            }
+        return false;
+    };
+    AlignSink s{A.ops + i * A.stride, A.stride};
+    // the hit's distance is the least cost within the budgets
+    bool bad = !feasible(0, p, r, d, tb, (int32_t)dist) || feasible(0, p, r, d, tb, (int32_t)dist - 1);
+    uint32_t x = 0, iu = r, du = d, xu = tb;
+    int32_t C = (int32_t)dist;
+    int64_t t = p;
+    while (x < Q.m && !bad) {
+        const bool fx = fixed(x), nodel = fx || (x > 0 && fixed(x - 1));
+        if (t < E) {
+            const uint32_t mi = !Q.match(__ldg(A.text + t), Q.at(x));
+            if (!(fx && mi) && mi <= xu && feasible(x + 1, t + 1, iu, du, xu - mi, C - (int32_t)mi)) {
+                s.push(mi ? ALIGN_X : ALIGN_EQ);
+                x++;
+                t++;
+                xu -= mi;
+                C -= (int32_t)mi;
+                continue;
+            }
+        }
+        if (!fx && iu > 0 && feasible(x + 1, t, iu - 1, du, xu, C - 1)) {
+            s.push(ALIGN_I);
+            x++;
+            iu--;
+            C--;
+            continue;
+        }
+        if (!nodel && t < E && du > 0 && feasible(x, t + 1, iu, du - 1, xu, C - 1)) {
+            s.push(ALIGN_D);
+            t++;
+            du--;
+            C--;
+            continue;
+        }
+        bad = true;
+    }
+    s.flush();
+    A.cnt[i] = s.n;
+    if (bad || C != 0 || s.n > A.stride) atomicOr(A.err, 1u);
 }
 
 // Hit i's cnt[i] words at its first entry seg[i]: d_pos gets p, d_mis the word with B200SA_APPROX_MINUS from the

@@ -117,6 +117,11 @@ struct CutPieces {
     static __device__ __forceinline__ uint32_t off(const ApproxArgs &A, uint32_t, uint32_t m, uint32_t j) {
         return approx_cut(m, A.P, j);
     }
+    // (offset, length) of piece i of query q of m bytes
+    static __device__ __forceinline__ uint2 piece(const ApproxArgs &A, uint32_t, uint32_t m, uint32_t i) {
+        const uint32_t a = approx_cut(m, A.P, i);
+        return make_uint2(a, approx_cut(m, A.P, i + 1) - a);
+    }
     // Whether the suffix at s, a candidate of the item's slot, starts an occurrence this slot reports; then
     // *p_out = its position and *mis_out = its mismatches.
     static __device__ __forceinline__ bool verify(const ApproxArgs &A, const ApproxItem &w, uint32_t s,

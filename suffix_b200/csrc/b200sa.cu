@@ -40,6 +40,7 @@
 #include "edit.cuh"
 #include "best.cuh"
 #include "iupac.cuh"
+#include "bulge.cuh"
 #include "strand.cuh"
 #include "approx_docs.cuh"
 #include "align.cuh"
@@ -94,6 +95,7 @@ struct b200sa_ctx {
     DevBuf strand, sstage;                     // with B200SA_APPROX_BOTH_STRANDS: the doubled batch, the staged hits
     DevBuf adoff, adocs;                       // with B200SA_APPROX_DOCUMENTS: the hit offsets, the staged hits
     DevBuf aops;                               // with B200SA_APPROX_ALIGN: each hit's operations
+    DevBuf abulge;                             // with B200SA_APPROX_ALIGN | _BULGES: the DP rows of a batch of hits
     uint32_t cls_calls = 0;
     // multi-GPU (SURVEY 8e): communicator owned or attached, NCCL resolved at run time
     ncclComm_t comm = nullptr;
@@ -1333,7 +1335,7 @@ void b200sa_ctx_destroy(b200sa_ctx *c) {
     DevBuf *bufs[] = {&c->text, &c->sa, &c->lcp, &c->pred, &c->stype, &c->lmsb, &c->lmsrank, &c->lmspos, &c->lmslist,
                       &c->lmspred, &c->sorted, &c->flag, &c->reduced, &c->sa_r, &c->blkstate, &c->carry, &c->tables,
                       &c->small, &c->scan_partial, &c->radix_cnt, &c->blkcnt, &c->k32b, &c->k64a, &c->k64b, &c->v0,
-                      &c->v1, &c->p0, &c->p1, &c->g0, &c->g1, &c->rank, &c->isa, &c->qbuf, &c->os_hist, &c->os_status, &c->packed, &c->phik, &c->phiv, &c->runscr, &c->plcp_samp, &c->scan_state, &c->cls_state, &c->lmsdesc, &c->steplog, &c->hist_copies, &c->tree_out, &c->docs_starts, &c->docs_out, &c->icode, &c->strand, &c->sstage, &c->adoff, &c->adocs, &c->aops, &c->sh_a, &c->sh_b, &c->sh_c, &c->sh_d, &c->sh_e, &c->sh_f, &c->sh_small};
+                      &c->v1, &c->p0, &c->p1, &c->g0, &c->g1, &c->rank, &c->isa, &c->qbuf, &c->os_hist, &c->os_status, &c->packed, &c->phik, &c->phiv, &c->runscr, &c->plcp_samp, &c->scan_state, &c->cls_state, &c->lmsdesc, &c->steplog, &c->hist_copies, &c->tree_out, &c->docs_starts, &c->docs_out, &c->icode, &c->strand, &c->sstage, &c->adoff, &c->adocs, &c->aops, &c->abulge, &c->sh_a, &c->sh_b, &c->sh_c, &c->sh_d, &c->sh_e, &c->sh_f, &c->sh_small};
     for (DevBuf *b : bufs) if (b->p) cudaFree(b->p);
     for (cudaEvent_t e : c->event_pool) cudaEventDestroy(e);
     if (c->h_pin) cudaFreeHost(c->h_pin);
@@ -2924,12 +2926,20 @@ int b200sa_unbwt_dev(b200sa_ctx *c, uint64_t n, uint32_t ndocs, const uint8_t *d
     return leave(c, unbwt_core(c, (uint32_t)n, ndocs, d_bwt, d_term_rows, d_text_out, d_doc_starts_out));
 }
 
-// ------------------------------------------------------------ approximate positions (DESIGN 6b f-14 .. f-21)
-// The k of a call as approx_args decodes it: the threshold, B200SA_APPROX_BEST's slack, and the flags.
+// ------------------------------------------------------------ approximate positions (DESIGN 6b f-14 .. f-22)
+// B200SA_APPROX_BULGES: on, with t substitutions, d DNA bulges and r RNA bulges.
+struct Bulges {
+    bool on;
+    uint32_t t, d, r;
+};
+
+// The k of a call as approx_args decodes it: the threshold (t + d + r with B200SA_APPROX_BULGES), B200SA_APPROX_BEST's
+// slack, and the flags.
 struct ApproxFlags {
     uint32_t k, s;
     bool edit, best, iupac, fixed, both, docs, align;
     bool stage;                                          // docs || align: the final lists go to staging
+    Bulges bulges;
 };
 
 // The words of c->small through which the approximate search hands results from its kernels to the host; a u64
@@ -3011,19 +3021,33 @@ static ApproxKernel approx_kernel(bool edit, bool iupac, bool fixed) {
     return edit ? k_approx_edit<EMIT> : k_approx<EMIT>;
 }
 
+// B200SA_APPROX_BULGES: the count (EMIT false) or emit pass of k_approx_bulge over the items, for the query alphabet.
+template <bool EMIT>
+static void launch_bulge(b200sa_ctx *c, bool iupac, bool fixed, uint64_t items, const BulgeArgs &B, uint32_t *cnt,
+                         const unsigned long long *item_off, int pbits, unsigned long long *key, uint32_t *val) {
+    typedef void (*Kernel)(BulgeArgs, uint32_t *, const unsigned long long *, int, unsigned long long *, uint32_t *);
+    const Kernel kern = fixed   ? k_approx_bulge<EMIT, FixedIupacPieces>
+                        : iupac ? k_approx_bulge<EMIT, IupacPieces>
+                                : k_approx_bulge<EMIT, CutPieces>;
+    kern<<<(uint32_t)cdiv(items, BULGE_WARPS), BULGE_BLK, 0, c->stream>>>(B, cnt, item_off, pbits, key, val);
+    c->launches++;
+}
+
 // One search of nq >= 1 queries at threshold k on n >= 1 bytes: d_offsets (nq + 1) and *total, read back.  When
 // 0 < total <= cap it also emits and sorts: *ko / *vo then hold the keys (q << *pbits) | p in (q, p) order and
 // their distances.  Phases: approx_pieces, approx_scan, approx_count, and approx_emit, approx_sort when it
 // emits.  B200SA_APPROX_EDIT picks k_approx_edit over k_approx; iupac (d_queries then the canonical copy) picks
 // the pieces of k_iupac_pieces and the kernels' IUPAC instantiations; d_fixed, the marks of the queries' fixed
 // symbols (B200SA_APPROX_FIXED, with iupac) or NULL, their fixed instantiations, with the pointer after the piece
-// table (iupac_marks); everything else is shared.
+// table (iupac_marks); bg.on (B200SA_APPROX_BULGES, k = t + d + r) the layered verification of k_approx_bulge in
+// place of the metric's; everything else is shared.
 template <class EndF>
 static int approx_search(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const uint32_t *d_sa,
                          const uint32_t *d_starts, uint32_t ndocs, const uint8_t *d_queries, const uint64_t *d_q_off,
                          const uint8_t *d_fixed, uint32_t nq, uint32_t k, bool edit, bool iupac, uint64_t *d_offsets,
                          uint64_t cap,
-                         uint64_t *total, EndF end, uint64_t **ko, uint32_t **vo, int *pbits_out) {
+                         uint64_t *total, EndF end, uint64_t **ko, uint32_t **vo, int *pbits_out,
+                         Bulges bg = Bulges{}) {
     typedef unsigned long long u64;
     uint32_t *words = ptr<uint32_t>(c->small);
     const uint32_t P = k + 1;
@@ -3051,6 +3075,9 @@ static int approx_search(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const
     const uint64_t items = pin_u64(c, 0);
     if (items > (uint64_t)0x7fffffff * NWARP)
         return fail(c, B200SA_ERR_TOO_LARGE, "approx positions: more than 2^31 * 8 chunks of 1024 candidates in one batch");
+    if (bg.on && items > (uint64_t)0x7fffffff * BULGE_WARPS)
+        return fail(c, B200SA_ERR_TOO_LARGE, "approx positions: with B200SA_APPROX_BULGES, more than 2^31 * 4 chunks of "
+                                             "1024 candidates in one batch");
     TRY(mark(c, "approx_count"));
     TRY(ensure(c, c->p0, (size_t)items * 4));
     TRY(ensure(c, c->k64b, ((size_t)items + 1) * 8));
@@ -3060,7 +3087,10 @@ static int approx_search(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const
     const ApproxArgs A{d_text, d_sa, d_starts, ndocs, n, d_queries, d_q_off, (uint32_t)nslots, P, k, ps, pe,
                        item_start, items};
     const int pbits = bit_length(n - 1);
-    if (items)
+    const BulgeArgs B{A, bg.t, bg.d, bg.r};
+    if (items && bg.on)
+        launch_bulge<false>(c, iupac, fixed, items, B, cnt, nullptr, pbits, nullptr, nullptr);
+    else if (items)
         LAUNCH(c, approx_kernel<false>(edit, iupac, fixed), cdiv(items, NWARP), A, cnt, (const u64 *)nullptr, pbits,
                (u64 *)nullptr, (uint32_t *)nullptr);
     TRY((dev_scan<OpSum64>(c, InCount64{cnt, items}, OutStoreExcl64{item_off}, items + 1, d_total)));
@@ -3075,8 +3105,11 @@ static int approx_search(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const
         TRY(ensure(c, c->g1, (size_t)*total * 8));
         TRY(ensure(c, c->v0, (size_t)*total * 4));
         TRY(ensure(c, c->v1, (size_t)*total * 4));
-        LAUNCH(c, approx_kernel<true>(edit, iupac, fixed), cdiv(items, NWARP), A, cnt, (const u64 *)item_off, pbits,
-               ptr<u64>(c->g0), ptr<uint32_t>(c->v0));
+        if (bg.on)
+            launch_bulge<true>(c, iupac, fixed, items, B, cnt, item_off, pbits, ptr<u64>(c->g0), ptr<uint32_t>(c->v0));
+        else
+            LAUNCH(c, approx_kernel<true>(edit, iupac, fixed), cdiv(items, NWARP), A, cnt, (const u64 *)item_off,
+                   pbits, ptr<u64>(c->g0), ptr<uint32_t>(c->v0));
         TRY(mark(c, "approx_sort"));                     // by (q, p)
         TRY(sort_pairs<uint64_t>(c, ptr<uint64_t>(c->g0), ptr<uint32_t>(c->v0), ptr<uint64_t>(c->g1),
                                  ptr<uint32_t>(c->v1), *total, bit_length(nq - 1) + pbits, ko, vo));
@@ -3203,11 +3236,13 @@ static int align_check(b200sa_ctx *c, const uint64_t *d_q_off, uint32_t nq, bool
 // caller's offsets and, when the listing fits cap, d_pos and d_mis; *total becomes the number of operations.  qs:
 // the queries (the canonical copy with iupac), k the threshold, mmax the longest query.  Phases align_count,
 // align_scan and align_emit.  fixed: the marks of qs with B200SA_APPROX_FIXED (k_align_edit<true>), after qs in
-// its buffer; else NULL.
+// its buffer; else NULL.  bg.on (B200SA_APPROX_BULGES, k = t + d + r): k_align_bulge, over batches of hits whose
+// DP rows fit ALIGN_BULGE_SCRATCH bytes.
+constexpr size_t ALIGN_BULGE_SCRATCH = 64u << 20;
 static int align_list(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const uint32_t *d_starts, uint32_t ndocs,
                       const uint8_t *qs, const uint64_t *d_q_off, const uint8_t *fixed, uint32_t nq, uint32_t k,
                       bool edit, bool iupac, uint32_t mmax, const uint64_t *hoff, uint64_t *d_offsets,
-                      uint32_t *d_pos, uint32_t *d_mis, uint64_t cap, uint64_t *total) {
+                      uint32_t *d_pos, uint32_t *d_mis, uint64_t cap, uint64_t *total, Bulges bg) {
     typedef unsigned long long u64;
     const uint64_t htotal = *total;
     TRY(mark(c, "align_count"));
@@ -3224,7 +3259,21 @@ static int align_list(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const ui
     const AlignArgs A{d_text, d_starts, ndocs, n, qs, d_q_off, nq, fixed ? (uint32_t)(fixed - qs) : 0u,
                       (const u64 *)hoff, hpos, hmis, htotal, iupac, stride, ptr<uint32_t>(c->aops), cnt,
                       words + AW_ALIGN_ERR};
-    if (edit) {
+    if (bg.on) {
+        const uint32_t rows = mmax + 1;
+        const size_t per_hit = (size_t)rows * (bg.d + bg.r + 1) * (bg.d + 1) * (bg.r + 1);
+        const uint64_t batch = std::max<uint64_t>(1, ALIGN_BULGE_SCRATCH / per_hit);
+        TRY(ensure(c, c->abulge, (size_t)std::min<uint64_t>(batch, htotal) * per_hit));
+        for (uint64_t h0 = 0; h0 < htotal; h0 += batch) {
+            const uint64_t h1 = std::min(htotal, h0 + batch);
+            if (fixed)
+                LAUNCH(c, k_align_bulge<true>, cdiv(h1 - h0, BLK), A, bg.t, bg.d, bg.r, h0, h1, rows,
+                       ptr<uint8_t>(c->abulge));
+            else
+                LAUNCH(c, k_align_bulge<false>, cdiv(h1 - h0, BLK), A, bg.t, bg.d, bg.r, h0, h1, rows,
+                       ptr<uint8_t>(c->abulge));
+        }
+    } else if (edit) {
         // 16 bytes of choices per query row and warp: as many warps per block (up to 8) as fit 48 KB, at least one
         const size_t per_warp = (size_t)max(mmax, 1u) * 16;
         const uint32_t aw = (uint32_t)std::max<size_t>(1, std::min<size_t>(NWARP, 49152 / per_warp));
@@ -3306,7 +3355,7 @@ static int approx_plain(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const 
     uint32_t *vo = nullptr;
     int pbits = 0;
     TRY(approx_search(c, d_text, n, d_sa, d_starts, ndocs, e.q, e.off, e.fx, e.ne, f.k, f.edit, f.iupac, e.out,
-                      fin.cap, total, end, &ko, &vo, &pbits));
+                      fin.cap, total, end, &ko, &vo, &pbits, f.bulges));
     const bool emitted = *total > 0 && *total <= fin.cap;
     if (f.stage && emitted) TRY(adocs_stage(c, *total, &fin.pos, &fin.mis));
     if (f.both)
@@ -3435,7 +3484,7 @@ static int approx_run(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const ui
     if (f.docs) TRY(adocs_reduce(c, d_starts, ndocs, nq, fin.off, d_offsets, d_pos, d_mis, cap, total));
     if (f.align)
         TRY(align_list(c, d_text, n, d_starts, ndocs, d_queries, d_q_off, d_fixed, nq, f.k, f.edit, f.iupac, mmax,
-                       fin.off, d_offsets, d_pos, d_mis, cap, total));
+                       fin.off, d_offsets, d_pos, d_mis, cap, total, f.bulges));
     TRY(mark(c, "end"));
     CU_TRY(c, cudaGetLastError());
     CU_TRY(c, cudaStreamSynchronize(c->stream));
@@ -3443,16 +3492,20 @@ static int approx_run(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const ui
 }
 
 // The argument checks shared by both entry points, and k decoded into *f.  docs: the documents entry, the only one
-// that takes B200SA_APPROX_DOCUMENTS, B200SA_APPROX_ALIGN and B200SA_APPROX_FIXED.
+// that takes B200SA_APPROX_DOCUMENTS, B200SA_APPROX_ALIGN, B200SA_APPROX_FIXED and B200SA_APPROX_BULGES (whose
+// budget fields are known bits only beside it).
 static int approx_args(b200sa_ctx *c, uint64_t n, const void *text, const void *sa, const void *q_off, uint32_t nq,
                        uint32_t k, const void *offsets, const void *pos, uint64_t cap, const void *total, bool docs,
                        ApproxFlags *f) {
     if (!c) return B200SA_ERR_BAD_ARG;
     if (!total || !offsets || (nq > 0 && !q_off) || (cap > 0 && !pos) || (n > 0 && (!text || !sa))) return null_ptr(c);
-    const bool best = (k & B200SA_APPROX_BEST) != 0;
+    const bool best = (k & B200SA_APPROX_BEST) != 0, bulges = (k & B200SA_APPROX_BULGES) != 0;
     const uint32_t accepted = 0xFFFFu | B200SA_APPROX_EDIT | B200SA_APPROX_IUPAC | B200SA_APPROX_BOTH_STRANDS |
                               (best ? B200SA_APPROX_BEST : 0u) |
-                              (docs ? B200SA_APPROX_DOCUMENTS | B200SA_APPROX_ALIGN | B200SA_APPROX_FIXED : 0u);
+                              (docs ? B200SA_APPROX_DOCUMENTS | B200SA_APPROX_ALIGN | B200SA_APPROX_FIXED : 0u) |
+                              (docs && bulges ? B200SA_APPROX_BULGES | B200SA_APPROX_DNA_BULGES(3) |
+                                                    B200SA_APPROX_RNA_BULGES(3)
+                                              : 0u);
     // with B200SA_APPROX_BEST the threshold and the slack are a byte each, and either above the limit is a bad k
     if ((k & ~accepted) || (best && ((k & 0xFFu) > B200SA_APPROX_MAX_K || ((k >> 8) & 0xFFu) > B200SA_APPROX_MAX_K))) {
         const std::string m =
@@ -3462,18 +3515,29 @@ static int approx_args(b200sa_ctx *c, uint64_t n, const void *text, const void *
             ", optionally | B200SA_APPROX_EDIT, | B200SA_APPROX_IUPAC" +
             (docs ? ", | B200SA_APPROX_BOTH_STRANDS, | B200SA_APPROX_FIXED with B200SA_APPROX_IUPAC and "
                     "| B200SA_APPROX_DOCUMENTS, or | B200SA_APPROX_ALIGN"
-                  : " and | B200SA_APPROX_BOTH_STRANDS");
+                  : " and | B200SA_APPROX_BOTH_STRANDS") +
+            (!docs && bulges ? "; B200SA_APPROX_BULGES is taken by b200sa_docs_approx_positions_dev only" : "");
         return fail(c, B200SA_ERR_BAD_ARG, m.c_str());
     }
     if ((k & B200SA_APPROX_FIXED) && !(k & B200SA_APPROX_IUPAC))
         return fail(c, B200SA_ERR_BAD_ARG, "approx positions: B200SA_APPROX_FIXED requires B200SA_APPROX_IUPAC");
+    if (bulges && !(k & B200SA_APPROX_EDIT))
+        return fail(c, B200SA_ERR_BAD_ARG, "approx positions: B200SA_APPROX_BULGES requires B200SA_APPROX_EDIT");
+    if (bulges && best)
+        return fail(c, B200SA_ERR_BAD_ARG,
+                    "approx positions: B200SA_APPROX_BULGES and B200SA_APPROX_BEST do not combine");
     if (!best && (k & 0xFFFFu) > B200SA_APPROX_MAX_K)
         return fail(c, B200SA_ERR_BAD_ARG, "approx positions: k above B200SA_APPROX_MAX_K");
+    const Bulges bg{bulges, k & 0xFFFFu, (k >> 17) & 3u, (k >> 22) & 3u};
+    if (bulges && bg.t + bg.d + bg.r > B200SA_APPROX_MAX_K)
+        return fail(c, B200SA_ERR_BAD_ARG, "approx positions: with B200SA_APPROX_BULGES, the threshold plus the DNA "
+                                           "and RNA bulges above B200SA_APPROX_MAX_K");
     if (n > B200SA_MAX_N) return too_long(c);
     const bool listing = (k & B200SA_APPROX_DOCUMENTS) != 0, align = (k & B200SA_APPROX_ALIGN) != 0;
-    *f = ApproxFlags{best ? k & 0xFFu : k & 0xFFFFu, best ? (k >> 8) & 0xFFu : 0u, (k & B200SA_APPROX_EDIT) != 0,
-                     best, (k & B200SA_APPROX_IUPAC) != 0, (k & B200SA_APPROX_FIXED) != 0,
-                     (k & B200SA_APPROX_BOTH_STRANDS) != 0, listing, align, listing || align};
+    *f = ApproxFlags{best ? k & 0xFFu : bulges ? bg.t + bg.d + bg.r : k & 0xFFFFu, best ? (k >> 8) & 0xFFu : 0u,
+                     (k & B200SA_APPROX_EDIT) != 0, best, (k & B200SA_APPROX_IUPAC) != 0,
+                     (k & B200SA_APPROX_FIXED) != 0, (k & B200SA_APPROX_BOTH_STRANDS) != 0, listing, align,
+                     listing || align, bg};
     return B200SA_OK;
 }
 

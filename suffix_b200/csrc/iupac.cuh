@@ -151,6 +151,9 @@ struct IupacPieces {
     static __device__ __forceinline__ uint32_t off(const ApproxArgs &A, uint32_t slot, uint32_t, uint32_t) {
         return iupac_table(A)[slot].x;
     }
+    static __device__ __forceinline__ uint2 piece(const ApproxArgs &A, uint32_t q, uint32_t, uint32_t i) {
+        return iupac_table(A)[(uint64_t)q * A.P + i];
+    }
     // The class test over all m symbols, then the pieces [0, j) of the query's table.
     static __device__ __forceinline__ bool verify(const ApproxArgs &A, const ApproxItem &w, uint32_t s,
                                                   uint32_t *p_out, uint32_t *mis_out) {
