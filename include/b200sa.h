@@ -559,7 +559,8 @@ int b200sa_unbwt_dev(b200sa_ctx *ctx, uint64_t n, uint32_t ndocs, const uint8_t 
  * names are as above.  m = 0 has no occurrences; 0 < m <= k makes every position an occurrence (dist <= m).
  * k = 0 gives exactly the set b200sa_positions_dev returns.  For every k the Hamming occurrences are a subset of
  * the edit occurrences, with dist(p) <= mis(p) on them.  One locus yields a run of neighbouring starts (an exact
- * hit at p also puts p - 1 and p + 1 at distance 1, when they lie in p's document); no filtering is applied.
+ * hit at p also puts p - 1 and p + 1 at distance 1, when they lie in p's document); no filtering is applied
+ * (B200SA_APPROX_LOCI, f-23 below, keeps one hit per locus).
  * Method: the same pieces and slots.  A candidate s of piece j (offset o_j) considers the starts p of s's
  * document with |p - (s - o_j)| <= k and computes their dist(p) by one banded reversed Sellers DP over the
  * diagonals [s - o_j - 2k, s - o_j + 2k].  It emits p iff dist(p) <= k and it is the least (i, s'') such that
@@ -803,7 +804,48 @@ int b200sa_unbwt_dev(b200sa_ctx *ctx, uint64_t n, uint32_t ndocs, const uint8_t 
  * #X, saturated at t + 1, in shared memory; the alignment recomputes the d + r + 1 diagonals of its hit, one thread
  * per hit, with every row kept in a device buffer of at most 64 MB per batch of hits.  Device workspace (computed,
  * not measured): what B200SA_APPROX_EDIT takes at threshold t + d + r, and with B200SA_APPROX_ALIGN up to 64 MB for
- * the rows.  Phases: those of the call without the flag. */
+ * the rows.  Phases: those of the call without the flag.
+ *
+ * ---- one hit per locus (DESIGN.md 6b f-23) ----
+ * With B200SA_APPROX_LOCI (bit 7) in k, b200sa_docs_approx_positions_dev lists one hit per locus instead of the run
+ * of neighbouring starts that one site yields (an exact hit at p also puts p - 1 and p + 1 at distance 1 under
+ * B200SA_APPROX_EDIT, and a bulge budget adds more), so that counts count sites.  On that entry the threshold is
+ * k & 0xFF7F (k & 0x7F with B200SA_APPROX_BEST, and likewise the t of B200SA_APPROX_BULGES); on
+ * b200sa_approx_positions_dev bit 7 stays a threshold bit, with its behaviour and error message unchanged.  The flag
+ * mixes freely with B200SA_APPROX_EDIT, B200SA_APPROX_BEST | B200SA_APPROX_SLACK(s), B200SA_APPROX_IUPAC,
+ * B200SA_APPROX_FIXED, B200SA_APPROX_BOTH_STRANDS, B200SA_APPROX_BULGES and B200SA_APPROX_ALIGN; a single text goes
+ * through that entry as one document.  B200SA_APPROX_LOCI | B200SA_APPROX_DOCUMENTS returns B200SA_ERR_BAD_ARG with
+ * a detail that names both (the document listing already keeps one entry per document).  Without the flag nothing
+ * changes.  Definition:
+ *  - L(q) is the list the same call with bit 7 cleared returns for q: hits (p, d, strand); best(q) and t(q) are
+ *    that call's.  m = |q| in bytes.
+ *  - Two hits of L(q) are linked when they are on the same strand, in the same document, and |p - p'| < m.  A locus
+ *    is a maximal chain of linked hits: in ascending p, one strand's hits in one document, cut wherever consecutive
+ *    starts differ by m or more.
+ *  - Each locus is represented by its hit with the least d, ties going to the least p.  q's list is its
+ *    representatives, ordered by (p, strand) with + first; each carries its own d, with B200SA_APPROX_MINUS on a
+ *    - hit.
+ *  - Protocol: the listing protocol; offsets and *total count loci.  With cap = 0 the call still stages every hit,
+ *    as B200SA_APPROX_DOCUMENTS does.  With B200SA_APPROX_ALIGN the output is the representatives' alignments,
+ *    exactly the words the call without bit 7 gives for those hits.
+ *  - Unchanged from the call without the flag: the argument checks and error codes, the TOO_LARGE checks, nq = 0,
+ *    n = 0, m = 0, the bytes read, synchronisation and b200sa_last_stats().doubling_rounds.
+ *  - So the loci are a subset of L(q), at equal distances; if no two same-strand hits of q in one document are
+ *    closer than m, the result is L(q) bit for bit; with m = 1 nothing merges; hits in different documents, or on
+ *    different strands, never merge.
+ * Method: the final list is staged as with B200SA_APPROX_DOCUMENTS.  Over the staged list, a max scan carries the
+ * last hit index of each strand (one 32-bit channel per strand), which marks the heads: a hit whose previous hit of
+ * its strand lies in another query or document, or m or more bytes before it.  A second max scan carries the last
+ * head index of each strand, which gives each hit its locus, and the least (d << 32) | p of a locus is taken with an
+ * atomicMin at its head, so the result does not depend on the order of the hits.  A chain as long as the text goes
+ * through the scans' carries, never through a serial loop.  A sum scan of the representatives gives their places
+ * and the offsets, and they are copied out (or, with B200SA_APPROX_ALIGN, back into staging for the alignment).
+ * A call with 2^32 - 1 or more staged hits returns B200SA_ERR_TOO_LARGE.  Device workspace (computed, not measured):
+ * what the call without the flag takes with the staged list (the fetch call's emission for the whole hit list, plus
+ * the staging's 20 bytes per hit and 8 per query), plus 20 bytes per hit for the least keys, the scan of the
+ * representatives and the heads, and with B200SA_APPROX_ALIGN 8 bytes per query.  Phases: those of the call without
+ * the flag (with its emission phases even at cap = 0), then loci_mark and, when the listing fits or with
+ * B200SA_APPROX_ALIGN, loci_emit, before the alignment's phases. */
 #define B200SA_APPROX_MAX_K 31
 #define B200SA_APPROX_EDIT 0x10000u
 #define B200SA_APPROX_BEST 0x100000u                      /* bit 20 */
@@ -818,6 +860,7 @@ int b200sa_unbwt_dev(b200sa_ctx *ctx, uint64_t n, uint32_t ndocs, const uint8_t 
 #define B200SA_APPROX_BULGES 0x200000u                    /* bit 21, in k, documents entry only, with B200SA_APPROX_EDIT */
 #define B200SA_APPROX_DNA_BULGES(d) ((uint32_t)(d) << 17)  /* bits 17-18, 0 <= d <= 3, only with B200SA_APPROX_BULGES */
 #define B200SA_APPROX_RNA_BULGES(r) ((uint32_t)(r) << 22)  /* bits 22-23, 0 <= r <= 3, only with B200SA_APPROX_BULGES */
+#define B200SA_APPROX_LOCI 0x80u                          /* bit 7, in k, documents entry only */
 int b200sa_approx_positions_dev(b200sa_ctx *ctx, const uint8_t *d_text, uint64_t n, const uint32_t *d_sa,
                                 const uint8_t *d_queries, const uint64_t *d_q_off, uint32_t nq, uint32_t k,
                                 uint64_t *d_offsets, uint32_t *d_pos, uint32_t *d_mismatches, uint64_t cap,

@@ -1,7 +1,7 @@
 """Approximate positions (occurrences with at most k mismatches, or within k edits with metric="edit", with
 best=s only each query's best hits, with iupac=True queries in IUPAC nucleotide codes, with fixed=True their
-lowercase symbols fixed, and with strands="both" the reverse complement's hits as well), the documents that hold
-them, and their alignments, over a device-resident table: the part SuffixTable and DocumentSuffixTable share.  A
+lowercase symbols fixed, with strands="both" the reverse complement's hits as well, and with loci=True one hit per
+locus), the documents that hold them, and their alignments, over a device-resident table: the part SuffixTable and DocumentSuffixTable share.  A
 table supplies `_device` and `_bwt_arrays()` -> (d_text, d_table, d_doc_starts or None, ndocs), its text and table
 on the device; the LCP array is not needed."""
 import numpy as np
@@ -19,6 +19,7 @@ DOCUMENTS = 0x20000000    # B200SA_APPROX_DOCUMENTS
 ALIGN = 0x8000000         # B200SA_APPROX_ALIGN
 FIXED = 0x2000000         # B200SA_APPROX_FIXED
 BULGES = 0x200000         # B200SA_APPROX_BULGES
+LOCI = 0x80               # B200SA_APPROX_LOCI
 MAX_BULGE = 3             # the most DNA or RNA bulges
 OPS = "MIDNSHP=X"         # the BAM operation codes
 METRICS = {"hamming": 0, "edit": EDIT}
@@ -69,6 +70,13 @@ def _bulges(bulges, k, metric, best):
     return BULGES | (dna << 17) | (rna << 22)
 
 
+def _loci(loci):
+    """The k bit of loci=: B200SA_APPROX_LOCI for True, 0 for False."""
+    if not isinstance(loci, (bool, np.bool_)):
+        raise ValueError("loci must be True or False, got %r" % (loci,))
+    return LOCI if loci else 0
+
+
 def _strands(strands):
     """The k bit of strands=: 0 for "forward", B200SA_APPROX_BOTH_STRANDS for "both"."""
     if not isinstance(strands, str) or strands not in ("forward", "both"):
@@ -77,7 +85,7 @@ def _strands(strands):
 
 
 def _call(table, queries, k, fetch, metric="hamming", best=None, iupac=False, strands="forward", documents=False,
-          align=False, fixed=False, bulges=None):
+          align=False, fixed=False, bulges=None, loci=False):
     """(offsets u64[nq + 1], positions u32[], distances u32[]); positions and distances are None without
     fetch (the cap = 0 call).  metric "hamming" counts mismatches, "edit" the Levenshtein distance; best=s keeps
     each query's occurrences within s of its least distance (include/b200sa.h, B200SA_APPROX_BEST); iupac=True reads
@@ -89,8 +97,10 @@ def _call(table, queries, k, fetch, metric="hamming", best=None, iupac=False, st
     fixed=True (with iupac=True) keeps the lowercase query symbols fixed: they must match their class and take no
     edit, and the threshold is spent on the uppercase ones (B200SA_APPROX_FIXED); bulges=(dna, rna) (with
     metric="edit" and best=None) makes k the substitution budget beside at most dna DNA bulges (text bytes with no
-    query byte) and rna RNA bulges (query bytes with no text byte) (B200SA_APPROX_BULGES).  With align, fixed or
-    bulges a single text goes through the documents entry as one document."""
+    query byte) and rna RNA bulges (query bytes with no text byte) (B200SA_APPROX_BULGES); loci=True keeps one hit
+    per locus, a chain of same-strand hits in one document whose starts are less than the query's length apart,
+    the one with the least distance, leftmost on a tie (B200SA_APPROX_LOCI).  With align, fixed, bulges or loci a
+    single text goes through the documents entry as one document."""
     import torch
     k = int(k)
     if not 0 <= k <= MAX_K:
@@ -98,12 +108,12 @@ def _call(table, queries, k, fetch, metric="hamming", best=None, iupac=False, st
     if metric not in METRICS:
         raise ValueError("metric must be 'hamming' or 'edit', got %r" % (metric,))
     kf = (k | METRICS[metric] | _flags(best) | _iupac(iupac) | _fixed(fixed, iupac) | _strands(strands) |
-          _bulges(bulges, k, metric, best) | (DOCUMENTS if documents else 0) | (ALIGN if align else 0))
+          _bulges(bulges, k, metric, best) | _loci(loci) | (DOCUMENTS if documents else 0) | (ALIGN if align else 0))
     qs = [_as_bytes(q) for q in queries]
     nq, n = len(qs), len(table)
     d_t, d_r, d_s, ndocs = table._bwt_arrays()
     dev = torch.device("cuda", table._device)
-    if (align or fixed or bulges is not None) and d_s is None:
+    if (align or fixed or bulges is not None or loci) and d_s is None:
         d_s, ndocs = _one_document(table, dev), 1
     off = np.zeros(nq + 1, dtype=np.uint64)
     off[1:] = np.cumsum([len(q) for q in qs])
@@ -142,22 +152,25 @@ def _split(dist):
 
 
 def positions_batch(table, queries, k, metric="hamming", best=None, iupac=False, strands="forward", fixed=False,
-                    bulges=None):
-    off, pos, dist = _call(table, queries, k, True, metric, best, iupac, strands, fixed=fixed, bulges=bulges)
+                    bulges=None, loci=False):
+    off, pos, dist = _call(table, queries, k, True, metric, best, iupac, strands, fixed=fixed, bulges=bulges,
+                           loci=loci)
     if strands == "forward":
         return off, pos, dist
     return (off, pos) + _split(dist)
 
 
-def positions(table, query, k, metric="hamming", best=None, iupac=False, strands="forward", fixed=False, bulges=None):
-    _, pos, dist = _call(table, [query], k, True, metric, best, iupac, strands, fixed=fixed, bulges=bulges)
+def positions(table, query, k, metric="hamming", best=None, iupac=False, strands="forward", fixed=False, bulges=None,
+              loci=False):
+    _, pos, dist = _call(table, [query], k, True, metric, best, iupac, strands, fixed=fixed, bulges=bulges, loci=loci)
     if strands == "forward":
         return pos, dist
     return (pos,) + _split(dist)
 
 
-def counts(table, queries, k, metric="hamming", best=None, iupac=False, strands="forward", fixed=False, bulges=None):
-    off, _, _ = _call(table, queries, k, False, metric, best, iupac, strands, fixed=fixed, bulges=bulges)
+def counts(table, queries, k, metric="hamming", best=None, iupac=False, strands="forward", fixed=False, bulges=None,
+           loci=False):
+    off, _, _ = _call(table, queries, k, False, metric, best, iupac, strands, fixed=fixed, bulges=bulges, loci=loci)
     return np.diff(off.astype(np.int64)).astype(np.uint64)
 
 

@@ -44,6 +44,7 @@
 #include "strand.cuh"
 #include "approx_docs.cuh"
 #include "align.cuh"
+#include "loci.cuh"
 #include "nccl_dyn.h"
 
 using namespace b200sa;
@@ -96,6 +97,7 @@ struct b200sa_ctx {
     DevBuf adoff, adocs;                       // with B200SA_APPROX_DOCUMENTS: the hit offsets, the staged hits
     DevBuf aops;                               // with B200SA_APPROX_ALIGN: each hit's operations
     DevBuf abulge;                             // with B200SA_APPROX_ALIGN | _BULGES: the DP rows of a batch of hits
+    DevBuf loci;                               // with B200SA_APPROX_LOCI: the locus keys, heads, marks and offsets
     uint32_t cls_calls = 0;
     // multi-GPU (SURVEY 8e): communicator owned or attached, NCCL resolved at run time
     ncclComm_t comm = nullptr;
@@ -1335,7 +1337,7 @@ void b200sa_ctx_destroy(b200sa_ctx *c) {
     DevBuf *bufs[] = {&c->text, &c->sa, &c->lcp, &c->pred, &c->stype, &c->lmsb, &c->lmsrank, &c->lmspos, &c->lmslist,
                       &c->lmspred, &c->sorted, &c->flag, &c->reduced, &c->sa_r, &c->blkstate, &c->carry, &c->tables,
                       &c->small, &c->scan_partial, &c->radix_cnt, &c->blkcnt, &c->k32b, &c->k64a, &c->k64b, &c->v0,
-                      &c->v1, &c->p0, &c->p1, &c->g0, &c->g1, &c->rank, &c->isa, &c->qbuf, &c->os_hist, &c->os_status, &c->packed, &c->phik, &c->phiv, &c->runscr, &c->plcp_samp, &c->scan_state, &c->cls_state, &c->lmsdesc, &c->steplog, &c->hist_copies, &c->tree_out, &c->docs_starts, &c->docs_out, &c->icode, &c->strand, &c->sstage, &c->adoff, &c->adocs, &c->aops, &c->abulge, &c->sh_a, &c->sh_b, &c->sh_c, &c->sh_d, &c->sh_e, &c->sh_f, &c->sh_small};
+                      &c->v1, &c->p0, &c->p1, &c->g0, &c->g1, &c->rank, &c->isa, &c->qbuf, &c->os_hist, &c->os_status, &c->packed, &c->phik, &c->phiv, &c->runscr, &c->plcp_samp, &c->scan_state, &c->cls_state, &c->lmsdesc, &c->steplog, &c->hist_copies, &c->tree_out, &c->docs_starts, &c->docs_out, &c->icode, &c->strand, &c->sstage, &c->adoff, &c->adocs, &c->aops, &c->abulge, &c->loci, &c->sh_a, &c->sh_b, &c->sh_c, &c->sh_d, &c->sh_e, &c->sh_f, &c->sh_small};
     for (DevBuf *b : bufs) if (b->p) cudaFree(b->p);
     for (cudaEvent_t e : c->event_pool) cudaEventDestroy(e);
     if (c->h_pin) cudaFreeHost(c->h_pin);
@@ -2937,8 +2939,8 @@ struct Bulges {
 // slack, and the flags.
 struct ApproxFlags {
     uint32_t k, s;
-    bool edit, best, iupac, fixed, both, docs, align;
-    bool stage;                                          // docs || align: the final lists go to staging
+    bool edit, best, iupac, fixed, both, docs, align, loci;
+    bool stage;                                          // docs || align || loci: the final lists go to staging
     Bulges bulges;
 };
 
@@ -2947,10 +2949,10 @@ struct ApproxFlags {
 // (the search clears [0, 6)); [8, 10) (batch size << 32) | batch bytes of best_batch, [10] the rounds where a query
 // ended, [12, 14) the best rounds' total (the rounds clear [8, 14)); [16, 18) the least (offset << 8) | byte that
 // iupac_canon rejects; [20, 22) the number of listed documents or alignment operations, [22] align_list's error
-// word; [24] the longest query.
+// word; [24] the longest query; [26, 28) the number of loci.
 enum ApproxWord : uint32_t {
     AW_FLAG = 0, AW_ITEMS = 2, AW_TOTAL = 4, AW_BATCH = 8, AW_ENDED = 10, AW_BEST_TOTAL = 12, AW_IUPAC_BAD = 16,
-    AW_LISTED = 20, AW_ALIGN_ERR = 22, AW_MMAX = 24
+    AW_LISTED = 20, AW_ALIGN_ERR = 22, AW_MMAX = 24, AW_LOCI = 26
 };
 
 // The checks of a call (nq >= 1, k its threshold): q_off on the device with q_off[nq] read back as *q_bytes,
@@ -3303,6 +3305,60 @@ static int align_list(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const ui
     return B200SA_OK;
 }
 
+// B200SA_APPROX_LOCI: the staged final lists (*total hits at offsets hoff, from adocs_stage) cut to one hit per
+// locus (loci.cuh); q_off gives each query's length.  *total becomes the number of loci.  With align the
+// representatives replace the staged lists, for align_list, at the offsets *loff; else they go to the caller's
+// offsets and, when they fit cap, d_pos and d_mis.  c->loci holds the least keys (8 bytes per hit), the scan of the
+// marks (8 per hit), the offsets with align (8 per query) and the marks, then heads (4 per hit).  Phases loci_mark
+// (three scans and the offsets) and loci_emit.
+static int loci_reduce(b200sa_ctx *c, const uint32_t *d_starts, uint32_t ndocs, const uint64_t *d_q_off, uint32_t nq,
+                       const uint64_t *hoff, bool align, uint64_t *d_offsets, uint32_t *d_pos, uint32_t *d_mis,
+                       uint64_t cap, uint64_t *total, const uint64_t **loff) {
+    typedef unsigned long long u64;
+    const uint64_t htotal = *total;
+    *loff = hoff;
+    TRY(mark(c, "loci_mark"));
+    if (htotal == 0) {
+        if (!align) CU_TRY(c, cudaMemsetAsync(d_offsets, 0, ((size_t)nq + 1) * 8, c->stream));
+        return B200SA_OK;
+    }
+    if (htotal >= 0xFFFFFFFFull)
+        return fail(c, B200SA_ERR_TOO_LARGE, "approx positions: with B200SA_APPROX_LOCI, 2^32 - 1 or more hits");
+    const size_t noff = align ? (size_t)nq + 1 : 0;
+    TRY(ensure(c, c->loci, (size_t)htotal * 20 + 8 + noff * 8));
+    u64 *least = ptr<u64>(c->loci), *keep = least + htotal, *aoff = keep + htotal + 1;
+    uint32_t *marks = reinterpret_cast<uint32_t *>(aoff + noff);
+    const uint32_t *hpos = reinterpret_cast<const uint32_t *>(ptr<u64>(c->adocs) + htotal + 1), *hmis = hpos + htotal;
+    uint32_t *words = ptr<uint32_t>(c->small);
+    const u64 *ho = reinterpret_cast<const u64 *>(hoff);
+    CU_TRY(c, cudaMemsetAsync(least, 0xFF, (size_t)htotal * 8, c->stream));
+    TRY((dev_scan<OpMax2x32>(c, LociPrevIn{hmis},
+                             LociPrevOut{hpos, hmis, ho, reinterpret_cast<const u64 *>(d_q_off), nq, d_starts, ndocs,
+                                         marks},
+                             htotal, nullptr)));
+    TRY((dev_scan<OpMax2x32>(c, LociHeadIn{hmis, marks}, LociHeadOut{hpos, hmis, marks, least}, htotal, nullptr)));
+    TRY((dev_scan<OpSum64>(c, LociKeepIn{hpos, hmis, marks, least, htotal}, OutStoreExcl64{keep}, htotal + 1,
+                           reinterpret_cast<u64 *>(words + AW_LOCI))));
+    u64 *off = align ? aoff : reinterpret_cast<u64 *>(d_offsets);
+    LAUNCH(c, k_adocs_offsets, cdiv((uint64_t)nq + 1, BLK), ho, (const u64 *)keep, nq, off);
+    TRY(read_words(c, words + AW_LOCI, 2));
+    *total = pin_u64(c, 0);
+    if (align) {                          // through the spent keys, then into the staging's layout for *total hits
+        *loff = reinterpret_cast<const uint64_t *>(off);
+        TRY(mark(c, "loci_emit"));
+        uint32_t *kpos = reinterpret_cast<uint32_t *>(least), *kmis = kpos + *total;
+        LAUNCH(c, k_loci_emit, cdiv(htotal, BLK), hpos, hmis, htotal, (const u64 *)keep, kpos, kmis);
+        uint32_t *spos, *smis;
+        TRY(adocs_stage(c, *total, &spos, &smis));
+        CU_TRY(c, cudaMemcpyAsync(spos, kpos, (size_t)*total * 8, cudaMemcpyDeviceToDevice, c->stream));
+        return B200SA_OK;
+    }
+    if (*total > cap) return B200SA_OK;
+    TRY(mark(c, "loci_emit"));
+    LAUNCH(c, k_loci_emit, cdiv(htotal, BLK), hpos, hmis, htotal, (const u64 *)keep, d_pos, d_mis);
+    return B200SA_OK;
+}
+
 // The batch a BestPick selects: *nb queries, map[i] the query of entry i; their bytes and offsets at *bq / *boff,
 // the call's own arrays when every query is picked, else gathered into c->qbuf and coff.  Pick: BestPick, or
 // StrandPick over the entries of the doubled batch.  fx (B200SA_APPROX_FIXED, else NULL): the queries' marks,
@@ -3453,9 +3509,11 @@ static int approx_best(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const u
 // B200SA_APPROX_FIXED the marks that follow the queries through every batch; with B200SA_APPROX_BOTH_STRANDS the
 // doubled batch; then approx_plain or approx_best writes each query's final list.
 // With B200SA_APPROX_DOCUMENTS that list is staged and adocs_reduce writes the caller's arrays; with
-// B200SA_APPROX_ALIGN align_list does.  `doubling_rounds` is set only with B200SA_APPROX_BEST.
-// Phases: approx_check; strand_queries with both strands; the middle's; adocs_mark, adocs_emit with
-// B200SA_APPROX_DOCUMENTS or align_count, align_scan, align_emit with B200SA_APPROX_ALIGN.
+// B200SA_APPROX_LOCI loci_reduce cuts it to one hit per locus first; with B200SA_APPROX_ALIGN align_list writes
+// them.  `doubling_rounds` is set only with B200SA_APPROX_BEST.
+// Phases: approx_check; strand_queries with both strands; the middle's; loci_mark, loci_emit with
+// B200SA_APPROX_LOCI; adocs_mark, adocs_emit with B200SA_APPROX_DOCUMENTS or align_count, align_scan, align_emit
+// with B200SA_APPROX_ALIGN.
 template <class EndF>
 static int approx_run(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const uint32_t *d_sa,
                       const uint32_t *d_starts, uint32_t ndocs, const uint8_t *d_queries, const uint64_t *d_q_off,
@@ -3481,10 +3539,13 @@ static int approx_run(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const ui
         TRY(approx_best(c, d_text, n, d_sa, d_starts, ndocs, end, f, e, nq, q_bytes, fin, total));
     else
         TRY(approx_plain(c, d_text, n, d_sa, d_starts, ndocs, end, f, e, nq, fin, total));
+    const uint64_t *hoff = fin.off;
+    if (f.loci)
+        TRY(loci_reduce(c, d_starts, ndocs, d_q_off, nq, fin.off, f.align, d_offsets, d_pos, d_mis, cap, total, &hoff));
     if (f.docs) TRY(adocs_reduce(c, d_starts, ndocs, nq, fin.off, d_offsets, d_pos, d_mis, cap, total));
     if (f.align)
         TRY(align_list(c, d_text, n, d_starts, ndocs, d_queries, d_q_off, d_fixed, nq, f.k, f.edit, f.iupac, mmax,
-                       fin.off, d_offsets, d_pos, d_mis, cap, total, f.bulges));
+                       hoff, d_offsets, d_pos, d_mis, cap, total, f.bulges));
     TRY(mark(c, "end"));
     CU_TRY(c, cudaGetLastError());
     CU_TRY(c, cudaStreamSynchronize(c->stream));
@@ -3492,14 +3553,16 @@ static int approx_run(b200sa_ctx *c, const uint8_t *d_text, uint32_t n, const ui
 }
 
 // The argument checks shared by both entry points, and k decoded into *f.  docs: the documents entry, the only one
-// that takes B200SA_APPROX_DOCUMENTS, B200SA_APPROX_ALIGN, B200SA_APPROX_FIXED and B200SA_APPROX_BULGES (whose
-// budget fields are known bits only beside it).
+// that takes B200SA_APPROX_DOCUMENTS, B200SA_APPROX_ALIGN, B200SA_APPROX_FIXED, B200SA_APPROX_BULGES (whose
+// budget fields are known bits only beside it) and B200SA_APPROX_LOCI (bit 7, a threshold bit on the other entry).
 static int approx_args(b200sa_ctx *c, uint64_t n, const void *text, const void *sa, const void *q_off, uint32_t nq,
                        uint32_t k, const void *offsets, const void *pos, uint64_t cap, const void *total, bool docs,
                        ApproxFlags *f) {
     if (!c) return B200SA_ERR_BAD_ARG;
     if (!total || !offsets || (nq > 0 && !q_off) || (cap > 0 && !pos) || (n > 0 && (!text || !sa))) return null_ptr(c);
     const bool best = (k & B200SA_APPROX_BEST) != 0, bulges = (k & B200SA_APPROX_BULGES) != 0;
+    const bool loci = docs && (k & B200SA_APPROX_LOCI) != 0;
+    const uint32_t tk = docs ? k & ~B200SA_APPROX_LOCI : k;  // k without bit 7 where it is the flag
     const uint32_t accepted = 0xFFFFu | B200SA_APPROX_EDIT | B200SA_APPROX_IUPAC | B200SA_APPROX_BOTH_STRANDS |
                               (best ? B200SA_APPROX_BEST : 0u) |
                               (docs ? B200SA_APPROX_DOCUMENTS | B200SA_APPROX_ALIGN | B200SA_APPROX_FIXED : 0u) |
@@ -3507,14 +3570,14 @@ static int approx_args(b200sa_ctx *c, uint64_t n, const void *text, const void *
                                                     B200SA_APPROX_RNA_BULGES(3)
                                               : 0u);
     // with B200SA_APPROX_BEST the threshold and the slack are a byte each, and either above the limit is a bad k
-    if ((k & ~accepted) || (best && ((k & 0xFFu) > B200SA_APPROX_MAX_K || ((k >> 8) & 0xFFu) > B200SA_APPROX_MAX_K))) {
+    if ((k & ~accepted) || (best && ((tk & 0xFFu) > B200SA_APPROX_MAX_K || ((k >> 8) & 0xFFu) > B200SA_APPROX_MAX_K))) {
         const std::string m =
             std::string("approx positions: ") + (best ? "with B200SA_APPROX_BEST, " : "") +
             "k must be a threshold up to B200SA_APPROX_MAX_K" +
             (best ? " | B200SA_APPROX_SLACK(s) with s up to B200SA_APPROX_MAX_K" : "") +
             ", optionally | B200SA_APPROX_EDIT, | B200SA_APPROX_IUPAC" +
-            (docs ? ", | B200SA_APPROX_BOTH_STRANDS, | B200SA_APPROX_FIXED with B200SA_APPROX_IUPAC and "
-                    "| B200SA_APPROX_DOCUMENTS, or | B200SA_APPROX_ALIGN"
+            (docs ? ", | B200SA_APPROX_BOTH_STRANDS, | B200SA_APPROX_FIXED with B200SA_APPROX_IUPAC, "
+                    "| B200SA_APPROX_LOCI and | B200SA_APPROX_DOCUMENTS, or | B200SA_APPROX_ALIGN"
                   : " and | B200SA_APPROX_BOTH_STRANDS") +
             (!docs && bulges ? "; B200SA_APPROX_BULGES is taken by b200sa_docs_approx_positions_dev only" : "");
         return fail(c, B200SA_ERR_BAD_ARG, m.c_str());
@@ -3526,18 +3589,18 @@ static int approx_args(b200sa_ctx *c, uint64_t n, const void *text, const void *
     if (bulges && best)
         return fail(c, B200SA_ERR_BAD_ARG,
                     "approx positions: B200SA_APPROX_BULGES and B200SA_APPROX_BEST do not combine");
-    if (!best && (k & 0xFFFFu) > B200SA_APPROX_MAX_K)
+    if (!best && (tk & 0xFFFFu) > B200SA_APPROX_MAX_K)
         return fail(c, B200SA_ERR_BAD_ARG, "approx positions: k above B200SA_APPROX_MAX_K");
-    const Bulges bg{bulges, k & 0xFFFFu, (k >> 17) & 3u, (k >> 22) & 3u};
+    const Bulges bg{bulges, tk & 0xFFFFu, (k >> 17) & 3u, (k >> 22) & 3u};
     if (bulges && bg.t + bg.d + bg.r > B200SA_APPROX_MAX_K)
         return fail(c, B200SA_ERR_BAD_ARG, "approx positions: with B200SA_APPROX_BULGES, the threshold plus the DNA "
                                            "and RNA bulges above B200SA_APPROX_MAX_K");
     if (n > B200SA_MAX_N) return too_long(c);
     const bool listing = (k & B200SA_APPROX_DOCUMENTS) != 0, align = (k & B200SA_APPROX_ALIGN) != 0;
-    *f = ApproxFlags{best ? k & 0xFFu : bulges ? bg.t + bg.d + bg.r : k & 0xFFFFu, best ? (k >> 8) & 0xFFu : 0u,
+    *f = ApproxFlags{best ? tk & 0xFFu : bulges ? bg.t + bg.d + bg.r : tk & 0xFFFFu, best ? (k >> 8) & 0xFFu : 0u,
                      (k & B200SA_APPROX_EDIT) != 0, best, (k & B200SA_APPROX_IUPAC) != 0,
-                     (k & B200SA_APPROX_FIXED) != 0, (k & B200SA_APPROX_BOTH_STRANDS) != 0, listing, align,
-                     listing || align, bg};
+                     (k & B200SA_APPROX_FIXED) != 0, (k & B200SA_APPROX_BOTH_STRANDS) != 0, listing, align, loci,
+                     listing || align || loci, bg};
     return B200SA_OK;
 }
 
@@ -3564,6 +3627,10 @@ int b200sa_docs_approx_positions_dev(b200sa_ctx *c, const uint8_t *d_text, uint6
     if (f.align && f.docs)
         return fail(c, B200SA_ERR_BAD_ARG,
                     "approx positions: B200SA_APPROX_ALIGN and B200SA_APPROX_DOCUMENTS do not combine");
+    if (f.loci && f.docs)
+        return fail(c, B200SA_ERR_BAD_ARG,
+                    "approx positions: B200SA_APPROX_LOCI and B200SA_APPROX_DOCUMENTS do not combine (the document "
+                    "listing already keeps one entry per document)");
     if (f.align && cap > 0 && !d_mismatches)
         return fail(c, B200SA_ERR_BAD_ARG,
                     "approx positions: with B200SA_APPROX_ALIGN, d_mismatches is required when cap > 0");

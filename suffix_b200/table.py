@@ -281,7 +281,7 @@ class SuffixTable:
 
     # ---- approximate positions (DESIGN 6b f-14 .. f-18, f-20, f-21)
     def approximate_positions(self, query, k, *, metric="hamming", best=None, iupac=False, strands="forward",
-                              fixed=False, bulges=None):
+                              fixed=False, bulges=None, loci=False):
         """(positions u32[], mismatches u32[]): every p with p + m <= n where text[p:p + m] differs from
         the query (m bytes) in at most k bytes, 0 <= k <= 31, by ascending p, with that number of
         mismatches beside it (b200sa_approx_positions_dev).  b"" matches nothing; for k = 0 the positions
@@ -314,6 +314,13 @@ class SuffixTable:
         substitutions, at most dna DNA bulges (text bases with no query base) and at most rna RNA bulges (query
         bases with no text base), with the least total of the three over those alignments beside it.
         bulges=(0, 0) gives exactly the Hamming call; combines with iupac=, fixed= and strands=.
+        loci=True (a non-bool value raises ValueError) lists one hit per locus in place of the run of
+        neighbouring starts that one site yields (B200SA_APPROX_LOCI (the text going through b200sa_docs_approx_positions_dev as one document on a
+        SuffixTable)): a locus is a
+        chain of hits on one strand whose consecutive starts are less than the query's length
+        apart, and its hit with the least distance, the leftmost on a tie, represents it.  So a planted site gives
+        one hit under metric="edit" and bulges= as under Hamming, and approximate_counts counts sites.  The result
+        is a subset of the call without it, at equal distances; combines with every other keyword.
         strands="both" also lists the occurrences of the query's reverse complement (A <-> T, C <-> G in either
         case; with iupac=True each code's class complemented, R <-> Y, K <-> M, B <-> V, D <-> H, U -> A) as
         minus-strand hits at the leftmost text position of their window or alignment
@@ -321,25 +328,26 @@ class SuffixTable:
         the plus hit first, minus a bool array; with best= best(q) is taken over both strands.  strands="forward"
         (the default) searches the query alone; any other value raises ValueError."""
         from . import _approx
-        return _approx.positions(self, query, k, metric, best, iupac, strands, fixed, bulges)
+        return _approx.positions(self, query, k, metric, best, iupac, strands, fixed, bulges, loci)
 
     def approximate_positions_batch(self, queries, k, *, metric="hamming", best=None, iupac=False, strands="forward",
-                                    fixed=False, bulges=None):
+                                    fixed=False, bulges=None, loci=False):
         """(offsets u64[nq + 1], positions u32[], mismatches u32[]): query q's occurrences with at most k
         mismatches (or within k edits, metric="edit") are positions[offsets[q]:offsets[q + 1]], as
         approximate_positions returns them; best=0 gives each query's best hits, with best(q) in the
-        distance column (best=, iupac=, fixed= and bulges= as in approximate_positions).  strands="both" returns (offsets,
+        distance column (best=, iupac=, fixed=, bulges= and loci= as in approximate_positions).  strands="both" returns (offsets,
         positions, distances, minus) with both strands in each query's list, as approximate_positions does."""
         from . import _approx
-        return _approx.positions_batch(self, queries, k, metric, best, iupac, strands, fixed, bulges)
+        return _approx.positions_batch(self, queries, k, metric, best, iupac, strands, fixed, bulges, loci)
 
     def approximate_counts(self, queries, k, *, metric="hamming", best=None, iupac=False, strands="forward",
-                           fixed=False, bulges=None):
+                           fixed=False, bulges=None, loci=False):
         """u64[nq]: the number of occurrences with at most k mismatches (or within k edits, metric="edit") of
         every query, without fetching them; best=0 counts each query's best hits, those at distance best(q)
-        (best=, iupac=, fixed= and bulges= as in approximate_positions); strands="both" counts the hits of both strands."""
+        (best=, iupac=, fixed= and bulges= as in approximate_positions); strands="both" counts the hits of both strands;
+        loci=True counts loci, the sites that approximate_positions(loci=True) lists."""
         from . import _approx
-        return _approx.counts(self, queries, k, metric, best, iupac, strands, fixed, bulges)
+        return _approx.counts(self, queries, k, metric, best, iupac, strands, fixed, bulges, loci)
 
     def approximate_alignments(self, query, k, *, metric="hamming", best=None, iupac=False, strands="forward"):
         """(positions u32[], distances u32[], ends u32[], cigar_offsets u64[h + 1], cigar u32[]): the hits of
