@@ -15,16 +15,11 @@
 extern "C" {
 #endif
 
-/* K1/K2: classification of `text` (reference SuffixTypes::compute,
- * src/table.rs:592-615; Bins::find_sizes, :686-704).  stype_words/lms_words:
- * ceil(n/32) u32 bitmaps; hist768: L / S-non-LMS / LMS counts per byte;
- * lmspos: up to cap_lms LMS positions in text order; *m_out their number. */
-int b200sa_test_classify(b200sa_ctx *ctx, const uint8_t *text, uint64_t n,
-                         uint32_t *stype_words, uint32_t *lms_words, uint32_t *hist768,
-                         uint32_t *lmspos, uint64_t cap_lms, uint64_t *m_out);
-
-/* The same through the fused single-pass classifier (classify2.cuh): lmspos_desc holds the
- * LMS positions in DESCENDING text order (the order the LMS sort is fed in). */
+/* K1/K2: classification of `text` by the fused single-pass byte classifier (classify2.cuh;
+ * reference SuffixTypes::compute, src/table.rs:592-615; Bins::find_sizes, :686-704).
+ * stype_words/lms_words: ceil(n/32) u32 bitmaps; hist768: L / S-non-LMS / LMS counts per byte;
+ * lmspos_desc: up to cap_lms LMS positions in DESCENDING text order (the order the LMS sort is
+ * fed in); *m_out their number. */
 int b200sa_test_classify_fused(b200sa_ctx *ctx, const uint8_t *text, uint64_t n,
                                uint32_t *stype_words, uint32_t *lms_words, uint32_t *hist768,
                                uint32_t *lmspos_desc, uint64_t cap_lms, uint64_t *m_out);

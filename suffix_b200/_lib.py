@@ -111,7 +111,6 @@ def lib():
         "b200sa_strerror": ([ci], ctypes.c_char_p),
         "b200sa_last_error": ([vp], ctypes.c_char_p),
         "b200sa_version": ([], ctypes.c_char_p),
-        "b200sa_test_classify": ([vp, vp, u64, vp, vp, vp, vp, u64, ctypes.POINTER(u64)], ci),
         "b200sa_test_classify_fused": ([vp, vp, u64, vp, vp, vp, vp, u64, ctypes.POINTER(u64)], ci),
         "b200sa_test_scan": ([vp, vp, u64, ci, vp, ctypes.POINTER(u32)], ci),
         "b200sa_test_sort_pairs32": ([vp, vp, vp, u64, ci], ci),

@@ -538,7 +538,7 @@ static int pack_text(b200sa_ctx *c, const uint8_t *text, uint64_t n, uint32_t si
     if (sigma <= 4) c->bits = 2; else if (sigma <= 16) c->bits = 4; else return B200SA_OK;
     uint32_t cpw = 32 / c->bits;
     uint64_t words = (n + cpw - 1) / cpw;
-    TRY(ensure(c, c->packed, words * 4 + 32));  // + padding for text_bits() / text_bits_wide()
+    TRY(ensure(c, c->packed, words * 4 + 32));  // + padding for text_bits()
     if (c->bits == 2 && !packed2)
         LAUNCH(c, (k_pack<2>), cdiv(words, BLK), text, n, tab + T_CODE, ptr<uint32_t>(c->packed), (const uint32_t *)nullptr,
                (const uint32_t *)nullptr, (const uint32_t *)nullptr, (uint32_t *)nullptr);
@@ -605,12 +605,10 @@ static int lms_direct_sort_t(b200sa_ctx *c, uint32_t n, uint32_t m, uint32_t **l
     bool bucketed = false;
     if (BITS == 2 && !getenv("B200SA_LMS_SORT4")) {
         TRY(mark(c, "lms_sort"));
-        if (c->lms_keys_ready)      // k_classify_packed wrote the keys to c->reduced and their digit counts
-            TRY((os_sort<FROM_KEYS>(c, kf, vf, ptr<uint32_t>(c->k32b), ptr<uint32_t>(c->v0), ptr<uint32_t>(c->reduced),
-                                    ptr<uint32_t>(c->v1), (uint64_t)m, 16, 16u, &Ks, &Ps)));
-        else
-            TRY(sort_pairs_from(c, kf, vf, ptr<uint32_t>(c->k32b), ptr<uint32_t>(c->v0), ptr<uint32_t>(c->reduced),
-                                ptr<uint32_t>(c->v1), m, 16, &Ks, &Ps, 16u));
+        // k_classify_packed wrote the keys to c->reduced and their digit counts (2-bit text is always classified
+        // from its packed words here: c->lms_keys_ready)
+        TRY((os_sort<FROM_KEYS>(c, kf, vf, ptr<uint32_t>(c->k32b), ptr<uint32_t>(c->v0), ptr<uint32_t>(c->reduced),
+                                ptr<uint32_t>(c->v1), (uint64_t)m, 16, 16u, &Ks, &Ps)));
         TRY(mark(c, "lms_groups"));
         uint32_t *Pout = ptr<uint32_t>(c->k32b);                    // keys of the first pass: dead after the second
         CU_TRY(c, cudaMemsetAsync(sm + 16, 0, 12, c->stream));      // [16] tied count, [18] bucket overflow
@@ -646,16 +644,11 @@ static int lms_direct_sort_t(b200sa_ctx *c, uint32_t n, uint32_t m, uint32_t **l
         CU_TRY(c, cudaMemsetAsync(forced, 0, fw * 4, c->stream));
         CU_TRY(c, cudaMemsetAsync(sm + 16, 0, 8, c->stream));
         LAUNCH(c, (k_lms_mark_trunc<BITS>), 1u, W, ptr<uint32_t>(c->lmsdesc), m, Ks, Ps, kc, forced);
-        if (getenv("B200SA_GROUPS_GENERIC")) {       // the generic scan with functors (cross-check)
-            InLmsActive1 in1{Ks, forced, m};
-            TRY((dev_scan<OpSum>(c, in1, OutLmsCompact1{in1, Ps, slotA, posA, grpA}, m, sm + 16)));
-        } else {
-            uint32_t nt = cdiv(m, LG_TILE);
-            ScanState S;
-            TRY(scan_state_for(c, nt, &S));
-            LAUNCH(c, k_lms_groups1, nt, Ks, Ps, forced, m, nt, S, slotA, posA, grpA, sm + 16);
-            CU_TRY(c, cudaGetLastError());
-        }
+        uint32_t nt = cdiv(m, LG_TILE);
+        ScanState S;
+        TRY(scan_state_for(c, nt, &S));
+        LAUNCH(c, k_lms_groups1, nt, Ks, Ps, forced, m, nt, S, slotA, posA, grpA, sm + 16);
+        CU_TRY(c, cudaGetLastError());
         TRY(read_words(c, sm + 16, 1));
     }
     uint32_t na = c->h_pin[0];
@@ -665,10 +658,9 @@ static int lms_direct_sort_t(b200sa_ctx *c, uint32_t n, uint32_t m, uint32_t **l
     if (const char *e = getenv("B200SA_DIRECT_ROUNDS")) { int v = atoi(e); if (v >= 1) max_rounds = (uint32_t)v; }
     if (getenv("B200SA_TRACE")) fprintf(stderr, "[b200sa] direct LMS sort: kc=%u, round 1 leaves %u of %u tied%s\n", kc, na, m,
                                         bucketed ? " (bucket sort)" : "");
-    const bool force = getenv("B200SA_DIRECT_FORCE") != nullptr;            // experiments: never bail out early
     // the window tells (almost) nothing apart: every suffix has a twin for kc characters -- repeats, not
     // a skewed alphabet (English leaves 99.5 % tied after 5 bytes and still converges in ~10 rounds)
-    if (!force && (uint64_t)na * 1000 > (uint64_t)m * 999 && m > 64) return direct_hand_over("round1-tied");
+    if ((uint64_t)na * 1000 > (uint64_t)m * 999 && m > 64) return direct_hand_over("round1-tied");
     if (na > 0 && !bucketed)     // group id of every tied element = slot of its group's head (the bucket sort writes it)
         TRY((dev_scan<OpMax>(c, InArray{grpA}, OutMaxInPlace{grpA}, na, nullptr)));
     uint64_t h = kc;
@@ -719,7 +711,7 @@ static int lms_direct_sort_t(b200sa_ctx *c, uint32_t n, uint32_t m, uint32_t **l
         uint32_t na_next = c->h_pin[0];
         if (getenv("B200SA_TRACE")) fprintf(stderr, "[b200sa] direct LMS sort: round %u (h=%llu): %u -> %u tied, %s\n", rounds, (unsigned long long)h, na, na_next, how);
         // slow convergence on a large residue means long repeats: stop early
-        if (!force && (uint64_t)na_next * 100 > (uint64_t)na * 85 && (uint64_t)na_next * 64 > m) return direct_hand_over("no-convergence");
+        if ((uint64_t)na_next * 100 > (uint64_t)na * 85 && (uint64_t)na_next * 64 > m) return direct_hand_over("no-convergence");
         na = na_next;
         uint32_t *t;
         t = slotA; slotA = slotB; slotB = t;
@@ -822,11 +814,10 @@ static int post_classify(b200sa_ctx *c, const uint8_t *text, uint64_t n, uint32_
 // text of at most 4 distinct bytes is packed at 2 bits and classified from its packed words by
 // k_classify_packed, which also writes the LMS sort's window keys (c->lms_keys_ready); for a larger
 // alphabet those kernels return at once and k_classify_fused classifies the bytes.  The one host read after
-// the classification stays the only one.  B200SA_CLASSIFY_BYTES=1 (or B200SA_NOPACK) keeps the byte
-// classifier on every text (cross-check).
+// the classification stays the only one.  B200SA_NOPACK keeps the byte classifier on every text.
 static int classify_fused_dev(b200sa_ctx *c, const uint8_t *text, uint64_t n, uint32_t *m_out,
                               ShardEdge edge = ShardEdge{-1, -1, ST_L}, bool pack = true, bool packed_first = false) {
-    const bool try2 = packed_first && pack && !getenv("B200SA_CLASSIFY_BYTES") && !getenv("B200SA_NOPACK");
+    const bool try2 = packed_first && pack && !getenv("B200SA_NOPACK");
     uint64_t nw = (n + 31) / 32;
     uint32_t nbc = cdiv(nw, CLS_WORDS);
     TRY(ensure(c, c->stype, nw * 4));
@@ -877,15 +868,8 @@ static int classify_fused_dev(b200sa_ctx *c, const uint8_t *text, uint64_t n, ui
                ptr<uint32_t>(c->stype), ptr<uint32_t>(c->lmsb), ptr<uint32_t>(c->hist_copies), ptr<uint32_t>(c->lmsdesc),
                ptr<uint32_t>(c->reduced), ptr<uint32_t>(c->os_hist), sm);
     }
-    // B200SA_CLASSIFY_TMA=1: the tile arrives by one cp.async.bulk (UBLKCP) + mbarrier instead of 512 vector
-    // loads.  With several resident one-tile CTAs per SM the load latency is already covered, so the bulk
-    // copy buys nothing here and stays opt-in.
-    if (getenv("B200SA_CLASSIFY_TMA") == nullptr)
-        LAUNCH(c, k_classify_fused<false>, nbc, text, n, nbc, S, CS, ptr<uint32_t>(c->stype), ptr<uint32_t>(c->lmsb),
-               ptr<uint32_t>(c->hist_copies), ptr<uint32_t>(c->lmsdesc), sm, edge, d_sigma2);
-    else
-        LAUNCH(c, k_classify_fused<true>, nbc, text, n, nbc, S, CS, ptr<uint32_t>(c->stype), ptr<uint32_t>(c->lmsb),
-               ptr<uint32_t>(c->hist_copies), ptr<uint32_t>(c->lmsdesc), sm, edge, d_sigma2);
+    LAUNCH(c, k_classify_fused, nbc, text, n, nbc, S, CS, ptr<uint32_t>(c->stype), ptr<uint32_t>(c->lmsb),
+           ptr<uint32_t>(c->hist_copies), ptr<uint32_t>(c->lmsdesc), sm, edge, d_sigma2);
     LAUNCH(c, k_hist_fold, 1u, ptr<uint32_t>(c->hist_copies), hist);
     LAUNCH(c, k_bucket_tables, 1, hist, tab + T_BSTART, tab + T_LCNT, tab + T_SCNT, tab + T_LMSOFF, tab + T_CODE,
            tab + T_ALPHA, sm + 3);
@@ -916,44 +900,6 @@ static int lms_ascending(b200sa_ctx *c, uint64_t n, uint32_t m) {
     return B200SA_OK;
 }
 
-
-static int classify_dev(b200sa_ctx *c, const uint8_t *text, uint64_t n, uint32_t *m_out,
-                        ShardEdge edge = ShardEdge{-1, -1, ST_L}) {
-    uint64_t nw = (n + 31) / 32;
-    uint32_t nbc = cdiv(nw, CLS_WORDS);
-    TRY(ensure(c, c->stype, nw * 4));
-    TRY(ensure(c, c->lmsb, nw * 4));
-    TRY(ensure(c, c->lmsrank, nw * 4));
-    TRY(ensure(c, c->blkstate, nbc));
-    TRY(ensure(c, c->carry, nbc));
-    TRY(ensure(c, c->tables, T_END * 4));
-    TRY(ensure(c, c->small, 4096));
-    uint32_t *tab = ptr<uint32_t>(c->tables);
-    uint32_t *hist = tab + T_HIST;
-    uint32_t *sm = ptr<uint32_t>(c->small);
-    CU_TRY(c, cudaMemsetAsync(hist, 0, 768 * 4, c->stream));
-    CU_TRY(c, cudaMemsetAsync(sm, 0, 4096, c->stream));
-    LAUNCH(c, k_cls_block_state, nbc, text, n, ptr<uint8_t>(c->blkstate), edge);
-    LAUNCH(c, k_cls_carry, 1, ptr<uint8_t>(c->blkstate), nbc, ptr<uint8_t>(c->carry), edge.next_char >= 0 ? edge.tail_carry : ST_L);
-    LAUNCH(c, k_cls_types, nbc, text, n, ptr<uint8_t>(c->carry), ptr<uint32_t>(c->stype), ptr<uint32_t>(c->lmsb), hist, edge);
-    LAUNCH(c, k_bucket_tables, 1, hist, tab + T_BSTART, tab + T_LCNT, tab + T_SCNT, tab + T_LMSOFF, tab + T_CODE,
-           tab + T_ALPHA, sm + 3);
-    CU_TRY(c, cudaGetLastError());
-    TRY((dev_scan<OpSum>(c, InPopcWords{ptr<uint32_t>(c->lmsb)}, OutStoreExcl{ptr<uint32_t>(c->lmsrank)}, nw, sm)));
-    if (c->early_sa_out)    // bucket layout for the early SA copy-out (same synchronisation as the read below)
-        CU_TRY(c, cudaMemcpyAsync(c->h_tab, tab + T_BSTART, 513 * sizeof(uint32_t), cudaMemcpyDeviceToHost, c->stream));
-    TRY(read_words(c, sm, 4));
-    uint32_t m = c->h_pin[0], sigma = c->h_pin[3];
-    TRY(post_classify(c, text, n, sigma));
-    TRY(ensure(c, c->lmspos, (size_t)m * 4));
-    if (m > 0) {
-        LAUNCH(c, k_lms_positions, cdiv(nw, BLK), ptr<uint32_t>(c->lmsb), ptr<uint32_t>(c->lmsrank), nw, ptr<uint32_t>(c->lmspos));
-        CU_TRY(c, cudaGetLastError());
-    }
-    c->lms_asc_ready = true;
-    *m_out = m;
-    return B200SA_OK;
-}
 
 // Host API only: the L parts of all buckets are final after the last L pass and the
 // S parts after the last S pass, so the SA can start leaving over PCIe one S-pass
@@ -991,14 +937,7 @@ static int build_dev(b200sa_ctx *c, const uint8_t *d_text, uint64_t n, uint32_t 
     uint32_t n32 = (uint32_t)n;
     TRY(mark(c, "classify"));
     uint32_t m = 0;
-    if (getenv("B200SA_CLASSIFY_V1")) {          // three-kernel classifier (classify.cuh) + reversed position list
-        TRY(classify_dev(c, text, n, &m));
-        c->lms_keys_ready = false;
-        TRY(ensure(c, c->lmsdesc, (size_t)m * 4 + 16));
-        if (m > 0) LAUNCH(c, k_reverse_u32, cdiv(m, BLK), ptr<uint32_t>(c->lmspos), m, ptr<uint32_t>(c->lmsdesc));
-    } else {
-        TRY(classify_fused_dev(c, text, n, &m, ShardEdge{-1, -1, ST_L}, true, true));
-    }
+    TRY(classify_fused_dev(c, text, n, &m, ShardEdge{-1, -1, ST_L}, true, true));
     c->stats.m = m; c->last_m = m;
     c->stats.induce_blocks = c->cur_induce_blocks;
     TRY(ensure(c, c->pred, 2 * n + 64));          // bytes (variant 1) or 16-bit carried words (variant 6)
@@ -1164,14 +1103,9 @@ static int lcp_dev(b200sa_ctx *c, const uint8_t *d_text, uint64_t n, const uint3
         sm = ptr<uint32_t>(c->small);
         CU_TRY(c, cudaMemsetAsync(sm + 8, 0, 4, c->stream));
         const uint32_t cap = 256;
-        int lk = 1;       // runs of 32 ranks per warp = window gathers in flight per lane: on an H100 one run
-                          // per warp is fastest for 2- and 4-bit text (B200SA_LCP_K=2|4 for the wider forms)
-        if (const char *e = getenv("B200SA_LCP_K")) lk = atoi(e);
-        if (c->bits == 2 && lk == 4) LAUNCH(c, (k_lcp_direct<2, 4>), cdiv(n, BLK * 4), c->ptext, n32, d_sa, d_lcp, cap, sm + 8);
-        else if (c->bits == 2 && lk == 2) LAUNCH(c, (k_lcp_direct<2, 2>), cdiv(n, BLK * 2), c->ptext, n32, d_sa, d_lcp, cap, sm + 8);
-        else if (c->bits == 2) LAUNCH(c, (k_lcp_direct<2, 1>), cdiv(n, BLK), c->ptext, n32, d_sa, d_lcp, cap, sm + 8);
-        else if (c->bits == 4) LAUNCH(c, (k_lcp_direct<4, 1>), cdiv(n, BLK), c->ptext, n32, d_sa, d_lcp, cap, sm + 8);
-        else LAUNCH(c, (k_lcp_direct<8, 1>), cdiv(n, BLK), c->ptext, n32, d_sa, d_lcp, cap, sm + 8);
+        if (c->bits == 2) LAUNCH(c, k_lcp_direct<2>, cdiv(n, BLK), c->ptext, n32, d_sa, d_lcp, cap, sm + 8);
+        else if (c->bits == 4) LAUNCH(c, k_lcp_direct<4>, cdiv(n, BLK), c->ptext, n32, d_sa, d_lcp, cap, sm + 8);
+        else LAUNCH(c, k_lcp_direct<8>, cdiv(n, BLK), c->ptext, n32, d_sa, d_lcp, cap, sm + 8);
         TRY(read_words(c, sm + 8, 1));
         if (c->h_pin[0] == 0) {
             TRY(mark(c, "end"));
@@ -1414,7 +1348,7 @@ static int host_build_inner(b200sa_ctx *c, const uint8_t *text, uint64_t n, uint
             if (cudaPointerGetAttributes(&pa, sa_out) == cudaSuccess) pinned = (pa.type == cudaMemoryTypeHost);
             else cudaGetLastError();
         }
-        c->early_sa_out = (pinned && n >= 2 && !getenv("B200SA_NO_EARLY_COPY")) ? sa_out : nullptr;
+        c->early_sa_out = (pinned && n >= 2) ? sa_out : nullptr;
         c->early_done = false;
         int brc = build_dev(c, ptr<uint8_t>(c->text), n, ptr<uint32_t>(c->sa));
         c->early_sa_out = nullptr;
@@ -1538,7 +1472,8 @@ static int shard_classify_core(b200sa_ctx *c, const uint8_t *d_shard, uint64_t l
                                uint64_t cap_lms, uint64_t *hist768, uint64_t *m_out) {
     uint32_t m = 0;
     ShardEdge edge{next_char, prev_char, next_char >= 0 ? (uint32_t)tail_carry : ST_L};
-    TRY(classify_dev(c, d_shard, len, &m, edge));
+    TRY(classify_fused_dev(c, d_shard, len, &m, edge, /*pack=*/false));
+    TRY(lms_ascending(c, len, m));                // text-order LMS positions from the descending list
     uint64_t nw = (len + 31) / 32;
     if (d_stype_words) CU_TRY(c, cudaMemcpyAsync(d_stype_words, c->stype.p, nw * 4, cudaMemcpyDeviceToDevice, c->stream));
     if (d_lms_words) CU_TRY(c, cudaMemcpyAsync(d_lms_words, c->lmsb.p, nw * 4, cudaMemcpyDeviceToDevice, c->stream));
@@ -4037,45 +3972,34 @@ int b200sa_lcp_sharded(b200sa_ctx *c, uint8_t *d_text, uint64_t n, uint32_t *d_s
 }
 
 // ------------------------------------------------------------ test hooks
-// The classification of a host text by the two-pass (fused = false) or the fused kernels, copied back.
-static int test_classify_core(b200sa_ctx *c, bool fused, const uint8_t *text, uint64_t n, uint32_t *stype_words,
-                              uint32_t *lms_words, uint32_t *hist768, uint32_t *lmspos, uint64_t cap_lms,
+// The classification of a host text by the fused byte classifier, copied back (LMS positions descending).
+static int test_classify_core(b200sa_ctx *c, const uint8_t *text, uint64_t n, uint32_t *stype_words,
+                              uint32_t *lms_words, uint32_t *hist768, uint32_t *lmspos_desc, uint64_t cap_lms,
                               uint64_t *m_out) {
     TRY(ensure(c, c->text, n));
     CU_TRY(c, cudaMemcpyAsync(c->text.p, text, n, cudaMemcpyHostToDevice, c->stream));
     uint32_t m = 0;
-    if (fused) TRY(classify_fused_dev(c, ptr<uint8_t>(c->text), n, &m));
-    else TRY(classify_dev(c, ptr<uint8_t>(c->text), n, &m));
+    TRY(classify_fused_dev(c, ptr<uint8_t>(c->text), n, &m));
     uint64_t nw = (n + 31) / 32;
     if (stype_words) CU_TRY(c, cudaMemcpyAsync(stype_words, c->stype.p, nw * 4, cudaMemcpyDeviceToHost, c->stream));
     if (lms_words) CU_TRY(c, cudaMemcpyAsync(lms_words, c->lmsb.p, nw * 4, cudaMemcpyDeviceToHost, c->stream));
     if (hist768) CU_TRY(c, cudaMemcpyAsync(hist768, ptr<uint32_t>(c->tables) + T_HIST, 768 * 4, cudaMemcpyDeviceToHost, c->stream));
-    if (lmspos && m > 0) {
+    if (lmspos_desc && m > 0) {
         uint64_t k = m < cap_lms ? m : cap_lms;
-        CU_TRY(c, cudaMemcpyAsync(lmspos, (fused ? c->lmsdesc : c->lmspos).p, k * 4, cudaMemcpyDeviceToHost, c->stream));
+        CU_TRY(c, cudaMemcpyAsync(lmspos_desc, c->lmsdesc.p, k * 4, cudaMemcpyDeviceToHost, c->stream));
     }
     CU_TRY(c, cudaStreamSynchronize(c->stream));
     if (m_out) *m_out = m;
     return B200SA_OK;
 }
 
-static int test_classify(b200sa_ctx *c, bool fused, const uint8_t *text, uint64_t n, uint32_t *stype_words,
-                         uint32_t *lms_words, uint32_t *hist768, uint32_t *lmspos, uint64_t cap_lms, uint64_t *m_out) {
+int b200sa_test_classify_fused(b200sa_ctx *c, const uint8_t *text, uint64_t n, uint32_t *stype_words, uint32_t *lms_words,
+                               uint32_t *hist768, uint32_t *lmspos_desc, uint64_t cap_lms, uint64_t *m_out) {
     if (!c) return B200SA_ERR_BAD_ARG;
     if (!text) return null_ptr(c);
     if (n < 1 || n > B200SA_MAX_N) return fail(c, B200SA_ERR_BAD_ARG, "test classify: n must be in [1, 2^32-4096]");
     TRY(enter(c, nullptr));
-    return leave(c, test_classify_core(c, fused, text, n, stype_words, lms_words, hist768, lmspos, cap_lms, m_out));
-}
-
-int b200sa_test_classify(b200sa_ctx *c, const uint8_t *text, uint64_t n, uint32_t *stype_words, uint32_t *lms_words,
-                         uint32_t *hist768, uint32_t *lmspos, uint64_t cap_lms, uint64_t *m_out) {
-    return test_classify(c, false, text, n, stype_words, lms_words, hist768, lmspos, cap_lms, m_out);
-}
-
-int b200sa_test_classify_fused(b200sa_ctx *c, const uint8_t *text, uint64_t n, uint32_t *stype_words, uint32_t *lms_words,
-                               uint32_t *hist768, uint32_t *lmspos_desc, uint64_t cap_lms, uint64_t *m_out) {
-    return test_classify(c, true, text, n, stype_words, lms_words, hist768, lmspos_desc, cap_lms, m_out);
+    return leave(c, test_classify_core(c, text, n, stype_words, lms_words, hist768, lmspos_desc, cap_lms, m_out));
 }
 
 // The classification of a host text of at most 4 distinct bytes from its 2-bit packed words

@@ -1,16 +1,18 @@
-// classify.cuh -- K1: S/L type classification, LMS flags, (char,type)
-// histogram; K2: bucket tables.  Replaces SuffixTypes::compute
-// (reference src/table.rs:592-615) and Bins::find_sizes / find_*_pointers
-// (src/table.rs:686-720) for the byte-level text.
+// classify.cuh -- the building blocks of the S/L type classification (K1, done
+// by k_classify_fused in classify2.cuh and k_classify_packed in
+// classify_packed.cuh), K2: bucket tables, and the text packing and access
+// helpers.  Together they replace SuffixTypes::compute (reference
+// src/table.rs:592-615) and Bins::find_sizes / find_*_pointers
+// (src/table.rs:686-720).
 //
 // Layout: position i lives in bit (i & 31) of word (i >> 5).
 //   stype[w]  bit set  <=> position is S-class (Ascending or Valley)
 //   lmsb[w]   bit set  <=> position is a Valley (LMS)
 // Algorithm: rel(i) = cmp(T[i],T[i+1]) (rel(n-1) := L, src/table.rs:602);
 // type(i) = first non-EQ rel(j), j >= i.  One block owns 256 words (8192
-// bytes); pass A reduces each block to {L,S,P(ropagate)}, pass B resolves the
-// carries right-to-left across blocks, pass C materialises the bitmaps and the
-// histogram with the carry known.
+// bytes).  The type of a shard's first position (multi-GPU summaries) takes
+// two passes: pass A reduces each block to {L,S,P(ropagate)}, pass B resolves
+// the carries right-to-left across blocks.
 #pragma once
 #include "common.cuh"
 
@@ -133,66 +135,6 @@ __global__ void __launch_bounds__(BLK) k_cls_carry(const uint8_t *blk_state, uin
         __syncthreads();
         carry = s_warp[0];
         __syncthreads();
-    }
-}
-
-// Pass C: bitmaps + histogram.  hist768: [0,256) L counts, [256,512) S
-// non-LMS counts, [512,768) LMS counts, per byte value.
-__global__ void __launch_bounds__(BLK) k_cls_types(const uint8_t *__restrict__ text, uint64_t n,
-                                                   const uint8_t *carry_in, uint32_t *stype, uint32_t *lmsb,
-                                                   uint32_t *hist768, ShardEdge edge) {
-    __shared__ uint32_t s_warp[NWARP];
-    __shared__ uint32_t s_sw[BLK];
-    __shared__ uint32_t s_hist[NWARP][768];        // per-warp private: plain RMW instead of ATOMS
-    for (int k = threadIdx.x; k < NWARP * 768; k += BLK) (&s_hist[0][0])[k] = 0;
-    uint64_t w = (uint64_t)blockIdx.x * CLS_WORDS + threadIdx.x;
-    uint64_t nw = (n + 31) / 32;
-    uint32_t c[8], nextc, lt, gt;
-    bool has_next;
-    uint32_t cnt = load_word(text, n, w, c, nextc, has_next, edge);
-    word_rel(c, cnt, nextc, has_next, lt, gt);
-    uint32_t ne = lt | gt;
-    uint32_t mine = ne ? ((lt >> (__ffs(ne) - 1)) & 1u) : ST_P;
-    uint32_t right = first_nonp_right(mine, s_warp);     // contains __syncthreads (covers s_hist init)
-    uint32_t cin = (right != ST_P) ? right : (uint32_t)carry_in[blockIdx.x];
-    // resolve S bits right-to-left inside the word
-    uint32_t sw = 0, cur = cin;
-#pragma unroll
-    for (int j = 31; j >= 0; j--) {
-        if ((ne >> j) & 1u) cur = (lt >> j) & 1u;
-        sw |= cur << j;
-    }
-    uint32_t vmask = (cnt >= 32) ? 0xffffffffu : ((1u << cnt) - 1u);
-    sw &= vmask;
-    s_sw[threadIdx.x] = sw;
-    __syncthreads();
-    // type bit of the position just before this word
-    uint32_t pb;
-    if (threadIdx.x > 0) pb = s_sw[threadIdx.x - 1] >> 31;
-    else if (w == 0 && edge.prev_char < 0) pb = 1u;  // position 0 is never a Valley (src/table.rs:465)
-    else if (w == 0) {                               // shard start: type of position lo-1 from the halo char
-        uint32_t c1 = (uint32_t)edge.prev_char, c2 = byte_of(c, 0);
-        pb = (c1 < c2) ? 1u : (c1 > c2) ? 0u : (sw & 1u);
-    }
-    else if (cnt == 0) pb = 0u;
-    else {
-        uint32_t c1 = __ldg(text + w * 32 - 1), c2 = byte_of(c, 0);
-        pb = (c1 < c2) ? 1u : (c1 > c2) ? 0u : (sw & 1u);
-    }
-    uint32_t lw = sw & ~((sw << 1) | pb);
-    if (w < nw) { stype[w] = sw; lmsb[w] = lw; }
-#pragma unroll
-    for (int j = 0; j < 32; j++) {
-        bool valid = (uint32_t)j < cnt;
-        uint32_t cls = ((sw >> j) & 1u) + ((lw >> j) & 1u);
-        hist_add_private<10>(s_hist[warp_id()], byte_of(c, j) + 256u * cls, valid);
-    }
-    __syncthreads();
-    for (int k = threadIdx.x; k < 768; k += BLK) {
-        uint32_t v = 0;
-#pragma unroll
-        for (int ww = 0; ww < NWARP; ww++) v += s_hist[ww][k];
-        if (v) atomicAdd(&hist768[k], v);
     }
 }
 
@@ -339,20 +281,6 @@ __device__ __forceinline__ uint32_t text_bits(const void *__restrict__ base, uin
     uint32_t lo = __ldg(pk + w), hi = __ldg(pk + w + 1);
     return __funnelshift_r(lo, hi, off);
 }
-// Same window from ONE 16-byte load in three cases out of four (the aligned 4-word group that
-// holds word w also holds w+1 unless w is its last word): the direct LCP and the naming are
-// bound by the number of divergent load instructions, not by bytes.  The packed buffer is
-// 16-byte aligned and padded by 32 bytes.
-template <int BITS>
-__device__ __forceinline__ uint32_t text_bits_wide(const void *__restrict__ base, uint32_t pos) {
-    constexpr int CPW = 32 / BITS;
-    const uint32_t *pk = reinterpret_cast<const uint32_t *>(base);
-    uint32_t w = pos / CPW, off = (pos % CPW) * BITS, k = w & 3u;
-    uint4 v = __ldg(reinterpret_cast<const uint4 *>(pk) + (w >> 2));
-    uint32_t lo = k == 0 ? v.x : k == 1 ? v.y : k == 2 ? v.z : v.w;
-    uint32_t hi = k == 0 ? v.y : k == 1 ? v.z : k == 2 ? v.w : __ldg(pk + w + 1);
-    return __funnelshift_r(lo, hi, off);
-}
 // Number of equal leading chars of text[a..) and text[b..), at most `limit`.
 template <int BITS>
 __device__ __forceinline__ uint32_t text_match(const void *__restrict__ base, uint32_t a, uint32_t b, uint32_t limit) {
@@ -456,21 +384,6 @@ __device__ __forceinline__ uint32_t next_lms_dist(const uint32_t *__restrict__ l
         dist += 32;
     }
     return 0;
-}
-
-// LMS positions in text order: lmspos[lmsrank[w] + k] = position of the k-th
-// set bit of lmsb[w].  (reference P15, src/table.rs:512-520)
-__global__ void __launch_bounds__(BLK) k_lms_positions(const uint32_t *lmsb, const uint32_t *lmsrank, uint64_t nw,
-                                                       uint32_t *lmspos) {
-    uint64_t w = (uint64_t)blockIdx.x * BLK + threadIdx.x;
-    if (w >= nw) return;
-    uint32_t bits = lmsb[w];
-    uint32_t r = lmsrank[w];
-    while (bits) {
-        uint32_t j = __ffs(bits) - 1;
-        bits &= bits - 1;
-        lmspos[r++] = (uint32_t)(w * 32 + j);
-    }
 }
 
 // rank of an LMS position among LMS positions in text order

@@ -2,7 +2,8 @@
 // bitmap, the (byte, L / S / LMS) histogram and the LMS positions (in DESCENDING text order,
 // the order the LMS sort is fed in).  Replaces SuffixTypes::compute (reference
 // src/table.rs:592-615), Bins::find_sizes (:686-704) and the LMS position fill (P15,
-// :512-520); same results as the three-kernel form in classify.cuh.
+// :512-520).  It classifies every text whose bytes are not classified from 2-bit packed
+// words (classify_packed.cuh), and every shard of a multi-GPU build.
 //
 // type(i) = first non-equal cmp(T[j], T[j+1]), j >= i, so information flows right to left:
 // tiles (8192 bytes) are claimed from the END of the text through an atomic ticket.  A tile
@@ -76,32 +77,11 @@ __global__ void __launch_bounds__(BLK) k_hist_fold(const uint32_t *__restrict__ 
     }
 }
 
-// ---- TMA 1-D bulk load of a whole text tile into shared memory (cp.async.bulk + mbarrier): one
-// elected thread arms the barrier with the byte count and issues the copy; the 256 threads then
-// read their 32 bytes from shared memory instead of issuing 512 16-byte global loads per tile.
-__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t *bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%1], %0;" :: "r"(count), "r"(smem_u32(bar)) : "memory");
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t *bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%1], %0;" :: "r"(bytes), "r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void bulk_g2s(void *dst, const void *src, uint32_t bytes, uint64_t *bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 :: "r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t phase) {
-    asm volatile("{\n\t.reg .pred P1;\n\tLAB_WAIT:\n\tmbarrier.try_wait.parity.shared::cta.b64 P1, [%0], %1;\n\t@P1 bra DONE;\n\tbra LAB_WAIT;\n\tDONE:\n\t}"
-                 :: "r"(smem_u32(bar)), "r"(phase) : "memory");
-}
-
 struct Cls2State {
     uint32_t *state;     // [tiles] epoch-tagged: tag + 1 + {ST_L, ST_S, ST_P}
     uint32_t tag;        // distinct per call
 };
 
-template <bool TMA>
 __global__ void __launch_bounds__(BLK) k_classify_fused(const uint8_t *__restrict__ text, uint64_t n, uint32_t ntiles,
                                                         ScanState S, Cls2State CS, uint32_t *stype, uint32_t *lmsb,
                                                         uint32_t *hist768, uint32_t *lmspos_desc, uint32_t *d_m,
@@ -112,23 +92,14 @@ __global__ void __launch_bounds__(BLK) k_classify_fused(const uint8_t *__restric
     __shared__ uint32_t s_warp[NWARP];
     __shared__ uint32_t s_sw[BLK];
     __shared__ uint32_t s_hist[NWARP][768];
-    __shared__ __align__(128) uint32_t s_lms[CLS_BYTES / 2];      // first the TMA landing zone of the text tile, then the LMS list
+    __shared__ __align__(128) uint32_t s_lms[CLS_BYTES / 2];      // the tile's LMS positions, descending
     __shared__ uint32_t s_w[NWARP + 1];
     __shared__ uint32_t s_tile, s_carry, s_prefix;
-    __shared__ __align__(8) uint64_t s_bar;
     const uint32_t tid = threadIdx.x, wp = warp_id(), l = lane_id();
     if (tid == 0) {
         uint32_t t = atomicAdd(S.ticket, 1u);
         if (t + 1 == ntiles) *S.ticket = 0u;
         s_tile = t;
-        if (TMA) {
-            mbar_init(&s_bar, 1u);
-            const uint64_t base = (uint64_t)(ntiles - 1u - t) * CLS_BYTES;
-            if (base + CLS_BYTES <= n) {                       // whole tile inside the text: one bulk copy
-                mbar_expect_tx(&s_bar, CLS_BYTES);
-                bulk_g2s(s_lms, text + base, CLS_BYTES, &s_bar);
-            }
-        }
     }
     for (int k = tid; k < NWARP * 768; k += BLK) (&s_hist[0][0])[k] = 0;
     __syncthreads();
@@ -138,25 +109,11 @@ __global__ void __launch_bounds__(BLK) k_classify_fused(const uint8_t *__restric
     const uint64_t nw = (n + 31) / 32;
     uint32_t c[8], nextc, lt, gt;
     bool has_next;
-    uint32_t cnt;
-    if (TMA && cb * CLS_BYTES + CLS_BYTES <= n) {
-        mbar_wait(&s_bar, 0u);
-        const uint4 *q = reinterpret_cast<const uint4 *>(s_lms) + 2u * tid;
-        uint4 a = q[0], b = q[1];
-        c[0] = a.x; c[1] = a.y; c[2] = a.z; c[3] = a.w;
-        c[4] = b.x; c[5] = b.y; c[6] = b.z; c[7] = b.w;
-        cnt = 32;
-        const uint64_t p1 = w * 32 + 32;
-        has_next = p1 < n;
-        nextc = has_next ? (tid + 1 < BLK ? (s_lms[8u * (tid + 1u)] & 0xffu) : (uint32_t)__ldg(text + p1)) : 0u;
-        if (!has_next && edge.next_char >= 0) { has_next = true; nextc = (uint32_t)edge.next_char; }
-    } else {
-        cnt = load_word(text, n, w, c, nextc, has_next, edge);
-    }
+    uint32_t cnt = load_word(text, n, w, c, nextc, has_next, edge);
     word_rel_swar(c, cnt, nextc, has_next, lt, gt);
     uint32_t ne = lt | gt;
     uint32_t mine = ne ? ((lt >> (__ffs(ne) - 1)) & 1u) : ST_P;
-    uint32_t right = first_nonp_right(mine, s_warp);        // two block barriers: the landing zone is free afterwards
+    uint32_t right = first_nonp_right(mine, s_warp);
     // ---- publish the tile's own state; fetch the carry from the right if any word needs it
     if (tid == 0) {
         uint32_t st = (mine != ST_P) ? mine : right;

@@ -120,34 +120,12 @@ __global__ void __launch_bounds__(BLK) k_lms_mark_trunc(LmsWin W, const uint32_t
         }
     }
 }
-struct InLmsActive1 {
-    const uint32_t *K, *forced; uint32_t m;
-    // branch-free: all five loads of an element are independent (a short-circuit chain would
-    // serialise them behind branches)
-    __device__ __forceinline__ bool head(uint32_t i) const {
-        uint32_t a = K[i], b = K[i > 0 ? i - 1 : 0], f = forced[i >> 5];
-        return (i == 0) | (a != b) | ((f >> (i & 31)) & 1u);
-    }
-    __device__ __forceinline__ uint32_t operator()(uint64_t ii) const {
-        uint32_t i = (uint32_t)ii, j = i + 1 < m ? i + 1 : i;
-        uint32_t a = K[i], b = K[i > 0 ? i - 1 : 0], c = K[j], f = forced[i >> 5], f2 = forced[j >> 5];
-        bool hd = (i == 0) | (a != b) | ((f >> (i & 31)) & 1u);
-        bool tl = (i + 1 == m) | (c != a) | ((f2 >> (j & 31)) & 1u);
-        return (hd & tl) ? 0u : 1u;
-    }
-};
-// compaction of the tied elements; ahead[k] = slot if the element starts its group, else 0
-// (a max-scan over the compacted list turns it into the group id)
-struct OutLmsCompact1 {
-    InLmsActive1 in; const uint32_t *P; uint32_t *aslot, *apos, *ahead;
-    __device__ void operator()(uint64_t i, uint32_t exc, uint32_t v) const {
-        if (v) { aslot[exc] = (uint32_t)i; apos[exc] = P[i]; ahead[exc] = in.head((uint32_t)i) ? (uint32_t)i : 0u; }
-    }
-};
-// The same compaction as ONE specialised single-pass kernel (the generic scan spends ~90
-// instructions per element on functor calls and 16 warp scans per thread; here a thread owns 16
+// Compaction of the elements tied with a neighbour (round-1 groups): aslot / apos get the slot and the
+// position, ahead[k] = slot if the element starts its group, else 0 (a max-scan over the compacted list
+// turns it into the group id).  ONE specialised single-pass kernel (the generic scan with functors spent
+// ~90 instructions per element on functor calls and 16 warp scans per thread): a thread owns 16
 // consecutive slots, reads its 18 keys with four 16-byte loads + 2, derives heads / tied flags in
-// registers and takes part in one block scan; tile offsets by the same look-back as k_scan_lb).
+// registers and takes part in one block scan; tile offsets by the same look-back as k_scan_lb.
 constexpr int LG_IPT = 16;
 constexpr int LG_TILE = BLK * LG_IPT;       // 4096 slots per tile
 __global__ void __launch_bounds__(BLK) k_lms_groups1(const uint32_t *__restrict__ K, const uint32_t *__restrict__ P,

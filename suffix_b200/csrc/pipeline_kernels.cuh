@@ -318,7 +318,7 @@ __global__ void __launch_bounds__(BLK) k_group_local_sort(const uint64_t *__rest
 // compares on the (L2-resident) packed text, capped at `cap` chars.  Pairs that
 // reach the cap are counted; if any exist the caller recomputes everything with
 // the linear Phi/PLCP path below (the direct form is quadratic on repetitive text).
-template <int BITS, int K = 1>
+template <int BITS>
 __global__ void __launch_bounds__(BLK) k_lcp_direct(const void *__restrict__ ptext, uint32_t n,
                                                     const uint32_t *__restrict__ sa, uint32_t *lcp, uint32_t cap,
                                                     uint32_t *capped) {
@@ -340,43 +340,30 @@ __global__ void __launch_bounds__(BLK) k_lcp_direct(const void *__restrict__ pte
         // Packed text: the first window of suffix sa[r] serves the pairs (r-1, r) AND (r, r+1): every lane
         // loads its own window once and takes its left neighbour's from the lane below (lane 0 loads
         // both) -- the kernel is bound by the number of divergent window loads, and this halves them.
-        // A warp owns K runs of 32 consecutive ranks; the K window gathers of a lane are in flight together.
+        // A warp owns one run of 32 consecutive ranks (two or four runs, with their window gathers in
+        // flight together, were slower on an H100).
         constexpr int PB = (BITS == 8 ? 4 : BITS);
         constexpr uint32_t CPW = 32 / PB;
-        const uint32_t wbase = (blockIdx.x * BLK + (threadIdx.x & ~31u)) * (uint32_t)K + lane_id();
-        uint32_t b[K], xb[K];
-        bool live[K];
-#pragma unroll
-        for (int k = 0; k < K; k++) {
-            uint32_t r = wbase + 32u * k;
-            live[k] = r < n;
-            b[k] = live[k] ? sa[r] : 0u;
+        const uint32_t r = blockIdx.x * BLK + (threadIdx.x & ~31u) + lane_id();      // the warp's run + the lane
+        const bool live = r < n;
+        const uint32_t b = live ? sa[r] : 0u;
+        const uint32_t xb = live ? text_bits<PB>(ptext, b) : 0u;
+        uint32_t a = __shfl_up_sync(FULL, b, 1), xa = __shfl_up_sync(FULL, xb, 1);
+        if (lane_id() == 0) {                       // left neighbour of the run's first rank
+            if (live && r > 0) { a = sa[r - 1]; xa = text_bits<PB>(ptext, a); }
         }
-#pragma unroll
-        for (int k = 0; k < K; k++) xb[k] = live[k] ? text_bits<PB>(ptext, b[k]) : 0u;
-#pragma unroll
-        for (int k = 0; k < K; k++) {
-            uint32_t r = wbase + 32u * k;
-            uint32_t a = __shfl_up_sync(FULL, b[k], 1), xa = __shfl_up_sync(FULL, xb[k], 1);
-            uint32_t pa = 0, pxa = 0;
-            if (k > 0) { pa = __shfl_sync(FULL, b[k > 0 ? k - 1 : 0], 31); pxa = __shfl_sync(FULL, xb[k > 0 ? k - 1 : 0], 31); }
-            if (lane_id() == 0) {                       // left neighbour of the run's first rank
-                if (k > 0) { a = pa; xa = pxa; }
-                else if (live[k] && r > 0) { a = sa[r - 1]; xa = text_bits<PB>(ptext, a); }
-            }
-            uint32_t h = 0, room = 0;
-            if (live[k] && r > 0) {
-                room = n - (a > b[k] ? a : b[k]);
-                uint32_t limit = room < cap ? room : cap;
-                uint32_t x = xa ^ xb[k];
-                uint32_t first = x ? (uint32_t)(__ffs(x) - 1) / PB : CPW;       // equal leading chars inside the window
-                if (first < CPW || limit <= CPW) h = first < limit ? first : limit;
-                else h = CPW + text_match<BITS>(ptext, a + CPW, b[k] + CPW, limit - CPW);
-            }
-            if (live[k]) {
-                lcp[r] = h;
-                if (r > 0 && h == cap && room > cap) atomicAdd(capped, 1u);
-            }
+        uint32_t h = 0, room = 0;
+        if (live && r > 0) {
+            room = n - (a > b ? a : b);
+            uint32_t limit = room < cap ? room : cap;
+            uint32_t x = xa ^ xb;
+            uint32_t first = x ? (uint32_t)(__ffs(x) - 1) / PB : CPW;       // equal leading chars inside the window
+            if (first < CPW || limit <= CPW) h = first < limit ? first : limit;
+            else h = CPW + text_match<BITS>(ptext, a + CPW, b + CPW, limit - CPW);
+        }
+        if (live) {
+            lcp[r] = h;
+            if (r > 0 && h == cap && room > cap) atomicAdd(capped, 1u);
         }
     }
 }

@@ -255,16 +255,6 @@ def test_value_sets(ctx, capfd, cache, sigma, kind, path):
     check(ctx, capfd, t, sa, lcp, bits_of(sigma), path, uniform=True)
 
 
-@pytest.mark.parametrize("path", ["build", "lcp"])
-@pytest.mark.parametrize("k", ["2", "4"])
-@pytest.mark.parametrize("sigma", [2, 3, 4])
-def test_lcp_k_two_bit(ctx, capfd, cache, sigma, k, path):
-    """B200SA_LCP_K=2|4: two or four runs of 32 ranks per warp in the direct compare of 2-bit text."""
-    t, sa, lcp = sweep_text(cache, sigma, "uniform")
-    assert lcp_route(sa, lcp, 2, {}) == ["lcp_direct"]
-    check(ctx, capfd, t, sa, lcp, 2, path, {"B200SA_LCP_K": k})
-
-
 # ------------------------------------------------------------------ text ends
 ENDS = [("2bit", 4, False, 16), ("4bit", 6, False, 8), ("4bit", 16, False, 8), ("8bit", 41, False, 4),
         ("8bit", 256, False, 4), ("nopack", 4, True, 4)]          # (packing, sigma, nopack, characters per word)
@@ -290,14 +280,12 @@ def test_text_end(ctx, capfd, cache, packing, sigma, nopack, r, ending, path):
 def test_lcp_thresholds(ctx, capfd, cache, sigma, nopack):
     """A repeats text just above 2^22 characters with more than 2^20 LMS suffixes: the direct compare
     meets capped pairs and hands over to Phi built by the partitioned scatter; B200SA_LCP_LINEAR=1 takes
-    that path at once, with B200SA_PHI_DIRECT=1 the plain Phi scatter; on 2-bit text B200SA_LCP_K=2|4."""
+    that path at once, with B200SA_PHI_DIRECT=1 the plain Phi scatter."""
     t, sa, lcp = cache(("phi", sigma), lambda: alpha_text(N_PHI, sigma, "repeats", seed=sigma))
     assert lcp_route(sa, lcp, 8, {}) == ["lcp_direct", "lcp_phi"]
     bits = bits_of(sigma, nopack)
     base = {"B200SA_NOPACK": "1"} if nopack else {}
     variants = [{}, {"B200SA_LCP_LINEAR": "1"}, {"B200SA_LCP_LINEAR": "1", "B200SA_PHI_DIRECT": "1"}]
-    if bits == 2:
-        variants += [{"B200SA_LCP_K": "2"}, {"B200SA_LCP_K": "4"}]
     for v in variants:
         st = check(ctx, capfd, t, sa, lcp, bits, "build", base | v)
         assert st["m"] >= 1 << 20

@@ -1,9 +1,8 @@
 """Classification of 2-bit text from its packed words (k_classify_packed): type / LMS bitmaps, the
 (byte, class) histogram, the LMS positions in descending order with their 16-character window keys and
 the digit counts of key bits 16-31, against oracle.types and numpy; then SA + LCP of the same texts
-against the oracle with the packed classifier and with the byte classifier (B200SA_CLASSIFY_BYTES=1).
-The packing is coded by the alphabet of the first 1 MiB; texts with bytes that first occur later take the
-second packing (or the byte classifier)."""
+against the oracle.  The packing is coded by the alphabet of the first 1 MiB; texts with bytes that first
+occur later take the second packing (or, with a fifth byte, the byte classifier)."""
 import ctypes
 import itertools
 
@@ -132,11 +131,8 @@ def test_classify_packed_every_short_dna(ctx):
 SA_CASES = CASES + [("late_N_1.2m", np.concatenate([gen.dna(1_200_000), _u8(b"N"), gen.dna(1000, seed=3)]))]
 
 
-@pytest.mark.parametrize("bytes_path", [False, True], ids=["packed", "bytes"])
 @pytest.mark.parametrize("name,t", SA_CASES, ids=[c[0] for c in SA_CASES])
-def test_sa_lcp(ctx, name, t, bytes_path, monkeypatch):
-    if bytes_path:
-        monkeypatch.setenv("B200SA_CLASSIFY_BYTES", "1")
+def test_sa_lcp(ctx, name, t):
     t = np.ascontiguousarray(t)
     sa, lcp = ctx.build_lcp(t)
     want = oracle.sais(t)
@@ -144,11 +140,8 @@ def test_sa_lcp(ctx, name, t, bytes_path, monkeypatch):
     assert np.array_equal(lcp, oracle.lcp_kasai(t, want))
 
 
-@pytest.mark.parametrize("bytes_path", [False, True], ids=["packed", "bytes"])
-def test_sa_lcp_every_short_dna(ctx, bytes_path, monkeypatch):
+def test_sa_lcp_every_short_dna(ctx):
     """Every text over {A,C,G,T} of length 2 to 6."""
-    if bytes_path:
-        monkeypatch.setenv("B200SA_CLASSIFY_BYTES", "1")
     for n in range(2, 7):
         for tup in itertools.product(b"ACGT", repeat=n):
             t = np.array(tup, np.uint8)

@@ -100,8 +100,6 @@ def _cases(p):
                                   BAD_ARG, "null"),
         "b200sa_lcp_sharded": (lambda L, h: L.b200sa_lcp_sharded(h, None, 8, None, None, 0, None), BAD_ARG, "null"),
         "b200sa_last_stats": (lambda L, h: L.b200sa_last_stats(h, None), BAD_ARG, "null"),
-        "b200sa_test_classify": (lambda L, h: L.b200sa_test_classify(h, None, 8, None, None, None, None, 0, None),
-                                 BAD_ARG, "null"),
         "b200sa_test_classify_fused": (lambda L, h: L.b200sa_test_classify_fused(h, None, 8, None, None, None, None, 0,
                                                                                  None), BAD_ARG, "null"),
         "b200sa_test_scan": (lambda L, h: L.b200sa_test_scan(h, None, 8, 0, None, None), BAD_ARG, "null"),

@@ -70,7 +70,7 @@ def test_sort_pairs64(ctx, n, bits):
     assert np.array_equal(v, vals[order])
 
 
-def _classify(ctx, t, fused=False):
+def _classify(ctx, t):
     n = len(t)
     nw = (n + 31) // 32
     st = np.zeros(nw, dtype=np.uint32)
@@ -78,12 +78,10 @@ def _classify(ctx, t, fused=False):
     hist = np.zeros(768, dtype=np.uint32)
     pos = np.zeros(max(1, n // 2 + 1), dtype=np.uint32)
     m = ctypes.c_uint64(0)
-    fn = _lib.lib().b200sa_test_classify_fused if fused else _lib.lib().b200sa_test_classify
-    _check(ctx, fn(ctx._h, t.ctypes.data, n, st.ctypes.data, lm.ctypes.data,
-                   hist.ctypes.data, pos.ctypes.data, len(pos), ctypes.byref(m)))
+    _check(ctx, _lib.lib().b200sa_test_classify_fused(ctx._h, t.ctypes.data, n, st.ctypes.data, lm.ctypes.data,
+                                                      hist.ctypes.data, pos.ctypes.data, len(pos), ctypes.byref(m)))
     bits = lambda w: np.unpackbits(w.view(np.uint8), bitorder="little")[:n]
-    p = pos[: m.value]
-    return bits(st), bits(lm), hist, (p[::-1] if fused else p)      # the fused kernel lists positions from the end
+    return bits(st), bits(lm), hist, pos[: m.value][::-1]      # the fused kernel lists positions from the end
 
 
 def _classify_cases():
@@ -102,15 +100,11 @@ def _classify_cases():
     return out
 
 
-@pytest.mark.parametrize("fused", [False, True, "tma"], ids=["three_kernel", "fused", "fused_bulk_copy"])
 @pytest.mark.parametrize("name,t", _classify_cases(), ids=lambda x: x if isinstance(x, str) else "")
-def test_classify(ctx, name, t, fused, monkeypatch):
-    if fused == "tma":                        # tile loads by cp.async.bulk + mbarrier (opt-in variant)
-        monkeypatch.setenv("B200SA_CLASSIFY_TMA", "1")
-    fused = bool(fused)
+def test_classify(ctx, name, t):
     t = np.ascontiguousarray(t)
     ty = oracle.types(t)                      # 0 S, 1 L, 2 Valley (reference semantics)
-    sbit, lbit, hist, pos = _classify(ctx, t, fused)
+    sbit, lbit, hist, pos = _classify(ctx, t)
     assert np.array_equal(sbit, (ty != 1).astype(np.uint8))
     assert np.array_equal(lbit, (ty == 2).astype(np.uint8))
     assert np.array_equal(pos, np.flatnonzero(ty == 2).astype(np.uint32))

@@ -8,8 +8,7 @@ A one-element add on the build's stream marks the start of every step, so the wi
 the events between its marker and its first `k_os_pass`.  Prints one JSON line: the card, its power
 limit, the mean time per step of every kernel and memset of the window, the idle time between them
 (split into the gap after the device-to-host copy of m and sigma -- the host read -- and the rest)
-and the window's length.  `--env NAME=VALUE` sets a library switch first (e.g.
-B200SA_CLASSIFY_BYTES=1)."""
+and the window's length.  `--env NAME=VALUE` sets a library switch first."""
 import argparse
 import json
 import os

@@ -18,6 +18,6 @@ cap() {  # name regex skip count
 }
 cap induce 'k_induce' 4 4
 cap ospass 'k_os_pass' 12 3
-cap stream 'k_cls_types|k_cls_block_state|k_pack|k_name_flags|k_lcp_direct|k_lms_positions|k_unrename' 7 7
+cap stream 'k_cls_block_state|k_pack|k_name_flags|k_lcp_direct|k_unrename' 7 7
 cap scans 'k_scan_apply|k_scan_reduce|k_os_hist|k_multi_key_list' 20 8
 du -sh gpurun_out

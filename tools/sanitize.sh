@@ -1,7 +1,7 @@
 #!/bin/bash
 # compute-sanitizer on small builds: every path of round 2 (direct / robust LMS sort, the 2-bit bucket sort and its
 # overflow, both induce kernels with and without cascade steps,
-# fused byte and packed classifiers (and the byte one forced on 2-bit text), sharded world-1 entry points, LCP paths, rows f, the suffix tree, the document suffix array,
+# fused byte and packed classifiers, sharded world-1 entry points, LCP paths, rows f, the suffix tree, the document suffix array,
 # the local-sort overflow, the direct path's probe and 64-bit round-0 keys)
 mkdir -p gpurun_out
 cat > /tmp/san.py <<'PY'
@@ -26,15 +26,12 @@ cases.append(("short_runs", np.concatenate(runs * 8)))
 # 2-bit text with one top-16 bucket of > 4096 LMS suffixes: k_lms_bucket_sort overflows, the four-pass sort reruns
 fill = np.frombuffer(b"ACGT", np.uint8)[rng.integers(0, 4, (4200, 6))]
 cases.append(("bucket_overflow", np.concatenate([gen.dna(20000)] + [np.concatenate([np.frombuffer(b"TACGTACGTC", np.uint8), f]) for f in fill] + [gen.dna(20000)])))
-for variant in ("", "1", "6:no_cascade", "6:cascade_4096", "6:classify_tma", "6:classify_bytes"):
-    os.environ.pop("B200SA_NO_CASCADE", None); os.environ.pop("B200SA_CASCADE_MAX", None); os.environ.pop("B200SA_CLASSIFY_TMA", None)
-    os.environ.pop("B200SA_CLASSIFY_BYTES", None)
+for variant in ("", "1", "6:no_cascade", "6:cascade_4096"):
+    os.environ.pop("B200SA_NO_CASCADE", None); os.environ.pop("B200SA_CASCADE_MAX", None)
     if variant:
         os.environ["B200SA_INDUCE"] = variant[0]
     if variant.endswith("no_cascade"): os.environ["B200SA_NO_CASCADE"] = "1"
     if variant.endswith("cascade_4096"): os.environ["B200SA_CASCADE_MAX"] = "4096"
-    if variant.endswith("classify_tma"): os.environ["B200SA_CLASSIFY_TMA"] = "1"
-    if variant.endswith("classify_bytes"): os.environ["B200SA_CLASSIFY_BYTES"] = "1"
     c2 = _lib.Context(0)
     for name, t in (cases if not variant else cases[:2] + cases[4:5] + cases[-1:]):
         sa, lcp = c2.build_lcp(t)
@@ -42,7 +39,7 @@ for variant in ("", "1", "6:no_cascade", "6:cascade_4096", "6:classify_tma", "6:
         assert np.array_equal(sa, want), (variant, name)
         assert np.array_equal(lcp, oracle.lcp_kasai(t, want)), (variant, name)
     c2.close()
-for k in ("B200SA_INDUCE", "B200SA_NO_CASCADE", "B200SA_CASCADE_MAX", "B200SA_CLASSIFY_TMA", "B200SA_CLASSIFY_BYTES"):
+for k in ("B200SA_INDUCE", "B200SA_NO_CASCADE", "B200SA_CASCADE_MAX"):
     os.environ.pop(k, None)
 os.environ["B200SA_LMS_SORT4"] = "1"            # the four-pass LMS sort on 2-bit text
 for name, t in cases[:1] + cases[-1:]:
@@ -65,9 +62,6 @@ for name, t in cases[:4]:
     os.environ["B200SA_NO_DIRECT"] = "1"
     assert np.array_equal(ctx.build(t), want), name
     del os.environ["B200SA_NO_DIRECT"]
-    os.environ["B200SA_CLASSIFY_V1"] = "1"
-    assert np.array_equal(ctx.build(t), want), name
-    del os.environ["B200SA_CLASSIFY_V1"]
     d_t = torch.from_numpy(t.copy()).cuda()
     g, nm, st = sharded.lms_sort_sharded(ctx, d_t)
     d_sa = torch.from_numpy(want.astype(np.int64)).cuda().to(torch.int32)
